@@ -49,9 +49,12 @@ typedef struct {
   uint32_t turbo_max_iter; /* max-log-MAP iterations, >= 1 (SURVEY.md App. B.7) */
   int32_t  device;         /* CUDA device ordinal */
   uint32_t flags;          /* LTEPHY_FLAG_* */
-  uint32_t symbol_sz;      /* FFT size of one OFDM symbol = samples per subframe / 15.  0: the standard LTE rate (128 * 2^k: 2048 at 100 PRB,
-                              30.72 Msps).  srsRAN built without FORCE_STANDARD_RATE -- the reference's default, CMakeLists.txt:289-292 --
-                              samples 25 / 50 / 100 PRB at 3/4 of that (384 / 768 / 1536, srsran_symbol_sz): pass that value then. */
+  uint32_t symbol_sz;      /* FFT size of one OFDM symbol = samples per subframe / 15: 2^k or 3 * 2^k (2^k >= 128), at most
+                              2048 and more than the 12 * nof_prb sub-carriers.
+                              0: 256 at 15 PRB, 512 at 25, 1024 at 50, 2048 at 75 and 100 PRB (2048 = 30.72 Msps).  At 75 PRB that is not
+                              the 3GPP rate: a 15 MHz capture at 23.04 Msps needs 1536.  srsRAN built without FORCE_STANDARD_RATE -- the
+                              reference's default, CMakeLists.txt:289-292 -- samples 25 / 50 / 75 / 100 PRB at 384 / 768 / 1024 / 1536
+                              (srsran_symbol_sz): pass that value then. */
   uint32_t phich_resources; /* phich-Resource of the MIB as srsran_phich_r_t (srsran_cell_t.phich_resources): 0 = Ng 1/6 (what the reference presets in file
                                mode, src/src/LTESniffer_Core.cc:242-247), 1 = 1/2, 2 = 1, 3 = 2.  Sets the PHICH groups of symbol 0 and with them the
                                CCE grid of the PDCCH. */

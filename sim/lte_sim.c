@@ -251,7 +251,7 @@ int lte_sim_subframe(lte_sim_t* s, uint32_t tti, cf_t* iq, lte_sim_truth_t* trut
     const uint32_t sfn = (tti / 10) % 1024;
     uint8_t        c40[40], d120[120], *e = (uint8_t*)malloc(1920), *sc = (uint8_t*)malloc(1920);
     cf_t*          dq = (cf_t*)malloc(sizeof(cf_t) * 960);
-    lte_mib_pack(N, 0, 0, sfn, c40);
+    lte_mib_pack(N, cell->phich_ext, cell->phich_ng, sfn, c40); /* the PHICH configuration this cell's control region is mapped with */
     const uint32_t crc = lte_crc(LTE_CRC16, 16, c40, 24) ^ lte_pbch_crc_mask(cell->nof_ports);
     for (int i = 0; i < 16; i++) c40[24 + i] = (crc >> (15 - i)) & 1;
     lte_conv_encode(c40, 40, d120);

@@ -16,14 +16,20 @@ pytestmark = pytest.mark.gpu
     ("cfg1_10sf_1rnti_tm1_qpsk", Cell(100, 1, 1, 1), 10, dict(seed=1, cfi=2, nof_ues=1, tm=1, mcs_min=5, mcs_max=5, snr_db=30.0, fixed_L=2, si_period=5)),
     ("cfg2_like_150ue_tm3", Cell(100, 2, 7, 2), 40, dict(seed=2, cfi=3, nof_ues=150, dl_min=8, dl_max=12, tm=3, mcs_min=17, mcs_max=26, snr_db=28.0, full_band=1)),
     ("mixed_10MHz", Cell(50, 2, 301, 2), 40, dict(seed=3, cfi=3, nof_ues=10, dl_min=3, dl_max=5, ul_min=1, ul_max=2, tm=13, mcs_min=2, mcs_max=18, snr_db=25.0, chan_delay=5)),
+    # Cell(nof_prb, ports, cell id, antennas, symbol size, phich-Resource Ng (3: Ng = 2), phich-Duration extended)
+    ("mixed_3MHz", Cell(15, 2, 33, 2), 20, dict(seed=5, cfi=3, nof_ues=6, dl_min=1, dl_max=3, ul_min=1, ul_max=1, tm=13, mcs_min=2, mcs_max=18, snr_db=26.0, si_period=4)),
+    ("mixed_15MHz_1536", Cell(75, 2, 34, 2, 1536), 20, dict(seed=6, cfi=2, nof_ues=10, dl_min=2, dl_max=5, ul_min=1, ul_max=2, tm=13, mcs_min=2, mcs_max=22, snr_db=26.0,
+                                                            chan_delay=4)),
+    ("tm3_20MHz_ng2_ext", Cell(100, 2, 35, 2, 0, 3, 1), 20, dict(seed=7, cfi=3, nof_ues=12, dl_min=3, dl_max=6, tm=3, mcs_min=4, mcs_max=22, snr_db=27.0)),
 ])
 def test_decode_subframes_matches_oracle_pipeline(infra, phylib, name, cell, n, kw):
     sim, iq, tti, truths, payloads = make_capture(cell, n, **kw)
     walk = ltelib.OracleWalk(cell, golden="oraclewalk_" + name)
     ref = ltelib.oracle_pipeline(cell, iq, tti, walk=walk)
     walk.save_record()
-    phy = capi.LtePhy(cell.nof_prb, cell.nof_ports, cell.cell_id, cell.nof_rx, max_subframes=n, turbo_max_iter=8, flags=capi.FLAG_SKIP_LOW_POWER)
-    srch = capi.Search(cell.nof_prb, cell.nof_ports, cell.cell_id, cell.nof_rx)
+    phy = capi.LtePhy(cell.nof_prb, cell.nof_ports, cell.cell_id, cell.nof_rx, max_subframes=n, turbo_max_iter=8, flags=capi.FLAG_SKIP_LOW_POWER,
+                      symbol_sz=cell.symbol_sz, phich_resources=cell.phich_ng, phich_length=cell.phich_ext)
+    srch = capi.Search(cell.nof_prb, cell.nof_ports, cell.cell_id, cell.nof_rx, phich_resources=cell.phich_ng | (cell.phich_ext << 8))
     info, dcis, tbs, payload = capi.decode_subframes(phy, srch, iq, tti)
     k = 0
     ntb_ok = 0

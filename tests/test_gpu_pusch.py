@@ -11,8 +11,11 @@ pytestmark = pytest.mark.gpu
 
 
 @pytest.mark.parametrize("cell,snr,nsf,ngr,table", [(Cell(50, 1, 17, 1), 25.0, 3, 4, 1), (Cell(100, 2, 301, 2), 23.0, 3, 6, 1), (Cell(25, 1, 5, 1), 20.0, 2, 2, 1),
-                                                      (Cell(50, 1, 9, 1), 34.0, 3, 4, 2)])     # table 2: 36.213 Table 8.6.1-3, Qm up to 8
+                                                      (Cell(50, 1, 9, 1), 34.0, 3, 4, 2),      # table 2: 36.213 Table 8.6.1-3, Qm up to 8
+                                                      (Cell(15, 1, 6, 1), 22.0, 3, 2, 1), (Cell(15, 2, 7, 2), 24.0, 2, 3, 2),
+                                                      (Cell(75, 1, 18, 1), 23.0, 3, 4, 1), (Cell(75, 2, 19, 2), 30.0, 2, 5, 2)])
 def test_pusch_bit_exact(infra, phylib, cell, snr, nsf, ngr, table):
+    """at 75 PRB the first subframe carries one grant of the whole band (75 = 3 * 5^2 PRB: the largest three- and five-point DFT steps)"""
     s = Sim(cell=cell, seed=21, snr_db=snr, nof_ues=1, chan_delay=3)
     o = Oracle(cell)
     rng = np.random.default_rng(cell.nof_prb)
@@ -23,7 +26,9 @@ def test_pusch_bit_exact(infra, phylib, cell, snr, nsf, ngr, table):
     tti = np.arange(4, 4 + nsf, dtype=np.uint32)
     grants_o, pls, offs, grants_p = [], [], [], []
     for i in range(nsf):
-        gr = ltelib.make_ul_grants(cell, rng, ngr, table=table)
+        full = i == 0 and cell.nof_prb == 75
+        gr = ltelib.make_ul_grants(cell, rng, 1 if full else ngr, table=table, min_prb=cell.nof_prb if full else 3)
+        assert not full or (gr[0].L_prb, gr[0].n_prb) == (75, 0)
         x, pl, off = ltelib.sim_ul_subframe(s, int(tti[i]), ucfg, gr)
         iq[i] = x
         grants_o.append(gr), pls.append(pl), offs.append(off)
@@ -116,7 +121,7 @@ def test_pusch_uci_multiplexed(infra, phylib):
 
 
 def test_pusch_hopping_group_hopping_timing(infra, phylib):
-    """type-1 hopping (slot 1 elsewhere), DMRS group / sequence hopping, timing offsets: product == oracle, estimate == truth"""
+    """type-1 hopping (slot 1 elsewhere), DMRS group / sequence hopping, timing offsets: product == oracle, estimate == truth; at 50 and at 75 PRB"""
     cell = Cell(50, 1, 301, 1)
     import ctypes as C
     S = ltelib.sim()
@@ -134,6 +139,9 @@ def test_pusch_hopping_group_hopping_timing(infra, phylib):
         g.ta_us = float(rng.uniform(-1.0, 1.0))
     nok, k = _run_ul_case(Cell(100, 1, 4, 1), UlCfg(n_dmrs1=0, delta_ss=0, group_hopping=1), ta_only, ngr=5, nsf=2, seed=70)
     assert nok == k
+    cell = Cell(75, 1, 302, 1)                      # hop() reads the cell at call time
+    nok, k = _run_ul_case(cell, UlCfg(n_dmrs1=1, delta_ss=5, group_hopping=1), hop, ngr=2, nsf=2, seed=71, min_prb=5)
+    assert nok == k == 4
 
 
 def test_pusch_every_dft_size(infra, phylib):

@@ -20,7 +20,27 @@ CASES = {
     "10MHz_tm3_tm4_cw_swap": dict(cell=Cell(50, 2, 21, 2), n=4, kw=dict(seed=16, cfi=2, nof_ues=8, dl_min=2, dl_max=4, tm=3, mcs_min=6, mcs_max=24, snr_db=29.0, tb_swap=1)),
     "10MHz_tm4_cw_swap": dict(cell=Cell(50, 2, 11, 2), n=3, kw=dict(seed=17, cfi=2, nof_ues=8, dl_min=2, dl_max=4, tm=4, mcs_min=4, mcs_max=20, snr_db=33.0, tb_swap=1)),
     "5MHz_2p1a": dict(cell=Cell(25, 2, 150, 1), n=3, kw=dict(seed=14, cfi=2, nof_ues=5, dl_min=1, dl_max=3, tm=1, mcs_min=2, mcs_max=12, snr_db=25.0, tti0=9)),
+    # Cell(nof_prb, ports, cell id, antennas, symbol size (0: the standard one), phich-Resource Ng (0..3 = 1/6, 1/2, 1, 2), phich-Duration extended).
+    # Every case decodes subframe 0 or 5: PBCH / synchronisation REs cut PRBs in half there at odd PRB counts.
+    "3MHz_1p1a_cfi3": dict(cell=Cell(15, 1, 31, 1), n=3, kw=dict(seed=41, cfi=3, nof_ues=4, dl_min=1, dl_max=3, tm=1, mcs_min=2, mcs_max=20, snr_db=28.0, si_period=2, tti0=4)),
+    "3MHz_2p2a_384": dict(cell=Cell(15, 2, 32, 2, 384), n=3, kw=dict(seed=42, cfi=2, nof_ues=4, dl_min=1, dl_max=3, tm=13, mcs_min=2, mcs_max=20, snr_db=28.0, tti0=9)),
+    "15MHz_2p2a_mix_delay": dict(cell=Cell(75, 2, 301, 2), n=3, kw=dict(seed=43, cfi=3, nof_ues=12, dl_min=3, dl_max=6, ul_min=1, ul_max=2, tm=13, mcs_min=0, mcs_max=24, snr_db=25.0, chan_delay=5)),
+    "15MHz_1p1a_1536": dict(cell=Cell(75, 1, 76, 1, 1536), n=3, kw=dict(seed=44, cfi=2, nof_ues=6, dl_min=2, dl_max=4, tm=1, mcs_min=2, mcs_max=24, snr_db=28.0, tti0=5)),
+    "15MHz_tm4_256qam_1024": dict(cell=Cell(75, 2, 77, 2, 1024), n=3, kw=dict(seed=45, cfi=2, nof_ues=8, dl_min=2, dl_max=4, tm=4, mcs_min=4, mcs_max=22, snr_db=33.0, alt_table=1, tti0=9)),
+    "10MHz_1p1a": dict(cell=Cell(50, 1, 9, 1), n=3, kw=dict(seed=46, cfi=2, nof_ues=6, dl_min=2, dl_max=4, tm=1, mcs_min=2, mcs_max=24, snr_db=27.0, si_period=3)),
+    "20MHz_ng2": dict(cell=Cell(100, 2, 301, 2, 0, 3), n=3, kw=dict(seed=47, cfi=2, nof_ues=10, dl_min=3, dl_max=6, tm=3, mcs_min=4, mcs_max=22, snr_db=27.0, tti0=4)),
+    "5MHz_ng1_ext_cfi3": dict(cell=Cell(25, 2, 150, 2, 0, 2, 1), n=3, kw=dict(seed=48, cfi=3, nof_ues=5, dl_min=1, dl_max=3, tm=13, mcs_min=2, mcs_max=20, snr_db=27.0, tti0=5)),
+    "15MHz_ng_half_ext": dict(cell=Cell(75, 2, 17, 2, 0, 1, 1), n=3, kw=dict(seed=49, cfi=3, nof_ues=8, dl_min=2, dl_max=5, tm=3, mcs_min=2, mcs_max=22, snr_db=27.0, tti0=9)),
 }
+
+
+def new_phy(cell, n, flags=0):
+    return capi.LtePhy(cell.nof_prb, cell.nof_ports, cell.cell_id, cell.nof_rx, max_subframes=n, turbo_max_iter=8, flags=flags, symbol_sz=cell.symbol_sz,
+                       phich_resources=cell.phich_ng, phich_length=cell.phich_ext)
+
+
+def new_search(cell):
+    return capi.Search(cell.nof_prb, cell.nof_ports, cell.cell_id, cell.nof_rx, phich_resources=cell.phich_ng | (cell.phich_ext << 8))
 
 
 @pytest.fixture(scope="module", params=list(CASES))
@@ -30,7 +50,8 @@ def case(request, infra, phylib):
     sim, iq, tti, truths, payloads = make_capture(cell, c["n"], **c["kw"])
     o = Oracle(cell)
     ref = oracle_frontend(o, iq, tti)
-    phy = capi.LtePhy(cell.nof_prb, cell.nof_ports, cell.cell_id, cell.nof_rx, max_subframes=c["n"], turbo_max_iter=8)
+    assert any(int(t) % 5 == 0 for t in tti), "every case decodes subframe 0 or 5"
+    phy = new_phy(cell, c["n"])
     phy.submit_iq(iq, tti)
     info, cands = phy.get_phase_a()
     yield dict(name=request.param, alt=c["kw"].get("alt_table", 0), cell=cell, iq=iq, tti=tti, truths=truths, payloads=payloads, o=o, ref=ref, phy=phy, info=info, cands=cands, n=c["n"])
@@ -79,11 +100,12 @@ def test_dci_table_bit_exact(case):
     distinct = {}
     for f in range(9):
         distinct[sidx[f]] = sizes[f]
-    nchecked = 0
+    nchecked = total = 0
     for i in range(n):
         r = case["ref"][i]
         nc, Ls = phy.locations(r["cfi"])
         assert case["info"][i].nof_locations == len(nc)
+        total += len(nc) * len(distinct)
         for li in range(len(nc)):
             e = r["llr"][72 * int(nc[li]):72 * int(nc[li]) + (72 << int(Ls[li]))]
             for si, nb in distinct.items():
@@ -105,7 +127,7 @@ def test_dci_table_bit_exact(case):
             c = case["cands"][i, li[0], sidx[d.format]]
             assert int(c["rnti"]) == d.rnti, "truth DCI not recovered: sf %d rnti %#x fmt %s" % (i, d.rnti, FORMATS[d.format])
             assert np.array_equal(capi.cand_bits(c["bits"], d.nbits), np.frombuffer(bytes(d.bits), np.uint8)[:d.nbits])
-    assert nchecked > 100
+    assert nchecked >= 0.9 * total, (nchecked, total)     # only an all-zero location decodes to nothing
 
 
 @pytest.mark.parametrize("flags", [0, capi.FLAG_SKIP_LOW_POWER])
@@ -114,13 +136,13 @@ def test_survivor_form_matches_host_restatement(case, flags):
     ltephy_compact_from_table applied to the GPU's own full table: same counts, location records and listed entries;
     and the walk over the survivor form accepts what the walk over the full table accepts."""
     cell, n = case["cell"], case["n"]
-    phy = capi.LtePhy(cell.nof_prb, cell.nof_ports, cell.cell_id, cell.nof_rx, max_subframes=n, turbo_max_iter=8, flags=flags)
+    phy = new_phy(cell, n, flags)
     phy.submit_iq(case["iq"], case["tti"])
     info, cands = phy.get_phase_a()
     info_c, comp = phy.get_phase_a_compact()
     assert bytes(info) == bytes(info_c)
-    sa = capi.Search(cell.nof_prb, cell.nof_ports, cell.cell_id, cell.nof_rx)
-    sb = capi.Search(cell.nof_prb, cell.nof_ports, cell.cell_id, cell.nof_rx)
+    sa = new_search(cell)
+    sb = new_search(cell)
     total = 0
     for i in range(n):
         ref = sa.compact_from_table(info[i], cands[i])[0]

@@ -129,7 +129,7 @@ def test_dci_to_grant_matches_oracle(infra):
     S = infra.sim()
     rng = np.random.default_rng(5)
     ncheck = nswap = 0
-    for cell in (Cell(100, 2, 3, 2), Cell(50, 1, 9, 1), Cell(25, 2, 100, 2), Cell(75, 2, 5, 2)):
+    for cell in (Cell(100, 2, 3, 2), Cell(50, 1, 9, 1), Cell(25, 2, 100, 2), Cell(75, 2, 5, 2), Cell(15, 1, 7, 1), Cell(15, 2, 8, 2)):
         srch = capi.Search(cell.nof_prb, cell.nof_ports, cell.cell_id, cell.nof_rx)
         for _ in range(1500):
             f = int(rng.choice([1, 2, 4, 6, 7]))

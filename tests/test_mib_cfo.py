@@ -17,11 +17,13 @@ def mib_fields(bits):
     return r, [x.value for x in v]
 
 
-@pytest.mark.parametrize("cellp,snr", [((25, 1, 3, 1), 8.0), ((50, 2, 301, 2), 6.0), ((100, 2, 77, 2), 10.0), ((15, 1, 10, 1), 12.0)])
+@pytest.mark.parametrize("cellp,snr", [((25, 1, 3, 1), 8.0), ((50, 2, 301, 2), 6.0), ((100, 2, 77, 2), 10.0), ((15, 1, 10, 1), 12.0),
+                                      ((75, 2, 40, 2, 0, 3, 1), 8.0)])
 def test_oracle_decodes_the_simulators_pbch(infra, cellp, snr):
     cell = Cell(*cellp)
     tti0 = 10 * 517            # SFN 517 = 0b1000000101: 8 MSBs 129, position 1 in the 40 ms period
-    sim, iq, tti, truths, payloads = make_capture(cell, 41, seed=5, cfi=2, nof_ues=2, dl_min=1, dl_max=2, tm=1, snr_db=snr, pbch=1, tti0=tti0)
+    sim, iq, tti, truths, payloads = make_capture(cell, 41, seed=5, cfi=3 if cell.phich_ext else 2, nof_ues=2, dl_min=1, dl_max=2, tm=1, snr_db=snr, pbch=1,
+                                                  tti0=tti0)
     o = ltelib.Oracle(cell)
     seen = set()
     for i in range(0, 41, 10):
@@ -30,7 +32,7 @@ def test_oracle_decodes_the_simulators_pbch(infra, cellp, snr):
         sfn = (tti0 + i) // 10
         assert found == 1 and nports == cell.nof_ports and fq == sfn % 4
         r, (nof_prb, phich_ext, phich_res, sfn8) = mib_fields(mib)
-        assert r == 0 and (nof_prb, phich_ext, phich_res) == (cell.nof_prb, 0, 0) and sfn8 == (sfn // 4) * 4
+        assert r == 0 and (nof_prb, phich_ext, phich_res) == (cell.nof_prb, cell.phich_ext, cell.phich_ng) and sfn8 == (sfn // 4) * 4
         seen.add(fq)
     assert seen == {0, 1, 2, 3}
     # a subframe without PBCH (subframe 1) must not produce a MIB
@@ -63,16 +65,19 @@ def test_cfo_correction_restores_the_decode(infra):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("cellp,snr", [((25, 1, 3, 1), 8.0), ((50, 2, 301, 2), 6.0), ((100, 2, 77, 2), 2.0)])
+@pytest.mark.parametrize("cellp,snr", [((25, 1, 3, 1), 8.0), ((50, 2, 301, 2), 6.0), ((100, 2, 77, 2), 2.0), ((15, 1, 10, 1), 8.0), ((15, 2, 11, 2), 6.0),
+                                      ((75, 1, 12, 1), 8.0), ((75, 2, 40, 2, 0, 3, 1), 6.0), ((25, 2, 150, 2, 0, 2, 1), 8.0), ((100, 1, 9, 1, 0, 1, 0), 8.0)])
 def test_gpu_mib_matches_oracle(infra, phylib, cellp, snr):
     """ltephy_mib_decode == oracle PBCH decode on every subframe of the batch (found flag, port count, frame position, the 24 bits), and both
-    equal what the simulated eNB broadcast; 2 dB at 20 MHz: some frames fail in both"""
+    equal what the simulated eNB broadcast, PHICH configuration included (cellp: nof_prb, ports, cell id, antennas[, symbol_sz, Ng, extended]);
+    2 dB at 20 MHz: some frames fail in both"""
     from ltesniffer_b200 import capi
     cell = Cell(*cellp)
     tti0 = 10 * 1022
-    sim, iq, tti, truths, payloads = make_capture(cell, 42, seed=5, cfi=2, nof_ues=2, dl_min=1, dl_max=2, tm=1, snr_db=snr, pbch=1, tti0=tti0)
+    sim, iq, tti, truths, payloads = make_capture(cell, 42, seed=5, cfi=3 if cell.phich_ext else 2, nof_ues=2, dl_min=1, dl_max=2, tm=1, snr_db=snr, pbch=1,
+                                                  tti0=tti0)       # the extended duration spans three symbols: CFI 3
     o = ltelib.Oracle(cell)
-    phy = capi.LtePhy(cell.nof_prb, cell.nof_ports, cell.cell_id, cell.nof_rx, max_subframes=42)
+    phy = capi.LtePhy(cell.nof_prb, cell.nof_ports, cell.cell_id, cell.nof_rx, max_subframes=42, phich_resources=cell.phich_ng, phich_length=cell.phich_ext)
     phy.submit_iq(iq, tti)
     phy.get_phase_a(want_cands=False)
     mibs = phy.mib_decode()
@@ -91,7 +96,7 @@ def test_gpu_mib_matches_oracle(infra, phylib, cellp, snr):
         packed = np.packbits(bits)
         assert (m.nof_ports, m.sfn_offset, bytes(m.bch_payload)) == (nports, fq, bytes(packed))
         sfn = (int(tti[i]) // 10) % 1024
-        assert (m.nof_prb, m.phich_length, m.phich_resources, m.sfn) == (cell.nof_prb, 0, 0, sfn)
+        assert (m.nof_prb, m.phich_length, m.phich_resources, m.sfn) == (cell.nof_prb, cell.phich_ext, cell.phich_ng, sfn)
     assert nfound >= 3
     phy.close()
 

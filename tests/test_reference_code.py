@@ -379,7 +379,7 @@ def test_rb_power_equals_reference(infra):
 
 
 @needs_ref
-@pytest.mark.parametrize("cellp", [(100, 2, 7, 2), (75, 2, 3, 2), (50, 2, 301, 2), (25, 1, 5, 1)])
+@pytest.mark.parametrize("cellp", [(100, 2, 7, 2), (75, 2, 3, 2), (50, 2, 301, 2), (25, 1, 5, 1), (15, 1, 4, 1), (15, 2, 9, 2)])
 def test_random_dcis_grants_equal_reference(infra, cellp):
     """2 500 random payloads per cell over the downlink formats LTESniffer decodes (1, 1A, 1C, 2, 2A), C-RNTIs and the SI / P / RA-RNTIs, every CFI
     and subframe index: ltephy_dci_to_grant against the reference's own dl_sniffer_ra_dl_dci_to_grant + dl_sniffer_config_mimo
@@ -423,7 +423,8 @@ def test_random_dcis_grants_equal_reference(infra, cellp):
 
 
 @needs_ref
-@pytest.mark.parametrize("cellp,n_rb_ho", [((100, 2, 7, 2), 0), ((100, 2, 7, 2), 5), ((75, 2, 3, 2), 2), ((50, 2, 301, 2), 8), ((25, 1, 5, 1), 0), ((25, 1, 5, 1), 3)])
+@pytest.mark.parametrize("cellp,n_rb_ho", [((100, 2, 7, 2), 0), ((100, 2, 7, 2), 5), ((75, 2, 3, 2), 2), ((50, 2, 301, 2), 8), ((25, 1, 5, 1), 0), ((25, 1, 5, 1), 3),
+                                           ((15, 2, 9, 2), 0), ((15, 1, 4, 1), 2)])
 def test_random_format0_grants_equal_reference(infra, cellp, n_rb_ho):
     """3 000 random format-0 payloads per cell and pusch-HoppingOffset (half of them with the hopping flag set, i.e. all four hop kinds of 36.213
     Tables 8.4-1/2): ltephy_ul_dci_to_grant against the reference's own ul_sniffer_ra_ul_dci_to_grant / ulsniffer_ra_ul_dci_to_grant_256 over
@@ -469,7 +470,8 @@ def test_random_format0_grants_equal_reference(infra, cellp, n_rb_ho):
 
 
 @needs_ref
-@pytest.mark.parametrize("cellp,n_rb_ho", [((100, 2, 7, 2), 0), ((100, 2, 7, 2), 6), ((50, 2, 301, 2), 0), ((25, 1, 5, 1), 2)])
+@pytest.mark.parametrize("cellp,n_rb_ho", [((100, 2, 7, 2), 0), ((100, 2, 7, 2), 6), ((50, 2, 301, 2), 0), ((25, 1, 5, 1), 2),
+                                           ((15, 2, 9, 2), 0), ((15, 1, 4, 1), 1)])
 def test_random_rar_grants_equal_reference(infra, cellp, n_rb_ho):
     """4 000 random 20-bit RAR grants per cell (inside random MAC RAR PDUs of 1-3 RARs): ltephy_rar_unpack against the reference's own
     ul_sniffer_dci_rar_unpack + ul_sniffer_dci_rar_to_ul_dci + ul_sniffer_ra_ul_dci_to_grant (falcon_dci.c:648-684, ul_sniffer_pusch.c:205-245, called at

@@ -1,13 +1,14 @@
 """Symbol sizes of srsRAN's default build (3/4 of the standard LTE rate: srsran_symbol_sz = 1536 at 100 PRB, 768 at 50, 384 at 25 -- the rate a
 stock LTESniffer records at, srsran_sampling_freq_hz at src/src/LTESniffer_Core.cc:222): the simulator, the oracle and the product handle the
-3 * 2^k-point OFDM symbols; GPU: symbols bit-exact against the oracle, and the whole pipeline decodes such a capture."""
+3 * 2^k-point OFDM symbols; GPU: symbols bit-exact against the oracle, and the whole pipeline decodes such a capture.  Also the other sizes a 15 MHz
+capture comes in (1536 at the 3GPP rate of 23.04 Msps, 1024 from srsRAN's default build; the library's default there is 2048) and a 3 * 2^k size at 3 MHz."""
 import numpy as np
 import pytest
 import ltelib
 from ltelib import Cell
 from helpers import make_capture, oracle_frontend, truth_grants
 
-CASES = [(100, 1536), (50, 768), (25, 384)]
+CASES = [(100, 1536), (50, 768), (25, 384), (75, 1536), (75, 1024), (15, 384)]     # 75 PRB: the 3GPP 15 MHz rate, srsRAN's 75 PRB size; 15 PRB: 3 * 2^7
 KW = dict(seed=3, cfi=2, nof_ues=3, dl_min=2, dl_max=2, tm=13, mcs_min=8, mcs_max=20, snr_db=28.0)
 
 
