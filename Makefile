@@ -5,13 +5,17 @@ CXX ?= g++
 CFLAGS = -O3 -g -fPIC -std=gnu11 -Wall -Wno-unused-function -ffp-contract=off -fno-fast-math
 CXXFLAGS = -O2 -g -fPIC -std=c++17 -Wall -ffp-contract=off -fno-fast-math
 
-all: sim/libltesim.so oracle/liblteoracle.so
+all: sim/libltesim.so oracle/liblteoracle.so oracle/liblteosync.so
 
 sim/libltesim.so: sim/lte_common.c sim/lte_sim.c sim/lte_common.h sim/lte_sim.h include/lte_tables.h
 	$(CC) $(CFLAGS) -shared -o $@ sim/lte_common.c sim/lte_sim.c -lm
 
 oracle/liblteoracle.so: oracle/lte_oracle.c oracle/lte_oracle.h sim/lte_common.c sim/lte_common.h include/lte_tables.h
 	$(CC) $(CFLAGS) -shared -o $@ oracle/lte_oracle.c sim/lte_common.c -lm -lpthread
+
+# cell search oracle: lteo_det_sum and the shared PSS / SSS sequences come from liblteoracle.so
+oracle/liblteosync.so: oracle/lte_sync_oracle.c oracle/lte_sync_oracle.h oracle/lte_oracle.h oracle/liblteoracle.so
+	$(CC) $(CFLAGS) -shared -o $@ oracle/lte_sync_oracle.c -Loracle -llteoracle -Wl,-rpath,'$$ORIGIN' -lm
 
 # C++ example of the C-ABI (needs ltesniffer_b200/libltephy_b200.so, built by ltesniffer_b200/build.py)
 examples/offline_decode: examples/offline_decode.cpp include/ltephy_b200.h include/ltephy_search.h include/ltephy_sinks.h
@@ -20,8 +24,11 @@ examples/offline_decode: examples/offline_decode.cpp include/ltephy_b200.h inclu
 examples/offline_ul: examples/offline_ul.cpp include/ltephy_b200.h include/ltephy_search.h include/ltephy_sinks.h
 	$(CXX) -O2 -std=c++17 -Wall -Iinclude -o $@ examples/offline_ul.cpp -Lltesniffer_b200 -lltephy_b200 -Wl,-rpath,'$$ORIGIN/../ltesniffer_b200'
 
+examples/cell_search: examples/cell_search.cpp include/ltephy_b200.h
+	$(CXX) -O2 -std=c++17 -Wall -Iinclude -o $@ examples/cell_search.cpp -Lltesniffer_b200 -lltephy_b200 -Wl,-rpath,'$$ORIGIN/../ltesniffer_b200'
+
 examples/compat_check: examples/compat_check.cpp compat/srsran/srsran.h include/ltephy_b200.h
 	$(CXX) -O2 -std=c++17 -Wall -Iinclude -Icompat -o $@ examples/compat_check.cpp -Lltesniffer_b200 -lltephy_srsran_compat -lltephy_b200 -Wl,-rpath,'$$ORIGIN/../ltesniffer_b200'
 
 clean:
-	rm -f sim/*.so oracle/*.so examples/offline_decode examples/offline_ul examples/compat_check
+	rm -f sim/*.so oracle/*.so examples/offline_decode examples/offline_ul examples/compat_check examples/cell_search

@@ -228,6 +228,46 @@ typedef struct {
  * own (no soft combining across the 40 ms period). */
 int ltephy_mib_decode(ltephy_t* h, ltephy_mib_t* out);
 
+/* Cell search: the PSS / SSS half of rf_search_and_decode_mib (reference src/src/LTESniffer_Core.cc:193-204) on a continuous FDD recording with
+ * normal CP.  For each N_ID_2 it finds the PSS timing, the carrier offset and N_ID_1 with the subframe-0 / subframe-5 decision, and from them the
+ * first sample of a subframe 0 -- what ltephy_create (PCI), ltephy_submit_iq (subframe alignment) and ltephy_set_cfo need.  The algorithm and
+ * its summation orders are DESIGN.md §2 ("cell search"); the CPU oracle lteo_cell_search defines the results bit for bit. */
+typedef struct ltephy_sync ltephy_sync_t;
+typedef struct {
+  uint32_t symbol_sz;   /* N: 128, 256, 384, 512, 768, 1024, 1536 or 2048 samples per symbol (sample rate 15 kHz * N) */
+  uint32_t nof_rx;      /* 1 or 2 antennas */
+  uint64_t max_samples; /* longest recording per antenna this handle accepts (device memory is sized for it) */
+  int32_t  device;      /* CUDA device ordinal */
+  uint32_t reserved[4];
+} ltephy_sync_cfg_t;
+typedef struct {
+  uint8_t  detected;        /* psr >= 2.5 and sss_ratio >= 1.75 */
+  uint8_t  n_id_2, pad[2];
+  uint16_t n_id_1, pci;     /* n_id_1 = pci = 0xFFFF when no half-frame had both PSS and SSS inside the capture */
+  uint64_t frame_offset;    /* first sample of a subframe 0, in [0, 150 * symbol_sz) */
+  uint32_t nof_half_frames; /* half-frames whose PSS and SSS both lie inside the capture */
+  float    pss_peak;        /* PSS metric at the refined timing (0..1) */
+  float    psr;             /* folded coarse peak / the largest folded value more than 2 bins away */
+  float    sss_peak, sss_ratio; /* best SSS hypothesis, and its ratio to the second best */
+  float    cfo_hz;          /* carrier offset: the value to pass to ltephy_set_cfo */
+  float    cfo_re, cfo_im;  /* the device sum it comes from (cfo_hz = atan2f(im, re) * 15000 / pi) */
+} ltephy_cell_t;
+int  ltephy_sync_create(const ltephy_sync_cfg_t* cfg, ltephy_sync_t** h);
+void ltephy_sync_destroy(ltephy_sync_t* h);
+/* iq: cf32 [nof_rx][nof_samples], antenna-major, host memory; HF + N <= nof_samples <= max_samples (HF = 75 N, 5 ms).  out[3]: one result per
+ * N_ID_2, by pss_peak descending, ties to the lower N_ID_2.  Blocks until done. */
+int  ltephy_cell_search(ltephy_sync_t* h, const float* iq, uint64_t nof_samples, ltephy_cell_t out[3]);
+/* same, with the samples already in device memory */
+int  ltephy_cell_search_device(ltephy_sync_t* h, const void* iq_dev, uint64_t nof_samples, ltephy_cell_t out[3]);
+enum {
+  LTEPHY_SYNC_TAP_COARSE  = 0, /* f32 [3][9600]       folded coarse metric per N_ID_2 */
+  LTEPHY_SYNC_TAP_REFINED = 1, /* f32 [3][2 D - 1]    folded stride-1 metric around the coarse peak, D = N / 128 */
+  LTEPHY_SYNC_TAP_CFO     = 2, /* f32 [3][2]          the CFO sum S (re, im) */
+  LTEPHY_SYNC_TAP_SSS     = 3  /* f32 [3][168][2]     the SSS table A(N_ID_1, q) */
+};
+/* copies an intermediate of the last search; bytes must be at least its size */
+int  ltephy_sync_tap(ltephy_sync_t* h, int what, void* dst, size_t bytes);
+
 /* nslots HARQ slots of LTEPHY_HARQ_SLOT_BYTES each (150 RNTIs x 8 processes x 2 TBs = 2400 slots = 1.4 GB); contents survive across batches */
 int ltephy_harq_reserve(ltephy_t* h, uint32_t nslots);
 

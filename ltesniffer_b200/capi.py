@@ -672,3 +672,81 @@ def pack_phase_a(phy):
     _bind_search(phy.L)
     phy._chk(phy.L.ltephy_pack_phase_a(phy.h, _p(out), out.nbytes, _p(offs)), "pack_phase_a")
     return out[:offs[n]].copy(), offs
+
+
+# ------------------------------------------------------------------------------------------------
+# cell search (ltephy_sync_*, include/ltephy_b200.h)
+SYNC_TAP_COARSE, SYNC_TAP_REFINED, SYNC_TAP_CFO, SYNC_TAP_SSS = 0, 1, 2, 3
+SYNC_BINS = 9600
+
+
+class SyncCfg(C.Structure):
+    _fields_ = [("symbol_sz", C.c_uint32), ("nof_rx", C.c_uint32), ("max_samples", C.c_uint64), ("device", C.c_int32), ("reserved", C.c_uint32 * 4)]
+
+
+class CellInfo(C.Structure):
+    """ltephy_cell_t"""
+    _fields_ = [("detected", C.c_uint8), ("n_id_2", C.c_uint8), ("pad", C.c_uint8 * 2), ("n_id_1", C.c_uint16), ("pci", C.c_uint16),
+                ("frame_offset", C.c_uint64), ("nof_half_frames", C.c_uint32), ("pss_peak", C.c_float), ("psr", C.c_float), ("sss_peak", C.c_float),
+                ("sss_ratio", C.c_float), ("cfo_hz", C.c_float), ("cfo_re", C.c_float), ("cfo_im", C.c_float)]
+
+
+assert C.sizeof(CellInfo) == 48
+
+
+class CellSearch:
+    """PSS / SSS cell search of continuous recordings of symbol_sz samples per symbol and nof_rx antennas, up to max_samples per antenna."""
+
+    def __init__(self, symbol_sz, nof_rx, max_samples, device=0):
+        self.L = load_library()
+        L = self.L
+        L.ltephy_sync_create.argtypes = [C.POINTER(SyncCfg), C.POINTER(C.c_void_p)]
+        L.ltephy_sync_destroy.argtypes = [C.c_void_p]
+        L.ltephy_cell_search.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]
+        L.ltephy_cell_search_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]
+        L.ltephy_sync_tap.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t]
+        self.cfg = SyncCfg(symbol_sz=symbol_sz, nof_rx=nof_rx, max_samples=max_samples, device=device)
+        self.h = C.c_void_p()
+        r = L.ltephy_sync_create(C.byref(self.cfg), C.byref(self.h))
+        if r != 0:
+            self.h = None
+            raise RuntimeError("ltephy_sync_create failed (%d): %s" % (r, L.ltephy_last_error().decode()))
+
+    def close(self):
+        if self.h:
+            self.L.ltephy_sync_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def _done(self, r, out):
+        if r != 0:
+            raise RuntimeError("ltephy_cell_search failed (%d): %s" % (r, self.L.ltephy_last_error().decode()))
+        return [CellInfo.from_buffer_copy(out[i]) for i in range(3)]
+
+    def search(self, iq):
+        """iq: complex64 [nof_rx][nof_samples] (host) -> three CellInfo, by pss_peak descending"""
+        iq = np.ascontiguousarray(iq, np.complex64)
+        assert iq.ndim == 2 and iq.shape[0] == self.cfg.nof_rx, iq.shape
+        out = (CellInfo * 3)()
+        return self._done(self.L.ltephy_cell_search(self.h, _p(iq), iq.shape[1], out), out)
+
+    def search_device(self, iq):
+        """iq: torch complex64 tensor [nof_rx][nof_samples], contiguous, on this handle's device"""
+        assert iq.is_cuda and iq.is_contiguous() and iq.dim() == 2 and iq.shape[0] == self.cfg.nof_rx
+        out = (CellInfo * 3)()
+        return self._done(self.L.ltephy_cell_search_device(self.h, C.c_void_p(iq.data_ptr()), iq.shape[1], out), out)
+
+    def tap(self, what):
+        """intermediate of the last search as float32: coarse [3][9600], refined [3][2D-1], cfo [3][2], sss [3][168][2]"""
+        D = self.cfg.symbol_sz // 128
+        shape = {SYNC_TAP_COARSE: (3, SYNC_BINS), SYNC_TAP_REFINED: (3, 2 * D - 1), SYNC_TAP_CFO: (3, 2), SYNC_TAP_SSS: (3, 168, 2)}[what]
+        out = np.zeros(shape, np.float32)
+        r = self.L.ltephy_sync_tap(self.h, what, _p(out), out.nbytes)
+        if r != 0:
+            raise RuntimeError("ltephy_sync_tap failed (%d): %s" % (r, self.L.ltephy_last_error().decode()))
+        return out

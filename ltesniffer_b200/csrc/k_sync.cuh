@@ -1,0 +1,36 @@
+// k_sync.cuh -- arguments shared by the cell search kernels (k_sync.cu) and their host code (sync.cu).  Private to libltephy_b200.
+#pragma once
+#include <cstdint>
+#include <cuda_runtime.h>
+
+#define SYNC_BINS 9600 // coarse bins per half-frame: 75 N / D
+
+struct SyncArgs {
+  const float2* x;   // [A][lda] samples
+  uint64_t      lda, L, J; // J: coarse offsets whose window fits, (L - N) / D + 1
+  uint32_t      N, D, A, nh; // nh: half-frames with a window start below L - N + 1, (L - N) / HF + 1
+  const float2* rep; // [3][N] PSS replicas
+  const float2* W;   // [N] exp(-j 2 pi i / N)
+  float         ep[3];
+};
+
+struct SyncPeak {
+  uint32_t bin;   // coarse peak bin
+  float    peak;  // folded coarse peak
+  float    side;  // largest folded value more than 2 bins away
+  uint32_t tau;   // refined timing in [0, HF)
+  float    rpeak; // folded stride-1 metric at tau
+  float    s_re, s_im; // CFO sum
+};
+
+struct SyncSss {
+  uint64_t      tau[3];
+  uint32_t      h0[3], nH[3], nhmax; // half-frames h0 .. h0 + nH - 1 have both windows inside the capture
+  float         rot[3][2];            // exp(-j phi) of the CFO estimate over N + 9 D samples
+  const float2* dpss;                 // [3][62] d_u
+  const float*  seq;                  // [3][168][2][62] SSS of subframe 0 / 5
+};
+
+extern "C" int launch_sync_pss(const SyncArgs& g, float* m, float* fold, SyncPeak* pk, float* rm, float4* c12, float* refined, cudaStream_t st,
+                               uint64_t* launches);
+extern "C" int launch_sync_sss(const SyncArgs& g, const SyncSss& s, float2* Y, float* sss, cudaStream_t st, uint64_t* launches);

@@ -1128,3 +1128,34 @@ int lte_mib_unpack(const uint8_t* bits, uint32_t* nof_prb, uint32_t* phich_ext, 
   return BW[bw] ? 0 : -1;
 }
 uint32_t lte_pbch_crc_mask(uint32_t nof_ports) { return nof_ports == 1 ? 0x0000u : nof_ports == 2 ? 0xFFFFu : nof_ports == 4 ? 0x5555u : 0u; }
+
+/* ------------------------------------------------------------------ PSS / SSS, 36.211 6.11.1.1 / 6.11.2.1 */
+void lte_pss(uint32_t n_id_2, cf_t* d)
+{
+  static const uint32_t ROOT[3] = {25, 29, 34};
+  const uint32_t        u       = ROOT[n_id_2 % 3];
+  for (uint32_t n = 0; n < 62; n++) {
+    const uint32_t m  = n < 31 ? n * (n + 1) : (n + 1) * (n + 2);
+    const double   ph = -M_PI * (double)((u * m) % 126u) / 63.0; /* exp(-j pi u m / 63) */
+    d[n]              = (cf_t){(float)cos(ph), (float)sin(ph)};
+  }
+}
+
+void lte_sss(uint32_t n_id_1, uint32_t n_id_2, uint32_t sf5, float* d)
+{
+  uint8_t xs[31] = {0, 0, 0, 0, 1}, xc[31] = {0, 0, 0, 0, 1}, xz[31] = {0, 0, 0, 0, 1};
+  for (uint32_t i = 0; i + 5 < 31; i++) {
+    xs[i + 5] = (xs[i + 2] + xs[i]) & 1;
+    xc[i + 5] = (xc[i + 3] + xc[i]) & 1;
+    xz[i + 5] = (xz[i + 4] + xz[i + 2] + xz[i + 1] + xz[i]) & 1;
+  }
+  const uint32_t qp = n_id_1 / 30, q = (n_id_1 + qp * (qp + 1) / 2) / 30, mp = n_id_1 + q * (q + 1) / 2;
+  const uint32_t m0 = mp % 31, m1 = (m0 + mp / 31 + 1) % 31;
+  for (uint32_t n = 0; n < 31; n++) {
+    const int s0 = 1 - 2 * xs[(n + m0) % 31], s1 = 1 - 2 * xs[(n + m1) % 31];
+    const int c0 = 1 - 2 * xc[(n + n_id_2) % 31], c1 = 1 - 2 * xc[(n + n_id_2 + 3) % 31];
+    const int z0 = 1 - 2 * xz[(n + m0 % 8) % 31], z1 = 1 - 2 * xz[(n + m1 % 8) % 31];
+    d[2 * n]     = (float)(sf5 ? s1 * c0 : s0 * c0);
+    d[2 * n + 1] = (float)(sf5 ? s0 * c1 * z1 : s1 * c1 * z0);
+  }
+}

@@ -228,6 +228,11 @@ void lte_mib_pack(uint32_t nof_prb, uint32_t phich_ext, uint32_t phich_res, uint
 int  lte_mib_unpack(const uint8_t* bits, uint32_t* nof_prb, uint32_t* phich_ext, uint32_t* phich_res, uint32_t* sfn);
 /* CRC mask of the antenna-port count (36.212 Table 5.3.1.1-1): 1 -> 0x0000, 2 -> 0xFFFF, 4 -> 0x5555; 0 for anything else */
 uint32_t lte_pbch_crc_mask(uint32_t nof_ports);
+/* synchronisation signals (36.211 6.11, FDD): d[n], n = 0..61, goes to the sub-carrier n - 31 (n < 31) or n - 30 (n >= 31) around DC.
+ * PSS: Zadoff-Chu root 25 / 29 / 34 of N_ID_2 = 0 / 1 / 2, each value computed in double and rounded to float.
+ * SSS: the +-1 sequence of subframe 0 (sf5 = 0) or subframe 5 (sf5 = 1) of N_ID_1 (0..167) and N_ID_2 (6.11.2.1). */
+void lte_pss(uint32_t n_id_2, cf_t* d /* [62] */);
+void lte_sss(uint32_t n_id_1, uint32_t n_id_2, uint32_t sf5, float* d /* [62] */);
 #ifdef __cplusplus
 }
 #endif

@@ -246,6 +246,18 @@ int lte_sim_subframe(lte_sim_t* s, uint32_t tti, cf_t* iq, lte_sim_truth_t* trut
     map_ctrl(s, d, ks, ls, 16);
   }
 
+  /* ---- PSS / SSS: the 62 sub-carriers around DC, d[n] on grid index n - 31 + nsc / 2 ---- */
+  if (cfg->sync && (sf_idx == 0 || sf_idx == 5)) {
+    cf_t  pss[62];
+    float sss[62];
+    lte_pss(cell->cell_id % 3, pss);
+    lte_sss(cell->cell_id / 3, cell->cell_id % 3, sf_idx == 5, sss);
+    for (uint32_t n = 0; n < 62; n++) {
+      s->grid[0][6 * nsc + n - 31 + nsc / 2] = pss[n];
+      s->grid[0][5 * nsc + n - 31 + nsc / 2] = (cf_t){sss[n], 0.0f};
+    }
+  }
+
   /* ---- PBCH ---- */
   if (cfg->pbch && sf_idx == 0) {
     const uint32_t sfn = (tti / 10) % 1024;

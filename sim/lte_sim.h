@@ -33,7 +33,8 @@ typedef struct {
   uint32_t   harq_retx;    /* 1: subframes with (tti / 8) odd repeat the DCIs and transport blocks of tti - 8 with rv = 2 (same NDI, same HARQ process) */
   uint32_t   pbch;         /* 1: subframe 0 of every frame carries the PBCH (MIB: bandwidth, PHICH, SFN = tti / 10) */
   float      cfo_hz;       /* carrier frequency offset applied to the generated samples (phase restarts every subframe, as srsran_cfo_correct sees it) */
-  uint32_t   reserved[2];
+  uint32_t   sync;         /* 1: subframes 0 and 5 carry the PSS (symbol 6) and SSS (symbol 5) on port 0 (36.211 6.11, FDD); 0 leaves those REs empty */
+  uint32_t   reserved[1];
 } lte_sim_cfg_t;
 
 #define LTE_SIM_MAX_DCI 32
