@@ -2,8 +2,9 @@
 // One CTA decodes a PAIR of code blocks of equal size K: the two trellises live in the low and high
 // halves of packed int16x2 registers (VIADD.16x2 / VIADDMNMX.S16x2 / VIMNMX.S16x2), one thread per
 // 32-step window, 8 state metrics per thread in registers, window-boundary metrics carried over from
-// the previous iteration (next-iteration initialisation), alpha kept in shared memory for 16 steps at a
-// time.  Restates the srsran_tdec_* behaviour reached through srsran_dlsch_decode2 (reference
+// the previous iteration (next-iteration initialisation), alpha kept in shared memory for 8 steps at a
+// time, the pair's systematic, extrinsic and interleaver arrays in shared memory for the whole pair.
+// Restates the srsran_tdec_* behaviour reached through srsran_dlsch_decode2 (reference
 // src/src/DL_Sniffer_PDSCH.cc:997): int16 LLRs, CRC24B/CRC24A early stop, at least one iteration.
 // The arithmetic is the CPU oracle's (oracle/lte_oracle.c, siso()): outputs are offset-invariant, so
 // the int16 normalisation schedule below does not change any decision.
@@ -12,58 +13,71 @@
 #include "turbo_arith.cuh"
 
 struct TurboView {
-  const uint32_t *sysT, *p1T, *p2T, *tails;
-  uint32_t*       ext; // [32][NW] a-priori / extrinsic values, window-transposed, updated in place by both constituent decoders
-  uint32_t*       bnd; // [2 siso][2 (A,B)][NW][8]
-  const uint16_t* piT;
+  const uint32_t *p1T, *p2T, *tails; // global: parity streams [32][NW] of both constituent codes, termination words
+  const uint32_t* sys;               // shared: [32][NW] systematic values, window-transposed
+  uint32_t*       ext;               // shared: [32][NW] a-priori / extrinsic values, updated in place by both constituent decoders
+  const uint16_t* pi;                // shared: [32][NW] natural bit index of step j of window w in the interleaved order
+  uint32_t*       bnd;               // global scratch slot: [2 siso][2 (A,B)][NW][8]
   uint32_t        K, NW;
 };
 
 #define TD_SUB 8 // alpha is kept in shared memory for TD_SUB steps at a time
 #define TD_NSUB (TD_WL / TD_SUB)
 
+// bit index and window-transposed word of step j of window w: the identity in the natural pass, the QPP interleaver in the other
+template <bool IL>
+__device__ __forceinline__ uint32_t step_bit(const TurboView& tv, uint32_t j, uint32_t w)
+{
+  return IL ? (uint32_t)tv.pi[j * tv.NW + w] : w * TD_WL + j;
+}
+__device__ __forceinline__ uint32_t bit_word(uint32_t k, uint32_t NW) { return (k & 31u) * NW + (k >> 5); }
+
+// (2 xa, 2 p) packed for the step at word pos with parity p: xa = systematic + a-priori
+__device__ __forceinline__ uint2 branch_in(const TurboView& tv, uint32_t pos, uint32_t p)
+{
+  const uint32_t xa = vadd(tv.sys[pos], tv.ext[pos]);
+  return make_uint2(vadd(xa, xa), vadd(p, p));
+}
+// parity of the 8 steps j0 .. j0 + 7 of window w (coalesced across the CTA)
+template <bool FULL>
+__device__ __forceinline__ void load_par(uint32_t (&p)[TD_SUB], const uint32_t* par, uint32_t j0, uint32_t w, uint32_t NW, uint32_t len)
+{
+#pragma unroll
+  for (uint32_t jj = 0; jj < TD_SUB; jj++)
+    if (FULL || j0 + jj < len) p[jj] = __ldg(par + (j0 + jj) * NW + w);
+}
+
 // one SISO pass for window w.  IL = second constituent decoder (interleaved order); NT = threads per CTA
 // (compile time, so every shared-memory access is base + immediate); FULL = every window has 32 steps.
-// Shared memory per thread: g_s[32] ((2 xa, 2 p) packed, staged once per pass with all the global loads of the window in flight
-// together), pos_s[32] (natural bit index of the step in the interleaved pass), alpha_s[TD_SUB][2] (uint4).
+// The systematic and a-priori values come from shared memory when a step needs them, with no staged copy: within a pass window w
+// reads and writes ext only at its own 32 words (the identity in the natural pass, the QPP bijection in the interleaved one), and
+// reads the a-priori value of step j before it writes the extrinsic value of step j, so no other window's write can reach them.
+// The window is walked in 8-step chunks: forward over sub-windows 0 .. 3, then sub-windows 3 .. 0.  The parity words of the next
+// chunk are loaded while the current one is computed, so their global-memory latency is hidden behind 8 trellis steps.
+// Shared memory per thread: alpha_t[TD_SUB][2] (uint4).
 template <bool IL, int NT, bool FULL>
-__device__ __forceinline__ void siso_pass(const TdConst& c, const TurboView& tv, uint4* __restrict__ alpha_t, uint2* __restrict__ g_t,
-                                          uint16_t* __restrict__ pos_t, uint32_t* bits_s, uint32_t w, bool active, const uint32_t* btail,
-                                          bool first_iter)
+__device__ __forceinline__ void siso_pass(const TdConst& c, const TurboView& tv, uint4* __restrict__ alpha_t, uint32_t* bits_s, uint32_t w,
+                                          bool active, const uint32_t* btail)
 {
   const uint32_t  K = tv.K, NW = tv.NW;
   const uint32_t  len = FULL ? (uint32_t)TD_WL : (active ? min((uint32_t)TD_WL, K - w * TD_WL) : 0u);
   uint32_t*       A  = tv.bnd + (size_t)(IL ? 2 : 0) * NW * 8;
   uint32_t*       B  = A + (size_t)NW * 8;
   const uint32_t* par = IL ? tv.p2T : tv.p1T;
-  uint32_t*       ext = tv.ext;
 
-  St8 a0, b;
+  St8      a0, b;
+  uint32_t pn[TD_SUB]; // parity of the next chunk
   if (active) {
 #pragma unroll
     for (int s = 0; s < 8; s++) {
       a0.s[s] = (w == 0) ? (s ? pk2(TD_NINF + (int)TD_BIAS, TD_NINF + (int)TD_BIAS) : TD_BIASW) : A[(size_t)w * 8 + s];
       b.s[s]  = (w == NW - 1) ? btail[s] : B[(size_t)w * 8 + s];
     }
-    // ---- stage the window: every load of the pass is issued here, independent of the recursions ----
-#pragma unroll 16
-    for (uint32_t j = 0; j < TD_WL; j++) {
-      if (FULL || j < len) {
-        uint32_t pos;
-        if (!IL)
-          pos = j * NW + w;
-        else {
-          const uint32_t pi = tv.piT[j * NW + w];
-          pos               = (pi & 31u) * NW + (pi >> 5);
-          pos_t[j * NT]     = (uint16_t)pi;
-        }
-        const uint32_t sy = tv.sysT[pos], ap = (!IL && first_iter) ? 0u : ext[pos], p = par[j * NW + w];
-        const uint32_t xa = vadd(sy, ap);
-        g_t[j * NT]       = make_uint2(vadd(xa, xa), vadd(p, p));
-      }
-    }
+    load_par<FULL>(pn, par, 0, w, NW, len);
   }
-  __syncthreads(); // every window has read its boundaries (and inputs) before anybody overwrites them
+  // every window has read its boundary metrics (A, B) before any window overwrites them below: windows w - 1 and w + 1 write
+  // the slots window w has just read
+  __syncthreads();
 
   if (active) {
     // ---- forward over the whole window, remembering alpha at the start of every sub-window ----------
@@ -71,11 +85,15 @@ __device__ __forceinline__ void siso_pass(const TdConst& c, const TurboView& tv,
 #pragma unroll 1
     for (uint32_t sw = 0; sw < TD_NSUB; sw++) {
       ck[sw] = a;
+      uint32_t pc[TD_SUB];
+#pragma unroll
+      for (uint32_t jj = 0; jj < TD_SUB; jj++) pc[jj] = pn[jj];
+      load_par<FULL>(pn, par, (sw + 1 < TD_NSUB ? sw + 1 : sw) * TD_SUB, w, NW, len); // after sub-window 3 comes sub-window 3 again
 #pragma unroll
       for (uint32_t jj = 0; jj < TD_SUB; jj++) {
         const uint32_t j = sw * TD_SUB + jj;
         if (FULL || j < len) {
-          const uint2 g = g_t[j * NT];
+          const uint2 g = branch_in(tv, bit_word(step_bit<IL>(tv, j, w), NW), pc[jj]);
           alpha_step(c, a, to32(c, g.x), g.y, vadd(g.x, g.y));
           if ((jj & 1u) == 1u) norm8(c, a);
         }
@@ -90,8 +108,23 @@ __device__ __forceinline__ void siso_pass(const TdConst& c, const TurboView& tv,
 #pragma unroll 1
     for (int sw = TD_NSUB - 1; sw >= 0; sw--) {
       const uint32_t j0 = (uint32_t)sw * TD_SUB;
+      uint32_t       pc[TD_SUB];
+#pragma unroll
+      for (uint32_t jj = 0; jj < TD_SUB; jj++) pc[jj] = pn[jj];
+      if (sw > 0) load_par<FULL>(pn, par, j0 - TD_SUB, w, NW, len);
       if (!FULL && j0 >= len) continue;
       St8 af = ck[sw];
+      // inputs of the sub-window's 8 steps, read once for both recursions and before any of its extrinsic values is written
+      uint2    g[TD_SUB];
+      uint32_t kb[TD_SUB];
+#pragma unroll
+      for (uint32_t jj = 0; jj < TD_SUB; jj++) {
+        const uint32_t j = j0 + jj;
+        if (FULL || j < len) {
+          kb[jj] = step_bit<IL>(tv, j, w);
+          g[jj]  = branch_in(tv, bit_word(kb[jj], NW), pc[jj]);
+        }
+      }
 #pragma unroll
       for (uint32_t jj = 0; jj < TD_SUB; jj++) {
         const uint32_t j = j0 + jj;
@@ -99,35 +132,29 @@ __device__ __forceinline__ void siso_pass(const TdConst& c, const TurboView& tv,
           alpha_t[(jj * 2 + 0) * NT] = make_uint4(af.s[0], af.s[1], af.s[2], af.s[3]);
           alpha_t[(jj * 2 + 1) * NT] = make_uint4(af.s[4], af.s[5], af.s[6], af.s[7]);
           if (jj + 1 < TD_SUB) {
-            const uint2 g = g_t[j * NT];
-            alpha_step(c, af, to32(c, g.x), g.y, vadd(g.x, g.y));
+            alpha_step(c, af, to32(c, g[jj].x), g[jj].y, vadd(g[jj].x, g[jj].y));
             if ((jj & 1u) == 1u) norm8(c, af);
           }
         }
       }
-#pragma unroll 4
+#pragma unroll
       for (int jj = TD_SUB - 1; jj >= 0; jj--) {
         const uint32_t j = j0 + (uint32_t)jj;
         if (FULL || j < len) {
-          const uint2 g  = g_t[j * NT];
           const uint4 u0 = alpha_t[(jj * 2 + 0) * NT], u1 = alpha_t[(jj * 2 + 1) * NT];
           St8         al;
           al.s[0] = u0.x, al.s[1] = u0.y, al.s[2] = u0.z, al.s[3] = u0.w, al.s[4] = u1.x, al.s[5] = u1.y, al.s[6] = u1.z, al.s[7] = u1.w;
-          const uint32_t X32 = to32(c, g.x), P32 = to32(c, g.y);
+          const uint32_t X32 = to32(c, g[jj].x), P32 = to32(c, g[jj].y);
           uint32_t       m1, m0;
           beta_llr_step(c, b, al, X32, P32, add32(c, X32, P32), m1, m0);
           if ((jj & 1) == 0) norm8(c, b);
           const uint32_t L = vsub(m1, m0); // the double bias cancels
-          uint32_t       ps;
-          if (!IL)
-            ps = j * NW + w;
-          else {
-            const uint32_t pi = pos_t[j * NT];
-            ps                = (pi & 31u) * NW + (pi >> 5);
-            if ((int)(L << 16) > 0) atomicOr(&bits_s[pi >> 5], 0x80000000u >> (pi & 31u));
-            if ((int)L >= 0x10000) atomicOr(&bits_s[(TD_WL * 6) + (pi >> 5)], 0x80000000u >> (pi & 31u));
+          const uint32_t k = kb[jj];
+          if (IL) {
+            if ((int)(L << 16) > 0) atomicOr(&bits_s[k >> 5], 0x80000000u >> (k & 31u));
+            if ((int)L >= 0x10000) atomicOr(&bits_s[(TD_WL * 6) + (k >> 5)], 0x80000000u >> (k & 31u));
           }
-          ext[ps] = ext_pair(c, L, g.x);
+          tv.ext[bit_word(k, NW)] = ext_pair(c, L, g[jj].x);
         }
       }
     }
@@ -163,12 +190,15 @@ __device__ __forceinline__ uint32_t gf_mod24(uint32_t v, uint32_t nbits, uint32_
 }
 
 // Persistent CTAs: the grid is sized to the number of CTAs the GPU can hold; each CTA takes code-block pairs from a queue
-// (early CRC stop makes the pairs' run times vary by up to 8x) and keeps the extrinsic values and the window-boundary metrics of
-// the pair it is working on in ITS OWN scratch slot (scratch + slot * slot_words).  A slot is rewritten for every pair, so its
-// lines stay dirty in L2 and are never written back for a finished pair: round 1 kept this state inside each pair's buffer and
-// paid 433 MB of DRAM write-back per 1000-subframe step for it.
+// (early CRC stop makes the pairs' run times vary by up to 8x).  The pair's systematic values, interleaver table and
+// extrinsic values live in shared memory for the whole pair: the systematic stream and the table are read from global memory once
+// per pair, and the interleaved pass gathers and scatters in shared memory (a few bank conflicts per warp access) instead of
+// touching a different 128-byte line per lane.  The window-boundary metrics stay in the CTA's OWN scratch slot
+// (scratch + slot * slot_words), which is rewritten for every pair, so its lines stay dirty in L2 and are never written back
+// for a finished pair.  At most 168 registers per thread (384 threads per SM) in every size class: unbounded, the 32-thread
+// variants take more and fit fewer CTAs per SM than shared memory allows.
 template <int NT, bool FULL>
-__global__ void __launch_bounds__(NT, (NT > 128 ? 2 : (NT > 64 ? 3 : 6))) turbo_kernel(const DevPair* __restrict__ pairs, uint32_t npairs, uint32_t* __restrict__ queue,
+__global__ void __launch_bounds__(NT, 384 / NT) turbo_kernel(const DevPair* __restrict__ pairs, uint32_t npairs, uint32_t* __restrict__ queue,
                                                     const uint32_t* __restrict__ pool, uint32_t* __restrict__ scratch, uint32_t slot_words,
                                                     const uint16_t* __restrict__ pi_pool,
                                                     const uint32_t* __restrict__ pi_off, const uint32_t* __restrict__ xpowA,
@@ -177,8 +207,9 @@ __global__ void __launch_bounds__(NT, (NT > 128 ? 2 : (NT > 64 ? 3 : 6))) turbo_
 {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   uint4*             alpha_t = reinterpret_cast<uint4*>(smem_raw) + threadIdx.x;                          // [TD_SUB][2][NT]
-  uint2*             g_t     = reinterpret_cast<uint2*>(reinterpret_cast<uint4*>(smem_raw) + TD_SUB * 2 * NT) + threadIdx.x; // [TD_WL][NT]
-  uint16_t*          pos_t   = reinterpret_cast<uint16_t*>(reinterpret_cast<uint2*>(reinterpret_cast<uint4*>(smem_raw) + TD_SUB * 2 * NT) + TD_WL * NT) + threadIdx.x;
+  uint32_t*          sys_s   = reinterpret_cast<uint32_t*>(reinterpret_cast<uint4*>(smem_raw) + TD_SUB * 2 * NT); // [TD_WL][NW], NW <= NT
+  uint32_t*          ext_s   = sys_s + TD_WL * NT;                                                         // [TD_WL][NW]
+  uint16_t*          pi_s    = reinterpret_cast<uint16_t*>(ext_s + TD_WL * NT);                            // [TD_WL][NW]
   __shared__ uint32_t bits_s[2 * TD_WL * 6];                       // 2 x 6144 bits
   __shared__ uint32_t btail[2][8];
   __shared__ uint32_t red_s[8];
@@ -196,18 +227,44 @@ __global__ void __launch_bounds__(NT, (NT > 128 ? 2 : (NT > 64 ? 3 : 6))) turbo_
   const DevPair  P = pairs[pidx];
   const uint32_t K = P.K, NW = P.NW;
   const bool     active = tid < NW;
-  TurboView      tv;
-  tv.sysT  = pool + P.buf_off;
-  tv.p1T   = tv.sysT + 32 * NW;
+  const uint32_t* sysT = pool + P.buf_off;
+  const uint16_t* piT  = pi_pool + pi_off[pidx];
+  TurboView       tv;
+  tv.p1T   = sysT + 32 * NW;
   tv.p2T   = tv.p1T + 32 * NW;
   tv.tails = tv.p2T + 32 * NW;
-  tv.ext   = my_scratch;
-  tv.bnd   = my_scratch + 32 * NW;
-  tv.piT   = pi_pool + pi_off[pidx];
+  tv.sys   = sys_s;
+  tv.ext   = ext_s;
+  tv.pi    = pi_s;
+  tv.bnd   = my_scratch;
   tv.K = K, tv.NW = NW;
 
   // boundary metrics start "unknown" (all equal: the bias); the a-priori input of the very first half iteration is zero
   for (uint32_t i = tid; i < 4 * NW * 8; i += nthreads) tv.bnd[i] = TD_BIASW;
+  {
+    // the pair's systematic values and interleaver table into shared memory, the a-priori values to zero, in 16-byte chunks (pair
+    // buffers are 96 NW + 16 words and tables 32 NW entries, so both start 16-byte aligned; NW <= NT), 4 loads in flight per thread
+    const uint4* s4 = reinterpret_cast<const uint4*>(sysT);
+    const uint4* p4 = reinterpret_cast<const uint4*>(piT);
+#pragma unroll
+    for (uint32_t k0 = 0; k0 < 12; k0 += 4) {
+      uint4 v[4];
+#pragma unroll
+      for (uint32_t k = k0; k < k0 + 4; k++) {
+        const uint32_t i = (k & 7u) * NT + tid;
+        if (i < (k < 8 ? 8 : 4) * NW) v[k - k0] = __ldg((k < 8 ? s4 : p4) + i);
+      }
+#pragma unroll
+      for (uint32_t k = k0; k < k0 + 4; k++) {
+        const uint32_t i = (k & 7u) * NT + tid;
+        if (k < 8 && i < 8 * NW) {
+          reinterpret_cast<uint4*>(sys_s)[i] = v[k - k0];
+          reinterpret_cast<uint4*>(ext_s)[i] = make_uint4(0u, 0u, 0u, 0u);
+        } else if (k >= 8 && i < 4 * NW)
+          reinterpret_cast<uint4*>(pi_s)[i] = v[k - k0];
+      }
+    }
+  }
   if (tid < 2) done_s[tid] = (tid < P.ncb) ? 0u : 1u;
   if (tid == 0) {
     // beta at K from the termination bits, both constituent codes, both code blocks (scalar int32)
@@ -253,8 +310,8 @@ __global__ void __launch_bounds__(NT, (NT > 128 ? 2 : (NT > 64 ? 3 : 6))) turbo_
   uint32_t it = 0;
   while (it < max_iter) {
     for (uint32_t i = tid; i < 2 * TD_WL * 6; i += nthreads) bits_s[i] = 0u;
-    siso_pass<false, NT, FULL>(c, tv, alpha_t, g_t, pos_t, bits_s, tid, active, btail[0], it == 0);
-    siso_pass<true, NT, FULL>(c, tv, alpha_t, g_t, pos_t, bits_s, tid, active, btail[1], false);
+    siso_pass<false, NT, FULL>(c, tv, alpha_t, bits_s, tid, active, btail[0]);
+    siso_pass<true, NT, FULL>(c, tv, alpha_t, bits_s, tid, active, btail[1]);
     it++;
     // ---- CRC over the K decided bits of each code block -------------------------------------------
     bool all_done = true;
@@ -347,14 +404,14 @@ static void launch_turbo_t(const DevPair* pairs, uint32_t npairs, uint32_t* queu
                            const uint16_t* pi_pool, const uint32_t* pi_off, const uint32_t* xpowA, const uint32_t* xpowB, uint8_t* payload,
                            uint8_t* cb_iters, uint8_t* cb_crc, uint32_t max_iter, cudaStream_t st)
 {
-  const size_t smem = (size_t)NT * (TD_SUB * 2 * sizeof(uint4) + TD_WL * sizeof(uint2) + TD_WL * sizeof(uint16_t));
+  const size_t smem = (size_t)NT * (TD_SUB * 2 * sizeof(uint4) + 2 * TD_WL * sizeof(uint32_t) + TD_WL * sizeof(uint16_t));
   // the attribute belongs to the current device / context (handles may live on different devices): set it on every launch
   cudaFuncSetAttribute(turbo_kernel<NT, FULL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   int dev = 0, sms = 132, per_sm = 1;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, turbo_kernel<NT, FULL>, NT, smem);
-  const uint32_t slot_words = 64u * NT; // extrinsic [32][NW] + boundary metrics [4][NW][8], NW <= NT
+  const uint32_t slot_words = 32u * NT; // boundary metrics [4][NW][8], NW <= NT
   uint32_t       grid       = (uint32_t)(sms * (per_sm > 0 ? per_sm : 1));
   grid                      = grid < npairs ? grid : npairs;
   if ((size_t)grid * slot_words > scratch_words) grid = (uint32_t)(scratch_words / slot_words);

@@ -433,15 +433,15 @@ extern "C" const ltephy_compact_t* ltephy_phase_a_compact_buffer(const ltephy_t*
 
 // ---------------------------------------------------------------------------------------- phase B
 // words of one code-block pair in the turbo pool: the three window-transposed input streams (sys, p1, p2: [32][NW] each) and the
-// 12 termination words; the decoder's own state (extrinsic values, window-boundary metrics) lives in per-CTA scratch
+// 12 termination words; the decoder keeps its extrinsic values in shared memory and its window-boundary metrics in per-CTA scratch
 static inline size_t ltephy_pair_words(uint32_t NW) { return (size_t)3 * 32 * NW + 16; }
-// per-CTA scratch of the persistent turbo kernel: 64 * NT words per resident CTA (k_turbo.cu); sized for the largest launch
+// per-CTA scratch of the persistent turbo kernel: 32 * NT words per resident CTA (k_turbo.cu); sized for the largest launch
 static int ltephy_turbo_scratch(ltephy* h)
 {
   int sms = 132;
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->cfg.device);
-  // resident CTAs x threads is at most 2048 threads per SM; 64 words per thread
-  if (h->d_tscratch.reserve((size_t)sms * 2048 * 64)) return -1;
+  // resident CTAs x threads is at most 2048 threads per SM; 32 words per thread
+  if (h->d_tscratch.reserve((size_t)sms * 2048 * 32)) return -1;
   if (h->d_tqueue.reserve(16)) return -1;
   return 0;
 }
