@@ -5,7 +5,7 @@ CXX ?= g++
 CFLAGS = -O3 -g -fPIC -std=gnu11 -Wall -Wno-unused-function -ffp-contract=off -fno-fast-math
 CXXFLAGS = -O2 -g -fPIC -std=c++17 -Wall -ffp-contract=off -fno-fast-math
 
-all: sim/libltesim.so oracle/liblteoracle.so oracle/liblteosync.so
+all: sim/libltesim.so oracle/liblteoracle.so oracle/liblteosync.so oracle/liblteomib.so
 
 sim/libltesim.so: sim/lte_common.c sim/lte_sim.c sim/lte_common.h sim/lte_sim.h include/lte_tables.h
 	$(CC) $(CFLAGS) -shared -o $@ sim/lte_common.c sim/lte_sim.c -lm
@@ -16,6 +16,10 @@ oracle/liblteoracle.so: oracle/lte_oracle.c oracle/lte_oracle.h sim/lte_common.c
 # cell search oracle: lteo_det_sum and the shared PSS / SSS sequences come from liblteoracle.so
 oracle/liblteosync.so: oracle/lte_sync_oracle.c oracle/lte_sync_oracle.h oracle/lte_oracle.h oracle/liblteoracle.so
 	$(CC) $(CFLAGS) -shared -o $@ oracle/lte_sync_oracle.c -Loracle -llteoracle -Wl,-rpath,'$$ORIGIN' -lm
+
+# PBCH combining oracle: lteo_dci_decode and the shared primitives come from liblteoracle.so
+oracle/liblteomib.so: oracle/lte_mib_oracle.c oracle/lte_mib_oracle.h oracle/lte_oracle.h oracle/liblteoracle.so
+	$(CC) $(CFLAGS) -shared -o $@ oracle/lte_mib_oracle.c -Loracle -llteoracle -Wl,-rpath,'$$ORIGIN' -lm
 
 # C++ example of the C-ABI (needs ltesniffer_b200/libltephy_b200.so, built by ltesniffer_b200/build.py)
 examples/offline_decode: examples/offline_decode.cpp include/ltephy_b200.h include/ltephy_search.h include/ltephy_sinks.h

@@ -1,6 +1,7 @@
 // cell_search.cpp -- what a recording needs before offline_decode can read it: find the cell in a continuous cf32 capture with
 // ltephy_cell_search (PCI, frame timing, carrier offset), then decode its MIB (bandwidth, ports, PHICH, SFN) at that timing with the
-// offset corrected, the PSS / SSS search and MIB decode of rf_search_and_decode_mib (reference src/src/LTESniffer_Core.cc:193-204).
+// offset corrected, the PSS / SSS search and MIB decode of rf_search_and_decode_mib (reference src/src/LTESniffer_Core.cc:193-204).  The MIB is
+// decoded with soft combining across the 40 ms period and a search over the port count, over every frame of the capture.
 // Host code only; without a GPU ltephy_sync_create fails.
 //
 //   cell_search <iq.cf32> <symbol_sz> <nof_rx>
@@ -77,29 +78,30 @@ int main(int argc, char** argv)
         sf[2 * d] = iq[2 * (a * L + s)], sf[2 * d + 1] = iq[2 * (a * L + s) + 1];
       }
   }
+  // one 2-port handle reads both port counts: port 0 is equalised alone for 1 port and with port 1 (SFBC) for 2.  The combining decoder keeps the
+  // soft bits of up to four consecutive frames, so a MIB too weak to decode from one frame is still read from the frames after it.
+  ltephy_cfg_t cfg{};
+  cfg.nof_prb = 15, cfg.nof_ports = 2, cfg.cell_id = c->pci, cfg.nof_rx = A, cfg.max_subframes = nframes, cfg.symbol_sz = N;
+  ltephy_t* phy = nullptr;
+  if (ltephy_create(&cfg, &phy) != LTEPHY_SUCCESS) {
+    fprintf(stderr, "ltephy_create: %s\n", ltephy_last_error());
+    return 1;
+  }
+  std::vector<ltephy_mib_comb_t> m(nframes);
+  if (ltephy_set_cfo(phy, c->cfo_hz) != LTEPHY_SUCCESS || ltephy_submit_iq(phy, sf.data(), tti.data(), nframes) != LTEPHY_SUCCESS ||
+      ltephy_mib_decode_combined(phy, LTEPHY_MIB_SEARCH_PORTS, m.data()) != LTEPHY_SUCCESS) {
+    fprintf(stderr, "MIB decode: %s\n", ltephy_last_error());
+    return 1;
+  }
+  ltephy_destroy(phy);
   ltephy_mib_t mib{};
   uint32_t     ports = 0;
-  for (uint32_t np : {2u, 1u}) {
-    ltephy_cfg_t cfg{};
-    cfg.nof_prb = 15, cfg.nof_ports = np, cfg.cell_id = c->pci, cfg.nof_rx = A, cfg.max_subframes = nframes, cfg.symbol_sz = N;
-    ltephy_t* phy = nullptr;
-    if (ltephy_create(&cfg, &phy) != LTEPHY_SUCCESS) {
-      fprintf(stderr, "ltephy_create: %s\n", ltephy_last_error());
-      return 1;
+  for (uint32_t f = 0; f < nframes && !ports; f++)
+    if (m[f].mib.found) {
+      mib = m[f].mib, ports = mib.nof_ports;
+      mib.sfn = (mib.sfn + 1024 - f % 1024) % 1024; // the SFN of frame f, counted back to the frame at frame_offset
     }
-    std::vector<ltephy_mib_t> m(nframes);
-    if (ltephy_set_cfo(phy, c->cfo_hz) != LTEPHY_SUCCESS || ltephy_submit_iq(phy, sf.data(), tti.data(), nframes) != LTEPHY_SUCCESS ||
-        ltephy_mib_decode(phy, m.data()) != LTEPHY_SUCCESS) {
-      fprintf(stderr, "MIB decode: %s\n", ltephy_last_error());
-      return 1;
-    }
-    ltephy_destroy(phy);
-    if (m[0].found && m[0].nof_ports == np) {
-      mib = m[0], ports = np;
-      break;
-    }
-  }
-  if (!ports) {
+  if (!ports) { // no window of any frame passed its CRC (too weak even combined, or a cell with four CRS ports)
     fprintf(stderr, "cell %u found, MIB not decoded\n", c->pci);
     return 3;
   }

@@ -225,8 +225,32 @@ typedef struct {
 } ltephy_mib_t;
 /* PBCH decode of every subframe of the last ltephy_submit_iq whose tti % 10 == 0 (found = 0 elsewhere): srsran_ue_mib_decode +
  * srsran_pbch_mib_unpack (src/src/LTESniffer_Core.cc:382-396).  out[n].  The equaliser uses the handle's port count; one frame is decoded on its
- * own (no soft combining across the 40 ms period). */
+ * own, any of the three CRC masks is accepted and the lowest position in the 40 ms period wins.  ltephy_mib_decode_combined is the
+ * combining decoder; this call neither reads nor changes its state. */
 int ltephy_mib_decode(ltephy_t* h, ltephy_mib_t* out);
+
+/* MIB decode with soft combining across the 40 ms PBCH period: srsran_ue_mib_decode as the reference calls it in its DECODE_MIB state
+ * (src/src/LTESniffer_Core.cc:382-396), whose PBCH decoder keeps the soft bits of up to four consecutive frames between calls and tries every
+ * way to combine them.  The rules are DESIGN.md §2 ("PBCH combining"): the subframes 0 of the last submit are consumed in batch order; a frame
+ * that does not follow the last one consumed (SFN 1023 -> 0 does) empties the buffer first; the first hypothesis that passes, in srsRAN's
+ * order, wins and empties the buffer; with four frames held and no pass the oldest is dropped.  The state persists across submits and calls.
+ * A hypothesis tried with k ports passes only if the CRC remainder is the mask of k ports; 4-port cells are not decoded.
+ * flags: LTEPHY_MIB_SEARCH_PORTS tries 1 and then (on a 2-port handle) 2 ports for every frame, as srsRAN's cell search does; without it only
+ * the handle's port count is tried (the reference's file mode).  out[n], one entry per subframe of the last submit; found = 0 on subframes
+ * other than 0 and on frames where nothing passed (a pass whose bandwidth code is reserved also reports found = 0, after emptying the buffer).
+ * Returns LTEPHY_ERROR_INVALID_INPUTS without a submit, with a NULL out or with unknown flags. */
+#define LTEPHY_MIB_SEARCH_PORTS 1u
+typedef struct {
+  ltephy_mib_t mib;        /* as ltephy_mib_decode, except: nof_ports is the port count of the passing hypothesis, and sfn_offset is srsRAN's
+                              dst - src + window - 1 (0..6), so that mib.sfn = ((8 MSBs << 2) + sfn_offset) mod 1024 is the SFN of this frame */
+  uint8_t      nof_frames; /* n: frames combined (1..4) */
+  uint8_t      src;        /* the first of them, as an index into the frames held (0 = oldest) */
+  uint8_t      dst;        /* its position in the 40 ms period (0..3) */
+  uint8_t      window;     /* frames held when the hypothesis passed, this one included (srsRAN's frame_idx) */
+} ltephy_mib_comb_t;
+int ltephy_mib_decode_combined(ltephy_t* h, uint32_t flags, ltephy_mib_comb_t* out);
+/* empties the combining buffer of ltephy_mib_decode_combined: srsran_ue_mib_reset */
+int ltephy_mib_reset(ltephy_t* h);
 
 /* Cell search: the PSS / SSS half of rf_search_and_decode_mib (reference src/src/LTESniffer_Core.cc:193-204) on a continuous FDD recording with
  * normal CP.  For each N_ID_2 it finds the PSS timing, the carrier offset and N_ID_1 with the subframe-0 / subframe-5 decision, and from them the

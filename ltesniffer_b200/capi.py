@@ -70,6 +70,14 @@ class Mib(C.Structure):
                 ("bch_payload", C.c_uint8 * 3), ("nof_prb", C.c_uint32), ("sfn", C.c_uint32)]
 
 
+class MibComb(C.Structure):
+    """ltephy_mib_comb_t: one result of ltephy_mib_decode_combined"""
+    _fields_ = [("mib", Mib), ("nof_frames", C.c_uint8), ("src", C.c_uint8), ("dst", C.c_uint8), ("window", C.c_uint8)]
+
+
+MIB_SEARCH_PORTS = 1
+
+
 class UlChest(C.Structure):
     _fields_ = [("noise", C.c_float), ("rsrp", C.c_float), ("snr_db", C.c_float), ("ta_us", C.c_float)]
 
@@ -223,6 +231,18 @@ class LtePhy:
         self.L.ltephy_mib_decode.argtypes = [C.c_void_p, C.c_void_p]
         self._chk(self.L.ltephy_mib_decode(self.h, out), "mib_decode")
         return out
+
+    def mib_decode_combined(self, search_ports=False):
+        """ltephy_mib_decode_combined over the subframes of the last submit: [MibComb] * n; the combining state persists across calls"""
+        out = (MibComb * self.n)()
+        self.L.ltephy_mib_decode_combined.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p]
+        self._chk(self.L.ltephy_mib_decode_combined(self.h, MIB_SEARCH_PORTS if search_ports else 0, out), "mib_decode_combined")
+        return out
+
+    def mib_reset(self):
+        """ltephy_mib_reset: empty the combining buffer"""
+        self.L.ltephy_mib_reset.argtypes = [C.c_void_p]
+        self._chk(self.L.ltephy_mib_reset(self.h), "mib_reset")
 
     def harq_reserve(self, nslots):
         self.L.ltephy_harq_reserve.argtypes = [C.c_void_p, C.c_uint32]

@@ -21,7 +21,8 @@ static cudaEvent_t g_h2d_last[64]; // per device: completion of the most recentl
 extern "C" {
 void launch_frontend(const DevCell&, const float2*, float2*, float2*, float*, DevSfInfo*, uint32_t, cudaStream_t, uint64_t*);
 void launch_chest_interp(const DevCell&, const float2*, float2*, uint32_t, cudaStream_t, uint64_t*);
-void launch_pbch(const DevCell&, const float2*, const float2*, const DevSfInfo*, void*, uint32_t, cudaStream_t, uint64_t*);
+void launch_pbch(const DevCell&, const float2*, const float2*, const uint32_t*, uint32_t, uint32_t, uint32_t, float*, const uint32_t*, uint32_t, void*, cudaStream_t,
+                 uint64_t*);
 void launch_viterbi(const DevCell&, const float*, const DevSfInfo*, ltephy_cand_t*, uint32_t*, uint32_t, cudaStream_t, uint64_t*);
 void launch_compact(const DevCell&, const DevSfInfo*, const ltephy_cand_t*, ltephy_compact_t*, uint32_t, cudaStream_t, uint64_t*);
 void launch_pdsch_front(const DevCell&, const DevGrant*, uint32_t, uint32_t, const float2*, const float2*, const uint32_t*, const uint32_t*, uint32_t,
@@ -274,7 +275,7 @@ extern "C" void ltephy_destroy(ltephy_t* h)
   h->d_iq.release(), h->d_sym.release(), h->d_ce.release(), h->d_pil.release(), h->d_llr.release(), h->d_info.release(), h->d_cands.release();
   h->h_info.release(), h->d_compact.release(), h->h_compact.release(), h->d_grants.release(), h->d_cbs.release(), h->d_pairs.release(), h->d_tbs.release(), h->d_pair_pi_off.release();
   h->d_tscratch.release(), h->d_tqueue.release();
-  h->d_seq.release(), h->d_rm.release(), h->d_turbo.release(), h->d_pllr.release(), h->d_pi.release(), h->d_payload.release(), h->d_harq.release(), h->d_cfo.release(), h->d_mib.release(), h->d_vwork.release();
+  h->d_seq.release(), h->d_rm.release(), h->d_turbo.release(), h->d_pllr.release(), h->d_pi.release(), h->d_payload.release(), h->d_harq.release(), h->d_cfo.release(), h->d_mib.release(), h->d_pbch.release(), h->d_vwork.release();
   h->d_cb_iters.release(), h->d_cb_crc.release(), h->d_res.release(), h->h_res.release(), h->h_payload.release(), h->h_stage.release();
   h->d_uliq.release(), h->d_ulsym.release(), h->d_ulpool.release(), h->d_ulgrants.release(), h->d_ulchest.release(), h->h_ulchest.release();
   for (auto& e : h->ev)
@@ -804,31 +805,149 @@ extern "C" int ltephy_set_cfo(ltephy_t* h, float cfo_hz)
   h->dc.cfo_rot = h->d_cfo.p;
   return LTEPHY_SUCCESS;
 }
-// PBCH / MIB of every subframe 0 of the last phase A: srsran_ue_mib_decode + srsran_pbch_mib_unpack (LTESniffer_Core.cc:382-396)
+// PBCH work of one call (k_pbch.cu): pbch_llr_kernel fills frame-store rows 3.. with the soft bits of the listed subframes 0 for the port counts
+// nant_first .. nant_last, then pbch_hyp_kernel decodes the hypothesis jobs; res receives {port count of the CRC mask or 0, 24 MIB bits} per job.
+static int pbch_run(ltephy* h, const std::vector<uint32_t>& frame_sf, uint32_t nant_first, uint32_t nant_last, const std::vector<uint32_t>& jobs,
+                    std::vector<uint32_t>& res)
+{
+  const size_t F = frame_sf.size(), J = jobs.size();
+  if (h->d_pbch.reserve((size_t)(3 + h->cfg.max_subframes) * 960) || h->d_mib.reserve(F + 3 * J + 1)) return fail(LTEPHY_ERROR, "device allocation failed");
+  const size_t R = (F + J + 1) & ~(size_t)1; // the results are uint2: an 8-byte aligned word offset
+  std::vector<uint32_t> up(frame_sf);
+  up.insert(up.end(), jobs.begin(), jobs.end());
+  res.assign(2 * J, 0);
+  if (!up.empty()) CU(cudaMemcpyAsync(h->d_mib.p, up.data(), up.size() * 4, cudaMemcpyHostToDevice, h->stream));
+  launch_pbch(h->dc, h->d_sym.p, h->d_pil.p, h->d_mib.p, (uint32_t)F, nant_first - 1, nant_last - nant_first + 1, h->d_pbch.p, h->d_mib.p + F, (uint32_t)J, h->d_mib.p + R, h->stream, &h->launches);
+  CU(cudaGetLastError());
+  if (J) CU(cudaMemcpyAsync(res.data(), h->d_mib.p + R, res.size() * 4, cudaMemcpyDeviceToHost, h->stream));
+  CU(cudaStreamSynchronize(h->stream));
+  return LTEPHY_SUCCESS;
+}
+// job word (k_pbch.cu): bit 0 port count - 1, bits 1..2 n - 1, bits 3..4 dst, bits 5..31 the row.  Rows go up to 3 + max_subframes, far below 2^27:
+// a handle's sample buffer for 2^27 subframes would take more than 2 TB, so ltephy_create fails long before
+static uint32_t pbch_job(uint32_t newest_row, uint32_t nant, uint32_t n, uint32_t dst) { return (nant - 1) | (n - 1) << 1 | dst << 3 | newest_row << 5; }
+// the fields of an ltephy_mib_t from the 24 MIB bits (first bit in bit 23): srsran_pbch_mib_unpack; found = 0 for a reserved bandwidth code
+static ltephy_mib_t mib_unpack(uint32_t bits, uint32_t nof_ports, uint32_t sfn_offset)
+{
+  static const uint32_t BW[8] = {6, 15, 25, 50, 75, 100, 0, 0};
+  ltephy_mib_t          m{};
+  m.found = 1, m.nof_ports = (uint8_t)nof_ports, m.sfn_offset = (uint8_t)sfn_offset;
+  m.nof_prb = BW[(bits >> 21) & 7u], m.phich_length = (uint8_t)((bits >> 20) & 1u), m.phich_resources = (uint8_t)((bits >> 18) & 3u);
+  m.sfn = ((((bits >> 10) & 0xFFu) << 2) + sfn_offset) % 1024u; // sfn = (sfn + sfn_offset) % 1024, LTESniffer_Core.cc:392
+  m.bch_payload[0] = (uint8_t)(bits >> 16), m.bch_payload[1] = (uint8_t)(bits >> 8), m.bch_payload[2] = (uint8_t)bits;
+  if (!m.nof_prb) m.found = 0;
+  return m;
+}
+
+// PBCH / MIB of every subframe 0 of the last phase A: srsran_ue_mib_decode + srsran_pbch_mib_unpack (LTESniffer_Core.cc:382-396), one frame at a
+// time: the four one-frame hypotheses dst = 0..3 with the handle's port count; the lowest dst whose remainder is any of the three masks wins
 extern "C" int ltephy_mib_decode(ltephy_t* h, ltephy_mib_t* out)
 {
   if (!h || !out) return fail(LTEPHY_ERROR_INVALID_INPUTS, "mib_decode: bad arguments");
   const uint32_t n = (uint32_t)h->n_cur;
   if (!n) return fail(LTEPHY_ERROR_INVALID_INPUTS, "mib_decode: no subframes submitted");
   CU(cudaSetDevice(h->cfg.device));
-  if (h->d_mib.reserve((size_t)4 * h->cfg.max_subframes)) return fail(LTEPHY_ERROR, "device allocation failed");
-  launch_pbch(h->dc, h->d_sym.p, h->d_pil.p, h->d_info.p, h->d_mib.p, n, h->stream, &h->launches);
-  std::vector<uint32_t> raw((size_t)4 * n);
-  CU(cudaMemcpyAsync(raw.data(), h->d_mib.p, raw.size() * 4, cudaMemcpyDeviceToHost, h->stream));
-  CU(cudaStreamSynchronize(h->stream));
-  static const uint32_t BW[8] = {6, 15, 25, 50, 75, 100, 0, 0};
-  for (uint32_t i = 0; i < n; i++) {
-    ltephy_mib_t m{};
-    const uint32_t bits = raw[4 * i + 3];
-    m.found = (uint8_t)raw[4 * i], m.nof_ports = (uint8_t)raw[4 * i + 1], m.sfn_offset = (uint8_t)raw[4 * i + 2];
-    if (m.found) {
-      m.nof_prb = BW[(bits >> 21) & 7u], m.phich_length = (uint8_t)((bits >> 20) & 1u), m.phich_resources = (uint8_t)((bits >> 18) & 3u);
-      m.sfn = ((((bits >> 10) & 0xFFu) << 2) + m.sfn_offset) % 1024u; // sfn = (sfn + sfn_offset) % 1024, LTESniffer_Core.cc:392
-      m.bch_payload[0] = (uint8_t)(bits >> 16), m.bch_payload[1] = (uint8_t)(bits >> 8), m.bch_payload[2] = (uint8_t)bits;
-      if (!m.nof_prb) m.found = 0;
+  std::vector<uint32_t> frame_sf, jobs, res;
+  for (uint32_t i = 0; i < n; i++)
+    if (h->h_info.p[i].tti % 10 == 0) {
+      for (uint32_t dst = 0; dst < 4; dst++) jobs.push_back(pbch_job(3 + (uint32_t)frame_sf.size(), h->dc.nof_ports, 1, dst));
+      frame_sf.push_back(i);
     }
-    out[i] = m;
+  if (int r = pbch_run(h, frame_sf, h->dc.nof_ports, h->dc.nof_ports, jobs, res)) return r;
+  for (uint32_t i = 0, f = 0; i < n; i++) {
+    out[i] = ltephy_mib_t{};
+    if (h->h_info.p[i].tti % 10) continue;
+    for (uint32_t dst = 0; dst < 4; dst++) {
+      const uint32_t j = 4 * f + dst;
+      if (res[2 * j]) {
+        out[i] = mib_unpack(res[2 * j + 1], res[2 * j], dst);
+        break;
+      }
+    }
+    f++;
   }
+  return LTEPHY_SUCCESS;
+}
+
+// Soft combining across the 40 ms period (DESIGN.md §2 "PBCH combining").  The hypotheses a window of frame_idx frames can try combine n
+// consecutive frames of it at positions dst..dst+n-1; every such (frames, dst, port count) is one job, evaluated for all candidate windows at once.
+// The walk below then replays srsRAN's sequential state machine over the results: which window each frame sees depends on earlier passes.
+extern "C" int ltephy_mib_decode_combined(ltephy_t* h, uint32_t flags, ltephy_mib_comb_t* out)
+{
+  if (!h || !out) return fail(LTEPHY_ERROR_INVALID_INPUTS, "mib_decode_combined: bad arguments");
+  if (flags & ~LTEPHY_MIB_SEARCH_PORTS) return fail(LTEPHY_ERROR_INVALID_INPUTS, "mib_decode_combined: unknown flags 0x%x", flags);
+  const uint32_t n = (uint32_t)h->n_cur;
+  if (!n) return fail(LTEPHY_ERROR_INVALID_INPUTS, "mib_decode_combined: no subframes submitted");
+  CU(cudaSetDevice(h->cfg.device));
+  const uint32_t P = h->dc.nof_ports;
+  std::vector<uint32_t> tries;
+  if (flags & LTEPHY_MIB_SEARCH_PORTS)
+    for (uint32_t k = 1; k <= P; k++) tries.push_back(k);
+  else
+    tries.push_back(P);
+  // frames in batch order: subframe index, SFN and run (consecutive frames ending here, the frames held before this call included)
+  std::vector<uint32_t> frame_sf, sfn, run;
+  for (uint32_t i = 0; i < n; i++)
+    if (h->h_info.p[i].tti % 10 == 0) frame_sf.push_back(i), sfn.push_back((h->h_info.p[i].tti / 10) % 1024);
+  const uint32_t F = (uint32_t)frame_sf.size();
+  const bool     cont = F && h->mib_held && (int32_t)sfn[0] == (h->mib_last_sfn + 1) % 1024;
+  const int32_t  held = cont ? (int32_t)h->mib_held : 0;
+  for (uint32_t k = 0; k < F; k++) run.push_back(k == 0 ? (uint32_t)held + 1 : sfn[k] == (sfn[k - 1] + 1) % 1024 ? run[k - 1] + 1 : 1);
+  // jobs: for every frame ordinal o (held frames are -held..-1, in rows 3 + o) as the newest of n <= min(4, run) frames, every dst <= 4 - n
+  auto run_of = [&](int32_t o) { return o < 0 ? (uint32_t)(o + held + 1) : run[o]; };
+  std::vector<int32_t>  jidx((size_t)(held + F) * 2 * 10, -1); // [(o + held) * 2 + nant - 1][(n, dst)]
+  auto slot = [&](int32_t o, uint32_t nant, uint32_t nn, uint32_t dst) -> int32_t& {
+    static const uint32_t base[5] = {0, 0, 4, 7, 9};
+    return jidx[((size_t)(o + held) * 2 + nant - 1) * 10 + base[nn] + dst];
+  };
+  std::vector<uint32_t> jobs, res;
+  for (int32_t o = -held; o < (int32_t)F; o++)
+    for (uint32_t nant : tries)
+      for (uint32_t nn = 1; nn <= std::min(4u, run_of(o)); nn++)
+        for (uint32_t dst = 0; dst + nn <= 4; dst++) {
+          slot(o, nant, nn, dst) = (int32_t)jobs.size();
+          jobs.push_back(pbch_job((uint32_t)(3 + o), nant, nn, dst));
+        }
+  if (int r = pbch_run(h, frame_sf, 1, P, jobs, res)) return r; // every port count: the carried rows serve later calls with either flag
+  for (uint32_t i = 0; i < n; i++) out[i] = ltephy_mib_comb_t{};
+  uint32_t fi = (uint32_t)held;
+  for (uint32_t k = 0; k < F; k++) {
+    if (run[k] == 1) fi = 0; // not the frame after the last one consumed: empty the buffer first
+    fi++;
+    bool done = false;
+    for (uint32_t t = 0; t < tries.size() && !done; t++) {
+      const uint32_t nant = tries[t];
+      for (uint32_t nb = 0; nb < fi && !done; nb++)
+        for (uint32_t dst = 0; dst < 4 - nb && !done; dst++)
+          for (uint32_t src = 0; src < fi - nb && !done; src++) {
+            const int32_t  o = (int32_t)k - (int32_t)fi + 1 + (int32_t)(src + nb); // newest combined frame
+            const uint32_t j = (uint32_t)slot(o, nant, nb + 1, dst);
+            if (res[2 * j] != nant) continue; // the remainder must be this port count's mask
+            ltephy_mib_comb_t& r = out[frame_sf[k]];
+            r.mib        = mib_unpack(res[2 * j + 1], nant, dst - src + fi - 1);
+            r.nof_frames = (uint8_t)(nb + 1), r.src = (uint8_t)src, r.dst = (uint8_t)dst, r.window = (uint8_t)fi;
+            done = true;
+          }
+    }
+    if (done)
+      fi = 0;
+    else if (fi == 4)
+      fi = 3; // drop the oldest frame
+  }
+  // carry the frames still held into rows 3 - fi .. 2, ascending (a source row always lies above its destination)
+  const int32_t first = (int32_t)F - (int32_t)fi;
+  for (uint32_t r = 0; r < fi; r++) {
+    const int32_t from = 3 + first + (int32_t)r, to = 3 - (int32_t)fi + (int32_t)r;
+    if (from != to) CU(cudaMemcpyAsync(h->d_pbch.p + (size_t)to * 960, h->d_pbch.p + (size_t)from * 960, 960 * sizeof(float), cudaMemcpyDeviceToDevice, h->stream));
+  }
+  CU(cudaStreamSynchronize(h->stream));
+  if (F) h->mib_held = fi, h->mib_last_sfn = (int32_t)sfn[F - 1];
+  return LTEPHY_SUCCESS;
+}
+extern "C" int ltephy_mib_reset(ltephy_t* h)
+{
+  if (!h) return fail(LTEPHY_ERROR_INVALID_INPUTS, "mib_reset: bad arguments");
+  h->mib_held = 0, h->mib_last_sfn = -1;
   return LTEPHY_SUCCESS;
 }
 

@@ -90,7 +90,10 @@ struct ltephy {
   cudaEvent_t        ev[6]{}, mark[2]{}, ev_h2d = nullptr;
   DevBuf<float2>     d_cfo;                  // per-sample rotation of ltephy_set_cfo
   DevBuf<uint32_t>   d_vwork;                // work list of the Viterbi kernel: count + (subframe, pair, size) items
-  DevBuf<uint32_t>   d_mib;                  // 4 words per subframe (pbch_kernel)
+  DevBuf<uint32_t>   d_mib;                  // PBCH work of one call: subframe of each frame, hypothesis jobs, 2 result words per job (k_pbch.cu)
+  DevBuf<float>      d_pbch;                 // PBCH frame store [3 + max_subframes][2][480]: rows 0..2 the frames the combiner carries over
+  uint32_t           mib_held     = 0;       // combiner: frames held (srsRAN's frame_idx between calls), in rows 3 - mib_held .. 2
+  int32_t            mib_last_sfn = -1;      // combiner: SFN of the last frame consumed, -1 after a reset
   DevBuf<short>      d_harq;                 // HARQ store: harq_slots x LTEPHY_HARQ_SLOT_BYTES
   uint32_t           harq_slots = 0, harq_max_gen = 0;
   std::map<uint32_t, uint32_t> harq_uses;    // slot -> uses in the batch being built
