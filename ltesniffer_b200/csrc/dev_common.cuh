@@ -78,8 +78,9 @@ struct DevCb {             // one code block
   uint32_t llr_off;        // first soft bit of this code block in the LLR pool
   uint32_t E;              // soft bits received
   uint32_t K, F;
-  uint32_t rm_tab;         // offset into the rate-matching table pool: order[k] = word of the pair buffer hit by soft bit k
-  uint32_t rm_nn;
+  uint32_t rm_tab;         // offset into the rate-matching table pool: inverse table of (K, F), one uint16 per pair-buffer word
+  uint32_t rm_nn;          // repeat period of the received soft bits
+  uint32_t rm_rot;         // redundancy version: soft bit k lands on the word whose table entry is (k + rm_rot) mod rm_nn
   uint32_t shift;          // conditioning shift from Qm
   uint32_t pair, half;     // turbo job and 16-bit lane it occupies
   uint32_t harq_op;        // LTEPHY_HARQ_*: 0 none, 1 overwrite the store, 2 add to it

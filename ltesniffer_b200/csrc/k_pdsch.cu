@@ -142,47 +142,89 @@ __global__ void __launch_bounds__(256) pdsch_demod_kernel(const __grid_constant_
   }
 }
 
-// ---- K7: one CTA per code block, iterating in RECEIVED order: soft bit k (and its repeats k+nn, ...) lands on
-// pair-buffer word order[k]; reads of e are coalesced, writes follow the runs of the sub-block interleaver
-// (consecutive k -> consecutive words of the window-transposed stream).  Unreceived positions are zeroed here,
-// so the stream buffers need no memset.
+// ---- K7: one CTA per code-block pair, iterating over the words of the pair buffer.  Word w of a code block sits at
+// position j = inv[w] of the rv-0 circular order (the table is shared by every redundancy version); it receives soft bits
+// k, k+nn, k+2nn, ... < E with k = (j - rot) mod nn, summed in that (received) order.  Consecutive words are consecutive
+// rows of one interleaver column, so the table reads and the stores are coalesced and the gathers of e nearly so.  Every
+// word is written, so the stream buffers need no memset.
 __device__ __forceinline__ int sat16(int v) { return v > 32767 ? 32767 : (v < -32768 ? -32768 : v); }
 
-__global__ void __launch_bounds__(256) rm_turbo_rx_kernel(const DevCb* __restrict__ cbs, const DevPair* __restrict__ pairs,
-                                                          const short* __restrict__ llr_pool, const uint32_t* __restrict__ rm_pool,
-                                                          uint32_t* __restrict__ turbo_pool, short* __restrict__ harq_pool, uint32_t gen)
+#define RM_UNROLL 4 // words per thread whose table reads and first gathers are in flight together
+
+struct RmHalf {
+  const short*    e;
+  const uint16_t* inv;
+  short*          hq; // HARQ accumulators, or nullptr
+  uint32_t        E, nn, rot, shift, retx;
+};
+__device__ __forceinline__ RmHalf rm_half(const DevCb& cb, const short* llr_pool, const uint16_t* rm_pool, short* harq_pool)
 {
-  const DevCb     cb = cbs[blockIdx.x];
-  if (cb.harq_gen != gen) return;
-  const DevPair&  pr = pairs[cb.pair];
-  const uint32_t  NW = pr.NW;
-  const bool      alone = pr.ncb == 1;
-  const short*    e   = llr_pool + cb.llr_off;
-  const uint32_t* ord = rm_pool + cb.rm_tab;
-  uint32_t*       bw  = turbo_pool + pr.buf_off;
-  short*          bh  = reinterpret_cast<short*>(bw);
   // HARQ store (reference src/src/HARQ.cc, DL_Sniffer_PDSCH.cc:955-985): the accumulators of this code block live at the pair-buffer word index,
   // which does not depend on the redundancy version; a retransmission starts from what earlier transmissions left there
-  short* hq = cb.harq_op ? harq_pool + cb.harq_off : nullptr;
-  for (uint32_t k = threadIdx.x; k < cb.rm_nn; k += blockDim.x) {
-    const uint32_t w = ord[k];
-    int            acc = cb.harq_op == LTEPHY_HARQ_RETX ? (int)hq[w] : 0;
-    for (uint32_t kk = k; kk < cb.E; kk += cb.rm_nn) acc = sat16(acc + (int)e[kk]);
-    if (hq) hq[w] = (short)acc;
-    int v = acc >> cb.shift;
-    v     = v > 255 ? 255 : (v < -255 ? -255 : v);
-    if (alone)
-      bw[w] = (uint32_t)v & 0xFFFFu;
-    else
-      bh[2 * w + cb.half] = (short)v;
+  return RmHalf{llr_pool + cb.llr_off, rm_pool + cb.rm_tab, cb.harq_op ? harq_pool + cb.harq_off : nullptr, cb.E, cb.rm_nn, cb.rm_rot, cb.shift,
+                cb.harq_op == LTEPHY_HARQ_RETX ? 1u : 0u};
+}
+// conditioned value of word w with table entry j of one code block: sat16 sum of its soft bits (first one, x0, already loaded)
+__device__ __forceinline__ int rm_word_value(const RmHalf& h, uint32_t w, uint32_t j, uint32_t k, int x0, int acc)
+{
+  if (j == LTEPHY_RM_NONE) return 0;
+  if (j == LTEPHY_RM_FILLER) return -255; // filler bits are known zeros: strong "0" in the systematic and first parity streams
+  if (k < h.E) {
+    acc = sat16(acc + x0);
+    for (uint32_t kk = k + h.nn; kk < h.E; kk += h.nn) acc = sat16(acc + (int)h.e[kk]);
   }
-  // filler bits are known zeros: strong "0" in the systematic and first parity streams
-  for (uint32_t i = threadIdx.x; i < 2 * cb.F; i += blockDim.x) {
-    const uint32_t st = i / cb.F, ii = i % cb.F, w = st * 32 * NW + (ii & 31u) * NW + (ii >> 5);
-    if (alone)
-      bw[w] = (uint32_t)(-255) & 0xFFFFu;
-    else
-      bh[2 * w + cb.half] = (short)-255;
+  if (h.hq) h.hq[w] = (short)acc;
+  const int v = acc >> h.shift;
+  return v > 255 ? 255 : (v < -255 ? -255 : v);
+}
+
+__global__ void __launch_bounds__(256) rm_turbo_rx_kernel(const DevCb* __restrict__ cbs, const DevPair* __restrict__ pairs,
+                                                          const short* __restrict__ llr_pool, const uint16_t* __restrict__ rm_pool,
+                                                          uint32_t* __restrict__ turbo_pool, short* __restrict__ harq_pool, uint32_t gen)
+{
+  const DevPair& pr  = pairs[blockIdx.x];
+  const uint32_t ncb = pr.ncb, nwords = 96 * pr.NW + 16;
+  const DevCb&   c0 = cbs[pr.cb_index[0]];
+  const DevCb&   c1 = cbs[pr.cb_index[ncb - 1]];
+  // a HARQ slot used twice in one batch puts its later use in a later launch: only the halves of this generation are written
+  const bool do0 = c0.harq_gen == gen, do1 = ncb == 2 && c1.harq_gen == gen;
+  if (!do0 && !do1) return;
+  const bool     full = do0 && (do1 || ncb == 1); // whole 32-bit words (a single code block keeps its high half at 0)
+  const RmHalf   h0 = rm_half(c0, llr_pool, rm_pool, harq_pool), h1 = rm_half(c1, llr_pool, rm_pool, harq_pool);
+  uint32_t*      bw = turbo_pool + pr.buf_off;
+  short*         bh = reinterpret_cast<short*>(bw);
+  for (uint32_t base = threadIdx.x; base < nwords; base += RM_UNROLL * blockDim.x) {
+    uint32_t j0[RM_UNROLL], j1[RM_UNROLL], k0[RM_UNROLL], k1[RM_UNROLL];
+    int      x0[RM_UNROLL], x1[RM_UNROLL], a0[RM_UNROLL], a1[RM_UNROLL];
+#pragma unroll
+    for (int u = 0; u < RM_UNROLL; u++) {
+      const uint32_t w = base + u * blockDim.x;
+      j0[u] = do0 && w < nwords ? h0.inv[w] : LTEPHY_RM_NONE;
+      j1[u] = do1 && w < nwords ? h1.inv[w] : LTEPHY_RM_NONE;
+    }
+#pragma unroll
+    for (int u = 0; u < RM_UNROLL; u++) {
+      const uint32_t w = base + u * blockDim.x;
+      const bool     r0 = j0[u] < h0.nn, r1 = j1[u] < h1.nn;
+      k0[u] = j0[u] >= h0.rot ? j0[u] - h0.rot : j0[u] + h0.nn - h0.rot;
+      k1[u] = j1[u] >= h1.rot ? j1[u] - h1.rot : j1[u] + h1.nn - h1.rot;
+      x0[u] = r0 && k0[u] < h0.E ? (int)h0.e[k0[u]] : 0;
+      x1[u] = r1 && k1[u] < h1.E ? (int)h1.e[k1[u]] : 0;
+      a0[u] = r0 && h0.retx ? (int)h0.hq[w] : 0;
+      a1[u] = r1 && h1.retx ? (int)h1.hq[w] : 0;
+    }
+#pragma unroll
+    for (int u = 0; u < RM_UNROLL; u++) {
+      const uint32_t w = base + u * blockDim.x;
+      if (w >= nwords) break;
+      const int v0 = rm_word_value(h0, w, j0[u], k0[u], x0[u], a0[u]), v1 = rm_word_value(h1, w, j1[u], k1[u], x1[u], a1[u]);
+      if (full)
+        bw[w] = ((uint32_t)v0 & 0xFFFFu) | ((uint32_t)v1 << 16);
+      else if (do0)
+        bh[2 * w] = (short)v0;
+      else
+        bh[2 * w + 1] = (short)v1;
+    }
   }
 }
 
@@ -195,10 +237,10 @@ extern "C" void launch_pdsch_front(const DevCell& c, const DevGrant* grants, uin
   pdsch_demod_kernel<<<ngrants, 256, 0, st>>>(c, grants, sym, ce, seq_pool, llr_pool);
   *launches += 2;
 }
-extern "C" void launch_rm_turbo_rx(const DevCb* cbs, uint32_t ncb, const DevPair* pairs, const short* llr_pool, const uint32_t* rm_pool,
+extern "C" void launch_rm_turbo_rx(const DevCb* cbs, const DevPair* pairs, uint32_t npairs, const short* llr_pool, const uint16_t* rm_pool,
                                    uint32_t* turbo_pool, short* harq_pool, uint32_t gen, cudaStream_t st, uint64_t* launches)
 {
-  if (!ncb) return;
-  rm_turbo_rx_kernel<<<ncb, 256, 0, st>>>(cbs, pairs, llr_pool, rm_pool, turbo_pool, harq_pool, gen);
+  if (!npairs) return;
+  rm_turbo_rx_kernel<<<npairs, 256, 0, st>>>(cbs, pairs, llr_pool, rm_pool, turbo_pool, harq_pool, gen);
   *launches += 1;
 }

@@ -1,5 +1,6 @@
 // lte_host.cpp -- see lte_host.hpp.  Product code (host side, C++17).
 #include "lte_host.hpp"
+#include "../../include/ltephy_b200.h"
 #include "../../include/lte_tables.h"
 #include <algorithm>
 #include <cmath>
@@ -373,6 +374,28 @@ RmTurboTable rm_turbo_table(uint32_t K, uint32_t F, uint32_t rv)
   }
   t.nn = (uint32_t)t.order.size();
   return t;
+}
+uint32_t rm_turbo_word(uint32_t K, uint32_t s)
+{
+  const uint32_t D = K + 4, NW = (K + 31) / 32, st = s / D, i = s % D;
+  return i < K ? st * 32 * NW + (i & 31u) * NW + (i >> 5) : 3 * 32 * NW + st * 4 + (i - K);
+}
+RmTurboInverse rm_turbo_inverse(uint32_t K, uint32_t F)
+{
+  const uint32_t D = K + 4, NW = (K + 31) / 32;
+  RmTurboInverse r;
+  r.inv.assign((size_t)96 * NW + 16, (uint16_t)LTEPHY_RM_NONE);
+  for (uint32_t st = 0; st < 2; st++)
+    for (uint32_t i = 0; i < F; i++) r.inv[rm_turbo_word(K, st * D + i)] = (uint16_t)LTEPHY_RM_FILLER;
+  for (uint32_t rv = 0; rv < 4; rv++) {
+    const RmTurboTable t = rm_turbo_table(K, F, rv);
+    if (rv == 0) {
+      r.nn = t.nn;
+      for (uint32_t j = 0; j < t.nn; j++) r.inv[rm_turbo_word(K, t.order[j])] = (uint16_t)j;
+    }
+    r.rot[rv] = t.nn ? r.inv[rm_turbo_word(K, t.order[0])] : 0;
+  }
+  return r;
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -89,6 +89,17 @@ struct RmTurboTable {
   std::vector<uint32_t> order; // [nn]
 };
 RmTurboTable rm_turbo_table(uint32_t K, uint32_t F, uint32_t rv);
+// word of the turbo pair buffer that holds stream position s = st*(K+4)+i: the window-transposed sys / p1 / p2 streams ([32][NW]
+// each, i < K), then the 12 tail words; 4 pad words end the buffer (96*NW + 16 words)
+uint32_t rm_turbo_word(uint32_t K, uint32_t s);
+// rm_turbo_table inverted per pair-buffer word, for every redundancy version at once: inv[w] = position j in [0, nn) of word w in the
+// rv-0 order, LTEPHY_RM_FILLER for a filler bit of sys / p1, LTEPHY_RM_NONE for a word no soft bit reaches.  nn does not depend on
+// rv (N_cb = K_w), so the order of rv is the rv-0 order rotated by rot[rv]: soft bit k of rv lands on the word with j = (k + rot[rv]) mod nn.
+struct RmTurboInverse {
+  uint32_t              nn = 0, rot[4]{};
+  std::vector<uint16_t> inv; // [96*NW + 16]
+};
+RmTurboInverse rm_turbo_inverse(uint32_t K, uint32_t F);
 
 // ---- PDSCH resource elements: count of data REs of symbol l in PRB prb (and which k) ---------
 uint32_t pdsch_re_in_prb(const Cell& c, uint32_t sf_idx, uint32_t cfi, uint32_t l, uint32_t prb, uint16_t* k /*12*/);

@@ -27,7 +27,7 @@ void launch_viterbi(const DevCell&, const float*, const DevSfInfo*, ltephy_cand_
 void launch_compact(const DevCell&, const DevSfInfo*, const ltephy_cand_t*, ltephy_compact_t*, uint32_t, cudaStream_t, uint64_t*);
 void launch_pdsch_front(const DevCell&, const DevGrant*, uint32_t, uint32_t, const float2*, const float2*, const uint32_t*, const uint32_t*, uint32_t,
                         uint32_t*, short*, cudaStream_t, uint64_t*);
-void launch_rm_turbo_rx(const DevCb*, uint32_t, const DevPair*, const short*, const uint32_t*, uint32_t*, short*, uint32_t, cudaStream_t, uint64_t*);
+void launch_rm_turbo_rx(const DevCb*, const DevPair*, uint32_t, const short*, const uint16_t*, uint32_t*, short*, uint32_t, cudaStream_t, uint64_t*);
 void launch_turbo(const DevPair*, uint32_t, uint32_t, int, uint32_t*, const uint32_t*, uint32_t*, size_t, const uint16_t*, const uint32_t*,
                   const uint32_t*, const uint32_t*, uint8_t*, uint8_t*, uint8_t*, uint32_t, cudaStream_t, uint64_t*);
 void launch_tb_crc(const DevTb*, uint32_t, const uint8_t*, const uint8_t*, const uint8_t*, const uint32_t*, ltephy_tb_result_t*, cudaStream_t,
@@ -109,7 +109,6 @@ extern "C" int ltephy_create(const ltephy_cfg_t* cfg, ltephy_t** out)
   h->cell = {cfg->nof_prb, cfg->nof_ports, cfg->cell_id, cfg->nof_rx, cfg->phich_resources, cfg->phich_length};
   if (!ltehost::build_ctrl_map(h->cell, h->cm)) return fail(LTEPHY_ERROR_INVALID_INPUTS, "control region map failed");
   h->st = ltehost::dci_size_table(h->cell);
-  memset(h->rm_fast, 0xFF, sizeof(h->rm_fast));
   memset(h->pi_fast, 0xFF, sizeof(h->pi_fast));
   h->segm_fast.assign(110000 / 8, ltehost::Segm{});
   CU(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
@@ -259,7 +258,7 @@ extern "C" int ltephy_create(const ltephy_cfg_t* cfg, ltephy_t** out)
   const size_t S = cfg->max_subframes, g = (size_t)14 * c.nsc;
   if (h->d_iq.reserve(S * c.nof_rx * c.sf_len) || h->d_sym.reserve(S * c.nof_rx * g) || h->d_pil.reserve(S * c.nof_ports * c.nof_rx * 4 * 2 * c.nof_prb) ||
       h->d_llr.reserve(S * LLR_STRIDE) || h->d_info.reserve(S) || h->d_cands.reserve(S * LTEPHY_MAX_LOC * LTEPHY_MAX_SIZES) || h->d_vwork.reserve(S * (LTEPHY_MAX_LOC / 2) * LTEPHY_MAX_SIZES + 16) ||
-      h->h_info.reserve(S) || h->d_compact.reserve(S) || h->h_compact.reserve(S) || h->d_rm.reserve((size_t)16 << 20) || h->d_pi.reserve((size_t)188 * 6144))
+      h->h_info.reserve(S) || h->d_compact.reserve(S) || h->h_compact.reserve(S) || h->d_rm.reserve((size_t)4 << 20) || h->d_pi.reserve((size_t)188 * 6144))
     return fail(LTEPHY_ERROR, "device allocation failed");
   CU(cudaMemset(h->d_cands.p, 0, h->d_cands.cap * sizeof(ltephy_cand_t)));
   guard.ok = true;
@@ -446,45 +445,45 @@ static int ltephy_turbo_scratch(ltephy* h)
   if (h->d_tqueue.reserve(16)) return -1;
   return 0;
 }
-static int rm_table_for(ltephy* h, uint32_t K, uint32_t F, uint32_t rv, uint32_t& off, uint32_t& nn)
+// inverse rate-matching table of (K, F) in the pool (one per code-block size and filler count; the redundancy version is a rotation)
+static const ltephy::RmEntry* rm_table_for(ltephy* h, uint32_t K, uint32_t F)
 {
   const int ki = lte_qpp_index_ge(K);
-  if (F == 0 && rv < 4 && ki >= 0 && h->rm_fast[ki][rv] >= 0) {
-    off = (uint32_t)h->rm_fast[ki][rv], nn = h->rm_fast_nn[ki][rv];
-    return 0;
-  }
-  auto key = std::make_tuple(K, F, rv);
-  auto it  = h->rm_cache.find(key);
-  if (it != h->rm_cache.end()) {
-    off = it->second.first, nn = it->second.second;
-    return 0;
-  }
-  auto t = ltehost::rm_turbo_table(K, F, rv);
-  { // stream position -> word index inside the pair buffer (window-transposed streams, then the 12 tail words)
-    const uint32_t D = K + 4, NW = (K + 31) / 32;
-    for (auto& v : t.order) {
-      const uint32_t st = v / D, i = v % D;
-      v = i < K ? st * 32 * NW + (i & 31u) * NW + (i >> 5) : 3 * 32 * NW + st * 4 + (i - K);
-    }
-  }
-  if (h->rm_used + t.order.size() > h->d_rm.cap) { // pool full: grow it and keep every offset handed out so far valid
-    const size_t want = 2 * h->d_rm.cap + t.order.size();
-    uint32_t*    np   = nullptr;
-    if (cudaStreamSynchronize(h->stream) != cudaSuccess || cudaMalloc(&np, want * sizeof(uint32_t)) != cudaSuccess) return -1;
-    if (cudaMemcpy(np, h->d_rm.p, h->rm_used * sizeof(uint32_t), cudaMemcpyDeviceToDevice) != cudaSuccess) {
+  if (ki < 0 || lte_qpp_K((uint32_t)ki) != K) return nullptr;
+  ltephy::RmEntry& e = F == 0 ? h->rm_fast[ki] : h->rm_cache[{K, F}];
+  if (e.off >= 0) return &e;
+  auto t = ltehost::rm_turbo_inverse(K, F);
+  if (h->rm_used + t.inv.size() > h->d_rm.cap) { // pool full: grow it and keep every offset handed out so far valid
+    const size_t want = 2 * h->d_rm.cap + t.inv.size();
+    uint16_t*    np   = nullptr;
+    if (cudaStreamSynchronize(h->stream) != cudaSuccess || cudaMalloc(&np, want * sizeof(uint16_t)) != cudaSuccess) return nullptr;
+    if (cudaMemcpy(np, h->d_rm.p, h->rm_used * sizeof(uint16_t), cudaMemcpyDeviceToDevice) != cudaSuccess) {
       cudaFree(np);
-      return -1;
+      return nullptr;
     }
     cudaFree(h->d_rm.p);
     h->d_rm.p = np, h->d_rm.cap = want;
   }
-  off = (uint32_t)h->rm_used, nn = t.nn;
-  if (cudaMemcpyAsync(h->d_rm.p + off, t.order.data(), t.order.size() * 4, cudaMemcpyHostToDevice, h->stream) != cudaSuccess) return -1;
+  if (cudaMemcpyAsync(h->d_rm.p + h->rm_used, t.inv.data(), t.inv.size() * sizeof(uint16_t), cudaMemcpyHostToDevice, h->stream) != cudaSuccess)
+    return nullptr;
   cudaStreamSynchronize(h->stream); // source vector dies at scope exit
-  h->rm_used += t.order.size();
-  h->rm_cache[key] = {off, nn};
-  if (F == 0 && rv < 4 && ki >= 0) h->rm_fast[ki][rv] = off, h->rm_fast_nn[ki][rv] = nn;
-  return 0;
+  e.off = (int64_t)h->rm_used, e.nn = t.nn;
+  memcpy(e.rot, t.rot, sizeof(e.rot));
+  h->rm_used += t.inv.size();
+  return &e;
+}
+extern "C" int ltephy_rm_turbo_tables(uint32_t K, uint32_t F, uint32_t rv, uint32_t* order, uint32_t* nn, uint16_t* inv, uint32_t* rot)
+{
+  const int ki = lte_qpp_index_ge(K);
+  if (ki < 0 || lte_qpp_K((uint32_t)ki) != K || F >= K || rv > 3 || !order || !nn || !inv || !rot)
+    return fail(LTEPHY_ERROR_INVALID_INPUTS, "rm_turbo_tables: bad arguments");
+  const auto t = ltehost::rm_turbo_table(K, F, rv);
+  for (uint32_t k = 0; k < t.nn; k++) order[k] = ltehost::rm_turbo_word(K, t.order[k]);
+  *nn          = t.nn;
+  const auto v = ltehost::rm_turbo_inverse(K, F);
+  memcpy(inv, v.inv.data(), v.inv.size() * sizeof(uint16_t));
+  memcpy(rot, v.rot, sizeof(v.rot));
+  return LTEPHY_SUCCESS;
 }
 static int pi_table_for(ltephy* h, uint32_t K, uint32_t& off)
 {
@@ -538,7 +537,9 @@ static int add_transport_block(ltephy* h, uint32_t tbs, uint32_t G, uint32_t qm,
     rp += cb.E;
     cb.shift = qm == 2 ? 0 : qm == 4 ? 1 : 2;
     cb.harq_op = harq_op, cb.harq_off = harq_op ? (uint32_t)((size_t)harq_slot * (LTEPHY_HARQ_SLOT_BYTES / 2) + (size_t)r * 18448u) : 0u, cb.harq_gen = harq_gen;
-    if (rm_table_for(h, cb.K, cb.F, rv, cb.rm_tab, cb.rm_nn)) return fail(LTEPHY_ERROR, "rate-matching table upload failed");
+    const ltephy::RmEntry* rm = rm_table_for(h, cb.K, cb.F);
+    if (!rm) return fail(LTEPHY_ERROR, "rate-matching table upload failed");
+    cb.rm_tab = (uint32_t)rm->off, cb.rm_nn = rm->nn, cb.rm_rot = rm->rot[rv & 3u];
     const int kq = lte_qpp_index_ge(cb.K);
     uint32_t  pi;
     if (open_pair[kq] >= 0) {
@@ -688,7 +689,7 @@ static int run_turbo_stage(ltephy* h, uint32_t max_iter)
   stage_and_pull(h, h->d_pair_pi_off.p, h->pair_pi_off.data(), h->pairs.size() * 4);
   stage_and_pull(h, h->d_cbs.p, h->cbs.data(), h->cbs.size() * sizeof(DevCb));
   for (uint32_t gen = 0; gen <= h->harq_max_gen; gen++) // one launch unless a HARQ slot is used more than once in this batch
-    launch_rm_turbo_rx(h->d_cbs.p, (uint32_t)h->cbs.size(), h->d_pairs.p, h->d_pllr.p, h->d_rm.p, h->d_turbo.p, h->d_harq.p, gen, h->stream, &h->launches);
+    launch_rm_turbo_rx(h->d_cbs.p, h->d_pairs.p, (uint32_t)h->pairs.size(), h->d_pllr.p, h->d_rm.p, h->d_turbo.p, h->d_harq.p, gen, h->stream, &h->launches);
   if (ltephy_turbo_scratch(h)) return fail(LTEPHY_ERROR, "device allocation failed");
   CU(cudaMemsetAsync(h->d_tqueue.p, 0, 16 * sizeof(uint32_t), h->stream));
   CU(cudaEventRecord(h->ev[4], h->stream));

@@ -123,7 +123,8 @@ struct ltephy {
   DevBuf<DevPair>       d_pairs;
   DevBuf<DevTb>         d_tbs;
   DevBuf<uint32_t>      d_pair_pi_off;
-  DevBuf<uint32_t>      d_seq, d_rm, d_turbo;
+  DevBuf<uint32_t>      d_seq, d_turbo;
+  DevBuf<uint16_t>      d_rm;
   DevBuf<uint32_t>      d_tscratch, d_tqueue; // persistent turbo kernel: per-CTA state slots, pair counters of the launches
   DevBuf<short>         d_pllr;
   DevBuf<uint16_t>      d_pi;
@@ -137,9 +138,12 @@ struct ltephy {
   size_t                     payload_bytes = 0, pllr_elems = 0;
   uint32_t *                 d_gold_x1 = nullptr, *d_gold_basis = nullptr, gold_words = 0;
   uint32_t *                 d_xpowA = nullptr, *d_xpowB = nullptr;
-  std::map<std::tuple<uint32_t, uint32_t, uint32_t>, std::pair<uint32_t, uint32_t>> rm_cache; // (K,F,rv) -> (offset, nn)
-  int64_t  rm_fast[188][4];   // F == 0 fast path: offset or -1
-  uint32_t rm_fast_nn[188][4];
+  struct RmEntry {
+    int64_t  off = -1; // offset of the inverse table in d_rm, -1: not built yet
+    uint32_t nn = 0, rot[4]{};
+  };
+  std::map<std::pair<uint32_t, uint32_t>, RmEntry> rm_cache; // (K, F) -> inverse table
+  RmEntry                                          rm_fast[188]; // F == 0 fast path, by qpp index
   int64_t  pi_fast[188];
   std::vector<ltehost::Segm> segm_fast; // index tbs/8, C == 0 means "not computed"
   // uplink
