@@ -353,13 +353,21 @@ enum {
 int ltephy_tap(ltephy_t* h, int what, void* dst, size_t bytes);
 /* turbo rate-dematch tables of a code block of size K with F filler bits, as phase B uses them; no device needed.  LTEPHY_TAP_TURBO_IN
  * holds one buffer of 96*NW + 16 words (NW = ceil(K/32)) per code-block pair: the sys / p1 / p2 streams, stream index i at word
- * (i % 32) * NW + i / 32 of the stream, then 12 tail words and 4 pad words; code block 0 of the pair in the low 16 bits.
+ * (i % 32) * NW + i / 32 of the stream, then 12 tail words and 4 pad words; code block 0 of the pair in the low 16 bits.  The tap pairs
+ * code blocks of equal K in submission order, buffers in the order of their first code block (the decoder's own pairs are ltephy_turbo_pairing's).
  * order[k], k < *nn: word that soft bit k (and k + nn, k + 2 nn, ...) of redundancy version rv lands on (3*(K+4) entries of room).
  * inv[w] (96*NW + 16 entries): the word's position j in the order of rv 0, or LTEPHY_RM_FILLER / LTEPHY_RM_NONE; soft bit k of
  * redundancy version v lands on the word with j = (k + rot[v]) mod nn.  Returns -2 for a K that is not a turbo block size. */
 #define LTEPHY_RM_FILLER 0xFFFEu /* filler bit of the systematic or first parity stream: a known 0 */
 #define LTEPHY_RM_NONE   0xFFFFu /* ragged window slot or pad word: no soft bit lands here */
 int ltephy_rm_turbo_tables(uint32_t K, uint32_t F, uint32_t rv, uint32_t* order, uint32_t* nn, uint16_t* inv, uint32_t* rot);
+
+/* Turbo pairs of phase B (host only, needs no device): code block i of a batch -- block size K[i], TBS tbs[i] and rate-matched bits G[i]
+ * of its transport block -- is decoded in half half[i] (0 or 1) of pair pair[i], *npairs pairs in all.  Both halves of a pair have the
+ * same K.  Blocks of one K are paired in the order of their code rate TBS / G (in steps of 2^-16, saturating at 1), highest first, then
+ * by index: a pair decodes until both halves are done, and blocks of similar rate tend to need similar iteration counts.  Pairs are
+ * numbered by K (largest first), then in that order.  Returns -2 for bad arguments or a K that is not a turbo block size. */
+int ltephy_turbo_pairing(uint32_t ncb, const uint32_t* K, const uint32_t* tbs, const uint32_t* G, uint32_t* pair, uint32_t* half, uint32_t* npairs);
 
 /* timing of the last batch, from CUDA events on the library's stream (ms): [0] H2D+phase A, [1] phase B */
 int ltephy_last_timing(ltephy_t* h, float ms[4]);

@@ -107,15 +107,17 @@ template <int P0> __device__ __forceinline__ void vit_traceback(const uint32_t* 
 #undef TB_SLOW
 }
 
-// One work item = (subframe, pair of locations, payload size) whose pair holds at least one decodable candidate (vit_worklist_kernel).
+// One work item = (subframe, two decodable locations -- or one and VIT_LOC_NONE --, payload size) (vit_worklist_kernel).  Every step below
+// is per 16-bit field or per candidate, so a candidate's result does not depend on which location shares its warp.
+#define VIT_LOC_NONE 0xFFu
 __device__ __forceinline__ void vit_decode_item(const DevCell& c, const float* __restrict__ llr_all, const DevSfInfo* __restrict__ info,
                                                 ltephy_cand_t* __restrict__ cands, const VitConst& vc, VitWarpSmem& sm, const uint32_t lane,
-                                                const uint32_t pair, const uint32_t si, const uint32_t sf)
+                                                const uint32_t loc0, const uint32_t loc1, const uint32_t si, const uint32_t sf)
 {
   const uint32_t cfi = info[sf].cfi;
   if (cfi < 1 || cfi > 3) return;
   const uint32_t nloc = c.nloc[cfi - 1];
-  if (2 * pair >= nloc) return;
+  if (loc0 >= nloc) return;
   const uint32_t nb = c.sizes[si], K = nb + 16, n3 = 3 * K;
   const float*   llr = llr_all + (size_t)sf * LLR_STRIDE;
   const uint16_t* tab = c.conv_tab[si];
@@ -124,7 +126,7 @@ __device__ __forceinline__ void vit_decode_item(const DevCell& c, const float* _
   bool     valid[2];
   uint32_t loc_i[2], ncce_c[2], L_c[2];
   for (int cd = 0; cd < 2; cd++) {
-    loc_i[cd] = 2 * pair + cd;
+    loc_i[cd] = cd ? loc1 : loc0;
     valid[cd] = loc_i[cd] < nloc;
     ncce_c[cd] = 0, L_c[cd] = 0;
     if (valid[cd]) {
@@ -345,48 +347,49 @@ __device__ __forceinline__ void vit_decode_item(const DevCell& c, const float* _
   }
 }
 
-// Work list of the decoder: every (subframe, pair, size) whose pair has a location that exists and whose CCEs are all above the power floor
-// (the rule the decoder applies itself); table entries of all other pairs are zeroed here, so nothing stale survives a change of CFI.
-// One CTA per subframe, one thread per pair of locations; items = work[16 ...], work[0] = count.
+// Work list of the decoder.  A location is decodable when it exists and, with LTEPHY_FLAG_SKIP_LOW_POWER, all its CCEs are above the power
+// floor (the rule the decoder applies itself).  The decodable locations of a subframe are paired in index order, an odd count leaving one
+// single-candidate item, so a warp never decodes an idle half beside a valid one.  Table entries of every other location are zeroed here,
+// so nothing stale survives a change of CFI.  One CTA per subframe, one thread per location; work[0] = item count, item i =
+// (work[16 + 2 i], work[17 + 2 i]) = (subframe, loc0 | loc1 << 8 | size << 16), loc1 = VIT_LOC_NONE for a single candidate.
 #define VIT_WORK_HDR 16u
-__global__ void __launch_bounds__(128) vit_worklist_kernel(const __grid_constant__ DevCell c, const DevSfInfo* __restrict__ info, uint32_t* __restrict__ work,
-                                                           ltephy_cand_t* __restrict__ cands)
+__global__ void __launch_bounds__(LTEPHY_MAX_LOC) vit_worklist_kernel(const __grid_constant__ DevCell c, const DevSfInfo* __restrict__ info,
+                                                                      uint32_t* __restrict__ work, ltephy_cand_t* __restrict__ cands)
 {
-  __shared__ uint32_t scan[128];
+  static_assert(LTEPHY_MAX_LOC % 32 == 0 && LTEPHY_MAX_LOC <= VIT_LOC_NONE, "layout");
+  __shared__ uint32_t wcnt[LTEPHY_MAX_LOC / 32];
+  __shared__ uint8_t  order[LTEPHY_MAX_LOC]; // decodable locations, ascending
   __shared__ uint32_t base_s;
-  const uint32_t sf = blockIdx.x, pair = threadIdx.x, cfi = info[sf].cfi;
+  const uint32_t sf = blockIdx.x, li = threadIdx.x, lane = li & 31u, warp = li >> 5, cfi = info[sf].cfi;
   const uint32_t nloc = (cfi >= 1 && cfi <= 3) ? c.nloc[cfi - 1] : 0;
-  bool           any = false;
-  if (pair < LTEPHY_MAX_LOC / 2) {
-    for (uint32_t cd = 0; cd < 2; cd++) {
-      const uint32_t li = 2 * pair + cd;
-      bool           v  = li < nloc;
-      if (v && (c.flags & LTEPHY_FLAG_SKIP_LOW_POWER)) {
-        const uint32_t e = c.loc_tab[cfi - 1][li], ncce = e & 0xFFu, L = e >> 8;
-        for (uint32_t i = ncce; i < ncce + (1u << L); i++)
-          if (info[sf].cce_power[i] < 0.7f) v = false;
-      }
-      any |= v;
-    }
-    if (!any) {
-      const ltephy_cand_t z{};
-      for (uint32_t cd = 0; cd < 2; cd++)
-        for (uint32_t si = 0; si < c.nsizes; si++) cands[((size_t)sf * LTEPHY_MAX_LOC + 2 * pair + cd) * LTEPHY_MAX_SIZES + si] = z;
-    }
+  bool           v    = li < nloc;
+  if (v && (c.flags & LTEPHY_FLAG_SKIP_LOW_POWER)) {
+    const uint32_t e = c.loc_tab[cfi - 1][li], ncce = e & 0xFFu, L = e >> 8;
+    for (uint32_t i = ncce; i < ncce + (1u << L); i++)
+      if (info[sf].cce_power[i] < 0.7f) v = false;
   }
-  const uint32_t mine = any ? c.nsizes : 0u;
-  scan[threadIdx.x]   = mine;
-  __syncthreads();
-  for (uint32_t off = 1; off < 128; off <<= 1) { // inclusive scan
-    const uint32_t v = threadIdx.x >= off ? scan[threadIdx.x - off] : 0u;
-    __syncthreads();
-    scan[threadIdx.x] += v;
-    __syncthreads();
+  if (!v) {
+    const ltephy_cand_t z{};
+    for (uint32_t si = 0; si < c.nsizes; si++) cands[((size_t)sf * LTEPHY_MAX_LOC + li) * LTEPHY_MAX_SIZES + si] = z;
   }
-  if (threadIdx.x == 127) base_s = atomicAdd(&work[0], scan[127]);
+  const uint32_t bal = __ballot_sync(0xffffffffu, v);
+  if (lane == 0) wcnt[warp] = __popc(bal);
   __syncthreads();
-  uint32_t w = VIT_WORK_HDR + base_s + scan[threadIdx.x] - mine;
-  for (uint32_t si = 0; si < mine; si++) work[w + si] = (sf * 128u + pair) * 8u + si;
+  uint32_t rank = __popc(bal & ((1u << lane) - 1u)), total = 0;
+#pragma unroll
+  for (uint32_t w = 0; w < LTEPHY_MAX_LOC / 32; w++) {
+    if (w < warp) rank += wcnt[w];
+    total += wcnt[w];
+  }
+  if (v) order[rank] = (uint8_t)li;
+  const uint32_t nitems = (total + 1) / 2;
+  if (li == 0) base_s = atomicAdd(&work[0], nitems * c.nsizes);
+  __syncthreads();
+  if (li < nitems) {
+    const uint32_t l0 = order[2 * li], l1 = 2 * li + 1 < total ? order[2 * li + 1] : VIT_LOC_NONE;
+    uint2*         dst = reinterpret_cast<uint2*>(work + VIT_WORK_HDR) + base_s + li * c.nsizes;
+    for (uint32_t si = 0; si < c.nsizes; si++) dst[si] = make_uint2(sf, l0 | (l1 << 8) | (si << 16));
+  }
 }
 
 __global__ void __launch_bounds__(VIT_WARPS * 32) dci_viterbi_kernel(const __grid_constant__ DevCell c, const float* __restrict__ llr_all,
@@ -395,9 +398,10 @@ __global__ void __launch_bounds__(VIT_WARPS * 32) dci_viterbi_kernel(const __gri
 {
   __shared__ VitWarpSmem sm_all[VIT_WARPS];
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31, count = work[0];
+  const uint2*   items = reinterpret_cast<const uint2*>(work + VIT_WORK_HDR);
   for (uint32_t it = blockIdx.x * VIT_WARPS + warp; it < count; it += gridDim.x * VIT_WARPS) { // every warp of the grid decodes real work
-    const uint32_t item = work[VIT_WORK_HDR + it];
-    vit_decode_item(c, llr_all, info, cands, vc, sm_all[warp], lane, (item >> 3) & 127u, item & 7u, item >> 10);
+    const uint2 item = items[it];
+    vit_decode_item(c, llr_all, info, cands, vc, sm_all[warp], lane, item.y & 0xFFu, (item.y >> 8) & 0xFFu, item.y >> 16, item.x);
     __syncwarp(); // the next item's prologue reuses the decision store
   }
 }
@@ -412,7 +416,7 @@ extern "C" void launch_viterbi(const DevCell& c, const float* llr, const DevSfIn
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, dci_viterbi_kernel, VIT_WARPS * 32, 0);
   cudaMemsetAsync(work, 0, VIT_WORK_HDR * sizeof(uint32_t), st);
-  vit_worklist_kernel<<<n, 128, 0, st>>>(c, info, work, cands);
+  vit_worklist_kernel<<<n, LTEPHY_MAX_LOC, 0, st>>>(c, info, work, cands);
   const uint32_t max_items = n * (LTEPHY_MAX_LOC / 2) * c.nsizes, want = (max_items + VIT_WARPS - 1) / VIT_WARPS;
   const uint32_t grid = (uint32_t)sms * (uint32_t)(per_sm > 0 ? per_sm : 1);
   dci_viterbi_kernel<<<grid < want ? grid : want, VIT_WARPS * 32, 0, st>>>(c, llr, info, cands, work, vc);

@@ -5,6 +5,7 @@
 #include "../../include/ltephy_search.h"
 #include "ltephy_internal.cuh"
 #include "../../include/lte_tables.h"
+#include <algorithm>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
@@ -257,7 +258,7 @@ extern "C" int ltephy_create(const ltephy_cfg_t* cfg, ltephy_t** out)
   }
   const size_t S = cfg->max_subframes, g = (size_t)14 * c.nsc;
   if (h->d_iq.reserve(S * c.nof_rx * c.sf_len) || h->d_sym.reserve(S * c.nof_rx * g) || h->d_pil.reserve(S * c.nof_ports * c.nof_rx * 4 * 2 * c.nof_prb) ||
-      h->d_llr.reserve(S * LLR_STRIDE) || h->d_info.reserve(S) || h->d_cands.reserve(S * LTEPHY_MAX_LOC * LTEPHY_MAX_SIZES) || h->d_vwork.reserve(S * (LTEPHY_MAX_LOC / 2) * LTEPHY_MAX_SIZES + 16) ||
+      h->d_llr.reserve(S * LLR_STRIDE) || h->d_info.reserve(S) || h->d_cands.reserve(S * LTEPHY_MAX_LOC * LTEPHY_MAX_SIZES) || h->d_vwork.reserve(S * (LTEPHY_MAX_LOC / 2) * LTEPHY_MAX_SIZES * 2 + 16) ||
       h->h_info.reserve(S) || h->d_compact.reserve(S) || h->h_compact.reserve(S) || h->d_rm.reserve((size_t)4 << 20) || h->d_pi.reserve((size_t)188 * 6144))
     return fail(LTEPHY_ERROR, "device allocation failed");
   CU(cudaMemset(h->d_cands.p, 0, h->d_cands.cap * sizeof(ltephy_cand_t)));
@@ -512,9 +513,9 @@ static int pi_table_for(ltephy* h, uint32_t K, uint32_t& off)
   return 0;
 }
 
-// transport block -> code blocks -> turbo pairs (shared by the PDSCH and PUSCH paths)
-static int add_transport_block(ltephy* h, uint32_t tbs, uint32_t G, uint32_t qm, uint32_t rv, uint32_t NL, uint32_t llr_off, int32_t* open_pair,
-                               size_t& turbo_words, uint32_t& tb_index, uint32_t harq_op = LTEPHY_HARQ_NONE, uint32_t harq_slot = 0)
+// transport block -> code blocks (shared by the PDSCH and PUSCH paths); pair_code_blocks puts them into turbo pairs once the batch is complete
+static int add_transport_block(ltephy* h, uint32_t tbs, uint32_t G, uint32_t qm, uint32_t rv, uint32_t NL, uint32_t llr_off, uint32_t& tb_index,
+                               uint32_t harq_op = LTEPHY_HARQ_NONE, uint32_t harq_slot = 0)
 {
   if (tbs / 8 >= h->segm_fast.size() || (tbs & 7)) return fail(LTEPHY_ERROR_INVALID_INPUTS, "invalid TBS %u", tbs);
   if (h->segm_fast[tbs / 8].C == 0 && !ltehost::cb_segmentation(tbs, h->segm_fast[tbs / 8])) return fail(LTEPHY_ERROR_INVALID_INPUTS, "invalid TBS %u", tbs);
@@ -540,40 +541,88 @@ static int add_transport_block(ltephy* h, uint32_t tbs, uint32_t G, uint32_t qm,
     const ltephy::RmEntry* rm = rm_table_for(h, cb.K, cb.F);
     if (!rm) return fail(LTEPHY_ERROR, "rate-matching table upload failed");
     cb.rm_tab = (uint32_t)rm->off, cb.rm_nn = rm->nn, cb.rm_rot = rm->rot[rv & 3u];
-    const int kq = lte_qpp_index_ge(cb.K);
-    uint32_t  pi;
-    if (open_pair[kq] >= 0) {
-      pi            = (uint32_t)open_pair[kq];
-      open_pair[kq] = -1;
-      cb.half       = 1;
-    } else {
-      DevPair p{};
-      p.K = cb.K, p.NW = (cb.K + 31) / 32;
-      ltehost::qpp_params(cb.K, p.f1, p.f2);
-      p.buf_off = (uint32_t)turbo_words;
-      turbo_words += ltephy_pair_words(p.NW);
-      uint32_t po;
-      if (pi_table_for(h, cb.K, po)) return fail(LTEPHY_ERROR, "interleaver table upload failed");
-      pi = (uint32_t)h->pairs.size();
-      h->pairs.push_back(p);
-      h->pair_pi_off.push_back(po);
-      open_pair[kq] = (int32_t)pi;
-      cb.half       = 0;
-    }
-    cb.pair           = pi;
-    DevPair&       p  = h->pairs[pi];
-    const uint32_t hh = cb.half;
-    p.ncb             = hh + 1;
-    p.crc_type[hh]    = s.C > 1 ? 2 : 1;
-    p.out_skip[hh]    = cb.F;
-    p.out_bits[hh]    = cb.K - cb.F - (s.C > 1 ? 24 : 0);
-    p.out_byte[hh]    = tb.byte_off + wbit / 8;
-    p.cb_index[hh]    = (uint32_t)h->cbs.size();
-    wbit += p.out_bits[hh];
+    ltephy::CbHalf o;
+    o.tbs = tbs, o.G = G, o.crc_type = s.C > 1 ? 2 : 1, o.out_bits = cb.K - cb.F - (s.C > 1 ? 24 : 0), o.out_byte = tb.byte_off + wbit / 8;
+    wbit += o.out_bits;
     h->cbs.push_back(cb);
+    h->cb_half.push_back(o);
   }
   tb_index = (uint32_t)h->tbs.size();
   h->tbs.push_back(tb);
+  return LTEPHY_SUCCESS;
+}
+
+// Code blocks -> turbo pairs (two code blocks of equal K, one per 16-bit half).  A pair runs until both halves pass their CRC or reach the
+// iteration limit, so it costs K x the larger of the two iteration counts, while each half's result depends on its own inputs alone.
+// Blocks of one K are therefore paired in the order of their transport block's code rate TBS / G (highest first, in steps of 2^-16, then
+// index): neighbours in that order tend to need similar iteration counts.  Pairs are numbered in the same order, larger K first, so each
+// persistent turbo launch (one per CTA size, run_turbo_stage) takes its longest pairs off the queue first.  This runs on the host for every
+// batch, between the DCI walk and the launch of phase B, so it is a stable counting sort of a 24-bit key (187 - QPP index of K, then
+// 0xFFFF - rate), two passes of 12 bits: O(n), where a comparison sort of a cfg-2 batch's 25 000 code blocks took milliseconds.
+static uint32_t turbo_pairing(uint32_t ncb, const uint32_t* K, const uint32_t* tbs, const uint32_t* G, uint32_t* pair, uint32_t* half)
+{
+  std::vector<uint32_t> key(ncb), ord(ncb), tmp(ncb), cnt(4097);
+  for (uint32_t i = 0; i < ncb; i++) {
+    const uint64_t rate = G[i] ? std::min<uint64_t>(((uint64_t)tbs[i] << 16) / G[i], 0xFFFFu) : 0xFFFFu;
+    key[i] = ((187u - (uint32_t)lte_qpp_index_ge(K[i])) << 16) | (0xFFFFu - (uint32_t)rate);
+    ord[i] = i;
+  }
+  for (uint32_t shift = 0; shift < 24; shift += 12) {
+    std::fill(cnt.begin(), cnt.end(), 0u);
+    for (uint32_t i = 0; i < ncb; i++) cnt[((key[i] >> shift) & 0xFFFu) + 1]++;
+    for (uint32_t d = 0; d < 4096; d++) cnt[d + 1] += cnt[d];
+    for (uint32_t j = 0; j < ncb; j++) tmp[cnt[(key[ord[j]] >> shift) & 0xFFFu]++] = ord[j];
+    ord.swap(tmp);
+  }
+  uint32_t np = 0;
+  for (uint32_t j = 0; j < ncb; j++) {
+    const uint32_t ci = ord[j];
+    const bool     second = j > 0 && half[ord[j - 1]] == 0 && K[ord[j - 1]] == K[ci];
+    half[ci] = second ? 1u : 0u;
+    pair[ci] = second ? np - 1 : np++;
+  }
+  return np;
+}
+extern "C" int ltephy_turbo_pairing(uint32_t ncb, const uint32_t* K, const uint32_t* tbs, const uint32_t* G, uint32_t* pair, uint32_t* half,
+                                    uint32_t* npairs)
+{
+  if ((ncb && (!K || !tbs || !G || !pair || !half)) || !npairs) return fail(LTEPHY_ERROR_INVALID_INPUTS, "turbo_pairing: bad arguments");
+  for (uint32_t i = 0; i < ncb; i++) {
+    const int ki = lte_qpp_index_ge(K[i]);
+    if (ki < 0 || lte_qpp_K((uint32_t)ki) != K[i]) return fail(LTEPHY_ERROR_INVALID_INPUTS, "turbo_pairing: K=%u is not a turbo block size", K[i]);
+  }
+  *npairs = turbo_pairing(ncb, K, tbs, G, pair, half);
+  return LTEPHY_SUCCESS;
+}
+static int pair_code_blocks(ltephy* h, size_t& turbo_words)
+{
+  const uint32_t        ncb = (uint32_t)h->cbs.size();
+  std::vector<uint32_t> K(ncb), tbs(ncb), G(ncb), pair(ncb), half(ncb);
+  for (uint32_t i = 0; i < ncb; i++) K[i] = h->cbs[i].K, tbs[i] = h->cb_half[i].tbs, G[i] = h->cb_half[i].G;
+  h->pairs.assign(turbo_pairing(ncb, K.data(), tbs.data(), G.data(), pair.data(), half.data()), DevPair{});
+  for (uint32_t ci = 0; ci < ncb; ci++) {
+    DevCb&                cb = h->cbs[ci];
+    DevPair&              p  = h->pairs[pair[ci]];
+    const ltephy::CbHalf& o  = h->cb_half[ci];
+    const uint32_t        hh = half[ci];
+    cb.pair = pair[ci], cb.half = hh;
+    p.K = cb.K, p.ncb = std::max(p.ncb, hh + 1);
+    p.crc_type[hh] = o.crc_type;
+    p.out_skip[hh] = cb.F;
+    p.out_bits[hh] = o.out_bits;
+    p.out_byte[hh] = o.out_byte;
+    p.cb_index[hh] = ci;
+  }
+  turbo_words = 0;
+  h->pair_pi_off.resize(h->pairs.size());
+  for (uint32_t pi = 0; pi < h->pairs.size(); pi++) {
+    DevPair& p = h->pairs[pi];
+    p.NW = (p.K + 31) / 32;
+    ltehost::qpp_params(p.K, p.f1, p.f2);
+    p.buf_off = (uint32_t)turbo_words;
+    turbo_words += ltephy_pair_words(p.NW);
+    if (pi_table_for(h, p.K, h->pair_pi_off[pi])) return fail(LTEPHY_ERROR, "interleaver table upload failed");
+  }
   return LTEPHY_SUCCESS;
 }
 
@@ -581,13 +630,12 @@ static int build_jobs(ltephy* h, const ltephy_grant_t* gin, uint32_t n, size_t& 
 {
   const DevCell& c = h->dc;
   const uint32_t N = c.nof_prb;
-  h->grants.clear(), h->cbs.clear(), h->pairs.clear(), h->tbs.clear(), h->pair_pi_off.clear(), h->harq_uses.clear(), h->harq_max_gen = 0;
+  h->grants.clear(), h->cbs.clear(), h->cb_half.clear(), h->pairs.clear(), h->tbs.clear(), h->pair_pi_off.clear(), h->harq_uses.clear(), h->harq_max_gen = 0;
   h->tb_slot.assign((size_t)n * 2, 0xFFFFFFFFu);
   h->pllr_elems = 0, h->payload_bytes = 0;
   seq_words = 0, turbo_words = 0, max_scr_words = 0;
-  int32_t open_pair[188]; // qpp index of K -> pair index with a free half, or -1
-  memset(open_pair, 0xFF, sizeof(open_pair));
-  h->grants.reserve(n), h->cbs.reserve((size_t)n * 4), h->pairs.reserve((size_t)n * 2), h->tbs.reserve((size_t)n * 2), h->pair_pi_off.reserve((size_t)n * 2);
+  h->grants.reserve(n), h->cbs.reserve((size_t)n * 4), h->cb_half.reserve((size_t)n * 4), h->pairs.reserve((size_t)n * 2), h->tbs.reserve((size_t)n * 2),
+      h->pair_pi_off.reserve((size_t)n * 2);
   for (uint32_t gi = 0; gi < n; gi++) {
     const ltephy_grant_t& g = gin[gi];
     if (g.sf >= h->n_cur) return fail(LTEPHY_ERROR_INVALID_INPUTS, "grant %u: subframe %u outside the batch", gi, g.sf);
@@ -648,7 +696,7 @@ static int build_jobs(ltephy* h, const ltephy_grant_t* gin, uint32_t n, size_t& 
       h->pllr_elems += (G + 7) & ~7u;
       if (g.tb[t].tbs > 0) {
         uint32_t tbi;
-        int r = add_transport_block(h, (uint32_t)g.tb[t].tbs, G, qm, g.tb[t].rv, g.tx_scheme == LTEPHY_TX_DIVERSITY ? 2 : 1, d.llr_off[cw], open_pair, turbo_words, tbi,
+        int r = add_transport_block(h, (uint32_t)g.tb[t].tbs, G, qm, g.tb[t].rv, g.tx_scheme == LTEPHY_TX_DIVERSITY ? 2 : 1, d.llr_off[cw], tbi,
                                     g.tb[t].harq_op, g.tb[t].harq_slot);
         if (r) return r;
         h->tb_slot[(size_t)gi * 2 + t] = tbi;
@@ -657,7 +705,7 @@ static int build_jobs(ltephy* h, const ltephy_grant_t* gin, uint32_t n, size_t& 
     d.ncw = n_en;
     h->grants.push_back(d);
   }
-  return LTEPHY_SUCCESS;
+  return pair_code_blocks(h, turbo_words);
 }
 
 static int run_turbo_stage(ltephy* h, uint32_t max_iter)
@@ -665,7 +713,7 @@ static int run_turbo_stage(ltephy* h, uint32_t max_iter)
   // pairs are launched in buckets of equal CTA size so that small code blocks do not pay for 192 threads
   std::vector<uint32_t> order(h->pairs.size());
   for (uint32_t i = 0; i < order.size(); i++) order[i] = i;
-  // (pairs were appended in arbitrary K order: bucket by rounded thread count)
+  // (bucket by rounded thread count; the pair order of pair_code_blocks is kept inside a bucket)
   std::map<uint32_t, std::vector<uint32_t>> buckets; // key = 2 * threads + (ragged last window)
   for (uint32_t i = 0; i < h->pairs.size(); i++) buckets[2 * (((h->pairs[i].NW + 31) / 32) * 32) + ((h->pairs[i].K & 31u) ? 1 : 0)].push_back(i);
   std::vector<DevPair>  sorted;
@@ -1055,13 +1103,11 @@ extern "C" int ltephy_submit_ul(ltephy_t* h, const float* iq_ul, const uint32_t*
   }
   h->n_ul = n;
   // jobs
-  h->ulgrants.clear(), h->cbs.clear(), h->pairs.clear(), h->tbs.clear(), h->pair_pi_off.clear(), h->harq_uses.clear(), h->harq_max_gen = 0;
+  h->ulgrants.clear(), h->cbs.clear(), h->cb_half.clear(), h->pairs.clear(), h->tbs.clear(), h->pair_pi_off.clear(), h->harq_uses.clear(), h->harq_max_gen = 0;
   h->tb_slot.assign((size_t)ng, 0xFFFFFFFFu);
   h->pllr_elems = 0, h->payload_bytes = 0;
   size_t   seq_words = 0, turbo_words = 0;
   uint32_t max_words = 0, max_M = 36;
-  int32_t  open_pair[188];
-  memset(open_pair, 0xFF, sizeof(open_pair));
   for (uint32_t gi = 0; gi < ng; gi++) {
     const ltephy_ul_grant_t& g = gin[gi];
     if (g.sf >= n) return fail(LTEPHY_ERROR_INVALID_INPUTS, "UL grant %u: subframe outside the batch", gi);
@@ -1096,11 +1142,12 @@ extern "C" int ltephy_submit_ul(ltephy_t* h, const float* iq_ul, const uint32_t*
     h->pllr_elems += (G + 7) & ~7u;
     max_words = std::max(max_words, w), max_M = std::max(max_M, M);
     uint32_t tbi;
-    int      r = add_transport_block(h, (uint32_t)g.tbs, G, g.qm, g.rv, 1, d.llr_off, open_pair, turbo_words, tbi);
+    int      r = add_transport_block(h, (uint32_t)g.tbs, G, g.qm, g.rv, 1, d.llr_off, tbi);
     if (r) return r;
     h->tb_slot[gi] = tbi;
     h->ulgrants.push_back(d);
   }
+  if (int r = pair_code_blocks(h, turbo_words)) return r;
   if (h->stage_busy) CU(cudaStreamSynchronize(h->stream));
   h->stage_used = 0, h->stage_busy = true;
   if (h->h_stage.reserve(h->ulgrants.size() * sizeof(DevUlGrant) + h->tbs.size() * sizeof(DevTb) + h->pairs.size() * (sizeof(DevPair) + 4) +
@@ -1254,6 +1301,40 @@ extern "C" int ltephy_turbo_batch(ltephy_t* h, const int16_t* d, uint32_t K, uin
   return LTEPHY_SUCCESS;
 }
 
+// LTEPHY_TAP_TURBO_IN after a phase B: the decoder's pairs follow pair_code_blocks, but the tap lays each code block's stream out as if
+// equal-K code blocks were paired in submission order (buffers in the order of their first block), so that what it shows depends on the
+// grants and the soft bits alone, not on the pairing policy.
+static int tap_turbo_in(ltephy* h, void* dst, size_t bytes)
+{
+  std::vector<uint32_t> pool(h->d_turbo.cap);
+  CU(cudaStreamSynchronize(h->stream));
+  CU(cudaMemcpy(pool.data(), h->d_turbo.p, pool.size() * 4, cudaMemcpyDeviceToHost));
+  if (h->cbs.empty()) { // ltephy_turbo_batch: the pool is already in submission order
+    memcpy(dst, pool.data(), bytes);
+    return LTEPHY_SUCCESS;
+  }
+  std::vector<uint16_t>      out(pool.size() * 2, 0);
+  const uint16_t*            src = reinterpret_cast<const uint16_t*>(pool.data());
+  std::map<uint32_t, size_t> open; // K -> buffer with a free high half
+  size_t                     words = 0;
+  for (const DevCb& cb : h->cbs) {
+    const size_t n = ltephy_pair_words((cb.K + 31) / 32), from = h->pairs[cb.pair].buf_off;
+    size_t       to;
+    uint32_t     hh = 0;
+    auto         it = open.find(cb.K);
+    if (it != open.end()) {
+      to = it->second, hh = 1;
+      open.erase(it);
+    } else {
+      to = words, open[cb.K] = words;
+      words += n;
+    }
+    for (size_t w = 0; w < n; w++) out[2 * (to + w) + hh] = src[2 * (from + w) + cb.half];
+  }
+  memcpy(dst, out.data(), bytes);
+  return LTEPHY_SUCCESS;
+}
+
 extern "C" int ltephy_tap(ltephy_t* h, int what, void* dst, size_t bytes)
 {
   if (!h || !dst) return fail(LTEPHY_ERROR_INVALID_INPUTS, "tap: bad arguments");
@@ -1275,6 +1356,7 @@ extern "C" int ltephy_tap(ltephy_t* h, int what, void* dst, size_t bytes)
     default: return fail(LTEPHY_ERROR_INVALID_INPUTS, "tap: unknown buffer");
   }
   if (bytes > avail) return fail(LTEPHY_ERROR_INVALID_INPUTS, "tap: %zu bytes requested, %zu available", bytes, avail);
+  if (what == LTEPHY_TAP_TURBO_IN) return tap_turbo_in(h, dst, bytes);
   CU(cudaStreamSynchronize(h->stream));
   CU(cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost));
   return LTEPHY_SUCCESS;

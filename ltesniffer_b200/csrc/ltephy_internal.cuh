@@ -89,7 +89,7 @@ struct ltephy {
   cudaStream_t       stream = nullptr;
   cudaEvent_t        ev[6]{}, mark[2]{}, ev_h2d = nullptr;
   DevBuf<float2>     d_cfo;                  // per-sample rotation of ltephy_set_cfo
-  DevBuf<uint32_t>   d_vwork;                // work list of the Viterbi kernel: count + (subframe, pair, size) items
+  DevBuf<uint32_t>   d_vwork;                // work list of the Viterbi kernel: count + two-word (subframe, locations, size) items
   DevBuf<uint32_t>   d_mib;                  // PBCH work of one call: subframe of each frame, hypothesis jobs, 2 result words per job (k_pbch.cu)
   DevBuf<float>      d_pbch;                 // PBCH frame store [3 + max_subframes][2][480]: rows 0..2 the frames the combiner carries over
   uint32_t           mib_held     = 0;       // combiner: frames held (srsRAN's frame_idx between calls), in rows 3 - mib_held .. 2
@@ -114,6 +114,10 @@ struct ltephy {
   // phase B
   std::vector<DevGrant> grants;
   std::vector<DevCb>    cbs;
+  struct CbHalf {                // what a code block's half of its turbo pair needs, and its pairing key TBS / G (pair_code_blocks)
+    uint32_t tbs, G, crc_type, out_bits, out_byte;
+  };
+  std::vector<CbHalf>   cb_half; // [code block]
   std::vector<DevPair>  pairs;
   std::vector<DevTb>    tbs;
   std::vector<uint32_t> pair_pi_off;
