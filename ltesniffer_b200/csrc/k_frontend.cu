@@ -4,6 +4,7 @@
 // (src/src/SubframePower.cc:18-58).  Compiled with -fmad=false: every float expression is evaluated
 // in the order written, which is the order of the CPU oracle, so results are compared bit-for-bit.
 #include "dev_common.cuh"
+#include "k_launch.cuh"
 #include "dev_eq.cuh"
 
 // =================================================================================================

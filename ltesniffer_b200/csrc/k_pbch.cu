@@ -13,6 +13,7 @@
 //                    whose mask the remainder is (0x0000 / 0xFFFF / 0x5555 -> 1 / 2 / 4, 0 for none) and the 24 bits.  The host picks the winner.
 // A one-frame hypothesis at dst = q is, bit for bit, the decode of position q of lteo_pbch_decode: same arithmetic and tie rules.
 #include "dev_common.cuh"
+#include "k_launch.cuh"
 #include "dev_eq.cuh"
 
 #define PBCH_ROW 960 // floats per frame-store row: [port count - 1][480]

@@ -4,6 +4,7 @@
 // (reference src/src/DL_Sniffer_PDSCH.cc:997): srsran_predecoding_type, srsran_demod_soft_demodulate_s
 // (int16, scales 100*sqrt2/400/700/1000), srsran_scrambling, srsran_rm_turbo_rx_lut.
 #include "dev_common.cuh"
+#include "k_launch.cuh"
 #include "dev_eq.cuh"
 
 // ---- scrambling sequences: c = x1 ^ XOR_{b in c_init} basis[b]  (36.211 7.2 without the 1600-step warm-up)

@@ -8,6 +8,7 @@
 // The IDFT is a Stockham autosort with radices 5.., 3.., 4.., 2 whose butterflies are plain sums in index order, the same expression tree
 // as the oracle's, so the soft bits are bit-identical for every 2^a 3^b 5^c size.
 #include "dev_common.cuh"
+#include "k_launch.cuh"
 #include "dev_ul.cuh"
 
 __device__ __forceinline__ short ul_f2s(float v)

@@ -9,6 +9,7 @@
 // The arithmetic is the CPU oracle's (oracle/lte_oracle.c, siso()): outputs are offset-invariant, so
 // the int16 normalisation schedule below does not change any decision.
 #include "dev_common.cuh"
+#include "k_launch.cuh"
 
 #include "turbo_arith.cuh"
 

@@ -21,6 +21,7 @@
 //  * Survivor decisions are ballot words in the layout of the step; the traceback walks in the same rotated coordinates (one bit
 //    of the lane index is replaced per step), so it needs no permutation either.  CRC16 by GF(2) folding across the warp.
 #include "dev_common.cuh"
+#include "k_launch.cuh"
 
 #define VIT_KMAX 80          // nof_bits <= 64 -> K = nof_bits + 16 <= 80
 #define VIT_WARPS 4

@@ -4,6 +4,7 @@
 #include "../../include/ltephy_b200.h"
 #include "../../include/ltephy_search.h"
 #include "ltephy_internal.cuh"
+#include "k_launch.cuh"
 #include "../../include/lte_tables.h"
 #include <algorithm>
 #include <cmath>
@@ -18,25 +19,6 @@
 
 static std::mutex  g_h2d_mtx;
 static cudaEvent_t g_h2d_last[64]; // per device: completion of the most recently issued sample upload (phase_a_common)
-
-extern "C" {
-void launch_frontend(const DevCell&, const float2*, float2*, float2*, float*, DevSfInfo*, uint32_t, cudaStream_t, uint64_t*);
-void launch_chest_interp(const DevCell&, const float2*, float2*, uint32_t, cudaStream_t, uint64_t*);
-void launch_pbch(const DevCell&, const float2*, const float2*, const uint32_t*, uint32_t, uint32_t, uint32_t, float*, const uint32_t*, uint32_t, void*, cudaStream_t,
-                 uint64_t*);
-void launch_viterbi(const DevCell&, const float*, const DevSfInfo*, ltephy_cand_t*, uint32_t*, uint32_t, cudaStream_t, uint64_t*);
-void launch_compact(const DevCell&, const DevSfInfo*, const ltephy_cand_t*, ltephy_compact_t*, uint32_t, cudaStream_t, uint64_t*);
-void launch_pdsch_front(const DevCell&, const DevGrant*, uint32_t, uint32_t, const float2*, const float2*, const uint32_t*, const uint32_t*, uint32_t,
-                        uint32_t*, short*, cudaStream_t, uint64_t*);
-void launch_rm_turbo_rx(const DevCb*, const DevPair*, uint32_t, const short*, const uint16_t*, uint32_t*, short*, uint32_t, cudaStream_t, uint64_t*);
-void launch_turbo(const DevPair*, uint32_t, uint32_t, int, uint32_t*, const uint32_t*, uint32_t*, size_t, const uint16_t*, const uint32_t*,
-                  const uint32_t*, const uint32_t*, uint8_t*, uint8_t*, uint8_t*, uint32_t, cudaStream_t, uint64_t*);
-void launch_tb_crc(const DevTb*, uint32_t, const uint8_t*, const uint8_t*, const uint8_t*, const uint32_t*, ltephy_tb_result_t*, cudaStream_t,
-                   uint64_t*);
-void launch_ul_ofdm(const DevCell&, const float2*, float2*, uint32_t, cudaStream_t, uint64_t*);
-void launch_pusch(const DevCell&, const DevUlGrant*, uint32_t, uint32_t, uint32_t, const float2*, const float2*, const float2*, const uint32_t*,
-                  const uint32_t*, uint32_t, uint32_t*, short*, DevUlChest*, cudaStream_t, uint64_t*);
-}
 
 thread_local std::string ltephy_g_err;
 template <typename T>
@@ -325,10 +307,10 @@ extern "C" float ltephy_mark_elapsed_ms(ltephy_t* h)
 extern "C" int ltephy_last_turbo_work(ltephy_t* h, uint64_t* bytes, uint64_t* code_blocks, uint64_t* info_bits)
 {
   uint64_t b = 0, ib = 0;
-  for (auto& cb : h->cbs) b += 3ull * (cb.K + 4) * 2 + cb.K / 8;
-  for (auto& tb : h->tbs) ib += 8ull * tb.nbytes;
+  for (auto& cb : h->pb.cbs) b += 3ull * (cb.K + 4) * 2 + cb.K / 8;
+  for (auto& tb : h->pb.tbs) ib += 8ull * tb.nbytes;
   if (bytes) *bytes = b;
-  if (code_blocks) *code_blocks = h->cbs.size();
+  if (code_blocks) *code_blocks = h->pb.cbs.size();
   if (info_bits) *info_bits = ib;
   return LTEPHY_SUCCESS;
 }
@@ -436,15 +418,27 @@ extern "C" const ltephy_compact_t* ltephy_phase_a_compact_buffer(const ltephy_t*
 // words of one code-block pair in the turbo pool: the three window-transposed input streams (sys, p1, p2: [32][NW] each) and the
 // 12 termination words; the decoder keeps its extrinsic values in shared memory and its window-boundary metrics in per-CTA scratch
 static inline size_t ltephy_pair_words(uint32_t NW) { return (size_t)3 * 32 * NW + 16; }
-// per-CTA scratch of the persistent turbo kernel: 32 * NT words per resident CTA (k_turbo.cu); sized for the largest launch
-static int ltephy_turbo_scratch(ltephy* h)
+// Append n values to a pool of lazily built device tables and return their offset, or -1.  A full pool is reallocated to 2 * cap + n once
+// the stream has drained, and its used part copied over, so every offset handed out earlier stays valid.  The upload is synchronous, so src
+// may be a temporary.
+template <typename T>
+static int64_t pool_append(ltephy* h, DevBuf<T>& pool, size_t& used, const T* src, size_t n)
 {
-  int sms = 132;
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->cfg.device);
-  // resident CTAs x threads is at most 2048 threads per SM; 32 words per thread
-  if (h->d_tscratch.reserve((size_t)sms * 2048 * 32)) return -1;
-  if (h->d_tqueue.reserve(16)) return -1;
-  return 0;
+  if (used + n > pool.cap) {
+    const size_t want = 2 * pool.cap + n;
+    T*           np   = nullptr;
+    if (cudaStreamSynchronize(h->stream) != cudaSuccess || cudaMalloc(&np, want * sizeof(T)) != cudaSuccess) return -1;
+    if (cudaMemcpy(np, pool.p, used * sizeof(T), cudaMemcpyDeviceToDevice) != cudaSuccess) {
+      cudaFree(np);
+      return -1;
+    }
+    cudaFree(pool.p);
+    pool.p = np, pool.cap = want;
+  }
+  if (cudaMemcpyAsync(pool.p + used, src, n * sizeof(T), cudaMemcpyHostToDevice, h->stream) != cudaSuccess) return -1;
+  cudaStreamSynchronize(h->stream);
+  used += n;
+  return (int64_t)(used - n);
 }
 // inverse rate-matching table of (K, F) in the pool (one per code-block size and filler count; the redundancy version is a rotation)
 static const ltephy::RmEntry* rm_table_for(ltephy* h, uint32_t K, uint32_t F)
@@ -454,23 +448,9 @@ static const ltephy::RmEntry* rm_table_for(ltephy* h, uint32_t K, uint32_t F)
   ltephy::RmEntry& e = F == 0 ? h->rm_fast[ki] : h->rm_cache[{K, F}];
   if (e.off >= 0) return &e;
   auto t = ltehost::rm_turbo_inverse(K, F);
-  if (h->rm_used + t.inv.size() > h->d_rm.cap) { // pool full: grow it and keep every offset handed out so far valid
-    const size_t want = 2 * h->d_rm.cap + t.inv.size();
-    uint16_t*    np   = nullptr;
-    if (cudaStreamSynchronize(h->stream) != cudaSuccess || cudaMalloc(&np, want * sizeof(uint16_t)) != cudaSuccess) return nullptr;
-    if (cudaMemcpy(np, h->d_rm.p, h->rm_used * sizeof(uint16_t), cudaMemcpyDeviceToDevice) != cudaSuccess) {
-      cudaFree(np);
-      return nullptr;
-    }
-    cudaFree(h->d_rm.p);
-    h->d_rm.p = np, h->d_rm.cap = want;
-  }
-  if (cudaMemcpyAsync(h->d_rm.p + h->rm_used, t.inv.data(), t.inv.size() * sizeof(uint16_t), cudaMemcpyHostToDevice, h->stream) != cudaSuccess)
-    return nullptr;
-  cudaStreamSynchronize(h->stream); // source vector dies at scope exit
-  e.off = (int64_t)h->rm_used, e.nn = t.nn;
+  if ((e.off = pool_append(h, h->d_rm, h->rm_used, t.inv.data(), t.inv.size())) < 0) return nullptr;
+  e.nn = t.nn;
   memcpy(e.rot, t.rot, sizeof(e.rot));
-  h->rm_used += t.inv.size();
   return &e;
 }
 extern "C" int ltephy_rm_turbo_tables(uint32_t K, uint32_t F, uint32_t rv, uint32_t* order, uint32_t* nn, uint16_t* inv, uint32_t* rot)
@@ -486,30 +466,20 @@ extern "C" int ltephy_rm_turbo_tables(uint32_t K, uint32_t F, uint32_t rv, uint3
   memcpy(rot, v.rot, sizeof(v.rot));
   return LTEPHY_SUCCESS;
 }
+// QPP interleaver table of K in the pool, window-transposed like the turbo streams
 static int pi_table_for(ltephy* h, uint32_t K, uint32_t& off)
 {
   const int ki = lte_qpp_index_ge(K);
-  if (ki >= 0 && h->pi_fast[ki] >= 0) {
-    off = (uint32_t)h->pi_fast[ki];
-    return 0;
+  if (ki < 0) return -1;
+  if (h->pi_fast[ki] < 0) {
+    uint32_t f1, f2;
+    if (!ltehost::qpp_params(K, f1, f2)) return -1;
+    const uint32_t        NW = (K + 31) / 32;
+    std::vector<uint16_t> t((size_t)32 * NW, 0);
+    for (uint64_t i = 0; i < K; i++) t[(i & 31) * NW + (i >> 5)] = (uint16_t)((f1 * i + f2 * i * i) % K);
+    if ((h->pi_fast[ki] = pool_append(h, h->d_pi, h->pi_used, t.data(), t.size())) < 0) return -1;
   }
-  auto it = h->pi_cache.find(K);
-  if (it != h->pi_cache.end()) {
-    off = it->second;
-    return 0;
-  }
-  uint32_t f1, f2;
-  if (!ltehost::qpp_params(K, f1, f2)) return -1;
-  const uint32_t        NW = (K + 31) / 32;
-  std::vector<uint16_t> t((size_t)32 * NW, 0);
-  for (uint64_t i = 0; i < K; i++) t[(i & 31) * NW + (i >> 5)] = (uint16_t)((f1 * i + f2 * i * i) % K);
-  if (h->pi_used + t.size() > h->d_pi.cap) return -1;
-  off = (uint32_t)h->pi_used;
-  if (cudaMemcpyAsync(h->d_pi.p + off, t.data(), t.size() * 2, cudaMemcpyHostToDevice, h->stream) != cudaSuccess) return -1;
-  cudaStreamSynchronize(h->stream);
-  h->pi_used += t.size();
-  h->pi_cache[K] = off;
-  if (ki >= 0) h->pi_fast[ki] = off;
+  off = (uint32_t)h->pi_fast[ki];
   return 0;
 }
 
@@ -520,16 +490,17 @@ static int add_transport_block(ltephy* h, uint32_t tbs, uint32_t G, uint32_t qm,
   if (tbs / 8 >= h->segm_fast.size() || (tbs & 7)) return fail(LTEPHY_ERROR_INVALID_INPUTS, "invalid TBS %u", tbs);
   if (h->segm_fast[tbs / 8].C == 0 && !ltehost::cb_segmentation(tbs, h->segm_fast[tbs / 8])) return fail(LTEPHY_ERROR_INVALID_INPUTS, "invalid TBS %u", tbs);
   const ltehost::Segm& s = h->segm_fast[tbs / 8];
+  ltephy::PhaseB&      b = h->pb;
   uint32_t             harq_gen = 0;
   if (harq_op != LTEPHY_HARQ_NONE) {
     if (harq_op > LTEPHY_HARQ_RETX || harq_slot >= h->harq_slots) return fail(LTEPHY_ERROR_INVALID_INPUTS, "HARQ slot %u outside the store (%u slots, ltephy_harq_reserve)", harq_slot, h->harq_slots);
     if (s.C > 16) return fail(LTEPHY_ERROR_INVALID_INPUTS, "transport block of %u code blocks does not fit a HARQ slot", s.C);
-    harq_gen        = h->harq_uses[harq_slot]++; // a slot used again inside one batch: its rate-dematch runs in a later launch, after the earlier use
-    h->harq_max_gen = std::max(h->harq_max_gen, harq_gen);
+    harq_gen       = b.harq_uses[harq_slot]++; // a slot used again inside one batch: its rate-dematch runs in a later launch, after the earlier use
+    b.harq_max_gen = std::max(b.harq_max_gen, harq_gen);
   }
   DevTb                tb{};
-  tb.byte_off = (uint32_t)h->payload_bytes, tb.nbytes = tbs / 8, tb.cb_first = (uint32_t)h->cbs.size(), tb.ncb = s.C;
-  h->payload_bytes += (tb.nbytes + 3 + 3) & ~3u;
+  tb.byte_off = (uint32_t)b.payload_bytes, tb.nbytes = tbs / 8, tb.cb_first = (uint32_t)b.cbs.size(), tb.ncb = s.C;
+  b.payload_bytes += (tb.nbytes + 3 + 3) & ~3u;
   uint32_t rp = llr_off, wbit = 0;
   for (uint32_t r = 0; r < s.C; r++) {
     DevCb cb{};
@@ -541,22 +512,35 @@ static int add_transport_block(ltephy* h, uint32_t tbs, uint32_t G, uint32_t qm,
     const ltephy::RmEntry* rm = rm_table_for(h, cb.K, cb.F);
     if (!rm) return fail(LTEPHY_ERROR, "rate-matching table upload failed");
     cb.rm_tab = (uint32_t)rm->off, cb.rm_nn = rm->nn, cb.rm_rot = rm->rot[rv & 3u];
-    ltephy::CbHalf o;
+    ltephy::PhaseB::CbHalf o;
     o.tbs = tbs, o.G = G, o.crc_type = s.C > 1 ? 2 : 1, o.out_bits = cb.K - cb.F - (s.C > 1 ? 24 : 0), o.out_byte = tb.byte_off + wbit / 8;
     wbit += o.out_bits;
-    h->cbs.push_back(cb);
-    h->cb_half.push_back(o);
+    b.cbs.push_back(cb);
+    b.cb_half.push_back(o);
   }
-  tb_index = (uint32_t)h->tbs.size();
-  h->tbs.push_back(tb);
+  tb_index = (uint32_t)b.tbs.size();
+  b.tbs.push_back(tb);
   return LTEPHY_SUCCESS;
+}
+// LLR and scrambling space of one codeword: G soft bits, scrambled with the first `bits` bits of the Gold sequence (PDSCH: G, PUSCH: 12 M Qm);
+// false if the scrambling basis is shorter
+static bool alloc_codeword(ltephy* h, uint32_t bits, uint32_t G, uint32_t& llr_off, uint32_t& scr_off)
+{
+  ltephy::PhaseB& b = h->pb;
+  const uint32_t  w = (bits + 31) / 32;
+  if (w > h->gold_words) return false;
+  llr_off = (uint32_t)b.pllr_elems, scr_off = (uint32_t)b.seq_words;
+  b.max_scr_words = std::max(b.max_scr_words, w);
+  b.seq_words += w + 1; // +1: the demapper reads a 64-bit window
+  b.pllr_elems += (G + 7) & ~7u;
+  return true;
 }
 
 // Code blocks -> turbo pairs (two code blocks of equal K, one per 16-bit half).  A pair runs until both halves pass their CRC or reach the
 // iteration limit, so it costs K x the larger of the two iteration counts, while each half's result depends on its own inputs alone.
 // Blocks of one K are therefore paired in the order of their transport block's code rate TBS / G (highest first, in steps of 2^-16, then
 // index): neighbours in that order tend to need similar iteration counts.  Pairs are numbered in the same order, larger K first, so each
-// persistent turbo launch (one per CTA size, run_turbo_stage) takes its longest pairs off the queue first.  This runs on the host for every
+// persistent turbo launch (one per CTA size, launch_turbo_buckets) takes its longest pairs off the queue first.  This runs on the host for every
 // batch, between the DCI walk and the launch of phase B, so it is a stable counting sort of a 24-bit key (187 - QPP index of K, then
 // 0xFFFF - rate), two passes of 12 bits: O(n), where a comparison sort of a cfg-2 batch's 25 000 code blocks took milliseconds.
 static uint32_t turbo_pairing(uint32_t ncb, const uint32_t* K, const uint32_t* tbs, const uint32_t* G, uint32_t* pair, uint32_t* half)
@@ -594,17 +578,18 @@ extern "C" int ltephy_turbo_pairing(uint32_t ncb, const uint32_t* K, const uint3
   *npairs = turbo_pairing(ncb, K, tbs, G, pair, half);
   return LTEPHY_SUCCESS;
 }
-static int pair_code_blocks(ltephy* h, size_t& turbo_words)
+static int pair_code_blocks(ltephy* h)
 {
-  const uint32_t        ncb = (uint32_t)h->cbs.size();
+  ltephy::PhaseB&       b   = h->pb;
+  const uint32_t        ncb = (uint32_t)b.cbs.size();
   std::vector<uint32_t> K(ncb), tbs(ncb), G(ncb), pair(ncb), half(ncb);
-  for (uint32_t i = 0; i < ncb; i++) K[i] = h->cbs[i].K, tbs[i] = h->cb_half[i].tbs, G[i] = h->cb_half[i].G;
-  h->pairs.assign(turbo_pairing(ncb, K.data(), tbs.data(), G.data(), pair.data(), half.data()), DevPair{});
+  for (uint32_t i = 0; i < ncb; i++) K[i] = b.cbs[i].K, tbs[i] = b.cb_half[i].tbs, G[i] = b.cb_half[i].G;
+  b.pairs.assign(turbo_pairing(ncb, K.data(), tbs.data(), G.data(), pair.data(), half.data()), DevPair{});
   for (uint32_t ci = 0; ci < ncb; ci++) {
-    DevCb&                cb = h->cbs[ci];
-    DevPair&              p  = h->pairs[pair[ci]];
-    const ltephy::CbHalf& o  = h->cb_half[ci];
-    const uint32_t        hh = half[ci];
+    DevCb&                        cb = b.cbs[ci];
+    DevPair&                      p  = b.pairs[pair[ci]];
+    const ltephy::PhaseB::CbHalf& o  = b.cb_half[ci];
+    const uint32_t                hh = half[ci];
     cb.pair = pair[ci], cb.half = hh;
     p.K = cb.K, p.ncb = std::max(p.ncb, hh + 1);
     p.crc_type[hh] = o.crc_type;
@@ -613,29 +598,27 @@ static int pair_code_blocks(ltephy* h, size_t& turbo_words)
     p.out_byte[hh] = o.out_byte;
     p.cb_index[hh] = ci;
   }
-  turbo_words = 0;
-  h->pair_pi_off.resize(h->pairs.size());
-  for (uint32_t pi = 0; pi < h->pairs.size(); pi++) {
-    DevPair& p = h->pairs[pi];
+  b.turbo_words = 0;
+  b.pair_pi_off.resize(b.pairs.size());
+  for (uint32_t pi = 0; pi < b.pairs.size(); pi++) {
+    DevPair& p = b.pairs[pi];
     p.NW = (p.K + 31) / 32;
     ltehost::qpp_params(p.K, p.f1, p.f2);
-    p.buf_off = (uint32_t)turbo_words;
-    turbo_words += ltephy_pair_words(p.NW);
-    if (pi_table_for(h, p.K, h->pair_pi_off[pi])) return fail(LTEPHY_ERROR, "interleaver table upload failed");
+    p.buf_off = (uint32_t)b.turbo_words;
+    b.turbo_words += ltephy_pair_words(p.NW);
+    if (pi_table_for(h, p.K, b.pair_pi_off[pi])) return fail(LTEPHY_ERROR, "interleaver table upload failed");
   }
   return LTEPHY_SUCCESS;
 }
 
-static int build_jobs(ltephy* h, const ltephy_grant_t* gin, uint32_t n, size_t& seq_words, size_t& turbo_words, uint32_t& max_scr_words)
+static int build_jobs(ltephy* h, const ltephy_grant_t* gin, uint32_t n)
 {
-  const DevCell& c = h->dc;
-  const uint32_t N = c.nof_prb;
-  h->grants.clear(), h->cbs.clear(), h->cb_half.clear(), h->pairs.clear(), h->tbs.clear(), h->pair_pi_off.clear(), h->harq_uses.clear(), h->harq_max_gen = 0;
-  h->tb_slot.assign((size_t)n * 2, 0xFFFFFFFFu);
-  h->pllr_elems = 0, h->payload_bytes = 0;
-  seq_words = 0, turbo_words = 0, max_scr_words = 0;
-  h->grants.reserve(n), h->cbs.reserve((size_t)n * 4), h->cb_half.reserve((size_t)n * 4), h->pairs.reserve((size_t)n * 2), h->tbs.reserve((size_t)n * 2),
-      h->pair_pi_off.reserve((size_t)n * 2);
+  const DevCell&  c = h->dc;
+  const uint32_t  N = c.nof_prb;
+  ltephy::PhaseB& b = h->pb;
+  b.reset((size_t)n * 2);
+  b.grants.reserve(n), b.cbs.reserve((size_t)n * 4), b.cb_half.reserve((size_t)n * 4), b.pairs.reserve((size_t)n * 2), b.tbs.reserve((size_t)n * 2),
+      b.pair_pi_off.reserve((size_t)n * 2);
   for (uint32_t gi = 0; gi < n; gi++) {
     const ltephy_grant_t& g = gin[gi];
     if (g.sf >= h->n_cur) return fail(LTEPHY_ERROR_INVALID_INPUTS, "grant %u: subframe %u outside the batch", gi, g.sf);
@@ -686,63 +669,33 @@ static int build_jobs(ltephy* h, const ltephy_grant_t* gin, uint32_t n, size_t& 
       const uint32_t cw = n_en == 2 ? g.tb[t].cw_idx : 0u;
       const uint32_t qm = g.tb[t].qm, G = acc * qm;
       if (qm != 2 && qm != 4 && qm != 6 && qm != 8) return fail(LTEPHY_ERROR_INVALID_INPUTS, "grant %u: bad modulation order", gi);
-      d.qm[cw]      = qm;
-      d.llr_off[cw] = (uint32_t)h->pllr_elems;
-      d.scr_off[cw] = (uint32_t)seq_words;
-      const uint32_t w = (G + 31) / 32;
-      if (w > h->gold_words) return fail(LTEPHY_ERROR, "grant %u: codeword longer than the scrambling basis", gi);
-      max_scr_words = std::max(max_scr_words, w);
-      seq_words += w + 1; // +1: the demapper reads a 64-bit window
-      h->pllr_elems += (G + 7) & ~7u;
+      d.qm[cw] = qm;
+      if (!alloc_codeword(h, G, G, d.llr_off[cw], d.scr_off[cw])) return fail(LTEPHY_ERROR, "grant %u: codeword longer than the scrambling basis", gi);
       if (g.tb[t].tbs > 0) {
         uint32_t tbi;
         int r = add_transport_block(h, (uint32_t)g.tb[t].tbs, G, qm, g.tb[t].rv, g.tx_scheme == LTEPHY_TX_DIVERSITY ? 2 : 1, d.llr_off[cw], tbi,
                                     g.tb[t].harq_op, g.tb[t].harq_slot);
         if (r) return r;
-        h->tb_slot[(size_t)gi * 2 + t] = tbi;
+        b.tb_slot[(size_t)gi * 2 + t] = tbi;
       }
     }
     d.ncw = n_en;
-    h->grants.push_back(d);
+    b.grants.push_back(d);
   }
-  return pair_code_blocks(h, turbo_words);
+  return pair_code_blocks(h);
 }
 
-static int run_turbo_stage(ltephy* h, uint32_t max_iter)
+// The persistent turbo launches of h->pb.pairs, which lie in bucket order: one launch per bucket (2 * threads + ragged last window, pairs)
+static int launch_turbo_buckets(ltephy* h, const std::vector<std::pair<uint32_t, uint32_t>>& buckets, uint32_t max_iter)
 {
-  // pairs are launched in buckets of equal CTA size so that small code blocks do not pay for 192 threads
-  std::vector<uint32_t> order(h->pairs.size());
-  for (uint32_t i = 0; i < order.size(); i++) order[i] = i;
-  // (bucket by rounded thread count; the pair order of pair_code_blocks is kept inside a bucket)
-  std::map<uint32_t, std::vector<uint32_t>> buckets; // key = 2 * threads + (ragged last window)
-  for (uint32_t i = 0; i < h->pairs.size(); i++) buckets[2 * (((h->pairs[i].NW + 31) / 32) * 32) + ((h->pairs[i].K & 31u) ? 1 : 0)].push_back(i);
-  std::vector<DevPair>  sorted;
-  std::vector<uint32_t> sorted_pi;
-  std::vector<std::pair<uint32_t, uint32_t>> ranges; // (threads, count)
-  std::vector<uint32_t> remap(h->pairs.size());
-  for (auto& b : buckets) {
-    ranges.push_back({b.first, (uint32_t)b.second.size()});
-    for (uint32_t i : b.second) {
-      remap[i] = (uint32_t)sorted.size();
-      sorted.push_back(h->pairs[i]);
-      sorted_pi.push_back(h->pair_pi_off[i]);
-    }
-  }
-  for (auto& cb : h->cbs) cb.pair = remap[cb.pair];
-  h->pairs.swap(sorted);
-  h->pair_pi_off.swap(sorted_pi);
-  if (h->d_pairs.reserve(h->pairs.size()) || h->d_pair_pi_off.reserve(h->pairs.size()) || h->d_cbs.reserve(h->cbs.size()))
-    return fail(LTEPHY_ERROR, "device allocation failed");
-  stage_and_pull(h, h->d_pairs.p, h->pairs.data(), h->pairs.size() * sizeof(DevPair));
-  stage_and_pull(h, h->d_pair_pi_off.p, h->pair_pi_off.data(), h->pairs.size() * 4);
-  stage_and_pull(h, h->d_cbs.p, h->cbs.data(), h->cbs.size() * sizeof(DevCb));
-  for (uint32_t gen = 0; gen <= h->harq_max_gen; gen++) // one launch unless a HARQ slot is used more than once in this batch
-    launch_rm_turbo_rx(h->d_cbs.p, h->d_pairs.p, (uint32_t)h->pairs.size(), h->d_pllr.p, h->d_rm.p, h->d_turbo.p, h->d_harq.p, gen, h->stream, &h->launches);
-  if (ltephy_turbo_scratch(h)) return fail(LTEPHY_ERROR, "device allocation failed");
+  // per-CTA scratch (k_turbo.cu), sized for the largest launch: at most 2048 resident threads per SM, 32 words per thread
+  int sms = 132;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->cfg.device);
+  if (h->d_tscratch.reserve((size_t)sms * 2048 * 32) || h->d_tqueue.reserve(16)) return fail(LTEPHY_ERROR, "device allocation failed");
   CU(cudaMemsetAsync(h->d_tqueue.p, 0, 16 * sizeof(uint32_t), h->stream));
   CU(cudaEventRecord(h->ev[4], h->stream));
   uint32_t first = 0, bi = 0;
-  for (auto& r : ranges) {
+  for (auto& r : buckets) {
     launch_turbo(h->d_pairs.p + first, r.second, r.first / 2, (r.first & 1u) == 0, h->d_tqueue.p + (bi++ & 15u), h->d_turbo.p, h->d_tscratch.p,
                  h->d_tscratch.cap, h->d_pi.p, h->d_pair_pi_off.p + first, h->d_xpowA, h->d_xpowB, h->d_payload.p, h->d_cb_iters.p, h->d_cb_crc.p,
                  max_iter, h->stream, &h->launches);
@@ -752,36 +705,74 @@ static int run_turbo_stage(ltephy* h, uint32_t max_iter)
   return LTEPHY_SUCCESS;
 }
 
+// The tail of every phase B, after the front kernel has written the soft bits: rate-dematch and turbo-decode the code blocks, then check
+// the transport-block CRCs
+static int decode_code_blocks(ltephy* h)
+{
+  ltephy::PhaseB& b = h->pb;
+  if (b.cbs.empty()) return LTEPHY_SUCCESS;
+  // pairs are launched in buckets of equal CTA size so that small code blocks do not pay for 192 threads
+  // (bucket by rounded thread count; the pair order of pair_code_blocks is kept inside a bucket)
+  std::map<uint32_t, std::vector<uint32_t>> buckets; // key = 2 * threads + (ragged last window)
+  for (uint32_t i = 0; i < b.pairs.size(); i++) buckets[2 * (((b.pairs[i].NW + 31) / 32) * 32) + ((b.pairs[i].K & 31u) ? 1 : 0)].push_back(i);
+  std::vector<DevPair>  sorted;
+  std::vector<uint32_t> sorted_pi;
+  std::vector<std::pair<uint32_t, uint32_t>> ranges; // (key, count)
+  std::vector<uint32_t> remap(b.pairs.size());
+  for (auto& bk : buckets) {
+    ranges.push_back({bk.first, (uint32_t)bk.second.size()});
+    for (uint32_t i : bk.second) {
+      remap[i] = (uint32_t)sorted.size();
+      sorted.push_back(b.pairs[i]);
+      sorted_pi.push_back(b.pair_pi_off[i]);
+    }
+  }
+  for (auto& cb : b.cbs) cb.pair = remap[cb.pair];
+  b.pairs.swap(sorted);
+  b.pair_pi_off.swap(sorted_pi);
+  if (h->d_pairs.reserve(b.pairs.size()) || h->d_pair_pi_off.reserve(b.pairs.size()) || h->d_cbs.reserve(b.cbs.size()))
+    return fail(LTEPHY_ERROR, "device allocation failed");
+  stage_and_pull(h, h->d_pairs.p, b.pairs.data(), b.pairs.size() * sizeof(DevPair));
+  stage_and_pull(h, h->d_pair_pi_off.p, b.pair_pi_off.data(), b.pairs.size() * 4);
+  stage_and_pull(h, h->d_cbs.p, b.cbs.data(), b.cbs.size() * sizeof(DevCb));
+  for (uint32_t gen = 0; gen <= b.harq_max_gen; gen++) // one launch unless a HARQ slot is used more than once in this batch
+    launch_rm_turbo_rx(h->d_cbs.p, h->d_pairs.p, (uint32_t)b.pairs.size(), h->d_pllr.p, h->d_rm.p, h->d_turbo.p, h->d_harq.p, gen, h->stream, &h->launches);
+  if (int r = launch_turbo_buckets(h, ranges, h->cfg.turbo_max_iter)) return r;
+  launch_tb_crc(h->d_tbs.p, (uint32_t)b.tbs.size(), h->d_payload.p, h->d_cb_crc.p, h->d_cb_iters.p, h->d_xpowA, h->d_res.p, h->stream, &h->launches);
+  return LTEPHY_SUCCESS;
+}
+
+// Once a submit has built its batch: reset the pinned staging arena and size it for the batch's descriptors (grant_bytes of them are the
+// grants), and reserve the buffers every phase B uses.  The grant-specific buffers are the caller's.
+static int reserve_phase_b(ltephy* h, size_t grant_bytes)
+{
+  const ltephy::PhaseB& b = h->pb;
+  if (h->stage_busy) CU(cudaStreamSynchronize(h->stream)); // a phase B that was never fetched may still be pulling from the arena
+  h->stage_used = 0, h->stage_busy = true;
+  if (h->h_stage.reserve(grant_bytes + b.tbs.size() * sizeof(DevTb) + b.pairs.size() * (sizeof(DevPair) + 4) + b.cbs.size() * sizeof(DevCb) + 256))
+    return fail(LTEPHY_ERROR, "pinned allocation failed");
+  if (h->d_tbs.reserve(b.tbs.size() + 1) || h->d_seq.reserve(b.seq_words + 1) || h->d_pllr.reserve(b.pllr_elems + 8) || h->d_turbo.reserve(b.turbo_words + 1) ||
+      h->d_payload.reserve(b.payload_bytes + 4) || h->d_cb_iters.reserve(b.cbs.size() + 1) || h->d_cb_crc.reserve(b.cbs.size() + 1) ||
+      h->d_res.reserve(b.tbs.size() + 1) || h->h_res.reserve(b.tbs.size() + 1) || h->h_payload.reserve(b.payload_bytes + 4))
+    return fail(LTEPHY_ERROR, "device allocation failed");
+  return LTEPHY_SUCCESS;
+}
+
 extern "C" int ltephy_submit_grants(ltephy_t* h, const ltephy_grant_t* gin, uint32_t n)
 {
   if (!h || (!gin && n)) return fail(LTEPHY_ERROR_INVALID_INPUTS, "submit_grants: bad arguments");
   CU(cudaSetDevice(h->cfg.device));
-  size_t   seq_words, turbo_words;
-  uint32_t max_scr_words;
-  int      r = build_jobs(h, gin, n, seq_words, turbo_words, max_scr_words);
-  if (r) return r;
-  if (h->stage_busy) CU(cudaStreamSynchronize(h->stream)); // a phase B that was never fetched may still be pulling from the arena
-  h->stage_used = 0, h->stage_busy = true;
-  if (h->h_stage.reserve(h->grants.size() * sizeof(DevGrant) + h->tbs.size() * sizeof(DevTb) + h->pairs.size() * (sizeof(DevPair) + 4) +
-                         h->cbs.size() * sizeof(DevCb) + 256))
-    return fail(LTEPHY_ERROR, "pinned allocation failed");
-  if (h->d_grants.reserve(n + 1) || h->d_tbs.reserve(h->tbs.size() + 1) || h->d_seq.reserve(seq_words + 1) || h->d_pllr.reserve(h->pllr_elems + 8) ||
-      h->d_turbo.reserve(turbo_words + 1) || h->d_payload.reserve(h->payload_bytes + 4) || h->d_cb_iters.reserve(h->cbs.size() + 1) ||
-      h->d_cb_crc.reserve(h->cbs.size() + 1) || h->d_res.reserve(h->tbs.size() + 1) || h->h_res.reserve(h->tbs.size() + 1) ||
-      h->h_payload.reserve(h->payload_bytes + 4))
-    return fail(LTEPHY_ERROR, "device allocation failed");
+  if (int r = build_jobs(h, gin, n)) return r;
+  if (int r = reserve_phase_b(h, n * sizeof(DevGrant))) return r;
+  if (h->d_grants.reserve(n + 1)) return fail(LTEPHY_ERROR, "device allocation failed");
+  const ltephy::PhaseB& b = h->pb;
   CU(cudaEventRecord(h->ev[2], h->stream));
   if (n) {
-    stage_and_pull(h, h->d_grants.p, h->grants.data(), n * sizeof(DevGrant));
-    stage_and_pull(h, h->d_tbs.p, h->tbs.data(), h->tbs.size() * sizeof(DevTb));
-    launch_pdsch_front(h->dc, h->d_grants.p, n, max_scr_words, h->d_sym.p, h->d_pil.p, h->d_gold_x1, h->d_gold_basis, h->gold_words, h->d_seq.p,
+    stage_and_pull(h, h->d_grants.p, b.grants.data(), n * sizeof(DevGrant));
+    stage_and_pull(h, h->d_tbs.p, b.tbs.data(), b.tbs.size() * sizeof(DevTb));
+    launch_pdsch_front(h->dc, h->d_grants.p, n, b.max_scr_words, h->d_sym.p, h->d_pil.p, h->d_gold_x1, h->d_gold_basis, h->gold_words, h->d_seq.p,
                        h->d_pllr.p, h->stream, &h->launches);
-    if (!h->cbs.empty()) {
-      r = run_turbo_stage(h, h->cfg.turbo_max_iter);
-      if (r) return r;
-      launch_tb_crc(h->d_tbs.p, (uint32_t)h->tbs.size(), h->d_payload.p, h->d_cb_crc.p, h->d_cb_iters.p, h->d_xpowA, h->d_res.p, h->stream,
-                    &h->launches);
-    }
+    if (int r = decode_code_blocks(h)) return r;
   }
   CU(cudaEventRecord(h->ev[3], h->stream));
   CU(cudaGetLastError());
@@ -794,30 +785,31 @@ extern "C" int ltephy_copy_phase_b_device(ltephy_t* h, void* dst_dev, size_t cap
 {
   if (!h || !dst_dev || !nbytes) return fail(LTEPHY_ERROR_INVALID_INPUTS, "copy_phase_b_device: bad arguments");
   CU(cudaSetDevice(h->cfg.device));
-  const size_t n = h->payload_bytes < cap ? h->payload_bytes : cap;
+  const size_t n = h->pb.payload_bytes < cap ? h->pb.payload_bytes : cap;
   if (n) CU(cudaMemcpyAsync(dst_dev, h->d_payload.p, n, cudaMemcpyDeviceToDevice, h->stream));
   CU(cudaStreamSynchronize(h->stream));
   *nbytes = n;
   return LTEPHY_SUCCESS;
 }
+// Results of the last phase B, downlink or uplink: one per slot of tb_slot, the payload packed in slot order
 extern "C" int ltephy_get_phase_b(ltephy_t* h, ltephy_tb_result_t* results, uint8_t* payload, size_t payload_cap)
 {
   if (!h || !results) return fail(LTEPHY_ERROR_INVALID_INPUTS, "get_phase_b: bad arguments");
-  const size_t ntb = h->tbs.size();
-  if (ntb) {
-    CU(cudaMemcpyAsync(h->h_res.p, h->d_res.p, ntb * sizeof(ltephy_tb_result_t), cudaMemcpyDeviceToHost, h->stream));
-    CU(cudaMemcpyAsync(h->h_payload.p, h->d_payload.p, h->payload_bytes, cudaMemcpyDeviceToHost, h->stream));
+  const ltephy::PhaseB& b = h->pb;
+  if (!b.tbs.empty()) {
+    CU(cudaMemcpyAsync(h->h_res.p, h->d_res.p, b.tbs.size() * sizeof(ltephy_tb_result_t), cudaMemcpyDeviceToHost, h->stream));
+    CU(cudaMemcpyAsync(h->h_payload.p, h->d_payload.p, b.payload_bytes, cudaMemcpyDeviceToHost, h->stream));
   }
   CU(cudaStreamSynchronize(h->stream));
   h->stage_busy = false;
-  cudaEventElapsedTime(&h->t_ms[1], h->ev[2], h->ev[3]);
-  if (!h->cbs.empty()) cudaEventElapsedTime(&h->t_ms[2], h->ev[4], h->ev[5]);
+  cudaEventElapsedTime(&h->t_ms[1], h->ev[2], h->ev[3]); // uplink: from before the H2D of its samples
+  if (!b.cbs.empty()) cudaEventElapsedTime(&h->t_ms[2], h->ev[4], h->ev[5]);
   size_t wp = 0;
-  for (size_t i = 0; i < h->tb_slot.size(); i++) {
+  for (size_t i = 0; i < b.tb_slot.size(); i++) {
     ltephy_tb_result_t o{};
-    if (h->tb_slot[i] != 0xFFFFFFFFu) {
-      const DevTb& tb = h->tbs[h->tb_slot[i]];
-      o               = h->h_res.p[h->tb_slot[i]];
+    if (b.tb_slot[i] != 0xFFFFFFFFu) {
+      const DevTb& tb = b.tbs[b.tb_slot[i]];
+      o               = h->h_res.p[b.tb_slot[i]];
       o.payload_off   = (uint32_t)wp;
       o.payload_len   = tb.nbytes;
       if (payload) {
@@ -1077,12 +1069,9 @@ static int ul_table_for(ltephy* h, uint32_t kind, uint32_t M, uint32_t ncs, uint
       t[m]            = make_float2((float)std::cos(ph), (float)std::sin(ph));
     }
   }
-  if (h->ulpool_used + M > h->d_ulpool.cap) return -1;
-  off = (uint32_t)h->ulpool_used;
-  if (cudaMemcpyAsync(h->d_ulpool.p + off, t.data(), M * sizeof(float2), cudaMemcpyHostToDevice, h->stream) != cudaSuccess) return -1;
-  cudaStreamSynchronize(h->stream);
-  h->ulpool_used += M;
-  h->ul_tab_cache[key] = off;
+  const int64_t o = pool_append(h, h->d_ulpool, h->ulpool_used, t.data(), M);
+  if (o < 0) return -1;
+  off = h->ul_tab_cache[key] = (uint32_t)o;
   return 0;
 }
 
@@ -1103,11 +1092,9 @@ extern "C" int ltephy_submit_ul(ltephy_t* h, const float* iq_ul, const uint32_t*
   }
   h->n_ul = n;
   // jobs
-  h->ulgrants.clear(), h->cbs.clear(), h->cb_half.clear(), h->pairs.clear(), h->tbs.clear(), h->pair_pi_off.clear(), h->harq_uses.clear(), h->harq_max_gen = 0;
-  h->tb_slot.assign((size_t)ng, 0xFFFFFFFFu);
-  h->pllr_elems = 0, h->payload_bytes = 0;
-  size_t   seq_words = 0, turbo_words = 0;
-  uint32_t max_words = 0, max_M = 36;
+  ltephy::PhaseB& b = h->pb;
+  b.reset(ng);
+  uint32_t max_M = 36;
   for (uint32_t gi = 0; gi < ng; gi++) {
     const ltephy_ul_grant_t& g = gin[gi];
     if (g.sf >= n) return fail(LTEPHY_ERROR_INVALID_INPUTS, "UL grant %u: subframe outside the batch", gi);
@@ -1134,38 +1121,25 @@ extern "C" int ltephy_submit_ul(ltephy_t* h, const float* iq_ul, const uint32_t*
       if (ul_table_for(h, 0, M, ncs, h->ul_u[ns], M >= 72 ? h->ul_v[ns] : 0, d.dmrs_off[sl])) return fail(LTEPHY_ERROR, "UL table upload failed");
     }
     if (ul_table_for(h, 1, M, 0, 0, 0, d.idft_off)) return fail(LTEPHY_ERROR, "UL table upload failed");
-    const uint32_t G = L.G, w = (12 * M * g.qm + 31) / 32;
-    if (w > h->gold_words) return fail(LTEPHY_ERROR, "UL grant %u: codeword longer than the scrambling basis", gi);
+    const uint32_t G = L.G;
+    if (!alloc_codeword(h, 12 * M * g.qm, G, d.llr_off, d.scr_off)) return fail(LTEPHY_ERROR, "UL grant %u: codeword longer than the scrambling basis", gi);
     if (G < g.qm * 12) return fail(LTEPHY_ERROR_INVALID_INPUTS, "UL grant %u: the control information leaves no room for the transport block", gi);
-    d.llr_off = (uint32_t)h->pllr_elems, d.scr_off = (uint32_t)seq_words;
-    seq_words += w + 1;
-    h->pllr_elems += (G + 7) & ~7u;
-    max_words = std::max(max_words, w), max_M = std::max(max_M, M);
+    max_M = std::max(max_M, M);
     uint32_t tbi;
     int      r = add_transport_block(h, (uint32_t)g.tbs, G, g.qm, g.rv, 1, d.llr_off, tbi);
     if (r) return r;
-    h->tb_slot[gi] = tbi;
-    h->ulgrants.push_back(d);
+    b.tb_slot[gi] = tbi;
+    b.ulgrants.push_back(d);
   }
-  if (int r = pair_code_blocks(h, turbo_words)) return r;
-  if (h->stage_busy) CU(cudaStreamSynchronize(h->stream));
-  h->stage_used = 0, h->stage_busy = true;
-  if (h->h_stage.reserve(h->ulgrants.size() * sizeof(DevUlGrant) + h->tbs.size() * sizeof(DevTb) + h->pairs.size() * (sizeof(DevPair) + 4) +
-                         h->cbs.size() * sizeof(DevCb) + 256))
-    return fail(LTEPHY_ERROR, "pinned allocation failed");
-  if (h->d_ulgrants.reserve(ng + 1) || h->d_ulchest.reserve(ng + 1) || h->h_ulchest.reserve(ng + 1) || h->d_tbs.reserve(h->tbs.size() + 1) ||
-      h->d_seq.reserve(seq_words + 1) || h->d_pllr.reserve(h->pllr_elems + 8) || h->d_turbo.reserve(turbo_words + 1) ||
-      h->d_payload.reserve(h->payload_bytes + 4) || h->d_cb_iters.reserve(h->cbs.size() + 1) || h->d_cb_crc.reserve(h->cbs.size() + 1) ||
-      h->d_res.reserve(h->tbs.size() + 1) || h->h_res.reserve(h->tbs.size() + 1) || h->h_payload.reserve(h->payload_bytes + 4))
-    return fail(LTEPHY_ERROR, "device allocation failed");
+  if (int r = pair_code_blocks(h)) return r;
+  if (int r = reserve_phase_b(h, ng * sizeof(DevUlGrant))) return r;
+  if (h->d_ulgrants.reserve(ng + 1) || h->d_ulchest.reserve(ng + 1) || h->h_ulchest.reserve(ng + 1)) return fail(LTEPHY_ERROR, "device allocation failed");
   if (ng) {
-    stage_and_pull(h, h->d_ulgrants.p, h->ulgrants.data(), ng * sizeof(DevUlGrant));
-    stage_and_pull(h, h->d_tbs.p, h->tbs.data(), h->tbs.size() * sizeof(DevTb));
-    launch_pusch(c, h->d_ulgrants.p, ng, max_M, max_words, h->d_ulsym.p, h->d_ulpool.p, h->d_ulpool.p, h->d_gold_x1, h->d_gold_basis, h->gold_words,
+    stage_and_pull(h, h->d_ulgrants.p, b.ulgrants.data(), ng * sizeof(DevUlGrant));
+    stage_and_pull(h, h->d_tbs.p, b.tbs.data(), b.tbs.size() * sizeof(DevTb));
+    launch_pusch(c, h->d_ulgrants.p, ng, max_M, b.max_scr_words, h->d_ulsym.p, h->d_ulpool.p, h->d_ulpool.p, h->d_gold_x1, h->d_gold_basis, h->gold_words,
                  h->d_seq.p, h->d_pllr.p, h->d_ulchest.p, h->stream, &h->launches);
-    int r = run_turbo_stage(h, h->cfg.turbo_max_iter);
-    if (r) return r;
-    launch_tb_crc(h->d_tbs.p, (uint32_t)h->tbs.size(), h->d_payload.p, h->d_cb_crc.p, h->d_cb_iters.p, h->d_xpowA, h->d_res.p, h->stream, &h->launches);
+    if (int r = decode_code_blocks(h)) return r;
   }
   CU(cudaEventRecord(h->ev[3], h->stream));
   CU(cudaGetLastError());
@@ -1175,45 +1149,17 @@ extern "C" int ltephy_submit_ul(ltephy_t* h, const float* iq_ul, const uint32_t*
 extern "C" int ltephy_get_ul(ltephy_t* h, ltephy_tb_result_t* results, ltephy_ul_chest_t* chest, uint8_t* payload, size_t payload_cap)
 {
   if (!h || !results) return fail(LTEPHY_ERROR_INVALID_INPUTS, "get_ul: bad arguments");
-  const size_t ng = h->ulgrants.size();
+  const size_t ng = h->pb.ulgrants.size();
   if (ng) CU(cudaMemcpyAsync(h->h_ulchest.p, h->d_ulchest.p, ng * sizeof(DevUlChest), cudaMemcpyDeviceToHost, h->stream));
-  // transport blocks come back through the shared phase-B path (one result per grant)
-  std::vector<ltephy_tb_result_t> res(ng + 1);
-  {
-    const size_t ntb = h->tbs.size();
-    if (ntb) {
-      CU(cudaMemcpyAsync(h->h_res.p, h->d_res.p, ntb * sizeof(ltephy_tb_result_t), cudaMemcpyDeviceToHost, h->stream));
-      CU(cudaMemcpyAsync(h->h_payload.p, h->d_payload.p, h->payload_bytes, cudaMemcpyDeviceToHost, h->stream));
-    }
-    CU(cudaStreamSynchronize(h->stream));
-    h->stage_busy = false;
-    cudaEventElapsedTime(&h->t_ms[1], h->ev[2], h->ev[3]); // H2D of the UL samples + UL OFDM + PUSCH + rate-dematch + turbo + CRC
-    if (!h->cbs.empty()) cudaEventElapsedTime(&h->t_ms[2], h->ev[4], h->ev[5]);
-  }
-  size_t wp = 0;
-  for (size_t i = 0; i < ng; i++) {
-    ltephy_tb_result_t o{};
-    if (h->tb_slot[i] != 0xFFFFFFFFu) {
-      const DevTb& tb = h->tbs[h->tb_slot[i]];
-      o               = h->h_res.p[h->tb_slot[i]];
-      o.payload_off   = (uint32_t)wp;
-      o.payload_len   = tb.nbytes;
-      if (payload) {
-        if (wp + tb.nbytes > payload_cap) return fail(LTEPHY_ERROR_INVALID_INPUTS, "payload buffer too small");
-        memcpy(payload + wp, h->h_payload.p + tb.byte_off, tb.nbytes);
-      }
-      wp += tb.nbytes;
-    }
-    results[i] = o;
-    if (chest) {
-      const DevUlChest& dcst = h->h_ulchest.p[i];
-      chest[i].noise = dcst.noise, chest[i].rsrp = dcst.rsrp;
-      chest[i].snr_db = 10.0f * log10f(dcst.rsrp / dcst.noise);
-      // timing offset: -arg(sum ls[n+1] conj(ls[n])) / 2 pi per slot (srsran_vec_estimate_frequency over the pilots, meas_ta_en), slot average, / 15e-3 -> us
-      float ta = 0.0f;
-      for (int sl = 0; sl < 2; sl++) ta = ta + (-atan2f(dcst.ci[sl], dcst.cr[sl]) / 6.28318530717958647692f) / 2.0f;
-      chest[i].ta_us = std::isnormal(ta) ? ta / 15e-3f : 0.0f;
-    }
+  if (int r = ltephy_get_phase_b(h, results, payload, payload_cap)) return r; // one transport block per grant
+  for (size_t i = 0; i < ng && chest; i++) {
+    const DevUlChest& dcst = h->h_ulchest.p[i];
+    chest[i].noise = dcst.noise, chest[i].rsrp = dcst.rsrp;
+    chest[i].snr_db = 10.0f * log10f(dcst.rsrp / dcst.noise);
+    // timing offset: -arg(sum ls[n+1] conj(ls[n])) / 2 pi per slot (srsran_vec_estimate_frequency over the pilots, meas_ta_en), slot average, / 15e-3 -> us
+    float ta = 0.0f;
+    for (int sl = 0; sl < 2; sl++) ta = ta + (-atan2f(dcst.ci[sl], dcst.cr[sl]) / 6.28318530717958647692f) / 2.0f;
+    chest[i].ta_us = std::isnormal(ta) ? ta / 15e-3f : 0.0f;
   }
   return LTEPHY_SUCCESS;
 }
@@ -1252,7 +1198,8 @@ extern "C" int ltephy_turbo_batch(ltephy_t* h, const int16_t* d, uint32_t K, uin
   CU(cudaSetDevice(h->cfg.device));
   const uint32_t NW = (K + 31) / 32, D = K + 4, npairs = (ncb + 1) / 2;
   const size_t   pw = ltephy_pair_words(NW); // words per pair
-  h->pairs.clear(), h->pair_pi_off.clear(), h->cbs.clear(), h->tbs.clear(), h->harq_uses.clear(), h->harq_max_gen = 0;
+  ltephy::PhaseB& b = h->pb;
+  b.reset(0);
   uint32_t po;
   if (pi_table_for(h, K, po)) return fail(LTEPHY_ERROR, "interleaver table upload failed");
   std::vector<uint32_t> pool(pw * npairs, 0u);
@@ -1272,22 +1219,16 @@ extern "C" int ltephy_turbo_batch(ltephy_t* h, const int16_t* d, uint32_t K, uin
           buf[2 * word + hh]  = (short)(v > 255 ? 255 : (v < -255 ? -255 : v));
         }
     }
-    h->pairs.push_back(pr);
-    h->pair_pi_off.push_back(po);
+    b.pairs.push_back(pr);
+    b.pair_pi_off.push_back(po);
   }
   if (h->d_turbo.reserve(pool.size()) || h->d_pairs.reserve(npairs) || h->d_pair_pi_off.reserve(npairs) || h->d_payload.reserve((size_t)ncb * out_bytes) ||
       h->d_cb_iters.reserve(ncb) || h->d_cb_crc.reserve(ncb))
     return fail(LTEPHY_ERROR, "device allocation failed");
   CU(cudaMemcpyAsync(h->d_turbo.p, pool.data(), pool.size() * 4, cudaMemcpyHostToDevice, h->stream));
-  CU(cudaMemcpyAsync(h->d_pairs.p, h->pairs.data(), npairs * sizeof(DevPair), cudaMemcpyHostToDevice, h->stream));
-  CU(cudaMemcpyAsync(h->d_pair_pi_off.p, h->pair_pi_off.data(), npairs * 4, cudaMemcpyHostToDevice, h->stream));
-  if (ltephy_turbo_scratch(h)) return fail(LTEPHY_ERROR, "device allocation failed");
-  CU(cudaMemsetAsync(h->d_tqueue.p, 0, 16 * sizeof(uint32_t), h->stream));
-  CU(cudaEventRecord(h->ev[4], h->stream));
-  launch_turbo(h->d_pairs.p, npairs, NW, (K & 31u) == 0, h->d_tqueue.p, h->d_turbo.p, h->d_tscratch.p, h->d_tscratch.cap, h->d_pi.p,
-               h->d_pair_pi_off.p, h->d_xpowA, h->d_xpowB, h->d_payload.p, h->d_cb_iters.p, h->d_cb_crc.p, max_iter ? max_iter : 1, h->stream,
-               &h->launches);
-  CU(cudaEventRecord(h->ev[5], h->stream));
+  CU(cudaMemcpyAsync(h->d_pairs.p, b.pairs.data(), npairs * sizeof(DevPair), cudaMemcpyHostToDevice, h->stream));
+  CU(cudaMemcpyAsync(h->d_pair_pi_off.p, b.pair_pi_off.data(), npairs * 4, cudaMemcpyHostToDevice, h->stream));
+  if (int r = launch_turbo_buckets(h, {{2 * NW + ((K & 31u) ? 1u : 0u), npairs}}, max_iter ? max_iter : 1)) return r; // one bucket: NW threads
   std::vector<uint8_t> packed((size_t)ncb * out_bytes), it(ncb), ok(ncb);
   CU(cudaMemcpyAsync(packed.data(), h->d_payload.p, packed.size(), cudaMemcpyDeviceToHost, h->stream));
   CU(cudaMemcpyAsync(it.data(), h->d_cb_iters.p, ncb, cudaMemcpyDeviceToHost, h->stream));
@@ -1309,7 +1250,7 @@ static int tap_turbo_in(ltephy* h, void* dst, size_t bytes)
   std::vector<uint32_t> pool(h->d_turbo.cap);
   CU(cudaStreamSynchronize(h->stream));
   CU(cudaMemcpy(pool.data(), h->d_turbo.p, pool.size() * 4, cudaMemcpyDeviceToHost));
-  if (h->cbs.empty()) { // ltephy_turbo_batch: the pool is already in submission order
+  if (h->pb.cbs.empty()) { // ltephy_turbo_batch: the pool is already in submission order
     memcpy(dst, pool.data(), bytes);
     return LTEPHY_SUCCESS;
   }
@@ -1317,8 +1258,8 @@ static int tap_turbo_in(ltephy* h, void* dst, size_t bytes)
   const uint16_t*            src = reinterpret_cast<const uint16_t*>(pool.data());
   std::map<uint32_t, size_t> open; // K -> buffer with a free high half
   size_t                     words = 0;
-  for (const DevCb& cb : h->cbs) {
-    const size_t n = ltephy_pair_words((cb.K + 31) / 32), from = h->pairs[cb.pair].buf_off;
+  for (const DevCb& cb : h->pb.cbs) {
+    const size_t n = ltephy_pair_words((cb.K + 31) / 32), from = h->pb.pairs[cb.pair].buf_off;
     size_t       to;
     uint32_t     hh = 0;
     auto         it = open.find(cb.K);
@@ -1350,7 +1291,7 @@ extern "C" int ltephy_tap(ltephy_t* h, int what, void* dst, size_t bytes)
       src = h->d_ce.p, avail = n * h->dc.nof_ports * h->dc.nof_rx * g * sizeof(float2);
       break;
     case LTEPHY_TAP_LLR: src = h->d_llr.p, avail = n * LLR_STRIDE * sizeof(float); break;
-    case LTEPHY_TAP_PDSCH_LLR: src = h->d_pllr.p, avail = h->pllr_elems * sizeof(short); break;
+    case LTEPHY_TAP_PDSCH_LLR: src = h->d_pllr.p, avail = h->pb.pllr_elems * sizeof(short); break;
     case LTEPHY_TAP_TURBO_IN: src = h->d_turbo.p, avail = h->d_turbo.cap * 4; break;
     case LTEPHY_TAP_UL_SYM: src = h->d_ulsym.p, avail = (size_t)h->n_ul * 14 * h->dc.nsc * sizeof(float2); break;
     default: return fail(LTEPHY_ERROR_INVALID_INPUTS, "tap: unknown buffer");

@@ -95,8 +95,7 @@ struct ltephy {
   uint32_t           mib_held     = 0;       // combiner: frames held (srsRAN's frame_idx between calls), in rows 3 - mib_held .. 2
   int32_t            mib_last_sfn = -1;      // combiner: SFN of the last frame consumed, -1 after a reset
   DevBuf<short>      d_harq;                 // HARQ store: harq_slots x LTEPHY_HARQ_SLOT_BYTES
-  uint32_t           harq_slots = 0, harq_max_gen = 0;
-  std::map<uint32_t, uint32_t> harq_uses;    // slot -> uses in the batch being built
+  uint32_t           harq_slots = 0;
   std::vector<void*> tables; // device tables freed at destroy
   uint64_t           launches = 0;
 
@@ -112,26 +111,42 @@ struct ltephy {
   std::vector<uint8_t>  re_cnt; // [3 sf class][3 cfi][14][nof_prb]
 
   // phase B
-  std::vector<DevGrant> grants;
-  std::vector<DevCb>    cbs;
-  struct CbHalf {                // what a code block's half of its turbo pair needs, and its pairing key TBS / G (pair_code_blocks)
-    uint32_t tbs, G, crc_type, out_bits, out_byte;
-  };
-  std::vector<CbHalf>   cb_half; // [code block]
-  std::vector<DevPair>  pairs;
-  std::vector<DevTb>    tbs;
-  std::vector<uint32_t> pair_pi_off;
-  std::vector<uint32_t> tb_slot; // result slot [grant*2 + tb] -> tb index or ~0
+  struct PhaseB { // the batch of the last ltephy_submit_grants, ltephy_submit_ul or ltephy_turbo_batch: every submit starts with reset()
+    std::vector<DevGrant>   grants;
+    std::vector<DevUlGrant> ulgrants;
+    std::vector<DevCb>      cbs;
+    struct CbHalf {           // what a code block's half of its turbo pair needs, and its pairing key TBS / G (pair_code_blocks)
+      uint32_t tbs, G, crc_type, out_bits, out_byte;
+    };
+    std::vector<CbHalf>     cb_half; // [code block]
+    std::vector<DevPair>    pairs;
+    std::vector<DevTb>      tbs;
+    std::vector<uint32_t>   pair_pi_off;
+    std::vector<uint32_t>   tb_slot; // result slot (DL: grant*2 + tb, UL: grant) -> tb index or ~0
+    std::map<uint32_t, uint32_t> harq_uses; // slot -> uses in this batch
+    uint32_t                harq_max_gen = 0;
+    size_t                  payload_bytes = 0, pllr_elems = 0;
+    size_t                  seq_words = 0, turbo_words = 0; // scrambling-sequence and turbo-pool words
+    uint32_t                max_scr_words = 0;              // longest codeword's scrambling words
+    void reset(size_t nslots)
+    {
+      grants.clear(), ulgrants.clear(), cbs.clear(), cb_half.clear(), pairs.clear(), tbs.clear(), pair_pi_off.clear(), harq_uses.clear();
+      tb_slot.assign(nslots, 0xFFFFFFFFu);
+      harq_max_gen = 0, payload_bytes = 0, pllr_elems = 0, seq_words = 0, turbo_words = 0, max_scr_words = 0;
+    }
+  } pb;
   DevBuf<DevGrant>      d_grants;
   DevBuf<DevCb>         d_cbs;
   DevBuf<DevPair>       d_pairs;
   DevBuf<DevTb>         d_tbs;
   DevBuf<uint32_t>      d_pair_pi_off;
   DevBuf<uint32_t>      d_seq, d_turbo;
-  DevBuf<uint16_t>      d_rm;
+  DevBuf<uint16_t>      d_rm;        // pool of rate-matching inverse tables (pool_append), rm_used entries filled
+  size_t                rm_used = 0;
   DevBuf<uint32_t>      d_tscratch, d_tqueue; // persistent turbo kernel: per-CTA state slots, pair counters of the launches
   DevBuf<short>         d_pllr;
-  DevBuf<uint16_t>      d_pi;
+  DevBuf<uint16_t>      d_pi;        // pool of QPP interleaver tables (pool_append), pi_used entries filled
+  size_t                pi_used = 0;
   DevBuf<uint8_t>       d_payload, d_cb_iters, d_cb_crc;
   DevBuf<ltephy_tb_result_t> d_res;
   PinBuf<ltephy_tb_result_t> h_res;
@@ -139,7 +154,6 @@ struct ltephy {
   PinBuf<uint8_t>            h_stage;      // pinned arena for the job descriptors of one phase B (see pull())
   size_t                     stage_used = 0;
   bool                       stage_busy = false; // descriptors staged and possibly still being pulled
-  size_t                     payload_bytes = 0, pllr_elems = 0;
   uint32_t *                 d_gold_x1 = nullptr, *d_gold_basis = nullptr, gold_words = 0;
   uint32_t *                 d_xpowA = nullptr, *d_xpowB = nullptr;
   struct RmEntry {
@@ -148,25 +162,20 @@ struct ltephy {
   };
   std::map<std::pair<uint32_t, uint32_t>, RmEntry> rm_cache; // (K, F) -> inverse table
   RmEntry                                          rm_fast[188]; // F == 0 fast path, by qpp index
-  int64_t  pi_fast[188];
+  int64_t  pi_fast[188];                // offset of K's interleaver table in d_pi by qpp index, -1: not built yet
   std::vector<ltehost::Segm> segm_fast; // index tbs/8, C == 0 means "not computed"
   // uplink
   ltephy_ul_cfg_t            ulcfg{};
   bool                       ulcfg_set = false;
   uint32_t                   n_prs[20]{}, ul_u[20]{}, ul_v[20]{}; // per slot: n_PRS, base-sequence group u and sequence v
-  DevBuf<float2>             d_uliq, d_ulsym, d_ulpool; // d_ulpool: DMRS sequences and IDFT twiddles
+  DevBuf<float2>             d_uliq, d_ulsym, d_ulpool; // d_ulpool: pool of DMRS sequences and IDFT twiddles (pool_append)
   DevBuf<DevUlGrant>         d_ulgrants;
   DevBuf<DevUlChest>         d_ulchest;
   PinBuf<DevUlChest>         h_ulchest;
-  std::vector<DevUlGrant>    ulgrants;
-  std::map<uint64_t, uint32_t> ul_tab_cache; // (kind, M, ncs) -> offset in d_ulpool
+  std::map<uint64_t, uint32_t> ul_tab_cache; // (kind, M, ncs, u, v) -> offset in d_ulpool
   size_t                     ulpool_used = 0;
   uint32_t                   n_ul = 0;
-  size_t                                                                            rm_used = 0;
-  std::map<uint32_t, uint32_t>                                                      pi_cache; // K -> offset
-  size_t                                                                            pi_used = 0;
-  std::map<uint32_t, ltehost::Segm>                                                 segm_cache;
-  float                                                                             t_ms[4]{};
+  float                      t_ms[4]{};
 };
 
 

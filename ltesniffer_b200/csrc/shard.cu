@@ -423,20 +423,20 @@ extern "C" int ltephy_decode_subframes_sharded(ltephy_shard_t* sh, ltephy_t* h, 
   // records + result structs; the payload bytes), so no size has to be agreed on first and the turn holds nothing but the NCCL calls.
   const size_t cap_m = 64 + (size_t)n * 64 * (sizeof(TbMeta) + sizeof(ltephy_tb_result_t)); // up to 32 grants (64 result slots) per subframe
   if (W > 1) {
-    const size_t ntb = h->tbs.size();
-    if (h->payload_bytes > cap_p)
-      return fail(LTEPHY_ERROR_INVALID_INPUTS, "%zu transport-block bytes in %u subframes exceed the gather capacity (ltephy_shard_set_gather_capacity)", h->payload_bytes, n);
+    const size_t ntb = h->pb.tbs.size();
+    if (h->pb.payload_bytes > cap_p)
+      return fail(LTEPHY_ERROR_INVALID_INPUTS, "%zu transport-block bytes in %u subframes exceed the gather capacity (ltephy_shard_set_gather_capacity)", h->pb.payload_bytes, n);
     if (64 + 2 * (size_t)ng * sizeof(TbMeta) + ntb * sizeof(ltephy_tb_result_t) > cap_m)
       return fail(LTEPHY_ERROR_INVALID_INPUTS, "%u grants in %u subframes exceed the gather message", ng, n);
     if (R != 0) {
       if (sl->h_msg.reserve(cap_m) || sl->d_msg.reserve(cap_m)) return fail(LTEPHY_ERROR, "allocation of the gather buffers failed");
-      GatherHdr gh{ng, (uint32_t)ntb, (uint64_t)h->payload_bytes};
+      GatherHdr gh{ng, (uint32_t)ntb, (uint64_t)h->pb.payload_bytes};
       memcpy(sl->h_msg.p, &gh, sizeof(gh));
       TbMeta* hm = reinterpret_cast<TbMeta*>(sl->h_msg.p + 64);
       for (uint32_t j = 0; j < 2 * ng; j++) {
-        const uint32_t ti = h->tb_slot[j];
+        const uint32_t ti = h->pb.tb_slot[j];
         hm[j].grant_dci = sl->grant_dci[j / 2], hm[j].tb_index = ti;
-        hm[j].byte_off = ti != 0xFFFFFFFFu ? h->tbs[ti].byte_off : 0, hm[j].nbytes = ti != 0xFFFFFFFFu ? h->tbs[ti].nbytes : 0;
+        hm[j].byte_off = ti != 0xFFFFFFFFu ? h->pb.tbs[ti].byte_off : 0, hm[j].nbytes = ti != 0xFFFFFFFFu ? h->pb.tbs[ti].nbytes : 0;
       }
       const size_t mb = 64 + 2 * (size_t)ng * sizeof(TbMeta);
       ltephy_pull(h, sl->d_msg.p, sl->h_msg.p, (mb + 15) & ~(size_t)15, h->stream);

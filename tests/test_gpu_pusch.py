@@ -62,13 +62,16 @@ def _to_capi(i, g):
                         I_offset_ack=g.I_offset_ack, I_offset_ri=g.I_offset_ri, I_offset_cqi=g.I_offset_cqi)
 
 
-def _run_ul_case(cell, ucfg, mutate, nsf=2, ngr=3, snr=30.0, seed=31, min_prb=3, table=1, llr_check=True):
-    """sim -> product (GPU) and oracle for mutated grants: soft bits, chest figures, CRC and payload bit-exact; returns the number of CRC passes"""
+def _run_ul_case(cell, ucfg, mutate, nsf=2, ngr=3, snr=30.0, seed=31, min_prb=3, table=1, llr_check=True, phy=None):
+    """sim -> product (GPU) and oracle for mutated grants: soft bits, chest figures, CRC and payload bit-exact; returns the number of CRC passes.
+    phy: a handle already configured with ucfg, kept open (default: a new one)"""
     s = Sim(cell=cell, seed=seed, snr_db=snr, nof_ues=1)
     o = Oracle(cell)
     rng = np.random.default_rng(seed)
-    phy = capi.LtePhy(cell.nof_prb, cell.nof_ports, cell.cell_id, cell.nof_rx, max_subframes=nsf)
-    phy.set_ul_cfg(ucfg.n_dmrs1, ucfg.delta_ss, ucfg.group_hopping, ucfg.seq_hopping)
+    own = phy is None
+    if own:
+        phy = capi.LtePhy(cell.nof_prb, cell.nof_ports, cell.cell_id, cell.nof_rx, max_subframes=nsf)
+        phy.set_ul_cfg(ucfg.n_dmrs1, ucfg.delta_ss, ucfg.group_hopping, ucfg.seq_hopping)
     iq = np.zeros((nsf, s.sf_len), np.complex64)
     tti = np.arange(3, 3 + nsf, dtype=np.uint32)
     grants_o, pls, offs, grants_p = [], [], [], []
@@ -102,7 +105,8 @@ def _run_ul_case(cell, ucfg, mutate, nsf=2, ngr=3, snr=30.0, seed=31, min_prb=3,
                 assert np.array_equal(payload[rr.payload_off:rr.payload_off + nby], pls[i][off:off + nby])
                 nok += 1
             k += 1
-    phy.close()
+    if own:
+        phy.close()
     return nok, k
 
 
