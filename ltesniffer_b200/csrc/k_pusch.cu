@@ -10,6 +10,7 @@
 #include "dev_common.cuh"
 #include "k_launch.cuh"
 #include "dev_ul.cuh"
+#include "dev_eq.cuh"
 
 __device__ __forceinline__ short ul_f2s(float v)
 {
@@ -195,7 +196,7 @@ __global__ void __launch_bounds__(256) pusch_kernel(const __grid_constant__ DevC
       const float2   h = hop ? sm[sl * M + n] : make_float2(A.x + (B.x - A.x) * t, A.y + (B.y - A.y) * t);
       const float2   v = y[l * nsc + g.k0[sl] + n];
       const float    den = h.x * h.x + h.y * h.y;
-      bufA[i]            = make_float2((v.x * h.x + v.y * h.y) / den, (v.y * h.x - v.x * h.y) / den);
+      bufA[i]            = make_float2(eq_div(v.x * h.x + v.y * h.y, den), eq_div(v.y * h.x - v.x * h.y, den)); // no channel: 0, not NaN
     }
     __syncthreads();
     float2 * src = bufA, *dst = bufB;
@@ -223,8 +224,8 @@ __global__ void __launch_bounds__(256) pusch_kernel(const __grid_constant__ DevC
       const uint32_t kind = uci_pos(M, k, cc, g.qp_ack, g.qp_ri, g.qp_cqi, dpos);
       if (kind != 0 && kind != 3) continue;
       const float2 zz = src[s * M + k];
-      short        z[8];
-      ul_demod_s(make_float2(zz.x * scl, zz.y * scl), qm, z);
+      short        z[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+      if (zz.x != 0.0f || zz.y != 0.0f) ul_demod_s(make_float2(zz.x * scl, zz.y * scl), qm, z); // an exactly zero sample is an erasure: LLR 0
       const uint32_t hb0 = (cc * M + k) * qm;
       for (uint32_t b = 0; b < qm; b++) {
         const uint32_t hb = hb0 + b, sbit = (seq[hb >> 5] >> (hb & 31)) & 1u;

@@ -1130,14 +1130,14 @@ int lteo_pusch_decode(lteo_t* q, const lte_ul_cfg_t* ucfg, uint32_t sf_idx, cons
       cf_t h = hop ? sm[sl * M + n] : (cf_t){A.re + (B.re - A.re) * t, A.im + (B.im - A.im) * t}; /* hopping: each slot stands alone */
       cf_t y = sym[l * nsc + k0 + n];
       float den = h.re * h.re + h.im * h.im;
-      x[n].re   = (y.re * h.re + y.im * h.im) / den;
-      x[n].im   = (y.im * h.re - y.re * h.im) / den;
+      x[n].re   = eq_div(y.re * h.re + y.im * h.im, den); /* no channel (zero-filled samples): 0, not 0/0 = NaN */
+      x[n].im   = eq_div(y.im * h.re - y.re * h.im, den);
     }
     const cf_t* zt = idft_mixed(W, M, x, x2);
     for (uint32_t k = 0; k < M; k++) {
-      cf_t    z = {zt[k].re * scl, zt[k].im * scl};
-      int16_t v[8];
-      demod_s(z, Qm, v);
+      cf_t    z    = {zt[k].re * scl, zt[k].im * scl};
+      int16_t v[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+      if (zt[k].re != 0.0f || zt[k].im != 0.0f) demod_s(z, Qm, v); /* an exactly zero de-precoded sample is an erasure: LLR 0 */
       const uint32_t p = k * 12 + c, kd = kind[p]; /* row k, column c of the channel interleaver (36.212 5.2.2.8) */
       if (kd != 0 && kd != 3) continue;            /* CQI / RI symbol: not part of the UL-SCH codeword */
       for (uint32_t b = 0; b < Qm; b++) {
