@@ -513,7 +513,7 @@ int lteo_dci_decode(const float* e, uint32_t E, uint32_t nof_bits, uint8_t* bits
   float gain = 32.0f / mx;
   for (uint32_t i = 0; i < n3; i++) {
     float v = rm[i] * gain + 127.5f;
-    if (v < 0.0f) v = 0.0f;
+    if (!(v >= 0.0f)) v = 0.0f; /* NaN (a NaN soft bit, 0 * an infinite gain, an infinite sum * 0) quantises as fmaxf does: to 0 */
     if (v > 255.0f) v = 255.0f;
     int qv = (int)v;
     r[i]   = 2 * qv - 255;

@@ -1,16 +1,16 @@
 """Test infrastructure for the MIB decode across the 40 ms PBCH period: ctypes bindings of oracle/liblteomib.so (lteo_pbch_llr and the
-combiner lteo_mib_*, oracle/lte_mib_oracle.h), an independent Python statement of srsRAN's combining loop over lteo_dci_decode, and a
-generator of simulated subframes 0.  Imported only by tests/."""
+combiner lteo_mib_*, oracle/lte_mib_oracle.h), an independent Python statement of srsRAN's combining loop over the integer reference
+ref_dec.pbch_hyp_ref, and a generator of simulated subframes 0.  Imported only by tests/."""
 import ctypes as C
 import os
 
 import numpy as np
 
 import ltelib
+import ref_dec
 from helpers import oracle_frontend
 from ref64 import gold
 
-MASK = {1: 0x0000, 2: 0xFFFF}
 BW = {0: 6, 1: 15, 2: 25, 3: 50, 4: 75, 5: 100}
 
 
@@ -81,10 +81,10 @@ class OracleCombiner:
 
 
 class PyCombiner:
-    """srsRAN 21.10's PBCH combiner stated again, from DESIGN.md §2, over lteo_dci_decode: a list of held frames per port count"""
+    """srsRAN 21.10's PBCH combiner stated again, from DESIGN.md §2, over ref_dec.pbch_hyp_ref: a list of held frames per port count"""
 
-    def __init__(self, cell, oracle):
-        self.cell, self.o = cell, oracle
+    def __init__(self, cell):
+        self.cell = cell
         self.scr = gold(cell.cell_id, 1920).astype(bool)
         self.reset()
 
@@ -104,12 +104,8 @@ class PyCombiner:
             for nb in range(w):
                 for dst in range(4 - nb):
                     for src in range(w - nb):
-                        e = np.zeros(1920, np.float32)
-                        for j in range(nb + 1):
-                            sl = slice(480 * (dst + j), 480 * (dst + j + 1))
-                            e[sl] = np.where(self.scr[sl], -self.held[nant][src + j], self.held[nant][src + j])
-                        r, bits, rem = self.o.dci_decode(e, 24)
-                        if r != 0 or rem != MASK[nant]:
+                        valid, bits, rem = ref_dec.pbch_hyp_ref(self.held[nant], src, dst, nb + 1, self.scr)
+                        if not valid or rem != ref_dec.PBCH_PORT_MASK[nant]:
                             continue
                         off = dst - src + w - 1
                         msb = int("".join(str(int(b)) for b in bits[6:14]), 2)

@@ -50,9 +50,10 @@ def tbs_of(itbs, nprb):
 # ------------------------------------------------------------------------------------------------ synthesis shared with the GPU file
 class Case:
     """One synthesised subframe: a cell, a PDSCH grant over prb_mask with the given scheme / codeword modulations, a designed channel, AWGN.
-    Attributes: iq complex64 [rx][sf_len], grant (ltelib.DlGrant), l / k (the grant's REs in mapping order), sf, cfi, rnti, qm per codeword."""
+    Attributes: iq complex64 [rx][sf_len], grant (ltelib.DlGrant), l / k (the grant's REs in mapping order), sf, cfi, rnti, qm per codeword.
+    cw_bits: the n_RE * Qm coded bits of each codeword (before scrambling); random when None."""
 
-    def __init__(self, cell, sf, cfi, scheme, qms, prbs, chan="selective", noise_var=1e-3, seed=0, cw_swap=0, pmi=0, H=None, rnti=0x4321, **_):
+    def __init__(self, cell, sf, cfi, scheme, qms, prbs, chan="selective", noise_var=1e-3, seed=0, cw_swap=0, pmi=0, H=None, rnti=0x4321, cw_bits=None, **_):
         rng = np.random.default_rng(seed)
         N, P, A = cell.nof_prb, cell.nof_ports, cell.nof_rx
         nsc = 12 * N
@@ -80,6 +81,8 @@ class Case:
         layers = []
         for q, qm in enumerate(qms):
             bits = rng.integers(0, 2, n * qm).astype(np.uint8)
+            if cw_bits is not None:                                       # given coded bits instead of random ones (same draws, so the noise is unchanged)
+                bits = np.asarray(cw_bits[q], np.uint8)
             layers.append(ref64.qam(bits ^ ref64.scrambling_seq(cell, sf, rnti, q, n * qm), qm))
         y = ref64.precode(scheme, np.array(layers), P, self.nof_layers, pmi)
         for p in range(y.shape[0]):

@@ -80,7 +80,7 @@ def test_oracle_equals_python_statement(infra, cellp, search_ports):
     cell = Cell(*cellp)
     o = ltelib.Oracle(cell)
     seq = _blocks(cell, o, PLAN)
-    oc, pc = M.OracleCombiner(cell), M.PyCombiner(cell, o)
+    oc, pc = M.OracleCombiner(cell), M.PyCombiner(cell)
     got, n_multi = 0, 0
     for i, (t, f) in enumerate(seq):
         if i == 20:                                   # srsran_ue_mib_reset in the middle of a run
@@ -142,6 +142,6 @@ def test_noise_only_frames(infra, cellp):
     cell = Cell(*cellp)
     o = ltelib.Oracle(cell)
     seq = _blocks(cell, o, [(100, 24, -40.0)], seed=23)
-    oc, pc = M.OracleCombiner(cell), M.PyCombiner(cell, o)
+    oc, pc = M.OracleCombiner(cell), M.PyCombiner(cell)
     for t, f in seq:
         assert oc.decode(t, f, True) == pc.decode(t, f, True)
