@@ -5,7 +5,7 @@ CXX ?= g++
 CFLAGS = -O3 -g -fPIC -std=gnu11 -Wall -Wno-unused-function -ffp-contract=off -fno-fast-math
 CXXFLAGS = -O2 -g -fPIC -std=c++17 -Wall -ffp-contract=off -fno-fast-math
 
-all: sim/libltesim.so oracle/liblteoracle.so oracle/liblteosync.so oracle/liblteomib.so
+all: sim/libltesim.so oracle/liblteoracle.so oracle/liblteosync.so oracle/liblteomib.so oracle_track/liblteotrack.so
 
 sim/libltesim.so: sim/lte_common.c sim/lte_sim.c sim/lte_common.h sim/lte_sim.h include/lte_tables.h
 	$(CC) $(CFLAGS) -shared -o $@ sim/lte_common.c sim/lte_sim.c -lm
@@ -21,6 +21,10 @@ oracle/liblteosync.so: oracle/lte_sync_oracle.c oracle/lte_sync_oracle.h oracle/
 oracle/liblteomib.so: oracle/lte_mib_oracle.c oracle/lte_mib_oracle.h oracle/lte_oracle.h oracle/liblteoracle.so
 	$(CC) $(CFLAGS) -shared -o $@ oracle/lte_mib_oracle.c -Loracle -llteoracle -Wl,-rpath,'$$ORIGIN' -lm
 
+# tracker oracle: stand-alone
+oracle_track/liblteotrack.so: oracle_track/lte_track_oracle.c oracle_track/lte_track_oracle.h
+	$(CC) $(CFLAGS) -shared -o $@ oracle_track/lte_track_oracle.c -lm
+
 # C++ example of the C-ABI (needs ltesniffer_b200/libltephy_b200.so, built by ltesniffer_b200/build.py)
 examples/offline_decode: examples/offline_decode.cpp include/ltephy_b200.h include/ltephy_search.h include/ltephy_sinks.h
 	$(CXX) -O2 -std=c++17 -Wall -Iinclude -o $@ examples/offline_decode.cpp -Lltesniffer_b200 -lltephy_b200 -Wl,-rpath,'$$ORIGIN/../ltesniffer_b200'
@@ -31,8 +35,11 @@ examples/offline_ul: examples/offline_ul.cpp include/ltephy_b200.h include/lteph
 examples/cell_search: examples/cell_search.cpp include/ltephy_b200.h
 	$(CXX) -O2 -std=c++17 -Wall -Iinclude -o $@ examples/cell_search.cpp -Lltesniffer_b200 -lltephy_b200 -Wl,-rpath,'$$ORIGIN/../ltesniffer_b200'
 
+examples/decode_recording: examples/decode_recording.cpp include/ltephy_b200.h include/ltephy_search.h include/ltephy_sinks.h
+	$(CXX) -O2 -std=c++17 -Wall -Iinclude -o $@ examples/decode_recording.cpp -Lltesniffer_b200 -lltephy_b200 -Wl,-rpath,'$$ORIGIN/../ltesniffer_b200'
+
 examples/compat_check: examples/compat_check.cpp compat/srsran/srsran.h include/ltephy_b200.h
 	$(CXX) -O2 -std=c++17 -Wall -Iinclude -Icompat -o $@ examples/compat_check.cpp -Lltesniffer_b200 -lltephy_srsran_compat -lltephy_b200 -Wl,-rpath,'$$ORIGIN/../ltesniffer_b200'
 
 clean:
-	rm -f sim/*.so oracle/*.so examples/offline_decode examples/offline_ul examples/compat_check examples/cell_search
+	rm -f sim/*.so oracle/*.so oracle_track/*.so examples/offline_decode examples/offline_ul examples/compat_check examples/cell_search examples/decode_recording

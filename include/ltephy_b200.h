@@ -292,6 +292,63 @@ enum {
 /* copies an intermediate of the last search; bytes must be at least its size */
 int  ltephy_sync_tap(ltephy_sync_t* h, int what, void* dst, size_t bytes);
 
+/* Tracking after acquisition: the track state of srsran_ue_sync_zerocopy (reference src/src/LTESniffer_Core.cc:365) on a recording.  From the
+ * cell search's frame_offset and cfo_hz, the tracker follows the PSS of every half-frame, corrects the subframe start in whole samples and the
+ * carrier offset with a first-order loop, and cuts every subframe into device memory, rotated by the carrier offset that held before it -- the
+ * input ltephy_submit_iq_device / ltephy_decode_subframes_device take, with ltephy_set_cfo left at 0.  The rule and its summation orders are
+ * DESIGN.md §2 ("tracking"); the CPU oracle lteo_track_* (oracle_track/) defines every record and cut sample bit for bit. */
+typedef struct ltephy_track ltephy_track_t;
+#define LTEPHY_TRACK_NO_CFO 1u /* keep cfo_hz at its initial value (the reference's disable_cfo) */
+typedef struct {
+  uint32_t symbol_sz;     /* N, as for ltephy_sync_cfg_t */
+  uint32_t nof_rx;        /* 1 or 2 antennas */
+  uint32_t pci;           /* 0..503: the PSS tracked is N_ID_2 = pci mod 3 */
+  uint32_t first_tti;     /* tti (10 sfn + subframe, 0..10239) of the subframe that starts at frame_offset */
+  uint64_t frame_offset;  /* absolute first sample of that subframe */
+  float    cfo_hz;        /* initial carrier offset (ltephy_cell_t.cfo_hz), |cfo_hz| <= 7500 */
+  float    max_ppm;       /* largest sampling-clock offset the measurement windows are sized for (0 = 50) */
+  uint32_t max_subframes; /* most subframes one push cuts (device memory is sized for it) */
+  uint32_t flags;         /* LTEPHY_TRACK_* */
+  int32_t  device;        /* CUDA device ordinal */
+  uint32_t reserved[5];
+} ltephy_track_cfg_t;
+#define LTEPHY_TRACK_LOCKED 1u /* subframe: the last half-frame measured before it was locked (or none was measured yet); half-frame: locked */
+#define LTEPHY_TRACK_LOST   2u /* 4 or more half-frames in a row were not locked */
+typedef struct {
+  int64_t  start;  /* absolute first sample of the subframe as cut */
+  uint32_t tti;
+  float    cfo_hz; /* carrier offset it was corrected with */
+  uint32_t flags;  /* LTEPHY_TRACK_LOCKED / _LOST */
+  uint32_t index;  /* subframe number since frame_offset */
+} ltephy_track_sf_t;
+typedef struct {
+  int64_t  tau;      /* expected first sample of the PSS useful part: start + 13 N / 2 */
+  uint32_t index;    /* subframe number (tti mod 5 = 0) */
+  int32_t  delta;    /* offset of the metric's argmax from tau, |delta| <= 9 N / 128 */
+  float    peak;     /* metric at tau + delta */
+  float    s_re, s_im; /* S = sum_a c2 conj(c1) at tau + delta */
+  float    f_meas;   /* atan2f(s_im, s_re) * 15000 / pi */
+  uint32_t flags;    /* LTEPHY_TRACK_LOCKED / _LOST, after this half-frame */
+  uint32_t pad;
+} ltephy_track_hf_t;
+typedef struct {
+  uint32_t                 nof_subframes, nof_half_frames;
+  const ltephy_track_sf_t* sf;          /* [nof_subframes], host memory owned by the tracker, valid until the next push */
+  const ltephy_track_hf_t* hf;          /* [nof_half_frames], likewise */
+  const void*              iq_dev;      /* cf32 [nof_subframes][nof_rx][15 N] in device memory, valid until the next push */
+  uint64_t                 next_sample; /* the first absolute sample the next push must still include */
+  uint32_t                 remeasured;  /* half-frames whose metric window had to be computed again (diagnostic) */
+  uint32_t                 reserved;
+} ltephy_track_out_t;
+int  ltephy_track_create(const ltephy_track_cfg_t* cfg, ltephy_track_t** h);
+void ltephy_track_destroy(ltephy_track_t* h);
+/* iq: cf32 [nof_rx][nof_samples], antenna-major, host memory, absolute samples first_sample .. first_sample + nof_samples - 1, with
+ * first_sample <= the previous push's next_sample.  Cuts every subframe (up to max_subframes) that lies wholly inside what has been fed.  The
+ * results do not depend on how the recording is split into pushes.  Blocks until the cut is complete. */
+int  ltephy_track_push(ltephy_track_t* h, const float* iq, uint64_t first_sample, uint64_t nof_samples, ltephy_track_out_t* out);
+/* same, with the samples already in device memory */
+int  ltephy_track_push_device(ltephy_track_t* h, const void* iq_dev, uint64_t first_sample, uint64_t nof_samples, ltephy_track_out_t* out);
+
 /* nslots HARQ slots of LTEPHY_HARQ_SLOT_BYTES each (150 RNTIs x 8 processes x 2 TBs = 2400 slots = 1.4 GB); contents survive across batches */
 int ltephy_harq_reserve(ltephy_t* h, uint32_t nslots);
 

@@ -770,3 +770,92 @@ class CellSearch:
         if r != 0:
             raise RuntimeError("ltephy_sync_tap failed (%d): %s" % (r, self.L.ltephy_last_error().decode()))
         return out
+
+
+# ------------------------------------------------------------------------------------------------
+# tracking after acquisition (ltephy_track_*, include/ltephy_b200.h)
+TRACK_NO_CFO = 1
+TRACK_LOCKED, TRACK_LOST = 1, 2
+
+
+class TrackCfg(C.Structure):
+    _fields_ = [("symbol_sz", C.c_uint32), ("nof_rx", C.c_uint32), ("pci", C.c_uint32), ("first_tti", C.c_uint32), ("frame_offset", C.c_uint64),
+                ("cfo_hz", C.c_float), ("max_ppm", C.c_float), ("max_subframes", C.c_uint32), ("flags", C.c_uint32), ("device", C.c_int32),
+                ("reserved", C.c_uint32 * 5)]
+
+
+TRACK_SF_DTYPE = np.dtype([("start", "<i8"), ("tti", "<u4"), ("cfo_hz", "<f4"), ("flags", "<u4"), ("index", "<u4")])
+TRACK_HF_DTYPE = np.dtype([("tau", "<i8"), ("index", "<u4"), ("delta", "<i4"), ("peak", "<f4"), ("s_re", "<f4"), ("s_im", "<f4"), ("f_meas", "<f4"),
+                           ("flags", "<u4"), ("pad", "<u4")])
+
+
+class TrackOut(C.Structure):
+    _fields_ = [("nof_subframes", C.c_uint32), ("nof_half_frames", C.c_uint32), ("sf", C.c_void_p), ("hf", C.c_void_p), ("iq_dev", C.c_void_p),
+                ("next_sample", C.c_uint64), ("remeasured", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+assert C.sizeof(TrackCfg) == 64 and C.sizeof(TrackOut) == 48 and TRACK_SF_DTYPE.itemsize == 24 and TRACK_HF_DTYPE.itemsize == 40
+
+
+class Tracker:
+    """PSS tracking and subframe cutting of a recording after the cell search: push the recording part by part (antenna-major complex64
+    [nof_rx][n] with its absolute first sample); each push returns the subframes that now lie wholly inside what was fed."""
+
+    def __init__(self, symbol_sz, nof_rx, pci, frame_offset, cfo_hz=0.0, first_tti=0, max_subframes=1000, max_ppm=50.0, flags=0, device=0):
+        self.L = load_library()
+        L = self.L
+        L.ltephy_track_create.argtypes = [C.POINTER(TrackCfg), C.POINTER(C.c_void_p)]
+        L.ltephy_track_destroy.argtypes = [C.c_void_p]
+        L.ltephy_track_push.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.POINTER(TrackOut)]
+        L.ltephy_track_push_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.POINTER(TrackOut)]
+        self.cfg = TrackCfg(symbol_sz=symbol_sz, nof_rx=nof_rx, pci=pci, first_tti=first_tti, frame_offset=frame_offset, cfo_hz=cfo_hz,
+                            max_ppm=max_ppm, max_subframes=max_subframes, flags=flags, device=device)
+        self.h = C.c_void_p()
+        r = L.ltephy_track_create(C.byref(self.cfg), C.byref(self.h))
+        if r != 0:
+            self.h = None
+            raise RuntimeError("ltephy_track_create failed (%d): %s" % (r, L.ltephy_last_error().decode()))
+        self.next_sample = frame_offset
+
+    def close(self):
+        if self.h:
+            self.L.ltephy_track_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def _done(self, r, o):
+        if r != 0:
+            raise RuntimeError("ltephy_track_push failed (%d): %s" % (r, self.L.ltephy_last_error().decode()))
+        import torch
+        sf = np.ctypeslib.as_array((C.c_uint8 * (o.nof_subframes * 24)).from_address(o.sf)).view(TRACK_SF_DTYPE).copy() if o.nof_subframes else \
+            np.zeros(0, TRACK_SF_DTYPE)
+        hf = np.ctypeslib.as_array((C.c_uint8 * (o.nof_half_frames * 40)).from_address(o.hf)).view(TRACK_HF_DTYPE).copy() if o.nof_half_frames else \
+            np.zeros(0, TRACK_HF_DTYPE)
+        shape = (o.nof_subframes, self.cfg.nof_rx, 15 * self.cfg.symbol_sz)
+        if o.nof_subframes:
+            view = type("_Cut", (), {"__cuda_array_interface__": dict(shape=shape, typestr="<c8", data=(o.iq_dev, False), version=2)})()
+            with torch.cuda.device(self.cfg.device):
+                iq = torch.as_tensor(view, device="cuda:%d" % self.cfg.device).clone()
+        else:
+            iq = torch.empty(shape, dtype=torch.complex64, device="cuda:%d" % self.cfg.device)
+        self.next_sample = o.next_sample
+        return dict(sf=sf, hf=hf, iq=iq, next_sample=o.next_sample, remeasured=o.remeasured)
+
+    def push(self, iq, first_sample):
+        """iq: complex64 [nof_rx][n] (host) of absolute samples first_sample ... -> dict(sf, hf: record arrays, iq: torch complex64
+        [k][nof_rx][15 N] on the device (a copy of the tracker's cut), next_sample, remeasured)"""
+        iq = np.ascontiguousarray(iq, np.complex64)
+        assert iq.ndim == 2 and iq.shape[0] == self.cfg.nof_rx, iq.shape
+        o = TrackOut()
+        return self._done(self.L.ltephy_track_push(self.h, _p(iq), first_sample, iq.shape[1], C.byref(o)), o)
+
+    def push_device(self, iq, first_sample):
+        """iq: torch complex64 tensor [nof_rx][n], contiguous, on this handle's device"""
+        assert iq.is_cuda and iq.is_contiguous() and iq.dim() == 2 and iq.shape[0] == self.cfg.nof_rx
+        o = TrackOut()
+        return self._done(self.L.ltephy_track_push_device(self.h, C.c_void_p(iq.data_ptr()), first_sample, iq.shape[1], C.byref(o)), o)

@@ -31,6 +31,9 @@ struct SyncSss {
   const float*  seq;                  // [3][168][2][62] SSS of subframe 0 / 5
 };
 
+// host (sync.cu): d_u and the replica of N_ID_2 = u, returns E_p
+float sync_pss_replica(uint32_t N, uint32_t u, float2* d, float2* rep);
+
 extern "C" int launch_sync_pss(const SyncArgs& g, float* m, float* fold, SyncPeak* pk, float* rm, float4* c12, float* refined, cudaStream_t st,
                                uint64_t* launches);
 extern "C" int launch_sync_sss(const SyncArgs& g, const SyncSss& s, float2* Y, float* sss, cudaStream_t st, uint64_t* launches);

@@ -37,6 +37,28 @@ static void pss_seq(uint32_t n_id_2, float2* d)
   }
 }
 
+// d_u (d[62]) and the replica p_u[k] = (1/sqrt N) sum_n d_u(n) exp(+j 2 pi f_n k / N) (rep[N]), in double rounded to float; returns E_p = sum |p|^2
+// (in double, rounded): as lteo_cell_search and lteo_track compute them.  Shared by the cell search and the tracker (track.cu).
+float sync_pss_replica(uint32_t N, uint32_t u, float2* d, float2* rep)
+{
+  pss_seq(u, d);
+  const double sc = 1.0 / std::sqrt((double)N);
+  double       e  = 0.0;
+  for (uint32_t k = 0; k < N; k++) {
+    double re = 0.0, im = 0.0;
+    for (uint32_t n = 0; n < 62; n++) {
+      const int64_t  f   = n < 31 ? (int64_t)n - 31 : (int64_t)n - 30;
+      const uint32_t idx = (uint32_t)(((f * (int64_t)k) % (int64_t)N + (int64_t)N) % (int64_t)N);
+      const double   ph = 2.0 * M_PI * (double)idx / (double)N, c = std::cos(ph), s = std::sin(ph);
+      re += (double)d[n].x * c - (double)d[n].y * s;
+      im += (double)d[n].x * s + (double)d[n].y * c;
+    }
+    rep[k] = make_float2((float)(re * sc), (float)(im * sc));
+    e += (double)rep[k].x * rep[k].x + (double)rep[k].y * rep[k].y;
+  }
+  return (float)e;
+}
+
 // 36.211 6.11.2.1: d[62] of subframe 0 (sf5 = 0) or 5 (sf5 = 1)
 static void sss_seq(uint32_t n_id_1, uint32_t n_id_2, uint32_t sf5, float* d)
 {
@@ -84,26 +106,7 @@ extern "C" int ltephy_sync_create(const ltephy_sync_cfg_t* cfg, ltephy_sync_t** 
   // replicas p_u[k] = (1/sqrt N) sum_n d_u(n) exp(+j 2 pi f_n k / N) and E_p, in double, as lteo_cell_search computes them
   std::vector<float2> rep((size_t)3 * N), W(N);
   h->dpss.resize(3 * 62);
-  const double sc = 1.0 / std::sqrt((double)N);
-  for (uint32_t u = 0; u < 3; u++) {
-    float2* d = &h->dpss[62 * u];
-    pss_seq(u, d);
-    double e = 0.0;
-    for (uint32_t k = 0; k < N; k++) {
-      double re = 0.0, im = 0.0;
-      for (uint32_t n = 0; n < 62; n++) {
-        const int64_t  f   = n < 31 ? (int64_t)n - 31 : (int64_t)n - 30;
-        const uint32_t idx = (uint32_t)(((f * (int64_t)k) % (int64_t)N + (int64_t)N) % (int64_t)N);
-        const double   ph = 2.0 * M_PI * (double)idx / (double)N, c = std::cos(ph), s = std::sin(ph);
-        re += (double)d[n].x * c - (double)d[n].y * s;
-        im += (double)d[n].x * s + (double)d[n].y * c;
-      }
-      float2& p = rep[(size_t)u * N + k];
-      p         = make_float2((float)(re * sc), (float)(im * sc));
-      e += (double)p.x * p.x + (double)p.y * p.y;
-    }
-    h->ep[u] = (float)e;
-  }
+  for (uint32_t u = 0; u < 3; u++) h->ep[u] = sync_pss_replica(N, u, &h->dpss[62 * u], &rep[(size_t)u * N]);
   for (uint32_t i = 0; i < N; i++) {
     const double ph = -2.0 * M_PI * (double)i / (double)N;
     W[i]            = make_float2((float)std::cos(ph), (float)std::sin(ph));

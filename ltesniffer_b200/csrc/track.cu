@@ -1,0 +1,281 @@
+// track.cu -- host side of the tracker (include/ltephy_b200.h, DESIGN.md §2 "tracking"): predicts the measurement windows of a push, runs the
+// metric kernel over them, replays the rule on its bit-exact results in the order lteo_track states it (measuring a window again when the
+// tracked position left the predicted one), then the CFO sums, the carrier-offset loop and the cut.
+#include "../../include/ltephy_b200.h"
+#include "k_sync.cuh"
+#include "k_track.cuh"
+#include "ltephy_internal.cuh"
+#include <algorithm>
+#include <cmath>
+#include <cstring>
+#include <vector>
+
+#define TRACK_P      4u    // locked half-frames per timing correction
+#define TRACK_ALPHA  0.05f // gain of the carrier-offset loop
+#define TRACK_MISS   4u    // half-frames in a row without lock after which records are flagged lost
+#define TRACK_LOCK_K 20.0f // lock: peak metric >= 20 / N; on noise-only captures no half-frame's peak came above 10.2 / N (DESIGN.md §2)
+
+struct ltephy_track {
+  ltephy_track_cfg_t cfg{};
+  uint32_t           N = 0, A = 0, W = 0, SF = 0;
+  float              ep = 0.0f, thr = 0.0f, max_ppm = 50.0f;
+  cudaStream_t       stream = nullptr;
+  DevBuf<float2>     d_rep, d_x, d_cut, d_tabA, d_tabB, d_c;
+  DevBuf<float>      d_m;
+  DevBuf<TrackWin>   d_win;
+  DevBuf<uint64_t>   d_pos, d_start;
+  // state: as lteo_track
+  int64_t  s = 0;
+  uint32_t k = 0;
+  float    f = 0.0f, d = 0.0f, acc = 0.0f;
+  uint32_t miss = 0, nhf = 0, ncor = 0, nl = 0;
+  int64_t  sd = 0, sh = 0, shh = 0, shd = 0;
+  std::vector<ltephy_track_sf_t> sf;
+  std::vector<ltephy_track_hf_t> hf;
+};
+
+static bool track_symbol_ok(uint32_t N)
+{
+  const uint32_t M = N % 3 ? N : N / 3;
+  return N >= 128 && N <= 2048 && N % 128 == 0 && !(M & (M - 1));
+}
+
+extern "C" int ltephy_track_create(const ltephy_track_cfg_t* cfg, ltephy_track_t** out)
+{
+  if (!cfg || !out) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_create: null argument");
+  const uint32_t N = cfg->symbol_sz;
+  if (!track_symbol_ok(N) || cfg->nof_rx < 1 || cfg->nof_rx > 2)
+    return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_create: symbol size %u / %u antennas not supported", N, cfg->nof_rx);
+  if (cfg->pci > 503 || cfg->first_tti > 10239) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_create: pci %u / first_tti %u out of range", cfg->pci, cfg->first_tti);
+  if (!(std::fabs(cfg->cfo_hz) <= 7500.0f)) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_create: cfo_hz outside +-7500 Hz");
+  if (!(cfg->max_ppm >= 0.0f && cfg->max_ppm <= 1000.0f)) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_create: max_ppm outside 0..1000");
+  if (cfg->max_subframes < 1 || cfg->max_subframes > 20000) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_create: max_subframes outside 1..20000");
+  if (cfg->flags & ~LTEPHY_TRACK_NO_CFO) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_create: unknown flags 0x%x", cfg->flags);
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail(LTEPHY_ERROR, "no CUDA device: this library has no CPU path");
+  CU(cudaSetDevice(cfg->device));
+  ltephy_track* h = new ltephy_track();
+  struct Guard {
+    ltephy_track* h;
+    bool          ok = false;
+    ~Guard()
+    {
+      if (!ok) ltephy_track_destroy(h);
+    }
+  } guard{h};
+  h->cfg = *cfg, h->N = N, h->A = cfg->nof_rx, h->W = 9 * N / 128, h->SF = 15 * N;
+  h->max_ppm = cfg->max_ppm > 0.0f ? cfg->max_ppm : 50.0f;
+  h->thr     = TRACK_LOCK_K / (float)N;
+  h->s = (int64_t)cfg->frame_offset, h->f = cfg->cfo_hz;
+  CU(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
+  // the replica of N_ID_2 = pci mod 3 and its energy: the cell search's (sync.cu), as lteo_track_create computes them
+  std::vector<float2> rep(N), d62(62);
+  h->ep = sync_pss_replica(N, cfg->pci % 3, d62.data(), rep.data());
+  const size_t nsf = cfg->max_subframes;
+  if (h->d_rep.reserve(N) || h->d_cut.reserve(nsf * h->A * h->SF) || h->d_tabA.reserve(nsf * (h->SF / 128)) || h->d_tabB.reserve(nsf * 128) ||
+      h->d_start.reserve(nsf) || h->d_pos.reserve(nsf / 5 + 1) || h->d_c.reserve((nsf / 5 + 1) * h->A * 2) || h->d_win.reserve(nsf / 5 + 1))
+    return fail(LTEPHY_ERROR, "track_create: device allocation failed");
+  CU(cudaMemcpy(h->d_rep.p, rep.data(), N * sizeof(float2), cudaMemcpyHostToDevice));
+  h->sf.reserve(nsf), h->hf.reserve(nsf / 5 + 1);
+  guard.ok = true;
+  *out     = h;
+  return LTEPHY_SUCCESS;
+}
+
+extern "C" void ltephy_track_destroy(ltephy_track_t* h)
+{
+  if (!h) return;
+  cudaSetDevice(h->cfg.device);
+  if (h->stream) cudaStreamSynchronize(h->stream);
+  h->d_rep.release(), h->d_x.release(), h->d_cut.release(), h->d_tabA.release(), h->d_tabB.release(), h->d_c.release(), h->d_m.release();
+  h->d_win.release(), h->d_pos.release(), h->d_start.release();
+  if (h->stream) cudaStreamDestroy(h->stream);
+  delete h;
+}
+
+// the metric at the positions of the given windows, back on the host (m[w * stride + i])
+static int track_metrics(ltephy_track_t* h, const TrackArgs& g, const std::vector<TrackWin>& win, std::vector<float>& m, uint32_t& stride)
+{
+  stride = 0;
+  for (const TrackWin& w : win) stride = std::max(stride, w.cnt);
+  m.assign((size_t)win.size() * stride, 0.0f);
+  if (win.empty()) return LTEPHY_SUCCESS;
+  if (h->d_win.reserve(win.size()) || h->d_m.reserve(m.size())) return fail(LTEPHY_ERROR, "track_push: device allocation failed");
+  CU(cudaMemcpyAsync(h->d_win.p, win.data(), win.size() * sizeof(TrackWin), cudaMemcpyHostToDevice, h->stream));
+  if (launch_track_metric(g, h->d_win.p, (uint32_t)win.size(), stride, stride, h->d_m.p, h->stream))
+    return fail(LTEPHY_ERROR, "track_push: metric kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
+  CU(cudaMemcpyAsync(m.data(), h->d_m.p, m.size() * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  CU(cudaStreamSynchronize(h->stream));
+  return LTEPHY_SUCCESS;
+}
+
+static int track_run(ltephy_track_t* h, const float2* x, uint64_t first, uint64_t n, ltephy_track_out_t* out)
+{
+  const uint32_t N = h->N, SF = h->SF, W = h->W, maxsf = h->cfg.max_subframes;
+  const uint64_t end = first + n;
+  TrackArgs      g{};
+  g.x = x, g.lda = n, g.N = N, g.A = h->A, g.rep = h->d_rep.p, g.ep = h->ep;
+  // 1. predict: the subframes of this push from the state at its start, without corrections; each half-frame's window is the tracker's +-W
+  //    plus the distance a clock max_ppm off moves the start over the predicted span, clamped to the samples fed
+  std::vector<TrackWin> win;
+  std::vector<uint32_t> wk; // subframe number of each window
+  {
+    int64_t  ps  = h->s;
+    float    pac = h->acc;
+    uint32_t pk = h->k, cnt = 0;
+    while (cnt < maxsf && ps >= (int64_t)first && (uint64_t)ps + SF <= end) {
+      if ((h->cfg.first_tti + pk) % 10240 % 5 == 0) {
+        const int64_t tau = ps + 13 * N / 2 - (int64_t)first;
+        const int64_t M   = (int64_t)std::ceil((double)h->max_ppm * 1e-6 * (double)(ps - h->s)) + 1; // half-width W + M
+        const int64_t lo = std::max<int64_t>(tau - W - M, 0), hi = std::min<int64_t>(tau + W + M, (int64_t)(n - N));
+        win.push_back(TrackWin{(uint64_t)lo, (uint32_t)(hi - lo + 1), 0});
+        wk.push_back(pk);
+      }
+      pac           = pac + h->d / 5.0f;
+      const float r = roundf(pac);
+      pac           = pac - r;
+      ps            = ps + SF + (int64_t)r;
+      pk++, cnt++;
+    }
+  }
+  std::vector<float> m;
+  uint32_t           stride = 0;
+  if (int r = track_metrics(h, g, win, m, stride)) return r;
+  // 2. replay the timing rule (lteo_track_push) subframe by subframe; the carrier offset waits for the sums of step 3
+  h->sf.clear(), h->hf.clear();
+  std::vector<uint64_t> spos, hpos;
+  uint32_t              remeasured = 0;
+  size_t                wi         = 0;
+  while (h->sf.size() < maxsf && h->s >= (int64_t)first && (uint64_t)h->s + SF <= end) {
+    const uint32_t    tti = (h->cfg.first_tti + h->k) % 10240;
+    ltephy_track_sf_t o{};
+    o.start = h->s, o.tti = tti, o.index = h->k;
+    o.flags = (h->miss == 0 ? LTEPHY_TRACK_LOCKED : 0) | (h->miss >= TRACK_MISS ? LTEPHY_TRACK_LOST : 0);
+    h->sf.push_back(o);
+    spos.push_back((uint64_t)(h->s - (int64_t)first));
+    if (tti % 5 == 0) {
+      ltephy_track_hf_t q{};
+      q.tau = h->s + 13 * N / 2, q.index = h->k;
+      const uint64_t tau = (uint64_t)(q.tau - (int64_t)first);
+      while (wi < wk.size() && wk[wi] < h->k) wi++;
+      const float* mv = nullptr;
+      uint64_t     t0 = 0;
+      if (wi < wk.size() && wk[wi] == h->k && win[wi].t0 + W <= tau && tau + W < win[wi].t0 + win[wi].cnt)
+        mv = &m[(size_t)wi * stride], t0 = win[wi].t0;
+      std::vector<float> mr;
+      if (!mv) { // the tracked window left the measured one: measure it now
+        std::vector<TrackWin> one{TrackWin{tau - W, 2 * W + 1, 0}};
+        uint32_t              st1 = 0;
+        if (int r = track_metrics(h, g, one, mr, st1)) return r;
+        mv = mr.data(), t0 = tau - W, remeasured++;
+      }
+      int32_t best = 0;
+      float   peak = mv[tau - t0];
+      for (int32_t d = 1; d <= (int32_t)W; d++)
+        for (int32_t sg = -1; sg <= 1; sg += 2) {
+          const float v = mv[tau + sg * d - t0];
+          if (v > peak) peak = v, best = sg * d;
+        }
+      q.delta = best, q.peak = peak;
+      const int64_t hn = h->nhf++;
+      if (peak >= h->thr) {
+        q.flags |= LTEPHY_TRACK_LOCKED;
+        h->miss = 0;
+        h->nl++, h->sd += best, h->sh += hn, h->shh += hn * hn, h->shd += hn * best;
+        if (h->nl == TRACK_P) {
+          const int64_t P = TRACK_P, c = h->sd >= 0 ? (h->sd + P / 2) / P : -((-h->sd + P / 2) / P);
+          h->s += c;
+          h->ncor++;
+          if (h->ncor == 1) {
+            const int64_t num = P * h->shd - h->sh * h->sd, den = P * h->shh - h->sh * h->sh;
+            h->d = h->d + (float)num / (float)den;
+          } else {
+            const int64_t moved = h->s - (int64_t)h->cfg.frame_offset - (int64_t)h->k * SF;
+            h->d = (float)moved / ((float)h->nhf - 0.5f * (float)(P - 1));
+          }
+          h->nl = 0, h->sd = h->sh = h->shh = h->shd = 0;
+        }
+      } else
+        h->miss++;
+      if (h->miss >= TRACK_MISS) q.flags |= LTEPHY_TRACK_LOST;
+      h->hf.push_back(q);
+      hpos.push_back(tau + best);
+    }
+    h->acc        = h->acc + h->d / 5.0f;
+    const float r = roundf(h->acc);
+    h->acc        = h->acc - r;
+    h->s          = h->s + SF + (int64_t)r;
+    h->k++;
+  }
+  const uint32_t nsf = (uint32_t)h->sf.size(), nh = (uint32_t)h->hf.size();
+  // 3. the CFO sums at the chosen positions, then the loop in subframe order: each subframe keeps the offset that held before its half-frame
+  std::vector<float2> c((size_t)nh * h->A * 2);
+  if (nh) {
+    CU(cudaMemcpyAsync(h->d_pos.p, hpos.data(), nh * sizeof(uint64_t), cudaMemcpyHostToDevice, h->stream));
+    if (launch_track_sums(g, h->d_pos.p, nh, h->d_c.p, h->stream))
+      return fail(LTEPHY_ERROR, "track_push: sum kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
+    CU(cudaMemcpyAsync(c.data(), h->d_c.p, c.size() * sizeof(float2), cudaMemcpyDeviceToHost, h->stream));
+    CU(cudaStreamSynchronize(h->stream));
+  }
+  std::vector<float2> tabA((size_t)nsf * (SF / 128)), tabB((size_t)nsf * 128);
+  for (uint32_t i = 0, j = 0; i < nsf; i++) {
+    ltephy_track_sf_t& o = h->sf[i];
+    o.cfo_hz             = h->f;
+    const double th      = 2.0 * M_PI * (double)h->f / (15000.0 * (double)N);
+    for (uint32_t q = 0; q < SF / 128; q++)
+      tabA[(size_t)i * (SF / 128) + q] = make_float2((float)std::cos(-th * 128.0 * (double)q), (float)std::sin(-th * 128.0 * (double)q));
+    for (uint32_t q = 0; q < 128; q++) tabB[(size_t)i * 128 + q] = make_float2((float)std::cos(-th * (double)q), (float)std::sin(-th * (double)q));
+    if (j < nh && h->hf[j].index == o.index) {
+      ltephy_track_hf_t& q  = h->hf[j];
+      float              sr = 0.0f, si = 0.0f;
+      for (uint32_t a = 0; a < h->A; a++) {
+        const float2 c1 = c[((size_t)j * h->A + a) * 2], c2 = c[((size_t)j * h->A + a) * 2 + 1];
+        sr              = sr + (c2.x * c1.x + c2.y * c1.y);
+        si              = si + (c2.y * c1.x - c2.x * c1.y);
+      }
+      q.s_re = sr, q.s_im = si;
+      q.f_meas = atan2f(si, sr) * (float)(15000.0 / M_PI);
+      if ((q.flags & LTEPHY_TRACK_LOCKED) && !(h->cfg.flags & LTEPHY_TRACK_NO_CFO)) h->f = h->f + TRACK_ALPHA * (q.f_meas - h->f);
+      j++;
+    }
+  }
+  // 4. the cut
+  if (nsf) {
+    CU(cudaMemcpyAsync(h->d_start.p, spos.data(), nsf * sizeof(uint64_t), cudaMemcpyHostToDevice, h->stream));
+    CU(cudaMemcpyAsync(h->d_tabA.p, tabA.data(), tabA.size() * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
+    CU(cudaMemcpyAsync(h->d_tabB.p, tabB.data(), tabB.size() * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
+    if (launch_track_cut(g, h->d_start.p, h->d_tabA.p, h->d_tabB.p, nsf, h->d_cut.p, h->stream))
+      return fail(LTEPHY_ERROR, "track_push: cut kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
+    CU(cudaStreamSynchronize(h->stream));
+  }
+  out->nof_subframes = nsf, out->nof_half_frames = nh;
+  out->sf = h->sf.data(), out->hf = h->hf.data(), out->iq_dev = h->d_cut.p;
+  out->next_sample = (uint64_t)h->s, out->remeasured = remeasured, out->reserved = 0;
+  return LTEPHY_SUCCESS;
+}
+
+static int track_check(ltephy_track_t* h, const void* iq, uint64_t first, uint64_t n, ltephy_track_out_t* out)
+{
+  if (!h || !out || (!iq && n)) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_push: null argument");
+  if ((int64_t)first > h->s)
+    return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_push: first_sample %llu is after the next sample needed, %lld", (unsigned long long)first, (long long)h->s);
+  return LTEPHY_SUCCESS;
+}
+
+extern "C" int ltephy_track_push(ltephy_track_t* h, const float* iq, uint64_t first_sample, uint64_t nof_samples, ltephy_track_out_t* out)
+{
+  if (int r = track_check(h, iq, first_sample, nof_samples, out)) return r;
+  CU(cudaSetDevice(h->cfg.device));
+  if (nof_samples) {
+    if (h->d_x.reserve((size_t)h->A * nof_samples)) return fail(LTEPHY_ERROR, "track_push: device allocation failed");
+    CU(cudaMemcpyAsync(h->d_x.p, iq, (size_t)h->A * nof_samples * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
+  }
+  return track_run(h, h->d_x.p, first_sample, nof_samples, out);
+}
+
+extern "C" int ltephy_track_push_device(ltephy_track_t* h, const void* iq_dev, uint64_t first_sample, uint64_t nof_samples, ltephy_track_out_t* out)
+{
+  if (int r = track_check(h, iq_dev, first_sample, nof_samples, out)) return r;
+  CU(cudaSetDevice(h->cfg.device));
+  return track_run(h, static_cast<const float2*>(iq_dev), first_sample, nof_samples, out);
+}

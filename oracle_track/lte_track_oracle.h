@@ -1,0 +1,58 @@
+/*
+ * lte_track_oracle.h -- CPU oracle of the tracker (DESIGN.md §2, "tracking"): PSS tracking of every half-frame after the cell search, whole-
+ * sample timing corrections with a drift estimate, a first-order carrier-offset loop, and the cut of every subframe rotated by the carrier
+ * offset that held before it.  Plain C, one subframe at a time, every float sum in the order DESIGN.md states; the product (ltephy_track_*,
+ * include/ltephy_b200.h) must equal its records and cut samples bit for bit.  The records have the layout of ltephy_track_sf_t / _hf_t.
+ */
+#pragma once
+#include <stdint.h>
+
+#ifdef __cplusplus
+extern "C" {
+#endif
+
+typedef struct {
+  float re, im;
+} lteo_tcf_t;
+
+#define LTEO_TRACK_NO_CFO 1u
+#define LTEO_TRACK_LOCKED 1u
+#define LTEO_TRACK_LOST   2u
+#define LTEO_TRACK_P      4u     /* locked half-frames per timing correction */
+#define LTEO_TRACK_ALPHA  0.05f  /* gain of the carrier-offset loop */
+#define LTEO_TRACK_MISS   4u     /* half-frames in a row without lock after which records are flagged lost */
+#define LTEO_TRACK_LOCK_K 20.0f  /* a half-frame is locked when its peak metric reaches LTEO_TRACK_LOCK_K / N */
+
+typedef struct {
+  int64_t  start;
+  uint32_t tti;
+  float    cfo_hz;
+  uint32_t flags;
+  uint32_t index;
+} lteo_track_sf_t;
+
+typedef struct {
+  int64_t  tau;
+  uint32_t index;
+  int32_t  delta;
+  float    peak;
+  float    s_re, s_im;
+  float    f_meas;
+  uint32_t flags;
+  uint32_t pad;
+} lteo_track_hf_t;
+
+typedef struct lteo_track lteo_track_t;
+
+/* N, A (1 or 2), pci, first_tti, frame_offset, cfo_hz and flags as in ltephy_track_cfg_t; NULL on invalid arguments */
+lteo_track_t* lteo_track_create(uint32_t N, uint32_t A, uint32_t pci, uint32_t first_tti, uint64_t frame_offset, float cfo_hz, uint32_t flags);
+void          lteo_track_destroy(lteo_track_t* t);
+/* x: [A][n] absolute samples first .. first + n - 1 (first <= *next of the previous call).  Processes up to max_sf subframes that lie wholly
+ * inside; writes their records to sf (and the half-frame records to hf, at most max_sf / 5 + 1), their cut samples to cut [k][A][15 N] (may be
+ * NULL), the counts to *nsf / *nhf and the next sample the caller must still include to *next.  0, or -2 on invalid arguments. */
+int lteo_track_push(lteo_track_t* t, const lteo_tcf_t* x, uint64_t first, uint64_t n, uint32_t max_sf, lteo_track_sf_t* sf, uint32_t* nsf,
+                    lteo_track_hf_t* hf, uint32_t* nhf, lteo_tcf_t* cut, uint64_t* next);
+
+#ifdef __cplusplus
+}
+#endif
