@@ -348,6 +348,26 @@ void ltephy_track_destroy(ltephy_track_t* h);
 int  ltephy_track_push(ltephy_track_t* h, const float* iq, uint64_t first_sample, uint64_t nof_samples, ltephy_track_out_t* out);
 /* same, with the samples already in device memory */
 int  ltephy_track_push_device(ltephy_track_t* h, const void* iq_dev, uint64_t first_sample, uint64_t nof_samples, ltephy_track_out_t* out);
+/* The uplink carrier of the same radio (the reference's -m 1: channel 1 of srsran_ue_sync_zerocopy, src/src/LTESniffer_Core.cc:174-181,365), cut
+ * at the downlink's tracked timing.  UL subframe k starts at start_k + ul_offset and is rotated, with the DL cut's rule, by
+ * f_ul = (float)(cfo_hz_k * cfo_ratio).  cfo_ratio = 1 applies the downlink's offset unchanged, as srsRAN's ue_sync does to every channel; with one
+ * reference oscillator f_UL / f_DL is the physical value (1747.5 / 1842.5 in band 3).  Call before the first push; afterwards only
+ * ltephy_track_push_ul / _device are accepted (ltephy_track_push / _device are refused).  INVALID_INPUTS for 0 >= cfo_ratio, cfo_ratio > 2, NaN,
+ * |ul_offset| >= 15 N or frame_offset + ul_offset < 0. */
+typedef struct {
+  double   cfo_ratio; /* f_UL / f_DL, in (0, 2] */
+  int32_t  ul_offset; /* whole samples the UL subframe starts after the DL one, |ul_offset| < 15 N */
+  uint32_t reserved[5];
+} ltephy_track_ul_cfg_t;
+int  ltephy_track_set_ul(ltephy_track_t* h, const ltephy_track_ul_cfg_t* cfg);
+/* iq as ltephy_track_push; iq_ul: cf32 [nof_samples] of one UL antenna, the same absolute samples.  A subframe is cut only when its DL window and
+ * its UL window both lie inside what has been fed; out->next_sample is the lowest sample either pending window still needs.  The DL records and
+ * cut equal those of a tracker without the uplink.  *ul_iq_dev: cf32 [nof_subframes][15 N] in device memory, valid until the next push. */
+int  ltephy_track_push_ul(ltephy_track_t* h, const float* iq, const float* iq_ul, uint64_t first_sample, uint64_t nof_samples, ltephy_track_out_t* out,
+                          const void** ul_iq_dev);
+/* same, with both carriers already in device memory */
+int  ltephy_track_push_ul_device(ltephy_track_t* h, const void* iq_dev, const void* iq_ul_dev, uint64_t first_sample, uint64_t nof_samples,
+                                 ltephy_track_out_t* out, const void** ul_iq_dev);
 
 /* nslots HARQ slots of LTEPHY_HARQ_SLOT_BYTES each (150 RNTIs x 8 processes x 2 TBs = 2400 slots = 1.4 GB); contents survive across batches */
 int ltephy_harq_reserve(ltephy_t* h, uint32_t nslots);
@@ -387,6 +407,13 @@ int ltephy_set_ul_cfg(ltephy_t* h, const ltephy_ul_cfg_t* cfg);
  * call demodulated the same n subframes: their symbols are decoded again with the new grants (srsran_enb_ul_fft once, decode_run per grant).
  * L_prb >= 3: the 1- and 2-PRB DMRS base sequences (36.211 Tables 5.5.1.2-1 / -2) are not carried. */
 int ltephy_submit_ul(ltephy_t* h, const float* iq_ul, const uint32_t* tti, uint32_t n, const ltephy_ul_grant_t* grants, uint32_t ngrants);
+/* same, with iq_ul_dev cf32 [n][sf_len] already in device memory on the handle's device (e.g. ltephy_track_push_ul's cut), read in place: the
+ * caller keeps it alive until ltephy_get_ul returns.  NULL re-decodes the previous call's symbols, as above. */
+int ltephy_submit_ul_device(ltephy_t* h, const void* iq_ul_dev, const uint32_t* tti, uint32_t n, const ltephy_ul_grant_t* grants, uint32_t ngrants);
+/* the uplink twin of ltephy_set_cfo: a constant carrier-offset correction of every UL subframe (phase restarting at each subframe, the table of
+ * ltephy_set_cfo), applied before the 7.5 kHz half-subcarrier rotation -- lteo_cfo_correct then lteo_ul_ofdm.  0 switches it off.  Kept apart
+ * from ltephy_set_cfo's value.  For pre-aligned captures; the tracked cut of ltephy_track_push_ul is already rotated. */
+int ltephy_set_ul_cfo(ltephy_t* h, float cfo_hz);
 /* results[ngrants], chest[ngrants]; payload receives the TB bytes back to back */
 int ltephy_get_ul(ltephy_t* h, ltephy_tb_result_t* results, ltephy_ul_chest_t* chest, uint8_t* payload, size_t payload_cap);
 

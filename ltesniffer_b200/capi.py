@@ -285,6 +285,28 @@ class LtePhy:
         self.n_ul = len(tti)
         return res, ch, pl
 
+    def decode_ul_device(self, iq_dev, tti, grants):
+        """ltephy_submit_ul_device: iq_dev a torch complex64 tensor [n][sf_len], contiguous, on this handle's device (None: decode the subframes
+        of the previous call again), read in place -> (results, chest, payload) as decode_ul"""
+        self.L.ltephy_submit_ul_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32]
+        tti = np.ascontiguousarray(tti, np.uint32)
+        if iq_dev is not None:
+            assert iq_dev.is_cuda and iq_dev.is_contiguous() and tuple(iq_dev.shape) == (len(tti), self.sf_len), tuple(iq_dev.shape)
+        arr = (UlGrant * max(1, len(grants)))(*grants)
+        ptr = None if iq_dev is None else C.c_void_p(iq_dev.data_ptr())
+        self._chk(self.L.ltephy_submit_ul_device(self.h, ptr, _p(tti), len(tti), arr, len(grants)), "submit_ul_device")
+        res = (TbResult * max(1, len(grants)))()
+        ch = (UlChest * max(1, len(grants)))()
+        pl = np.zeros(len(grants) * 10000 + 64, np.uint8)
+        self._chk(self.L.ltephy_get_ul(self.h, res, ch, _p(pl), pl.nbytes), "get_ul")
+        self.n_ul = len(tti)
+        return res, ch, pl
+
+    def set_ul_cfo(self, cfo_hz):
+        """ltephy_set_ul_cfo: constant carrier-offset correction of the uplink subframes (0 switches it off)"""
+        self.L.ltephy_set_ul_cfo.argtypes = [C.c_void_p, C.c_float]
+        self._chk(self.L.ltephy_set_ul_cfo(self.h, cfo_hz), "set_ul_cfo")
+
     # ---- stand-alone kernels
     def dci_sweep(self, llr, cfi):
         llr = np.ascontiguousarray(llr, np.float32)
@@ -794,20 +816,29 @@ class TrackOut(C.Structure):
                 ("next_sample", C.c_uint64), ("remeasured", C.c_uint32), ("reserved", C.c_uint32)]
 
 
+class TrackUlCfg(C.Structure):
+    _fields_ = [("cfo_ratio", C.c_double), ("ul_offset", C.c_int32), ("reserved", C.c_uint32 * 5)]
+
+
 assert C.sizeof(TrackCfg) == 64 and C.sizeof(TrackOut) == 48 and TRACK_SF_DTYPE.itemsize == 24 and TRACK_HF_DTYPE.itemsize == 40
+assert C.sizeof(TrackUlCfg) == 32
 
 
 class Tracker:
     """PSS tracking and subframe cutting of a recording after the cell search: push the recording part by part (antenna-major complex64
-    [nof_rx][n] with its absolute first sample); each push returns the subframes that now lie wholly inside what was fed."""
+    [nof_rx][n] with its absolute first sample); each push returns the subframes that now lie wholly inside what was fed.  With ul=dict(cfo_ratio=..., ul_offset=...) the tracker also cuts the
+    uplink carrier of the same radio (ltephy_track_set_ul); push both carriers with push_ul / push_ul_device."""
 
-    def __init__(self, symbol_sz, nof_rx, pci, frame_offset, cfo_hz=0.0, first_tti=0, max_subframes=1000, max_ppm=50.0, flags=0, device=0):
+    def __init__(self, symbol_sz, nof_rx, pci, frame_offset, cfo_hz=0.0, first_tti=0, max_subframes=1000, max_ppm=50.0, flags=0, device=0, ul=None):
         self.L = load_library()
         L = self.L
         L.ltephy_track_create.argtypes = [C.POINTER(TrackCfg), C.POINTER(C.c_void_p)]
         L.ltephy_track_destroy.argtypes = [C.c_void_p]
         L.ltephy_track_push.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.POINTER(TrackOut)]
         L.ltephy_track_push_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.POINTER(TrackOut)]
+        L.ltephy_track_set_ul.argtypes = [C.c_void_p, C.POINTER(TrackUlCfg)]
+        L.ltephy_track_push_ul.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.POINTER(TrackOut), C.POINTER(C.c_void_p)]
+        L.ltephy_track_push_ul_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.POINTER(TrackOut), C.POINTER(C.c_void_p)]
         self.cfg = TrackCfg(symbol_sz=symbol_sz, nof_rx=nof_rx, pci=pci, first_tti=first_tti, frame_offset=frame_offset, cfo_hz=cfo_hz,
                             max_ppm=max_ppm, max_subframes=max_subframes, flags=flags, device=device)
         self.h = C.c_void_p()
@@ -816,6 +847,15 @@ class Tracker:
             self.h = None
             raise RuntimeError("ltephy_track_create failed (%d): %s" % (r, L.ltephy_last_error().decode()))
         self.next_sample = frame_offset
+        self.ul = None
+        if ul is not None:
+            u = TrackUlCfg(cfo_ratio=float(ul.get("cfo_ratio", 1.0)), ul_offset=int(ul.get("ul_offset", 0)))
+            r = L.ltephy_track_set_ul(self.h, C.byref(u))
+            if r != 0:
+                self.close()
+                raise RuntimeError("ltephy_track_set_ul failed (%d): %s" % (r, L.ltephy_last_error().decode()))
+            self.ul = u
+            self.next_sample = min(frame_offset, frame_offset + u.ul_offset)
 
     def close(self):
         if self.h:
@@ -828,23 +868,28 @@ class Tracker:
         except Exception:
             pass
 
-    def _done(self, r, o):
+    def _view(self, ptr, shape):
+        """a torch copy of the tracker's device buffer at ptr (valid until the next push)"""
+        import torch
+        if shape[0]:
+            view = type("_Cut", (), {"__cuda_array_interface__": dict(shape=shape, typestr="<c8", data=(ptr, False), version=2)})()
+            with torch.cuda.device(self.cfg.device):
+                return torch.as_tensor(view, device="cuda:%d" % self.cfg.device).clone()
+        return torch.empty(shape, dtype=torch.complex64, device="cuda:%d" % self.cfg.device)
+
+    def _done(self, r, o, ul_ptr=None):
         if r != 0:
             raise RuntimeError("ltephy_track_push failed (%d): %s" % (r, self.L.ltephy_last_error().decode()))
-        import torch
         sf = np.ctypeslib.as_array((C.c_uint8 * (o.nof_subframes * 24)).from_address(o.sf)).view(TRACK_SF_DTYPE).copy() if o.nof_subframes else \
             np.zeros(0, TRACK_SF_DTYPE)
         hf = np.ctypeslib.as_array((C.c_uint8 * (o.nof_half_frames * 40)).from_address(o.hf)).view(TRACK_HF_DTYPE).copy() if o.nof_half_frames else \
             np.zeros(0, TRACK_HF_DTYPE)
-        shape = (o.nof_subframes, self.cfg.nof_rx, 15 * self.cfg.symbol_sz)
-        if o.nof_subframes:
-            view = type("_Cut", (), {"__cuda_array_interface__": dict(shape=shape, typestr="<c8", data=(o.iq_dev, False), version=2)})()
-            with torch.cuda.device(self.cfg.device):
-                iq = torch.as_tensor(view, device="cuda:%d" % self.cfg.device).clone()
-        else:
-            iq = torch.empty(shape, dtype=torch.complex64, device="cuda:%d" % self.cfg.device)
+        iq = self._view(o.iq_dev, (o.nof_subframes, self.cfg.nof_rx, 15 * self.cfg.symbol_sz))
         self.next_sample = o.next_sample
-        return dict(sf=sf, hf=hf, iq=iq, next_sample=o.next_sample, remeasured=o.remeasured)
+        out = dict(sf=sf, hf=hf, iq=iq, next_sample=o.next_sample, remeasured=o.remeasured)
+        if ul_ptr is not None:
+            out["ul_iq"] = self._view(ul_ptr.value, (o.nof_subframes, 15 * self.cfg.symbol_sz))
+        return out
 
     def push(self, iq, first_sample):
         """iq: complex64 [nof_rx][n] (host) of absolute samples first_sample ... -> dict(sf, hf: record arrays, iq: torch complex64
@@ -859,3 +904,20 @@ class Tracker:
         assert iq.is_cuda and iq.is_contiguous() and iq.dim() == 2 and iq.shape[0] == self.cfg.nof_rx
         o = TrackOut()
         return self._done(self.L.ltephy_track_push_device(self.h, C.c_void_p(iq.data_ptr()), first_sample, iq.shape[1], C.byref(o)), o)
+
+    def push_ul(self, iq, iq_ul, first_sample):
+        """iq as push, iq_ul: complex64 [n] of the uplink antenna, the same absolute samples -> push's dict plus ul_iq: torch complex64 [k][15 N]
+        on the device (a copy of the tracker's UL cut)"""
+        iq = np.ascontiguousarray(iq, np.complex64)
+        iq_ul = np.ascontiguousarray(iq_ul, np.complex64).reshape(-1)
+        assert iq.ndim == 2 and iq.shape[0] == self.cfg.nof_rx and iq_ul.shape[0] == iq.shape[1], (iq.shape, iq_ul.shape)
+        o, u = TrackOut(), C.c_void_p()
+        return self._done(self.L.ltephy_track_push_ul(self.h, _p(iq), _p(iq_ul), first_sample, iq.shape[1], C.byref(o), C.byref(u)), o, u)
+
+    def push_ul_device(self, iq, iq_ul, first_sample):
+        """iq: torch complex64 [nof_rx][n], iq_ul: torch complex64 [n], both contiguous on this handle's device"""
+        assert iq.is_cuda and iq.is_contiguous() and iq.dim() == 2 and iq.shape[0] == self.cfg.nof_rx
+        assert iq_ul.is_cuda and iq_ul.is_contiguous() and iq_ul.numel() == iq.shape[1]
+        o, u = TrackOut(), C.c_void_p()
+        return self._done(self.L.ltephy_track_push_ul_device(self.h, C.c_void_p(iq.data_ptr()), C.c_void_p(iq_ul.data_ptr()), first_sample, iq.shape[1],
+                                                             C.byref(o), C.byref(u)), o, u)

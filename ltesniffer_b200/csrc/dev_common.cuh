@@ -35,6 +35,7 @@ struct DevCell {
   const uint32_t* pbch_scr;       // [60] c(cell_id), 1920 bits
   const uint16_t* pbch_tab;       // [120] conv rate-matching table of K = 40
   const float2*   cfo_rot;        // [sf_len] e^{-j 2 pi f n / (15000 fft)} or nullptr (ltephy_set_cfo)
+  const float2*   ul_cfo_rot;     // the same for the uplink, or nullptr (ltephy_set_ul_cfo)
 };
 
 // per-subframe device record (layout mirrors the leading part of ltephy_sf_info_t)

@@ -81,7 +81,7 @@ __global__ void __launch_bounds__(256) ofdm_rx_kernel(const __grid_constant__ De
         const uint32_t m = ((j & 1u) << 2) | (j & 2u) | (j >> 2), idx = R3 ? 3 * (t + m * q8) + r : t + m * q8;
         float2         x = src[idx];
         if (CFO) { // constant frequency-offset correction of the file samples (srsran_cfo_correct in srsran_ue_sync's file mode)
-          const float2 rr = __ldg(&c.cfo_rot[c.sym_off[l] + idx]);
+          const float2 rr = __ldg(&(UL ? c.ul_cfo_rot : c.cfo_rot)[c.sym_off[l] + idx]);
           x               = make_float2(x.x * rr.x - x.y * rr.y, x.x * rr.y + x.y * rr.x);
         }
         if (UL) { // remove the 7.5 kHz half-subcarrier shift: multiply by exp(-j pi i / N) (srsran_enb_ul_fft)
@@ -360,9 +360,18 @@ extern "C" void launch_frontend(const DevCell& c, const float2* iq, float2* sym,
 extern "C" void launch_ul_ofdm(const DevCell& c, const float2* iq, float2* sym, uint32_t n, cudaStream_t st, uint64_t* launches)
 {
   const size_t smem_fft = (size_t)c.fft * sizeof(float2);
-  if (c.sub == c.fft)
-    ofdm_rx_kernel<true, false, false><<<dim3(14, 1, n), c.fft / 8 < 32 ? 32 : c.fft / 8, smem_fft, st>>>(c, iq, sym);
-  else
-    ofdm_rx_kernel<true, true, false><<<dim3(14, 1, n), 3 * (c.sub / 8), smem_fft, st>>>(c, iq, sym);
+  const dim3   grid(14, 1, n);
+  const uint32_t nt2 = c.fft / 8 < 32 ? 32 : c.fft / 8, nt3 = 3 * (c.sub / 8);
+  if (c.sub == c.fft) {
+    if (c.ul_cfo_rot)
+      ofdm_rx_kernel<true, false, true><<<grid, nt2, smem_fft, st>>>(c, iq, sym);
+    else
+      ofdm_rx_kernel<true, false, false><<<grid, nt2, smem_fft, st>>>(c, iq, sym);
+  } else {
+    if (c.ul_cfo_rot)
+      ofdm_rx_kernel<true, true, true><<<grid, nt3, smem_fft, st>>>(c, iq, sym);
+    else
+      ofdm_rx_kernel<true, true, false><<<grid, nt3, smem_fft, st>>>(c, iq, sym);
+  }
   *launches += 1;
 }

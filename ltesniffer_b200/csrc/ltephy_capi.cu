@@ -190,6 +190,7 @@ extern "C" int ltephy_create(const ltephy_cfg_t* cfg, ltephy_t** out)
     auto t40   = ltehost::conv_rm_table(40);
     c.pbch_tab = upload(h, t40.data(), t40.size());
     c.cfo_rot  = nullptr;
+    c.ul_cfo_rot = nullptr;
   }
   for (uint32_t cfi = 0; cfi < 3; cfi++) {
     c.nof_cce[cfi] = h->cm.nof_cce[cfi];
@@ -257,7 +258,7 @@ extern "C" void ltephy_destroy(ltephy_t* h)
   h->d_iq.release(), h->d_sym.release(), h->d_ce.release(), h->d_pil.release(), h->d_llr.release(), h->d_info.release(), h->d_cands.release();
   h->h_info.release(), h->d_compact.release(), h->h_compact.release(), h->d_grants.release(), h->d_cbs.release(), h->d_pairs.release(), h->d_tbs.release(), h->d_pair_pi_off.release();
   h->d_tscratch.release(), h->d_tqueue.release();
-  h->d_seq.release(), h->d_rm.release(), h->d_turbo.release(), h->d_pllr.release(), h->d_pi.release(), h->d_payload.release(), h->d_harq.release(), h->d_cfo.release(), h->d_mib.release(), h->d_pbch.release(), h->d_vwork.release();
+  h->d_seq.release(), h->d_rm.release(), h->d_turbo.release(), h->d_pllr.release(), h->d_pi.release(), h->d_payload.release(), h->d_harq.release(), h->d_cfo.release(), h->d_ulcfo.release(), h->d_mib.release(), h->d_pbch.release(), h->d_vwork.release();
   h->d_cb_iters.release(), h->d_cb_crc.release(), h->d_res.release(), h->h_res.release(), h->h_payload.release(), h->h_stage.release();
   h->d_uliq.release(), h->d_ulsym.release(), h->d_ulpool.release(), h->d_ulgrants.release(), h->d_ulchest.release(), h->h_ulchest.release();
   for (auto& e : h->ev)
@@ -827,13 +828,13 @@ extern "C" int ltephy_get_phase_b(ltephy_t* h, ltephy_tb_result_t* results, uint
 // ---------------------------------------------------------------------------------------- file-mode front matter (SURVEY 8f-1)
 // constant frequency-offset correction of every subframe of samples: srsran_cfo_correct(&q->file_cfo_correct, ..., file_cfo / 15000 / fft_size)
 // in srsran_ue_sync's file mode (args.file_offset_freq, reference src/src/LTESniffer_Core.cc:252-257); the rotation is applied by the OFDM kernel
-extern "C" int ltephy_set_cfo(ltephy_t* h, float cfo_hz)
+// the table both directions use: rot[n] = exp(-j 2 pi f n / (15000 fft)) over one subframe, in double, rounded to float (lteo_cfo_correct)
+static int cfo_table(ltephy_t* h, float cfo_hz, DevBuf<float2>& buf, const float2*& ptr)
 {
-  if (!h) return fail(LTEPHY_ERROR_INVALID_INPUTS, "set_cfo: bad arguments");
   CU(cudaSetDevice(h->cfg.device));
   CU(cudaStreamSynchronize(h->stream));
   if (cfo_hz == 0.0f) {
-    h->dc.cfo_rot = nullptr;
+    ptr = nullptr;
     return LTEPHY_SUCCESS;
   }
   std::vector<float2> rot(h->dc.sf_len);
@@ -841,10 +842,21 @@ extern "C" int ltephy_set_cfo(ltephy_t* h, float cfo_hz)
     const double ph = -2.0 * M_PI * (double)cfo_hz * (double)n / (15000.0 * (double)h->dc.fft);
     rot[n]          = make_float2((float)std::cos(ph), (float)std::sin(ph));
   }
-  if (h->d_cfo.reserve(rot.size())) return fail(LTEPHY_ERROR, "device allocation failed");
-  CU(cudaMemcpy(h->d_cfo.p, rot.data(), rot.size() * sizeof(float2), cudaMemcpyHostToDevice));
-  h->dc.cfo_rot = h->d_cfo.p;
+  if (buf.reserve(rot.size())) return fail(LTEPHY_ERROR, "device allocation failed");
+  CU(cudaMemcpy(buf.p, rot.data(), rot.size() * sizeof(float2), cudaMemcpyHostToDevice));
+  ptr = buf.p;
   return LTEPHY_SUCCESS;
+}
+extern "C" int ltephy_set_cfo(ltephy_t* h, float cfo_hz)
+{
+  if (!h) return fail(LTEPHY_ERROR_INVALID_INPUTS, "set_cfo: bad arguments");
+  return cfo_table(h, cfo_hz, h->d_cfo, h->dc.cfo_rot);
+}
+// the uplink's own table (DevCell::ul_cfo_rot), applied by ofdm_rx_kernel<UL> before the half-subcarrier rotation
+extern "C" int ltephy_set_ul_cfo(ltephy_t* h, float cfo_hz)
+{
+  if (!h) return fail(LTEPHY_ERROR_INVALID_INPUTS, "set_ul_cfo: bad arguments");
+  return cfo_table(h, cfo_hz, h->d_ulcfo, h->dc.ul_cfo_rot);
 }
 // PBCH work of one call (k_pbch.cu): pbch_llr_kernel fills frame-store rows 3.. with the soft bits of the listed subframes 0 for the port counts
 // nant_first .. nant_last, then pbch_hyp_kernel decodes the hypothesis jobs; res receives {port count of the CRC mask or 0, 24 MIB bits} per job.
@@ -1075,20 +1087,26 @@ static int ul_table_for(ltephy* h, uint32_t kind, uint32_t M, uint32_t ncs, uint
   return 0;
 }
 
-extern "C" int ltephy_submit_ul(ltephy_t* h, const float* iq_ul, const uint32_t* tti, uint32_t n, const ltephy_ul_grant_t* gin, uint32_t ng)
+// ltephy_submit_ul / _device: iq_host is copied into d_uliq first; iq_dev is demodulated in place; both NULL re-decodes the previous symbols
+static int submit_ul_common(ltephy_t* h, const float2* iq_host, const float2* iq_dev, const uint32_t* tti, uint32_t n, const ltephy_ul_grant_t* gin,
+                            uint32_t ng)
 {
   if (!h || !tti || n == 0 || n > h->cfg.max_subframes || (!gin && ng)) return fail(LTEPHY_ERROR_INVALID_INPUTS, "submit_ul: bad arguments");
   if (!h->ulcfg_set) return fail(LTEPHY_ERROR_INVALID_INPUTS, "submit_ul: ltephy_set_ul_cfg has not been called");
-  if (!iq_ul && h->n_ul != n) return fail(LTEPHY_ERROR_INVALID_INPUTS, "submit_ul: no IQ given and the previous call demodulated %u subframes, not %u", h->n_ul, n);
+  const bool have_iq = iq_host || iq_dev;
+  if (!have_iq && h->n_ul != n) return fail(LTEPHY_ERROR_INVALID_INPUTS, "submit_ul: no IQ given and the previous call demodulated %u subframes, not %u", h->n_ul, n);
   CU(cudaSetDevice(h->cfg.device));
   const DevCell& c = h->dc;
-  if (h->d_uliq.reserve((size_t)h->cfg.max_subframes * c.sf_len) || h->d_ulsym.reserve((size_t)h->cfg.max_subframes * 14 * c.nsc) ||
+  if ((iq_host && h->d_uliq.reserve((size_t)h->cfg.max_subframes * c.sf_len)) || h->d_ulsym.reserve((size_t)h->cfg.max_subframes * 14 * c.nsc) ||
       h->d_ulpool.reserve((size_t)1 << 20))
     return fail(LTEPHY_ERROR, "device allocation failed");
   CU(cudaEventRecord(h->ev[2], h->stream));
-  if (iq_ul) { // NULL: the demodulated symbols of the previous call stay (srsran_enb_ul_fft once, then one decode per grant)
-    CU(cudaMemcpyAsync(h->d_uliq.p, iq_ul, (size_t)n * c.sf_len * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
-    launch_ul_ofdm(c, h->d_uliq.p, h->d_ulsym.p, n, h->stream, &h->launches);
+  if (have_iq) { // NULL: the demodulated symbols of the previous call stay (srsran_enb_ul_fft once, then one decode per grant)
+    if (iq_host) {
+      CU(cudaMemcpyAsync(h->d_uliq.p, iq_host, (size_t)n * c.sf_len * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
+      iq_dev = h->d_uliq.p;
+    }
+    launch_ul_ofdm(c, iq_dev, h->d_ulsym.p, n, h->stream, &h->launches);
   }
   h->n_ul = n;
   // jobs
@@ -1144,6 +1162,14 @@ extern "C" int ltephy_submit_ul(ltephy_t* h, const float* iq_ul, const uint32_t*
   CU(cudaEventRecord(h->ev[3], h->stream));
   CU(cudaGetLastError());
   return LTEPHY_SUCCESS;
+}
+extern "C" int ltephy_submit_ul(ltephy_t* h, const float* iq_ul, const uint32_t* tti, uint32_t n, const ltephy_ul_grant_t* gin, uint32_t ng)
+{
+  return submit_ul_common(h, reinterpret_cast<const float2*>(iq_ul), nullptr, tti, n, gin, ng);
+}
+extern "C" int ltephy_submit_ul_device(ltephy_t* h, const void* iq_ul_dev, const uint32_t* tti, uint32_t n, const ltephy_ul_grant_t* gin, uint32_t ng)
+{
+  return submit_ul_common(h, nullptr, static_cast<const float2*>(iq_ul_dev), tti, n, gin, ng); // read in place until ltephy_get_ul
 }
 
 extern "C" int ltephy_get_ul(ltephy_t* h, ltephy_tb_result_t* results, ltephy_ul_chest_t* chest, uint8_t* payload, size_t payload_cap)

@@ -89,6 +89,7 @@ struct ltephy {
   cudaStream_t       stream = nullptr;
   cudaEvent_t        ev[6]{}, mark[2]{}, ev_h2d = nullptr;
   DevBuf<float2>     d_cfo;                  // per-sample rotation of ltephy_set_cfo
+  DevBuf<float2>     d_ulcfo;                // per-sample rotation of ltephy_set_ul_cfo
   DevBuf<uint32_t>   d_vwork;                // work list of the Viterbi kernel: count + two-word (subframe, locations, size) items
   DevBuf<uint32_t>   d_mib;                  // PBCH work of one call: subframe of each frame, hypothesis jobs, 2 result words per job (k_pbch.cu)
   DevBuf<float>      d_pbch;                 // PBCH frame store [3 + max_subframes][2][480]: rows 0..2 the frames the combiner carries over

@@ -32,7 +32,24 @@ struct ltephy_track {
   int64_t  sd = 0, sh = 0, shh = 0, shd = 0;
   std::vector<ltephy_track_sf_t> sf;
   std::vector<ltephy_track_hf_t> hf;
+  // the uplink carrier (ltephy_track_set_ul): one antenna cut at start + ul_off with its own rotation tables
+  bool             pushed = false, ul = false;
+  double           ul_ratio = 1.0;
+  int32_t          ul_off   = 0;
+  DevBuf<float2>   d_xu, d_cutu, d_tabAu, d_tabBu;
+  DevBuf<uint64_t> d_startu;
 };
+
+// the lowest absolute sample the pending DL window, and with the uplink set its UL window, still needs
+static int64_t track_needed(const ltephy_track* h) { return h->ul && h->ul_off < 0 ? h->s + h->ul_off : h->s; }
+
+// a subframe starting at s is cut only when its DL window, and with the uplink set its UL window, lie inside [first, end)
+static bool track_fits(const ltephy_track* h, int64_t s, uint64_t first, uint64_t end)
+{
+  if (!(s >= (int64_t)first && (uint64_t)s + h->SF <= end)) return false;
+  const int64_t su = s + (h->ul ? h->ul_off : 0);
+  return su >= (int64_t)first && (uint64_t)su + h->SF <= end;
+}
 
 static bool track_symbol_ok(uint32_t N)
 {
@@ -89,6 +106,7 @@ extern "C" void ltephy_track_destroy(ltephy_track_t* h)
   if (h->stream) cudaStreamSynchronize(h->stream);
   h->d_rep.release(), h->d_x.release(), h->d_cut.release(), h->d_tabA.release(), h->d_tabB.release(), h->d_c.release(), h->d_m.release();
   h->d_win.release(), h->d_pos.release(), h->d_start.release();
+  h->d_xu.release(), h->d_cutu.release(), h->d_tabAu.release(), h->d_tabBu.release(), h->d_startu.release();
   if (h->stream) cudaStreamDestroy(h->stream);
   delete h;
 }
@@ -109,7 +127,7 @@ static int track_metrics(ltephy_track_t* h, const TrackArgs& g, const std::vecto
   return LTEPHY_SUCCESS;
 }
 
-static int track_run(ltephy_track_t* h, const float2* x, uint64_t first, uint64_t n, ltephy_track_out_t* out)
+static int track_run(ltephy_track_t* h, const float2* x, const float2* xu, uint64_t first, uint64_t n, ltephy_track_out_t* out, const void** ul_iq_dev)
 {
   const uint32_t N = h->N, SF = h->SF, W = h->W, maxsf = h->cfg.max_subframes;
   const uint64_t end = first + n;
@@ -123,7 +141,7 @@ static int track_run(ltephy_track_t* h, const float2* x, uint64_t first, uint64_
     int64_t  ps  = h->s;
     float    pac = h->acc;
     uint32_t pk = h->k, cnt = 0;
-    while (cnt < maxsf && ps >= (int64_t)first && (uint64_t)ps + SF <= end) {
+    while (cnt < maxsf && track_fits(h, ps, first, end)) {
       if ((h->cfg.first_tti + pk) % 10240 % 5 == 0) {
         const int64_t tau = ps + 13 * N / 2 - (int64_t)first;
         const int64_t M   = (int64_t)std::ceil((double)h->max_ppm * 1e-6 * (double)(ps - h->s)) + 1; // half-width W + M
@@ -146,7 +164,7 @@ static int track_run(ltephy_track_t* h, const float2* x, uint64_t first, uint64_
   std::vector<uint64_t> spos, hpos;
   uint32_t              remeasured = 0;
   size_t                wi         = 0;
-  while (h->sf.size() < maxsf && h->s >= (int64_t)first && (uint64_t)h->s + SF <= end) {
+  while (h->sf.size() < maxsf && track_fits(h, h->s, first, end)) {
     const uint32_t    tti = (h->cfg.first_tti + h->k) % 10240;
     ltephy_track_sf_t o{};
     o.start = h->s, o.tti = tti, o.index = h->k;
@@ -217,14 +235,20 @@ static int track_run(ltephy_track_t* h, const float2* x, uint64_t first, uint64_
     CU(cudaMemcpyAsync(c.data(), h->d_c.p, c.size() * sizeof(float2), cudaMemcpyDeviceToHost, h->stream));
     CU(cudaStreamSynchronize(h->stream));
   }
-  std::vector<float2> tabA((size_t)nsf * (SF / 128)), tabB((size_t)nsf * 128);
+  // the cut's factor tables of subframe i for the offset f: exp(-j th 128 q) and exp(-j th q), th = 2 pi f / (15000 N), in double, rounded to float
+  auto tables = [&](std::vector<float2>& tA, std::vector<float2>& tB, uint32_t i, float f) {
+    const double th = 2.0 * M_PI * (double)f / (15000.0 * (double)N);
+    for (uint32_t q = 0; q < SF / 128; q++)
+      tA[(size_t)i * (SF / 128) + q] = make_float2((float)std::cos(-th * 128.0 * (double)q), (float)std::sin(-th * 128.0 * (double)q));
+    for (uint32_t q = 0; q < 128; q++) tB[(size_t)i * 128 + q] = make_float2((float)std::cos(-th * (double)q), (float)std::sin(-th * (double)q));
+  };
+  std::vector<float2> tabA((size_t)nsf * (SF / 128)), tabB((size_t)nsf * 128), tabAu, tabBu;
+  if (xu) tabAu.resize(tabA.size()), tabBu.resize(tabB.size());
   for (uint32_t i = 0, j = 0; i < nsf; i++) {
     ltephy_track_sf_t& o = h->sf[i];
     o.cfo_hz             = h->f;
-    const double th      = 2.0 * M_PI * (double)h->f / (15000.0 * (double)N);
-    for (uint32_t q = 0; q < SF / 128; q++)
-      tabA[(size_t)i * (SF / 128) + q] = make_float2((float)std::cos(-th * 128.0 * (double)q), (float)std::sin(-th * 128.0 * (double)q));
-    for (uint32_t q = 0; q < 128; q++) tabB[(size_t)i * 128 + q] = make_float2((float)std::cos(-th * (double)q), (float)std::sin(-th * (double)q));
+    tables(tabA, tabB, i, h->f);
+    if (xu) tables(tabAu, tabBu, i, (float)((double)h->f * h->ul_ratio)); // f_ul = (float)(cfo_hz cfo_ratio)
     if (j < nh && h->hf[j].index == o.index) {
       ltephy_track_hf_t& q  = h->hf[j];
       float              sr = 0.0f, si = 0.0f;
@@ -246,36 +270,92 @@ static int track_run(ltephy_track_t* h, const float2* x, uint64_t first, uint64_
     CU(cudaMemcpyAsync(h->d_tabB.p, tabB.data(), tabB.size() * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
     if (launch_track_cut(g, h->d_start.p, h->d_tabA.p, h->d_tabB.p, nsf, h->d_cut.p, h->stream))
       return fail(LTEPHY_ERROR, "track_push: cut kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
+    if (xu) { // the same kernel on the UL carrier: one antenna, start + ul_offset, the UL tables
+      std::vector<uint64_t> upos(nsf);
+      for (uint32_t i = 0; i < nsf; i++) upos[i] = (uint64_t)((int64_t)spos[i] + h->ul_off);
+      TrackArgs gu = g;
+      gu.x = xu, gu.A = 1;
+      CU(cudaMemcpyAsync(h->d_startu.p, upos.data(), nsf * sizeof(uint64_t), cudaMemcpyHostToDevice, h->stream));
+      CU(cudaMemcpyAsync(h->d_tabAu.p, tabAu.data(), tabAu.size() * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
+      CU(cudaMemcpyAsync(h->d_tabBu.p, tabBu.data(), tabBu.size() * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
+      if (launch_track_cut(gu, h->d_startu.p, h->d_tabAu.p, h->d_tabBu.p, nsf, h->d_cutu.p, h->stream))
+        return fail(LTEPHY_ERROR, "track_push: UL cut kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
+    }
     CU(cudaStreamSynchronize(h->stream));
   }
+  if (ul_iq_dev) *ul_iq_dev = h->d_cutu.p;
   out->nof_subframes = nsf, out->nof_half_frames = nh;
   out->sf = h->sf.data(), out->hf = h->hf.data(), out->iq_dev = h->d_cut.p;
-  out->next_sample = (uint64_t)h->s, out->remeasured = remeasured, out->reserved = 0;
+  out->next_sample = (uint64_t)track_needed(h), out->remeasured = remeasured, out->reserved = 0;
   return LTEPHY_SUCCESS;
 }
 
-static int track_check(ltephy_track_t* h, const void* iq, uint64_t first, uint64_t n, ltephy_track_out_t* out)
+static int track_check(ltephy_track_t* h, const void* iq, uint64_t first, uint64_t n, ltephy_track_out_t* out, bool ul)
 {
   if (!h || !out || (!iq && n)) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_push: null argument");
-  if ((int64_t)first > h->s)
-    return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_push: first_sample %llu is after the next sample needed, %lld", (unsigned long long)first, (long long)h->s);
+  if (ul != h->ul)
+    return fail(LTEPHY_ERROR_INVALID_INPUTS, h->ul ? "track_push: the uplink is set: push with ltephy_track_push_ul" : "track_push_ul: ltephy_track_set_ul has not been called");
+  if ((int64_t)first > track_needed(h))
+    return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_push: first_sample %llu is after the next sample needed, %lld", (unsigned long long)first,
+                (long long)track_needed(h));
+  h->pushed = true;
   return LTEPHY_SUCCESS;
 }
 
 extern "C" int ltephy_track_push(ltephy_track_t* h, const float* iq, uint64_t first_sample, uint64_t nof_samples, ltephy_track_out_t* out)
 {
-  if (int r = track_check(h, iq, first_sample, nof_samples, out)) return r;
+  if (int r = track_check(h, iq, first_sample, nof_samples, out, false)) return r;
   CU(cudaSetDevice(h->cfg.device));
   if (nof_samples) {
     if (h->d_x.reserve((size_t)h->A * nof_samples)) return fail(LTEPHY_ERROR, "track_push: device allocation failed");
     CU(cudaMemcpyAsync(h->d_x.p, iq, (size_t)h->A * nof_samples * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
   }
-  return track_run(h, h->d_x.p, first_sample, nof_samples, out);
+  return track_run(h, h->d_x.p, nullptr, first_sample, nof_samples, out, nullptr);
 }
 
 extern "C" int ltephy_track_push_device(ltephy_track_t* h, const void* iq_dev, uint64_t first_sample, uint64_t nof_samples, ltephy_track_out_t* out)
 {
-  if (int r = track_check(h, iq_dev, first_sample, nof_samples, out)) return r;
+  if (int r = track_check(h, iq_dev, first_sample, nof_samples, out, false)) return r;
   CU(cudaSetDevice(h->cfg.device));
-  return track_run(h, static_cast<const float2*>(iq_dev), first_sample, nof_samples, out);
+  return track_run(h, static_cast<const float2*>(iq_dev), nullptr, first_sample, nof_samples, out, nullptr);
+}
+
+extern "C" int ltephy_track_set_ul(ltephy_track_t* h, const ltephy_track_ul_cfg_t* cfg)
+{
+  if (!h || !cfg) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_set_ul: null argument");
+  if (h->pushed || h->ul) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_set_ul: only before the first push, once");
+  if (!(cfg->cfo_ratio > 0.0 && cfg->cfo_ratio <= 2.0)) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_set_ul: cfo_ratio outside (0, 2]");
+  const int64_t off = cfg->ul_offset;
+  if ((off < 0 ? -off : off) >= (int64_t)h->SF) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_set_ul: |ul_offset| %lld >= 15 N", (long long)off);
+  if ((int64_t)h->cfg.frame_offset + off < 0)
+    return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_set_ul: the first UL subframe would start before sample 0 (frame_offset + ul_offset < 0)");
+  CU(cudaSetDevice(h->cfg.device));
+  const size_t nsf = h->cfg.max_subframes;
+  if (h->d_cutu.reserve(nsf * h->SF) || h->d_tabAu.reserve(nsf * (h->SF / 128)) || h->d_tabBu.reserve(nsf * 128) || h->d_startu.reserve(nsf))
+    return fail(LTEPHY_ERROR, "track_set_ul: device allocation failed");
+  h->ul = true, h->ul_ratio = cfg->cfo_ratio, h->ul_off = cfg->ul_offset;
+  return LTEPHY_SUCCESS;
+}
+
+extern "C" int ltephy_track_push_ul(ltephy_track_t* h, const float* iq, const float* iq_ul, uint64_t first_sample, uint64_t nof_samples,
+                                    ltephy_track_out_t* out, const void** ul_iq_dev)
+{
+  if (!iq_ul && nof_samples) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_push_ul: null argument");
+  if (int r = track_check(h, iq, first_sample, nof_samples, out, true)) return r;
+  CU(cudaSetDevice(h->cfg.device));
+  if (nof_samples) {
+    if (h->d_x.reserve((size_t)h->A * nof_samples) || h->d_xu.reserve(nof_samples)) return fail(LTEPHY_ERROR, "track_push_ul: device allocation failed");
+    CU(cudaMemcpyAsync(h->d_x.p, iq, (size_t)h->A * nof_samples * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
+    CU(cudaMemcpyAsync(h->d_xu.p, iq_ul, nof_samples * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
+  }
+  return track_run(h, h->d_x.p, h->d_xu.p, first_sample, nof_samples, out, ul_iq_dev);
+}
+
+extern "C" int ltephy_track_push_ul_device(ltephy_track_t* h, const void* iq_dev, const void* iq_ul_dev, uint64_t first_sample, uint64_t nof_samples,
+                                           ltephy_track_out_t* out, const void** ul_iq_dev)
+{
+  if (!iq_ul_dev && nof_samples) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_push_ul: null argument");
+  if (int r = track_check(h, iq_dev, first_sample, nof_samples, out, true)) return r;
+  CU(cudaSetDevice(h->cfg.device));
+  return track_run(h, static_cast<const float2*>(iq_dev), static_cast<const float2*>(iq_ul_dev), first_sample, nof_samples, out, ul_iq_dev);
 }

@@ -20,6 +20,11 @@ struct lteo_track {
   uint32_t miss, nhf, ncor;
   uint32_t nl;       /* locked half-frames since the last correction */
   int64_t  sd, sh, shh, shd; /* their sums of delta, h, h^2, h delta (h: half-frame number) */
+  /* uplink carrier (lteo_track_set_ul) */
+  int      pushed;   /* a push was accepted: the uplink can no longer be set */
+  int      ul;       /* set: pushes go through lteo_track_push_ul */
+  double   ul_ratio; /* f_UL / f_DL */
+  int32_t  ul_off;   /* UL subframe start - DL subframe start */
 };
 
 static int track_symbol_ok(uint32_t N)
@@ -125,13 +130,13 @@ static void track_measure(const lteo_track_t* t, const lteo_tcf_t* x, uint64_t l
 
 /* y[n] = x[n] exp(-j theta n), theta = 2 pi f / (15000 N), n = 128 i + j: the factors exp(-j theta 128 i) and exp(-j theta j) in double, rounded
  * to float, multiplied in float (a b), then x (a b) */
-static void track_cut(lteo_track_t* t, const lteo_tcf_t* x, uint64_t lda, uint64_t s, lteo_tcf_t* out)
+static void track_cut(lteo_track_t* t, const lteo_tcf_t* x, uint64_t lda, uint32_t A, float f, uint64_t s, lteo_tcf_t* out)
 {
   const uint32_t N = t->N, SF = 15 * N;
-  const double   th = 2.0 * M_PI * (double)t->f / (15000.0 * (double)N);
+  const double   th = 2.0 * M_PI * (double)f / (15000.0 * (double)N);
   for (uint32_t i = 0; i < SF / 128; i++) t->tabA[i] = (lteo_tcf_t){(float)cos(-th * 128.0 * (double)i), (float)sin(-th * 128.0 * (double)i)};
   for (uint32_t j = 0; j < 128; j++) t->tabB[j] = (lteo_tcf_t){(float)cos(-th * (double)j), (float)sin(-th * (double)j)};
-  for (uint32_t a = 0; a < t->A; a++) {
+  for (uint32_t a = 0; a < A; a++) {
     const lteo_tcf_t* xa = x + a * lda + s;
     lteo_tcf_t*       ya = out + (uint64_t)a * SF;
     for (uint32_t n = 0; n < SF; n++) {
@@ -142,20 +147,47 @@ static void track_cut(lteo_track_t* t, const lteo_tcf_t* x, uint64_t lda, uint64
   }
 }
 
-int lteo_track_push(lteo_track_t* t, const lteo_tcf_t* x, uint64_t first, uint64_t n, uint32_t max_sf, lteo_track_sf_t* sf, uint32_t* nsf,
-                    lteo_track_hf_t* hf, uint32_t* nhf, lteo_tcf_t* cut, uint64_t* next)
+int lteo_track_set_ul(lteo_track_t* t, double cfo_ratio, int32_t ul_offset)
 {
-  if (!t || !x || !sf || !nsf || !hf || !nhf || !next || (int64_t)first > t->s) return -2;
+  if (!t || t->pushed || t->ul || !(cfo_ratio > 0.0 && cfo_ratio <= 2.0)) return -2;
+  if ((int64_t)(ul_offset < 0 ? -(int64_t)ul_offset : ul_offset) >= 15 * (int64_t)t->N || (int64_t)t->s0 + ul_offset < 0) return -2;
+  t->ul = 1, t->ul_ratio = cfo_ratio, t->ul_off = ul_offset;
+  return 0;
+}
+
+/* the lowest absolute sample the pending DL window, and with the uplink set its UL window, still needs */
+static int64_t track_needed(const lteo_track_t* t)
+{
+  return t->ul && t->ul_off < 0 ? t->s + t->ul_off : t->s;
+}
+
+/* a subframe is processed only when its DL window (and its UL window) lie inside first .. first + n - 1 */
+static int track_fits(const lteo_track_t* t, uint64_t first, uint64_t n)
+{
+  const uint32_t SF = 15 * t->N;
+  if (!(t->s >= (int64_t)first && (uint64_t)t->s + SF <= first + n)) return 0;
+  if (!t->ul) return 1;
+  const int64_t su = t->s + t->ul_off;
+  return su >= (int64_t)first && (uint64_t)su + SF <= first + n;
+}
+
+static int track_push(lteo_track_t* t, const lteo_tcf_t* x, const lteo_tcf_t* xu, uint64_t first, uint64_t n, uint32_t max_sf, lteo_track_sf_t* sf,
+                      uint32_t* nsf, lteo_track_hf_t* hf, uint32_t* nhf, lteo_tcf_t* cut, lteo_tcf_t* cut_ul, uint64_t* next)
+{
+  if (!t || !x || !sf || !nsf || !hf || !nhf || !next || (int64_t)first > track_needed(t)) return -2;
   const uint32_t N = t->N, SF = 15 * N, P = LTEO_TRACK_P;
   uint32_t       ns = 0, nh = 0;
-  while (ns < max_sf && t->s >= (int64_t)first && (uint64_t)t->s + SF <= first + n) {
+  t->pushed = 1;
+  while (ns < max_sf && track_fits(t, first, n)) {
     const uint64_t   s   = (uint64_t)t->s - first;
     const uint32_t   tti = (t->first_tti + t->k) % 10240;
     lteo_track_sf_t* o   = &sf[ns];
     memset(o, 0, sizeof(*o));
     o->start  = t->s, o->tti = tti, o->cfo_hz = t->f, o->index = t->k;
     o->flags  = (t->miss == 0 ? LTEO_TRACK_LOCKED : 0) | (t->miss >= LTEO_TRACK_MISS ? LTEO_TRACK_LOST : 0);
-    if (cut) track_cut(t, x, n, s, cut + (uint64_t)ns * t->A * SF);
+    if (cut) track_cut(t, x, n, t->A, t->f, s, cut + (uint64_t)ns * t->A * SF);
+    /* UL: one antenna at start + ul_offset, rotated by f_ul = (float)(f cfo_ratio) with the DL rule */
+    if (xu && cut_ul) track_cut(t, xu, n, 1, (float)((double)t->f * t->ul_ratio), (uint64_t)(t->s + t->ul_off) - first, cut_ul + (uint64_t)ns * SF);
     ns++;
     if (tti % 5 == 0) {
       lteo_track_hf_t* h = &hf[nh++];
@@ -192,6 +224,20 @@ int lteo_track_push(lteo_track_t* t, const lteo_tcf_t* x, uint64_t first, uint64
     t->s           = t->s + SF + (int64_t)r;
     t->k++;
   }
-  *nsf = ns, *nhf = nh, *next = (uint64_t)t->s;
+  *nsf = ns, *nhf = nh, *next = (uint64_t)track_needed(t);
   return 0;
+}
+
+int lteo_track_push(lteo_track_t* t, const lteo_tcf_t* x, uint64_t first, uint64_t n, uint32_t max_sf, lteo_track_sf_t* sf, uint32_t* nsf,
+                    lteo_track_hf_t* hf, uint32_t* nhf, lteo_tcf_t* cut, uint64_t* next)
+{
+  if (t && t->ul) return -2;
+  return track_push(t, x, NULL, first, n, max_sf, sf, nsf, hf, nhf, cut, NULL, next);
+}
+
+int lteo_track_push_ul(lteo_track_t* t, const lteo_tcf_t* x, const lteo_tcf_t* x_ul, uint64_t first, uint64_t n, uint32_t max_sf, lteo_track_sf_t* sf,
+                       uint32_t* nsf, lteo_track_hf_t* hf, uint32_t* nhf, lteo_tcf_t* cut, lteo_tcf_t* cut_ul, uint64_t* next)
+{
+  if (!t || !t->ul || !x_ul) return -2;
+  return track_push(t, x, x_ul, first, n, max_sf, sf, nsf, hf, nhf, cut, cut_ul, next);
 }
