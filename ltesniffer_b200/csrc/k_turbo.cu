@@ -22,6 +22,42 @@ struct TurboView {
   uint32_t        K, NW;
 };
 
+// Per-phase cycle counters for tools/turbo_phases.py, compiled in only with -DLTEPHY_TURBO_PHASES (the default build has none of it):
+// thread 0 of a CTA adds the clock64() time since its previous mark to the phase that ends at the mark, in shared memory, and the CTA
+// adds its sums to turbo_phase_cycles when it leaves.  Thread 0 waits at every barrier of the CTA, so its clock is the CTA's.
+#ifdef LTEPHY_TURBO_PHASES
+enum { PH_QUEUE, PH_STAGE, PH_BTAIL, PH_NATURAL, PH_INTERLEAVED, PH_CRC, PH_EMIT, PH_COUNT };
+__device__ unsigned long long turbo_phase_cycles[PH_COUNT];
+#define PH_BEGIN()                                                                                                                               \
+  __shared__ long long          ph_t;                                                                                                            \
+  __shared__ unsigned long long ph_s[PH_COUNT];                                                                                                  \
+  if (threadIdx.x == 0) {                                                                                                                        \
+    for (int i_ = 0; i_ < PH_COUNT; i_++) ph_s[i_] = 0;                                                                                          \
+    ph_t = clock64();                                                                                                                            \
+  }
+#define PH_MARK(p)                                                                                                                               \
+  if (threadIdx.x == 0) {                                                                                                                        \
+    const long long t_ = clock64();                                                                                                              \
+    ph_s[p] += (unsigned long long)(t_ - ph_t);                                                                                                  \
+    ph_t = t_;                                                                                                                                   \
+  }
+#define PH_END()                                                                                                                                 \
+  if (threadIdx.x == 0)                                                                                                                          \
+    for (int i_ = 0; i_ < PH_COUNT; i_++) atomicAdd(&turbo_phase_cycles[i_], ph_s[i_]);
+// reads (and optionally clears) the counters of the current device: PH_COUNT values
+extern "C" int ltephy_turbo_phases(unsigned long long* out, int reset)
+{
+  static const unsigned long long zero[PH_COUNT] = {};
+  if (cudaDeviceSynchronize() != cudaSuccess || cudaMemcpyFromSymbol(out, turbo_phase_cycles, sizeof(zero)) != cudaSuccess) return -1;
+  if (reset && cudaMemcpyToSymbol(turbo_phase_cycles, zero, sizeof(zero)) != cudaSuccess) return -1;
+  return PH_COUNT;
+}
+#else
+#define PH_BEGIN()
+#define PH_MARK(p)
+#define PH_END()
+#endif
+
 #define TD_SUB 8 // alpha is kept in shared memory for TD_SUB steps at a time
 #define TD_NSUB (TD_WL / TD_SUB)
 
@@ -53,8 +89,10 @@ __device__ __forceinline__ void load_par(uint32_t (&p)[TD_SUB], const uint32_t* 
 // The systematic and a-priori values come from shared memory when a step needs them, with no staged copy: within a pass window w
 // reads and writes ext only at its own 32 words (the identity in the natural pass, the QPP bijection in the interleaved one), and
 // reads the a-priori value of step j before it writes the extrinsic value of step j, so no other window's write can reach them.
-// The window is walked in 8-step chunks: forward over sub-windows 0 .. 3, then sub-windows 3 .. 0.  The parity words of the next
-// chunk are loaded while the current one is computed, so their global-memory latency is hidden behind 8 trellis steps.
+// The window is walked in 8-step chunks: forward over sub-windows 0 .. 2, then sub-windows 3 .. 0 forward with storage and backward.
+// Sub-window 3 is walked forward once: its stored pass also takes the eighth step, which gives the alpha the next window starts from.
+// The parity words of the next chunk are loaded while the current one is computed, so their global-memory latency is hidden behind
+// 8 trellis steps.
 // Shared memory per thread: alpha_t[TD_SUB][2] (uint4).
 template <bool IL, int NT, bool FULL>
 __device__ __forceinline__ void siso_pass(const TdConst& c, const TurboView& tv, uint4* __restrict__ alpha_t, uint32_t* bits_s, uint32_t w,
@@ -81,15 +119,15 @@ __device__ __forceinline__ void siso_pass(const TdConst& c, const TurboView& tv,
   __syncthreads();
 
   if (active) {
-    // ---- forward over the whole window, remembering alpha at the start of every sub-window ----------
+    // ---- forward over all sub-windows but the last, remembering alpha at the start of every sub-window ----------
     St8 a = a0, ck[TD_NSUB];
 #pragma unroll 1
-    for (uint32_t sw = 0; sw < TD_NSUB; sw++) {
+    for (uint32_t sw = 0; sw + 1 < TD_NSUB; sw++) {
       ck[sw] = a;
       uint32_t pc[TD_SUB];
 #pragma unroll
       for (uint32_t jj = 0; jj < TD_SUB; jj++) pc[jj] = pn[jj];
-      load_par<FULL>(pn, par, (sw + 1 < TD_NSUB ? sw + 1 : sw) * TD_SUB, w, NW, len); // after sub-window 3 comes sub-window 3 again
+      load_par<FULL>(pn, par, (sw + 1) * TD_SUB, w, NW, len);
 #pragma unroll
       for (uint32_t jj = 0; jj < TD_SUB; jj++) {
         const uint32_t j = sw * TD_SUB + jj;
@@ -100,11 +138,7 @@ __device__ __forceinline__ void siso_pass(const TdConst& c, const TurboView& tv,
         }
       }
     }
-    norm8(c, a);
-    if (w + 1 < NW) {
-#pragma unroll
-      for (int s = 0; s < 8; s++) A[(size_t)(w + 1) * 8 + s] = a.s[s];
-    }
+    ck[TD_NSUB - 1] = a;
     // ---- sub-windows, last first: forward with storage, then backward with LLR / extrinsic ----------
 #pragma unroll 1
     for (int sw = TD_NSUB - 1; sw >= 0; sw--) {
@@ -132,11 +166,16 @@ __device__ __forceinline__ void siso_pass(const TdConst& c, const TurboView& tv,
         if (FULL || j < len) {
           alpha_t[(jj * 2 + 0) * NT] = make_uint4(af.s[0], af.s[1], af.s[2], af.s[3]);
           alpha_t[(jj * 2 + 1) * NT] = make_uint4(af.s[4], af.s[5], af.s[6], af.s[7]);
-          if (jj + 1 < TD_SUB) {
+          if (jj + 1 < TD_SUB || sw == TD_NSUB - 1) {
             alpha_step(c, af, to32(c, g[jj].x), g[jj].y, vadd(g[jj].x, g[jj].y));
             if ((jj & 1u) == 1u) norm8(c, af);
           }
         }
+      }
+      if (sw == TD_NSUB - 1 && w + 1 < NW) { // only a full window has a successor
+        norm8(c, af);
+#pragma unroll
+        for (int s = 0; s < 8; s++) A[(size_t)(w + 1) * 8 + s] = af.s[s];
       }
 #pragma unroll
       for (int jj = TD_SUB - 1; jj >= 0; jj--) {
@@ -180,15 +219,22 @@ __device__ __forceinline__ uint32_t gf_mulmod24(uint32_t a, uint32_t b, uint32_t
   }
   return r;
 }
-__device__ __forceinline__ uint32_t gf_mod24(uint32_t v, uint32_t nbits, uint32_t poly)
+// the same product for both code blocks of a pair at once: two independent chains, so the 24 rounds of one hide the latency of the other
+__device__ __forceinline__ void gf_mulmod24x2(uint32_t (&a)[2], const uint32_t (&b)[2], const uint32_t (&poly)[2], uint32_t (&r)[2])
 {
-  uint32_t r = 0;
-  for (uint32_t i = 0; i < nbits; i++) {
-    r = (r << 1) | ((v >> (31 - i)) & 1u);
-    if (r & 0x1000000u) r ^= poly;
+  r[0] = r[1] = 0;
+#pragma unroll
+  for (int i = 0; i < 24; i++) {
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      if ((b[h] >> i) & 1u) r[h] ^= a[h];
+      a[h] <<= 1;
+      if (a[h] & 0x1000000u) a[h] ^= poly[h];
+    }
   }
-  return r;
 }
+// b(x) x^24 mod CRC24A / CRC24B for every byte b (turbo_arith.cuh); 2 KB of global memory, read through the read-only path
+__device__ const Crc24Tab crc24_tab = crc24_make_tab();
 
 // Persistent CTAs: the grid is sized to the number of CTAs the GPU can hold; each CTA takes code-block pairs from a queue
 // (early CRC stop makes the pairs' run times vary by up to 8x).  The pair's systematic values, interleaver table and
@@ -213,12 +259,13 @@ __global__ void __launch_bounds__(NT, 384 / NT) turbo_kernel(const DevPair* __re
   uint16_t*          pi_s    = reinterpret_cast<uint16_t*>(ext_s + TD_WL * NT);                            // [TD_WL][NW]
   __shared__ uint32_t bits_s[2 * TD_WL * 6];                       // 2 x 6144 bits
   __shared__ uint32_t btail[2][8];
-  __shared__ uint32_t red_s[8];
+  __shared__ uint32_t red_s[2][8];
   __shared__ uint32_t done_s[2];
   __shared__ uint32_t next_s;
 
   const uint32_t tid = threadIdx.x, nthreads = NT;
   uint32_t* const my_scratch = scratch + (size_t)blockIdx.x * slot_words;
+  PH_BEGIN()
   for (;;) {
     __syncthreads(); // the previous pair is completely done (shared memory and scratch slot are free)
     if (tid == 0) next_s = atomicAdd(queue, 1u);
@@ -240,8 +287,17 @@ __global__ void __launch_bounds__(NT, 384 / NT) turbo_kernel(const DevPair* __re
   tv.bnd   = my_scratch;
   tv.K = K, tv.NW = NW;
 
+  // the termination words of warp 0's lanes (below), asked for before the staging loads so that they arrive with them
+  uint32_t tx[3] = {0u, 0u, 0u}, tz[3] = {0u, 0u, 0u};
+  if (tid < 32) {
+    // d0 = xK, zK+1, x'K, z'K+1 ; d1 = zK, xK+2, z'K, x'K+2 ; d2 = xK+1, zK+2, x'K+1, z'K+2
+    const uint32_t* T = tv.tails + 2 * (tid >> 4); // the second constituent code's words lie two further
+    tx[0] = __ldg(T + 0), tx[1] = __ldg(T + 8), tx[2] = __ldg(T + 5);
+    tz[0] = __ldg(T + 4), tz[1] = __ldg(T + 1), tz[2] = __ldg(T + 9);
+  }
   // boundary metrics start "unknown" (all equal: the bias); the a-priori input of the very first half iteration is zero
   for (uint32_t i = tid; i < 4 * NW * 8; i += nthreads) tv.bnd[i] = TD_BIASW;
+  PH_MARK(PH_QUEUE)
   {
     // the pair's systematic values and interleaver table into shared memory, the a-priori values to zero, in 16-byte chunks (pair
     // buffers are 96 NW + 16 words and tables 32 NW entries, so both start 16-byte aligned; NW <= NT), 4 loads in flight per thread
@@ -266,79 +322,74 @@ __global__ void __launch_bounds__(NT, 384 / NT) turbo_kernel(const DevPair* __re
       }
     }
   }
+  PH_MARK(PH_STAGE)
   if (tid < 2) done_s[tid] = (tid < P.ncb) ? 0u : 1u;
-  if (tid == 0) {
-    // beta at K from the termination bits, both constituent codes, both code blocks (scalar int32)
-    for (int dec = 0; dec < 2; dec++) {
-      // d0 = xK, zK+1, x'K, z'K+1 ; d1 = zK, xK+2, z'K, x'K+2 ; d2 = xK+1, zK+2, x'K+1, z'K+2
-      const uint32_t* T = tv.tails;
-      uint32_t        tx[3], tz[3];
-      if (dec == 0) {
-        tx[0] = T[0], tx[1] = T[8], tx[2] = T[5];
-        tz[0] = T[4], tz[1] = T[1], tz[2] = T[9];
-      } else {
-        tx[0] = T[2], tx[1] = T[10], tx[2] = T[7];
-        tz[0] = T[6], tz[1] = T[3], tz[2] = T[11];
-      }
-      const uint8_t NEXT[8][2] = {{0, 4}, {4, 0}, {5, 1}, {1, 5}, {2, 6}, {6, 2}, {7, 3}, {3, 7}};
-      const uint8_t PAR[8][2]  = {{0, 1}, {0, 1}, {1, 0}, {1, 0}, {1, 0}, {1, 0}, {0, 1}, {0, 1}};
-      for (int h = 0; h < 2; h++) {
-        int bt[8], bn[8];
-        for (int s = 0; s < 8; s++) bt[s] = s ? TD_NINF : 0;
-        for (int k = 2; k >= 0; k--) {
-          const int x = h ? hi_s(tx[k]) : lo_s(tx[k]), z = h ? hi_s(tz[k]) : lo_s(tz[k]);
-          for (int s = 0; s < 8; s++) {
-            int best = -(1 << 30);
-            for (int u = 0; u < 2; u++) {
-              const int g = (u ? x : -x) + (PAR[s][u] ? z : -z), v = bt[NEXT[s][u]] + g;
-              best        = v > best ? v : best;
-            }
-            bn[s] = best;
-          }
-          for (int s = 0; s < 8; s++) bt[s] = bn[s];
-        }
-        const int ref = bt[0];
-        for (int s = 0; s < 8; s++) {
-          const int      v = bt[s] - ref + (int)TD_BIAS;
-          const uint32_t o = btail[dec][s];
-          btail[dec][s]    = h ? ((o & 0xFFFFu) | ((uint32_t)v << 16)) : ((uint32_t)v & 0xFFFFu);
-        }
-      }
+  if (tid < 32) {
+    // beta at K from the termination bits (int32): one lane per (constituent code, code block, state), lane = 16 dec + 8 h + s.
+    // Successor of state s on input u: NEXT[s][u] = {{0,4},{4,0},{5,1},{1,5},{2,6},{6,2},{7,3},{3,7}} (a nibble per state, the other
+    // edge is 4 away); parity of that edge: PAR[s][u] = {{0,1},{0,1},{1,0},{1,0},{1,0},{1,0},{0,1},{0,1}} (a bit per state, the other edge
+    // has the opposite parity).  The successors' metrics come from the lanes that hold them.
+    const uint32_t h = (tid >> 3) & 1u, s = tid & 7u, base = tid & 24u;
+    const uint32_t n0 = (0x37621540u >> (4 * s)) & 7u;
+    const bool     p0 = (0x3Cu >> s) & 1u;
+    int            bt = s ? TD_NINF : 0;
+#pragma unroll
+    for (int k = 2; k >= 0; k--) {
+      const int x = h ? hi_s(tx[k]) : lo_s(tx[k]), z = h ? hi_s(tz[k]) : lo_s(tz[k]), zz = p0 ? z : -z;
+      const int v0 = __shfl_sync(0xffffffffu, bt, base + n0) + (zz - x), v1 = __shfl_sync(0xffffffffu, bt, base + (n0 ^ 4u)) + (x - zz);
+      bt           = max(v0, v1);
     }
+    const int v = bt - __shfl_sync(0xffffffffu, bt, base) + (int)TD_BIAS;
+    const int o = __shfl_xor_sync(0xffffffffu, v, 8); // the other code block's value of the same state
+    if (!h) btail[tid >> 4][s] = ((uint32_t)v & 0xFFFFu) | ((uint32_t)o << 16);
   }
   __syncthreads();
+  PH_MARK(PH_BTAIL)
 
   uint32_t it = 0;
   while (it < max_iter) {
     for (uint32_t i = tid; i < 2 * TD_WL * 6; i += nthreads) bits_s[i] = 0u;
     siso_pass<false, NT, FULL>(c, tv, alpha_t, bits_s, tid, active, btail[0]);
+    PH_MARK(PH_NATURAL)
     siso_pass<true, NT, FULL>(c, tv, alpha_t, bits_s, tid, active, btail[1]);
+    PH_MARK(PH_INTERLEAVED)
     it++;
     // ---- CRC over the K decided bits of each code block -------------------------------------------
     bool all_done = true;
     const uint32_t was_done[2] = {done_s[0], done_s[1]}; // read before anybody can set it below (every path to here passed a barrier)
     __syncthreads();
+    // syndromes of the unfinished halves that carry a CRC, both in one round: word tid of a half is reduced by the byte table, moved
+    // to its place by x^after, and the words are summed over the CTA
+    const bool chk[2] = {!was_done[0] && P.crc_type[0], !was_done[1] && P.crc_type[1]};
+    uint32_t   tot[2] = {0u, 0u};
+    if (chk[0] || chk[1]) {
+      uint32_t r[2] = {0u, 0u};
+      if (active) {
+        const uint32_t k0 = tid * TD_WL, nb = min((uint32_t)TD_WL, K - k0), after = K - k0 - nb;
+        uint32_t       a[2], xp[2], poly[2];
+#pragma unroll
+        for (uint32_t h = 0; h < 2; h++) {
+          const bool     tA = P.crc_type[h] == 1; // a half without CRC goes through CRC24B's arithmetic and is ignored
+          const uint32_t v  = bits_s[h * TD_WL * 6 + tid] >> (32u - nb);
+          a[h]              = crc24_fold_word(__ldg(&crc24_tab.t[tA ? 0 : 1][v >> 24]), v);
+          xp[h]             = __ldg((tA ? xpowA : xpowB) + (after >> 3));
+          poly[h]           = tA ? TD_CRC24A : TD_CRC24B;
+        }
+        gf_mulmod24x2(a, xp, poly, r);
+      }
+#pragma unroll
+      for (int off = 16; off >= 1; off >>= 1) {
+        r[0] ^= __shfl_xor_sync(0xffffffffu, r[0], off);
+        r[1] ^= __shfl_xor_sync(0xffffffffu, r[1], off);
+      }
+      if ((tid & 31u) == 0) red_s[0][tid >> 5] = r[0], red_s[1][tid >> 5] = r[1];
+      __syncthreads(); // red_s is next written an iteration (several barriers) later
+      for (uint32_t i = 0; i < (nthreads + 31) / 32; i++) tot[0] ^= red_s[0][i], tot[1] ^= red_s[1][i];
+    }
+    PH_MARK(PH_CRC)
     for (uint32_t h = 0; h < 2; h++) {
       if (was_done[h]) continue;
-      const uint32_t ct = P.crc_type[h];
-      bool           ok = false;
-      if (ct) {
-        const uint32_t  poly = ct == 1 ? 0x1864CFBu : 0x1800063u;
-        const uint32_t* xp   = ct == 1 ? xpowA : xpowB;
-        uint32_t        r    = 0;
-        if (active) {
-          const uint32_t k0 = tid * TD_WL, nb = min((uint32_t)TD_WL, K - k0), after = K - k0 - nb;
-          r                 = gf_mulmod24(gf_mod24(bits_s[h * TD_WL * 6 + tid], nb, poly), xp[after >> 3], poly);
-        }
-#pragma unroll
-        for (int off = 16; off >= 1; off >>= 1) r ^= __shfl_xor_sync(0xffffffffu, r, off);
-        if ((tid & 31u) == 0) red_s[tid >> 5] = r;
-        __syncthreads();
-        uint32_t tot = 0;
-        for (uint32_t i = 0; i < (nthreads + 31) / 32; i++) tot ^= red_s[i];
-        ok = (tot == 0);
-        __syncthreads();
-      }
+      const bool ok = chk[h] && tot[h] == 0;
       if (ok || it == max_iter) {
         // emit the data bits (skip fillers, drop the CB CRC when C > 1): byte aligned by construction
         const uint32_t nbytes = P.out_bits[h] >> 3, skip = P.out_skip[h];
@@ -355,9 +406,11 @@ __global__ void __launch_bounds__(NT, 384 / NT) turbo_kernel(const DevPair* __re
         all_done = false;
     }
     __syncthreads();
+    PH_MARK(PH_EMIT)
     if (all_done) break;
   }
   } // pair queue
+  PH_END()
 }
 
 // ---- transport-block CRC24A over the assembled payload (tbs/8 data bytes + 3 CRC bytes) -------------
@@ -374,13 +427,8 @@ __global__ void __launch_bounds__(256) tb_crc_kernel(const DevTb* __restrict__ t
   const uint32_t per = (n + blockDim.x - 1) / blockDim.x, b0 = tid * per, b1 = min(n, b0 + per);
   if (b0 < b1) {
     uint32_t v = 0;
-    for (uint32_t i = b0; i < b1; i++) {
-      for (int bit = 7; bit >= 0; bit--) {
-        v = (v << 1) | ((p[i] >> bit) & 1u);
-        if (v & 0x1000000u) v ^= 0x1864CFBu;
-      }
-    }
-    r = gf_mulmod24(v, xpowA[n - b1], 0x1864CFBu);
+    for (uint32_t i = b0; i < b1; i++) v = crc24_fold_byte(__ldg(&crc24_tab.t[0][v >> 16]), v, p[i]);
+    r = gf_mulmod24(v, xpowA[n - b1], TD_CRC24A);
   }
 #pragma unroll
   for (int off = 16; off >= 1; off >>= 1) r ^= __shfl_xor_sync(0xffffffffu, r, off);

@@ -1,5 +1,5 @@
 // turbo_arith.cuh -- arithmetic core of the max-log-MAP decoder (K8), shared by the kernel (k_turbo.cu) and by the host model that
-// checks it against the CPU oracle without a GPU (tools/turbo_model.cu, tests/test_turbo_model.py): the packed int16x2 intrinsics
+// checks it against the CPU oracle without a GPU (tools/turbo_model.cpp, tests/test_turbo_model.py): the packed int16x2 intrinsics
 // get bit-identical host definitions below when this header is compiled for the host.
 #pragma once
 #include <cstdint>
@@ -143,3 +143,30 @@ TD_HD uint32_t ext_pair(const TdConst& c, uint32_t L, uint32_t Xp)
   return vmax(e, 0xFE01FE01u);                                   // -511
 }
 
+// ---- CRC24 of the hard decisions ---------------------------------------------------------------------------------------
+// Remainder of a 32-bit word v(x) modulo a CRC24 generator g: the low 24 bits are their own remainder, and the top byte b
+// contributes b(x) x^24 mod g, one entry of a 256-entry table per generator.  A word that holds only nb < 32 bits (in its top
+// bits) is shifted down first: leading zeros do not change a remainder.
+#define TD_CRC24A 0x1864CFBu
+#define TD_CRC24B 0x1800063u
+struct Crc24Tab {
+  uint32_t t[2][256]; // [0] CRC24A, [1] CRC24B: t[.][b] = b(x) x^24 mod g
+};
+constexpr Crc24Tab crc24_make_tab()
+{
+  Crc24Tab r{};
+  for (int p = 0; p < 2; p++)
+    for (uint32_t b = 0; b < 256; b++) {
+      uint32_t v = b << 16; // b(x) x^16, then 8 more shifts with reduction
+      for (int i = 0; i < 8; i++) {
+        v <<= 1;
+        if (v & 0x1000000u) v ^= (p ? TD_CRC24B : TD_CRC24A);
+      }
+      r.t[p][b] = v;
+    }
+  return r;
+}
+// top: the table entry of v's top byte (the caller reads it: __ldg on the device)
+TD_HD uint32_t crc24_fold_word(uint32_t top, uint32_t v) { return top ^ (v & 0xFFFFFFu); }
+// (r x^8 + byte) mod g for a remainder r < 2^24, top = table entry of r >> 16
+TD_HD uint32_t crc24_fold_byte(uint32_t top, uint32_t r, uint32_t byte) { return top ^ ((r << 8) & 0xFFFFFFu) ^ byte; }

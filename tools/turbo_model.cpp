@@ -152,3 +152,17 @@ extern "C" int turbo_model_decode(const int16_t* d0, const int16_t* d1, uint32_t
   memcpy(bits0, P.bits[0].data(), K), memcpy(bits1, P.bits[1].data(), K);
   return 0;
 }
+
+// The CRC24 byte tables of turbo_arith.cuh and the kernel's use of them: remainder of the top nb bits of a decision word
+// (which: 0 CRC24A, 1 CRC24B), and one byte folded into a remainder as tb_crc_kernel does it.
+static constexpr Crc24Tab crc24_tab_h = crc24_make_tab();
+extern "C" void turbo_model_crc24_table(uint32_t which, uint32_t* out) { memcpy(out, crc24_tab_h.t[which & 1u], sizeof(crc24_tab_h.t[0])); }
+extern "C" uint32_t turbo_model_crc24_word(uint32_t which, uint32_t word, uint32_t nb)
+{
+  const uint32_t v = word >> (32u - nb);
+  return crc24_fold_word(crc24_tab_h.t[which & 1u][v >> 24], v);
+}
+extern "C" uint32_t turbo_model_crc24_byte(uint32_t which, uint32_t r, uint32_t byte)
+{
+  return crc24_fold_byte(crc24_tab_h.t[which & 1u][r >> 16], r, byte);
+}
