@@ -432,7 +432,9 @@ enum {
   LTEPHY_TAP_LLR = 2, /* f32  [n][72*LTEPHY_MAX_CCE]           q->pdcch.llr */
   LTEPHY_TAP_PDSCH_LLR = 3, /* int16, all codewords of the submitted grants back to back */
   LTEPHY_TAP_TURBO_IN = 4,  /* int16 conditioned streams (debug) */
-  LTEPHY_TAP_UL_SYM = 5     /* cf32 [n][14][12*nof_prb]  UL grid after srsran_enb_ul_fft */
+  LTEPHY_TAP_UL_SYM = 5,    /* cf32 [n][14][12*nof_prb]  UL grid after srsran_enb_ul_fft */
+  LTEPHY_TAP_PBCH_LLR = 6   /* f32  [frames][2][480]     PBCH soft bits (not descrambled) of the subframes 0 of the last ltephy_mib_decode or
+                               ltephy_mib_decode_combined, in batch order, row [port count - 1]; ltephy_mib_decode writes only its handle's port count */
 };
 int ltephy_tap(ltephy_t* h, int what, void* dst, size_t bytes);
 /* turbo rate-dematch tables of a code block of size K with F filler bits, as phase B uses them; no device needed.  LTEPHY_TAP_TURBO_IN

@@ -83,6 +83,7 @@ class UlChest(C.Structure):
 
 
 TAP_UL_SYM = 5
+TAP_PBCH_LLR = 6                                      # f32 [frames][2][480]: PBCH soft bits of the last MIB decode, row [port count - 1]
 HARQ_NONE, HARQ_NEW, HARQ_RETX = 0, 1, 2            # grant.tb[t].harq_op
 HARQ_NEW_TX, HARQ_RE_TX, HARQ_FULL_BUFFER, HARQ_DECODED = 0, 1, 2, 3   # ltephy_harq_classify
 HARQ_SLOT_BYTES = 16 * 18448 * 2

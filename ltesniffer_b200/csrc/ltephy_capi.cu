@@ -872,6 +872,7 @@ static int pbch_run(ltephy* h, const std::vector<uint32_t>& frame_sf, uint32_t n
   if (!up.empty()) CU(cudaMemcpyAsync(h->d_mib.p, up.data(), up.size() * 4, cudaMemcpyHostToDevice, h->stream));
   launch_pbch(h->dc, h->d_sym.p, h->d_pil.p, h->d_mib.p, (uint32_t)F, nant_first - 1, nant_last - nant_first + 1, h->d_pbch.p, h->d_mib.p + F, (uint32_t)J, h->d_mib.p + R, h->stream, &h->launches);
   CU(cudaGetLastError());
+  h->pbch_frames = (uint32_t)F;
   if (J) CU(cudaMemcpyAsync(res.data(), h->d_mib.p + R, res.size() * 4, cudaMemcpyDeviceToHost, h->stream));
   CU(cudaStreamSynchronize(h->stream));
   return LTEPHY_SUCCESS;
@@ -1320,6 +1321,7 @@ extern "C" int ltephy_tap(ltephy_t* h, int what, void* dst, size_t bytes)
     case LTEPHY_TAP_PDSCH_LLR: src = h->d_pllr.p, avail = h->pb.pllr_elems * sizeof(short); break;
     case LTEPHY_TAP_TURBO_IN: src = h->d_turbo.p, avail = h->d_turbo.cap * 4; break;
     case LTEPHY_TAP_UL_SYM: src = h->d_ulsym.p, avail = (size_t)h->n_ul * 14 * h->dc.nsc * sizeof(float2); break;
+    case LTEPHY_TAP_PBCH_LLR: src = h->pbch_frames ? h->d_pbch.p + 3 * 960 : nullptr, avail = (size_t)h->pbch_frames * 960 * sizeof(float); break;
     default: return fail(LTEPHY_ERROR_INVALID_INPUTS, "tap: unknown buffer");
   }
   if (bytes > avail) return fail(LTEPHY_ERROR_INVALID_INPUTS, "tap: %zu bytes requested, %zu available", bytes, avail);

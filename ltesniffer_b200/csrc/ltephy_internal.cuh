@@ -95,6 +95,7 @@ struct ltephy {
   DevBuf<float>      d_pbch;                 // PBCH frame store [3 + max_subframes][2][480]: rows 0..2 the frames the combiner carries over
   uint32_t           mib_held     = 0;       // combiner: frames held (srsRAN's frame_idx between calls), in rows 3 - mib_held .. 2
   int32_t            mib_last_sfn = -1;      // combiner: SFN of the last frame consumed, -1 after a reset
+  uint32_t           pbch_frames  = 0;       // frames the last PBCH call wrote to rows 3.. of d_pbch (LTEPHY_TAP_PBCH_LLR)
   DevBuf<short>      d_harq;                 // HARQ store: harq_slots x LTEPHY_HARQ_SLOT_BYTES
   uint32_t           harq_slots = 0;
   std::vector<void*> tables; // device tables freed at destroy

@@ -11,6 +11,7 @@ import pytest
 
 import ltelib
 import ref64
+import ref64_ctrl
 from helpers import make_capture, oracle_frontend
 from ltelib import Cell, Oracle
 
@@ -29,14 +30,9 @@ def re_map_oracle(cell, sf, cfi, l, prb):
 
 
 def pdcch_index(cell, cfi):
-    """grid indices l * nsc + k of the PDCCH REs in reading order, and of the 16 PCFICH REs (symbol 0)"""
-    O = ltelib.oracle()
-    O.lteo_pdcch_re_index.restype = C.c_uint32
-    O.lteo_pdcch_re_index.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
-    o = Oracle(cell)
-    idx, pidx = np.zeros(4 * 9 * 88, np.uint16), np.zeros(16, np.uint16)
-    ncce = O.lteo_pdcch_re_index(o.h, cfi, ltelib.ptr(idx), ltelib.ptr(pidx))
-    return idx[:36 * ncce].astype(np.int64), pidx.astype(np.int64)
+    """grid indices l * nsc + k of the PDCCH REs in reading order, and of the 16 PCFICH REs (symbol 0), from ref64_ctrl's 36.211 map"""
+    m = ref64_ctrl.cell_map(cell, cfi)
+    return m.pdcch.ravel(), m.pcfich
 
 
 def pcfich_index(cell):
@@ -74,7 +70,7 @@ class Case:
                     for q in range(P):
                         free[ref64.crs_offset(cell, q, 0)::6] = False
                 grids[p, l, free] = ref64.qam(rng.integers(0, 2, 2 * free.sum()), 2)
-        # PCFICH (36.211 6.7): the CFI codeword scrambled, QPSK, port 0 or SFBC, on the four REGs of lteo_pdcch_re_index (pinned by test_phich_resources)
+        # PCFICH (36.211 6.7): the CFI codeword scrambled, QPSK, port 0 or SFBC, on the four REGs of ref64_ctrl (written from 36.211 6.7.4)
         pidx = pcfich_index(cell)
         d = ref64.qam(np.array(ref64.CFI_CODEWORDS[cfi - 1][:32], np.uint8) ^ ref64.gold((sf + 1) * (2 * cell.cell_id + 1) * 512 + cell.cell_id, 32), 2)
         grids[:, 0, pidx] = ref64.precode("port0" if P == 1 else "sfbc", d[None], P)
