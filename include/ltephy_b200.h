@@ -37,6 +37,8 @@ extern "C" {
 #define LTEPHY_NOF_FORMATS 9     /* falcon_ue_all_formats, src/src/DCISearch.cc:84-95 */
 #define LTEPHY_MAX_SIZES 8       /* distinct DCI payload sizes among the 9 formats */
 
+#define LTEPHY_MAX_BATCH_SUBFRAMES 65535 /* largest max_subframes ltephy_create accepts (65 s of air time per batch) */
+
 typedef struct ltephy ltephy_t;
 
 typedef struct {
@@ -44,7 +46,7 @@ typedef struct {
   uint32_t nof_ports;      /* CRS ports 1|2 */
   uint32_t cell_id;        /* PCI */
   uint32_t nof_rx;         /* rx antennas 1|2 */
-  uint32_t max_subframes;  /* batch capacity */
+  uint32_t max_subframes;  /* batch capacity, 1..LTEPHY_MAX_BATCH_SUBFRAMES */
   uint32_t max_grants;     /* phase-B capacity per batch (0 = 24 * max_subframes) */
   uint32_t turbo_max_iter; /* max-log-MAP iterations, >= 1 (SURVEY.md App. B.7) */
   int32_t  device;         /* CUDA device ordinal */

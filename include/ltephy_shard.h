@@ -91,7 +91,8 @@ typedef struct {
  *        ranks see only those of their own subframes (the rest stay zeroed)
  *   payload: transport-block bytes; tbs[].payload_off points into it.  Pinned memory keeps the device->host copy asynchronous.
  * Returns 0 or a negative LTEPHY_* code.  A rank that fails stops taking part in the collectives of later batches: treat
- * an error as fatal for the job, as with any collective program. */
+ * an error as fatal for the job, as with any collective program.  A failing call, a refused argument list included, still passes
+ * every ordered section on, and later batches of the rank return LTEPHY_ERROR at once. */
 int ltephy_decode_subframes_sharded(ltephy_shard_t* sh, ltephy_t* h, ltephy_search_t* s, const void* iq, int iq_on_device, const uint32_t* tti,
                                     uint32_t n, uint64_t seq, ltephy_sf_info_t* info, ltephy_dci_t* dcis, uint32_t max_dcis, uint32_t* n_dcis,
                                     ltephy_tb_result_t* tbs, uint8_t* payload, size_t payload_cap, ltephy_shard_stats_t* stats);

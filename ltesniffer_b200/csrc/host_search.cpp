@@ -1506,10 +1506,16 @@ static int decode_common(ltephy_t* h, ltephy_search_t* s, const void* iq, bool i
                          ltephy_sf_info_t* info, ltephy_cand_t* cand_scratch, ltephy_dci_t* dcis, uint32_t max_dcis, uint32_t* n_dcis,
                          ltephy_tb_result_t* tbs, uint8_t* payload, size_t payload_cap)
 {
-  if (!h || !s || !iq || !tti || !info || !cand_scratch || !dcis || !n_dcis || !tbs) return LTEPHY_ERROR_INVALID_INPUTS;
+  if (!s) return LTEPHY_ERROR_INVALID_INPUTS;
   double t0 = now_ms();
-  // Whatever happens before this batch's turn in the walk, the turn is taken and passed on: a failing batch must not leave the
-  // other pipelines of this search object waiting for a sequence number that never comes.
+  // A seq whose turn is over would wait forever: refuse it without touching the turn.  A second call with the same seq that gets past
+  // this check while the first still waits is refused at the walk (both waits below wake once next_seq reaches or passes seq).
+  if (seq != LTEPHY_SEQ_NONE) {
+    std::lock_guard<std::mutex> lk(s->mtx);
+    if (seq < s->next_seq) return LTEPHY_ERROR_INVALID_INPUTS;
+  }
+  // Whatever happens before this batch's turn in the walk, the argument check included, the turn is taken and passed on: a failing
+  // batch must not leave the other pipelines of this search object waiting for a sequence number that never comes.
   struct SeqGuard {
     ltephy_search_t* s;
     uint64_t         seq;
@@ -1519,14 +1525,15 @@ static int decode_common(ltephy_t* h, ltephy_search_t* s, const void* iq, bool i
       if (done || seq == LTEPHY_SEQ_NONE) return;
       {
         std::unique_lock<std::mutex> lk(s->mtx);
-        s->cv.wait(lk, [&] { return s->next_seq == seq; });
-        s->next_seq = seq + 1;
+        s->cv.wait(lk, [&] { return s->next_seq >= seq; });
+        if (s->next_seq == seq) s->next_seq = seq + 1;
       }
       s->cv.notify_all();
       done = true;
     }
     ~SeqGuard() { pass(); }
   } guard{s, seq};
+  if (!h || !iq || !tti || !info || !cand_scratch || !dcis || !n_dcis || !tbs) return LTEPHY_ERROR_INVALID_INPUTS;
   int r = iq_on_device ? ltephy_submit_iq_device(h, iq, tti, n) : ltephy_submit_iq(h, (const float*)iq, tti, n);
   if (r) return r;
   double t1 = now_ms();
@@ -1537,7 +1544,11 @@ static int decode_common(ltephy_t* h, ltephy_search_t* s, const void* iq, bool i
   uint32_t nd = 0;
   {
     std::unique_lock<std::mutex> lk(s->mtx);
-    s->cv.wait(lk, [&] { return s->next_seq == seq || seq == LTEPHY_SEQ_NONE; });
+    s->cv.wait(lk, [&] { return seq == LTEPHY_SEQ_NONE || s->next_seq >= seq; });
+    if (seq != LTEPHY_SEQ_NONE && s->next_seq != seq) { // a duplicate seq whose turn another call has taken meanwhile
+      guard.done = true;
+      return LTEPHY_ERROR_INVALID_INPUTS;
+    }
     r = ltephy_search_batch_compact(s, info, comp, nullptr, n, dcis, max_dcis, &nd);
     if (r == LTEPHY_NEED_FULL_TABLE) { // RAR-activated RNTIs or an overfull subframe: fetch the 20 KB / subframe table after all
       r = ltephy_get_phase_a(h, nullptr, cand_scratch);

@@ -8,15 +8,17 @@
 #include "dev_eq.cuh"
 
 // ---- scrambling sequences: c = x1 ^ XOR_{b in c_init} basis[b]  (36.211 7.2 without the 1600-step warm-up)
+// Grid: x = (grant, codeword), y = block of 256 words.  The grant count goes on x because gridDim.y stops at 65 535 and a batch
+// may carry more than 32 767 grants; a codeword needs a few dozen word blocks at most.
 __global__ void __launch_bounds__(256) scr_seq_kernel(const DevGrant* __restrict__ grants, const uint32_t* __restrict__ x1,
                                                       const uint32_t* __restrict__ basis, uint32_t basis_words, uint32_t cell_id,
                                                       uint32_t* __restrict__ seq_pool)
 {
-  const DevGrant& g  = grants[blockIdx.y >> 1];
-  const uint32_t  cw = blockIdx.y & 1u;
+  const DevGrant& g  = grants[blockIdx.x >> 1];
+  const uint32_t  cw = blockIdx.x & 1u;
   if (cw >= g.ncw) return;
   const uint32_t nwords = (g.nof_re * g.qm[cw] + 31) / 32;
-  const uint32_t wi     = blockIdx.x * blockDim.x + threadIdx.x;
+  const uint32_t wi     = blockIdx.y * blockDim.x + threadIdx.x;
   if (wi >= nwords || wi >= basis_words) return;
   const uint32_t c_init = (g.rnti << 14) + (cw << 13) + (g.sf_idx << 9) + cell_id;
   uint32_t       v      = x1[wi];
@@ -234,7 +236,7 @@ extern "C" void launch_pdsch_front(const DevCell& c, const DevGrant* grants, uin
                                    uint32_t* seq_pool, short* llr_pool, cudaStream_t st, uint64_t* launches)
 {
   if (!ngrants) return;
-  scr_seq_kernel<<<dim3((max_words + 255) / 256, 2 * ngrants), 256, 0, st>>>(grants, gold_x1, gold_basis, basis_words, c.cell_id, seq_pool);
+  scr_seq_kernel<<<dim3(2 * ngrants, (max_words + 255) / 256), 256, 0, st>>>(grants, gold_x1, gold_basis, basis_words, c.cell_id, seq_pool);
   pdsch_demod_kernel<<<ngrants, 256, 0, st>>>(c, grants, sym, ce, seq_pool, llr_pool);
   *launches += 2;
 }

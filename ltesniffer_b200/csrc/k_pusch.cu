@@ -46,8 +46,8 @@ __global__ void __launch_bounds__(256) scr_seq_ul_kernel(const DevUlGrant* __res
                                                          const uint32_t* __restrict__ basis, uint32_t basis_words, uint32_t cell_id,
                                                          uint32_t* __restrict__ seq_pool)
 {
-  const DevUlGrant& g = grants[blockIdx.y];
-  const uint32_t nwords = (12 * g.M * g.qm + 31) / 32, wi = blockIdx.x * blockDim.x + threadIdx.x;
+  const DevUlGrant& g = grants[blockIdx.x]; // grant on x, word block on y: gridDim.y stops at 65 535 (scr_seq_kernel, k_pdsch.cu)
+  const uint32_t nwords = (12 * g.M * g.qm + 31) / 32, wi = blockIdx.y * blockDim.x + threadIdx.x;
   if (wi >= nwords || wi >= basis_words) return;
   const uint32_t c_init = (g.rnti << 14) + (g.sf_idx << 9) + cell_id;
   uint32_t       v      = x1[wi];
@@ -241,7 +241,7 @@ extern "C" void launch_pusch(const DevCell& c, const DevUlGrant* grants, uint32_
                              uint32_t* seq_pool, short* llr_pool, DevUlChest* chest, cudaStream_t st, uint64_t* launches)
 {
   if (!ngrants) return;
-  scr_seq_ul_kernel<<<dim3((max_words + 255) / 256, ngrants), 256, 0, st>>>(grants, x1, basis, basis_words, c.cell_id, seq_pool);
+  scr_seq_ul_kernel<<<dim3(ngrants, (max_words + 255) / 256), 256, 0, st>>>(grants, x1, basis, basis_words, c.cell_id, seq_pool);
   const size_t smem = ((size_t)5 * max_M + 2 * PUSCH_PASS_CAP) * sizeof(float2);
   cudaFuncSetAttribute(pusch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (5 * 1200 + 2 * (int)PUSCH_PASS_CAP) * (int)sizeof(float2)); // per device / context
   pusch_kernel<<<ngrants, 256, smem, st>>>(c, grants, ulsym, dmrs_pool, idft_pool, seq_pool, llr_pool, chest, max_M);

@@ -65,6 +65,9 @@ extern "C" int ltephy_create(const ltephy_cfg_t* cfg, ltephy_t** out)
   if (cfg->nof_prb <= 10 || cfg->nof_prb > 100 || cfg->nof_ports < 1 || cfg->nof_ports > 2 || cfg->nof_rx < 1 || cfg->nof_rx > 2 ||
       cfg->max_subframes == 0)
     return fail(LTEPHY_ERROR_INVALID_INPUTS, "unsupported cell/batch configuration");
+  // the front end puts the subframe index on gridDim.y / gridDim.z (k_frontend.cu), which stop at 65 535
+  if (cfg->max_subframes > LTEPHY_MAX_BATCH_SUBFRAMES)
+    return fail(LTEPHY_ERROR_INVALID_INPUTS, "max_subframes %u: at most %u subframes per batch", cfg->max_subframes, (uint32_t)LTEPHY_MAX_BATCH_SUBFRAMES);
   // 2^k or 3 * 2^k samples per symbol, wide enough for the carrier: the standard LTE rate, or what srsran_symbol_sz answers in srsRAN's default
   // build (3/4 of it: 1536 at 100 PRB, 768 at 50, 384 at 25 -- the rate LTESniffer records at)
   if (cfg->symbol_sz) {
@@ -773,6 +776,7 @@ extern "C" int ltephy_submit_grants(ltephy_t* h, const ltephy_grant_t* gin, uint
     stage_and_pull(h, h->d_tbs.p, b.tbs.data(), b.tbs.size() * sizeof(DevTb));
     launch_pdsch_front(h->dc, h->d_grants.p, n, b.max_scr_words, h->d_sym.p, h->d_pil.p, h->d_gold_x1, h->d_gold_basis, h->gold_words, h->d_seq.p,
                        h->d_pllr.p, h->stream, &h->launches);
+    CU(cudaGetLastError()); // a front kernel that could not launch would leave the previous batch's sequences and soft bits behind
     if (int r = decode_code_blocks(h)) return r;
   }
   CU(cudaEventRecord(h->ev[3], h->stream));
@@ -1158,6 +1162,7 @@ static int submit_ul_common(ltephy_t* h, const float2* iq_host, const float2* iq
     stage_and_pull(h, h->d_tbs.p, b.tbs.data(), b.tbs.size() * sizeof(DevTb));
     launch_pusch(c, h->d_ulgrants.p, ng, max_M, b.max_scr_words, h->d_ulsym.p, h->d_ulpool.p, h->d_ulpool.p, h->d_gold_x1, h->d_gold_basis, h->gold_words,
                  h->d_seq.p, h->d_pllr.p, h->d_ulchest.p, h->stream, &h->launches);
+    CU(cudaGetLastError()); // as in ltephy_submit_grants
     if (int r = decode_code_blocks(h)) return r;
   }
   CU(cudaEventRecord(h->ev[3], h->stream));

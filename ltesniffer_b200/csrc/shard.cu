@@ -6,6 +6,7 @@
 #include "../../include/ltephy_shard.h"
 #include "ltephy_internal.cuh"
 #include "tb_merge.hpp"
+#include <atomic>
 #include <chrono>
 #include <condition_variable>
 #include <dlfcn.h>
@@ -151,16 +152,13 @@ struct TurnGuard { // a turn is always taken and given back exactly once, also o
     t.take(seq);
     state = 1;
   }
-  void give()
+  void give() // a section this batch skips (the gather at world size 1) still has to pass its turn on
   {
+    if (state == 0) take();
     if (state == 1) t.give();
     state = 2;
   }
-  ~TurnGuard()
-  {
-    if (state == 0) t.take(seq), state = 1;
-    give();
-  }
+  ~TurnGuard() { give(); }
 };
 
 struct TbMeta { // one per result slot (2 per grant) of the sending rank
@@ -208,7 +206,7 @@ struct ltephy_shard {
   uint32_t     gather_bytes_per_sf = 24576; // fixed payload capacity of one rank's gather message, per subframe of the batch
   std::mutex   slots_mtx;
   std::map<ltephy_t*, Slot*> slots;
-  bool         failed = false;
+  std::atomic<bool> failed{false}; // set and read by the pipelines' threads
   Slot*        slot_of(ltephy_t* h)
   {
     std::lock_guard<std::mutex> lk(slots_mtx);
@@ -320,9 +318,9 @@ extern "C" int ltephy_decode_subframes_sharded(ltephy_shard_t* sh, ltephy_t* h, 
                                                uint32_t n, uint64_t seq, ltephy_sf_info_t* info, ltephy_dci_t* dcis, uint32_t max_dcis, uint32_t* n_dcis,
                                                ltephy_tb_result_t* tbs, uint8_t* payload, size_t payload_cap, ltephy_shard_stats_t* stats)
 {
-  if (!sh || !h || !s || !iq || !tti || !info || !dcis || !n_dcis || !tbs || n == 0) return fail(LTEPHY_ERROR_INVALID_INPUTS, "decode_subframes_sharded: bad arguments");
+  if (!sh) return fail(LTEPHY_ERROR_INVALID_INPUTS, "decode_subframes_sharded: bad arguments");
   const uint32_t W = sh->world, R = sh->rank;
-  // the three ordered sections of this batch; the guards keep the order intact on every exit path
+  // the ordered sections of this batch; the guards keep the order intact on every exit path, a refused argument list included
   TurnGuard gx(sh->turn_x, seq), gf(sh->turn_f, seq), gw(sh->turn_w, seq), gg(sh->turn_g, seq);
   if (sh->failed) return fail(LTEPHY_ERROR, "decode_subframes_sharded: an earlier batch failed on this rank");
   struct FailMark {
@@ -333,6 +331,7 @@ extern "C" int ltephy_decode_subframes_sharded(ltephy_shard_t* sh, ltephy_t* h, 
       if (!ok) sh->failed = true;
     }
   } mark{sh};
+  if (!h || !s || !iq || !tti || !info || !dcis || !n_dcis || !tbs || n == 0) return fail(LTEPHY_ERROR_INVALID_INPUTS, "decode_subframes_sharded: bad arguments");
   CU(cudaSetDevice(sh->device));
   Slot*  sl = sh->slot_of(h);
   double t[10];

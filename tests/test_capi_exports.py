@@ -36,6 +36,11 @@ def test_invalid_inputs_are_rejected(phylib):
     cfg = capi.Cfg(nof_prb=6, nof_ports=1, cell_id=0, nof_rx=1, max_subframes=1)
     assert phylib.ltephy_create(C.byref(cfg), C.byref(h)) == -2   # LTEPHY_ERROR_INVALID_INPUTS (falcon_pdcch.c:121 convention)
     assert phylib.ltephy_create(None, C.byref(h)) == -2
+    # the front end's grids put the subframe on gridDim.y / z (at most 65 535): refused before any device is looked for
+    for ms in (65536, 100000, 0xFFFFFFFF):
+        cfg = capi.Cfg(nof_prb=25, nof_ports=1, cell_id=0, nof_rx=1, max_subframes=ms)
+        assert phylib.ltephy_create(C.byref(cfg), C.byref(h)) == -2
+        assert b"max_subframes" in phylib.ltephy_last_error()
 
 
 def test_srsran_compat_shim_exports(phylib):

@@ -4,6 +4,8 @@ against one GPU decoding the whole capture: rank 0 must end up with the same DCI
 import ctypes as C
 import os
 import sys
+import threading
+import time
 import numpy as np
 import pytest
 
@@ -28,7 +30,8 @@ def _tb_table(dcis, tbs, payload):
     return out
 
 
-def _sharded_decode(capi, shard, phy, srch, iq, tti, seq, max_dcis, world):
+def _sharded_call(capi, shard, phy, srch, iq, tti, seq, max_dcis, world, tbs_null=False):
+    """-> (return code, last error of this thread, info, dcis, tbs, payload, stats)"""
     L = phy.L
     capi._bind_search(L)
     n = len(tti)
@@ -41,10 +44,73 @@ def _sharded_decode(capi, shard, phy, srch, iq, tti, seq, max_dcis, world):
     nd = C.c_uint32(0)
     st = capi.ShardStats()
     r = L.ltephy_decode_subframes_sharded(shard.h, phy.h, srch.h, iq.ctypes.data_as(C.c_void_p), 0, tti.ctypes.data_as(C.c_void_p), n, seq, info,
-                                          dcis.ctypes.data_as(C.c_void_p), max_dcis, C.byref(nd), tbs, payload.ctypes.data_as(C.c_void_p), payload.nbytes,
-                                          C.byref(st))
-    assert r == 0, L.ltephy_last_error().decode()
-    return info, dcis[:nd.value], tbs, payload, st
+                                          dcis.ctypes.data_as(C.c_void_p), max_dcis, C.byref(nd), None if tbs_null else tbs,
+                                          payload.ctypes.data_as(C.c_void_p), payload.nbytes, C.byref(st))
+    return r, L.ltephy_last_error().decode(), info, dcis[:nd.value], tbs, payload, st
+
+
+def _sharded_decode(capi, shard, phy, srch, iq, tti, seq, max_dcis, world):
+    r, err, info, dcis, tbs, payload, st = _sharded_call(capi, shard, phy, srch, iq, tti, seq, max_dcis, world)
+    assert r == 0, err
+    return info, dcis, tbs, payload, st
+
+
+def _join_all(threads, timeout_s=60.0):
+    """daemon threads joined with one deadline: a turn never given back fails the test instead of hanging it"""
+    deadline = time.time() + timeout_s
+    for t in threads:
+        t.join(max(0.0, deadline - time.time()))
+    assert not any(t.is_alive() for t in threads), "a pipeline never finished: an ordered section was not given back"
+
+
+def _three_pipelines_on_one_shard(capi, cell, sh, srch, iq, tti, ref_dcis, ref_table, T):
+    """T host threads, one handle each, on one Shard of world size 1 (thread t takes batches t, t + T, ... with seq = batch index), against the
+    unsharded serial decode.  Then a batch refused for a NULL argument: it takes and gives back every turn and marks the rank failed, so the
+    batches after it return at once with the rank-failed error."""
+    sizes = [3, 3, 3, 3, 2, 2]
+    lo = np.cumsum([0] + sizes)
+    phys = [capi.LtePhy(cell.nof_prb, cell.nof_ports, cell.cell_id, cell.nof_rx, max_subframes=max(sizes), turbo_max_iter=8, flags=capi.FLAG_SKIP_LOW_POWER)
+            for _ in range(T)]
+    out, errs = {}, []
+
+    def worker(t, seqs, **kw):
+        try:
+            for k in seqs:
+                a, b = (int(lo[k]), int(lo[k + 1])) if k < len(sizes) else (0, sizes[0])
+                out[k] = _sharded_call(capi, sh, phys[t], srch, iq[a:b], tti[a:b], k, 32 * 16, 1, **kw)
+        except BaseException as e:  # noqa: B902 -- handed to the main thread
+            errs.append(e)
+
+    th = [threading.Thread(target=worker, args=(t, range(t, len(sizes), T)), daemon=True) for t in range(T)]
+    for x in th:
+        x.start()
+    _join_all(th)
+    assert not errs, errs
+    got, table = [], []
+    for k in range(len(sizes)):
+        r, err, info, dcis, tbs, pl, st = out[k]
+        assert r == 0, (k, err)
+        got += [(d[0] + int(lo[k]),) + d[1:] for d in (_key(d) for d in dcis)]
+        table += _tb_table(dcis, tbs, pl)
+    assert got == [_key(d) for d in ref_dcis]
+    assert table == ref_table
+    # the refused batch (seq 6), then two more from two threads
+    k = len(sizes)
+    th = [threading.Thread(target=worker, args=(0, [k]), kwargs=dict(tbs_null=True), daemon=True)]
+    th[0].start()
+    _join_all(th)
+    assert out[k][0] == -2, out[k][:2]                                       # LTEPHY_ERROR_INVALID_INPUTS
+    th = [threading.Thread(target=worker, args=(t, [k + t]), daemon=True) for t in (1, 2)]
+    t0 = time.time()
+    for x in th:
+        x.start()
+    _join_all(th)
+    assert not errs, errs
+    for j in (k + 1, k + 2):
+        assert out[j][0] == -1 and "an earlier batch failed on this rank" in out[j][1], out[j][:2]   # LTEPHY_ERROR
+    assert time.time() - t0 < 10.0
+    for p in phys:
+        p.close()
 
 
 def test_pack_kernel_matches_host_restatement(infra, phylib):
@@ -67,18 +133,22 @@ def test_pack_kernel_matches_host_restatement(infra, phylib):
     phy.close()
 
 
-def test_sharded_one_rank_equals_single_gpu_pipeline(infra, phylib):
+def _one_rank_setup(n):
+    """a capture of n subframes, its unsharded serial decode, a Shard of world size 1 and a fresh search"""
     import ltelib
     from helpers import make_capture
     from ltesniffer_b200 import capi
     cell = ltelib.Cell(*CELL)
-    n = 16
     sim, iq, tti, truths, payloads = make_capture(cell, n, **SIM_KW)
     phy = capi.LtePhy(cell.nof_prb, cell.nof_ports, cell.cell_id, cell.nof_rx, max_subframes=n, turbo_max_iter=8, flags=capi.FLAG_SKIP_LOW_POWER)
     ref_info, ref_dcis, ref_tbs, ref_pl = capi.decode_subframes(phy, capi.Search(*CELL), iq, tti)
-    ref_table = _tb_table(ref_dcis, ref_tbs, ref_pl)
     sh = capi.Shard(capi.Shard.unique_id(), 0, 1, 0)
-    srch = capi.Search(*CELL)
+    return capi, cell, iq, tti, phy, ref_info, ref_dcis, _tb_table(ref_dcis, ref_tbs, ref_pl), sh, capi.Search(*CELL)
+
+
+def test_sharded_one_rank_equals_single_gpu_pipeline(infra, phylib):
+    n = 16
+    capi, cell, iq, tti, phy, ref_info, ref_dcis, ref_table, sh, srch = _one_rank_setup(n)
     # two consecutive batches through the ordered sections (seq 0, 1): the second continues the RNTI history of the first
     info, dcis, tbs, pl, st = _sharded_decode(capi, sh, phy, srch, iq[:8], tti[:8], 0, 32 * n, 1)
     info2, dcis2, tbs2, pl2, st2 = _sharded_decode(capi, sh, phy, srch, iq[8:], tti[8:], 1, 32 * n, 1)
@@ -88,6 +158,13 @@ def test_sharded_one_rank_equals_single_gpu_pipeline(infra, phylib):
     assert sum(t[0] for t in ref_table) >= 4
     assert [info[i].snr_db for i in range(8)] == [ref_info[i].snr_db for i in range(8)]
     assert st.exchanged_bytes > 0 and st.used_full_table == 0
+    sh.close()
+    phy.close()
+
+
+def test_sharded_one_rank_three_threads_and_a_refused_batch(infra, phylib):
+    capi, cell, iq, tti, phy, ref_info, ref_dcis, ref_table, sh, srch = _one_rank_setup(16)
+    _three_pipelines_on_one_shard(capi, cell, sh, srch, iq, tti, ref_dcis, ref_table, 3)
     sh.close()
     phy.close()
 
