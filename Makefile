@@ -41,8 +41,11 @@ examples/decode_recording: examples/decode_recording.cpp include/ltephy_b200.h i
 examples/decode_recording_ul: examples/decode_recording_ul.cpp include/ltephy_b200.h include/ltephy_search.h include/ltephy_sinks.h
 	$(CXX) -O2 -std=c++17 -Wall -Iinclude -o $@ examples/decode_recording_ul.cpp -Lltesniffer_b200 -lltephy_b200 -Wl,-rpath,'$$ORIGIN/../ltesniffer_b200'
 
-examples/compat_check: examples/compat_check.cpp compat/srsran/srsran.h include/ltephy_b200.h
+examples/compat_check: examples/compat_check.cpp compat/srsran/srsran.h compat/ltephy_compat_ext.h include/ltephy_b200.h
 	$(CXX) -O2 -std=c++17 -Wall -Iinclude -Icompat -o $@ examples/compat_check.cpp -Lltesniffer_b200 -lltephy_srsran_compat -lltephy_b200 -Wl,-rpath,'$$ORIGIN/../ltesniffer_b200'
 
+examples/compat_ul_check: examples/compat_ul_check.cpp compat/srsran/srsran.h include/ltephy_b200.h
+	$(CXX) -O2 -std=c++17 -Wall -Iinclude -Icompat -o $@ examples/compat_ul_check.cpp -Lltesniffer_b200 -lltephy_srsran_compat -lltephy_b200 -Wl,-rpath,'$$ORIGIN/../ltesniffer_b200'
+
 clean:
-	rm -f sim/*.so oracle/*.so oracle_track/*.so examples/offline_decode examples/offline_ul examples/compat_check examples/cell_search examples/decode_recording examples/decode_recording_ul
+	rm -f sim/*.so oracle/*.so oracle_track/*.so examples/offline_decode examples/offline_ul examples/compat_check examples/compat_ul_check examples/cell_search examples/decode_recording examples/decode_recording_ul

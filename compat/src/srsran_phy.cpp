@@ -9,10 +9,18 @@
 #include <cmath>
 #include <cstddef>
 #include <cstring>
+#include <unordered_map>
 #include <vector>
 
 namespace {
 typedef struct { float re, im; } cfx_t; // layout of cf_t
+// One slot of the handle's HARQ store per soft-buffer object: the slot holds the soft values of the transmissions decoded into the
+// buffer since its identity (b200_id, renewed by every reset) last changed.
+struct HarqSlot {
+  const srsran_softbuffer_rx_t* buf;
+  uint64_t                      id;       // b200_id of the last decode into this slot
+  uint64_t                      last_use; // for least-recently-used replacement when every slot is taken
+};
 struct DlPriv {
   ltephy_t*                  phy = nullptr;
   cf_t*                      in[SRSRAN_MAX_PORTS]{};
@@ -27,6 +35,12 @@ struct DlPriv {
   uint32_t                   cur_cfi = 0;
   bool                       injected = false;
   ltephy_sf_info_t           inj_info{};
+  uint32_t                   harq_cap = LTEPHY_COMPAT_HARQ_SLOTS;
+  bool                       harq_reserved = false; // the store of phy holds harq_cap slots
+  std::vector<HarqSlot>      harq;                  // slots in use, by slot index
+  std::unordered_map<const srsran_softbuffer_rx_t*, uint32_t> harq_of;
+  uint64_t                   harq_clock = 0;
+  void clear_harq() { harq.clear(), harq_of.clear(), harq_clock = 0; }
 };
 DlPriv* P(srsran_ue_dl_t* q) { return q ? static_cast<DlPriv*>(q->b200) : nullptr; }
 
@@ -38,6 +52,7 @@ struct UlPriv {
   // result of the last srsran_chest_ul_estimate_pusch (the GPU decodes the grant in the same pass)
   bool               have = false, fft_done = false;
   ltephy_ul_grant_t  grant{};
+  uint32_t           tti = 0;
   ltephy_tb_result_t res{};
   ltephy_ul_chest_t  chest{};
   srsran_refsignal_dmrs_pusch_cfg_t dmrs{};
@@ -63,6 +78,7 @@ int srsran_ue_dl_set_cell(srsran_ue_dl_t* q, srsran_cell_t cell)
   if (!p || cell.cp != SRSRAN_CP_NORM || cell.nof_prb < 15 || cell.nof_prb > 100 || cell.nof_ports < 1 || cell.nof_ports > 2) return SRSRAN_ERROR_INVALID_INPUTS;
   if ((uint32_t)cell.phich_length > 1 || (uint32_t)cell.phich_resources > 3) return SRSRAN_ERROR_INVALID_INPUTS;
   if (p->phy) ltephy_destroy(p->phy), p->phy = nullptr;
+  p->harq_reserved = false, p->clear_harq(); // the store went with the handle: every soft buffer starts empty again
   // geometry from the host tables only: the CUDA handle is created with the first subframe that is really decoded, so a search
   // fed with ltephy_compat_inject needs no GPU
   const ltehost::Cell hc{cell.nof_prb, cell.nof_ports, cell.id, q->nof_rx_antennas, (uint32_t)cell.phich_resources, (uint32_t)cell.phich_length};
@@ -104,6 +120,35 @@ void srsran_ue_dl_free(srsran_ue_dl_t* q)
 }
 void srsran_ue_dl_set_rnti(srsran_ue_dl_t* q, uint16_t rnti) { if (q) q->pregen_rnti = rnti; }
 ltephy_t* ltephy_compat_phy(srsran_ue_dl_t* q) { return P(q) ? P(q)->phy : nullptr; }
+int ltephy_compat_harq_slots(srsran_ue_dl_t* q, uint32_t nslots)
+{
+  DlPriv* p = P(q);
+  if (!p || nslots == 0) return SRSRAN_ERROR_INVALID_INPUTS;
+  p->harq_cap = nslots, p->harq_reserved = false, p->clear_harq();
+  return SRSRAN_SUCCESS;
+}
+// LTEPHY_HARQ_* for soft buffer b of one TB, and the slot it uses; see ltephy_compat_ext.h for the rules
+static uint8_t harq_slot_of(DlPriv* p, const srsran_softbuffer_rx_t* b, uint32_t* slot)
+{
+  if (!b) return LTEPHY_HARQ_NONE;
+  auto     it = p->harq_of.find(b);
+  uint32_t s;
+  uint8_t  op = LTEPHY_HARQ_NEW;
+  if (it != p->harq_of.end()) {
+    s = it->second;
+    if (p->harq[s].id == b->b200_id) op = LTEPHY_HARQ_RETX;
+  } else if (p->harq.size() < p->harq_cap) {
+    s = (uint32_t)p->harq.size(), p->harq.push_back(HarqSlot{});
+  } else { // every slot taken: the least recently decoded buffer gives its slot up and starts empty at its next decode
+    s = 0;
+    for (uint32_t i = 1; i < p->harq.size(); i++)
+      if (p->harq[i].last_use < p->harq[s].last_use) s = i;
+    p->harq_of.erase(p->harq[s].buf);
+  }
+  p->harq_of[b] = s, p->harq[s] = HarqSlot{b, b->b200_id, ++p->harq_clock};
+  *slot = s;
+  return op;
+}
 
 static void publish(srsran_ue_dl_t* q, DlPriv* p, srsran_dl_sf_cfg_t* sf)
 {
@@ -161,8 +206,13 @@ int srsran_ue_dl_decode_fft_estimate_noguru(srsran_ue_dl_t* q, srsran_dl_sf_cfg_
 {
   DlPriv* p = P(q);
   if (!p || !input) return SRSRAN_ERROR_INVALID_INPUTS;
+  // input serves this call only: the next srsran_ue_dl_decode_fft_estimate reads the buffers of srsran_ue_dl_init again
+  cf_t* keep[SRSRAN_MAX_PORTS];
+  memcpy(keep, p->in, sizeof(keep));
   for (uint32_t a = 0; a < q->nof_rx_antennas; a++) p->in[a] = input[a];
-  return srsran_ue_dl_decode_fft_estimate(q, sf, cfg);
+  const int r = srsran_ue_dl_decode_fft_estimate(q, sf, cfg);
+  memcpy(p->in, keep, sizeof(keep));
+  return r;
 }
 // srsran_pdcch_dci_decode (lib/src/phy/falcon_phch/falcon_pdcch.c:142): (location, payload size) -> entry of the GPU's table
 int srsran_pdcch_dci_decode(srsran_pdcch_t* pd, float* e, uint8_t* data, uint32_t E, uint32_t nof_bits, uint16_t* crc)
@@ -211,6 +261,17 @@ int srsran_ue_dl_decode_pdsch(srsran_ue_dl_t* q, srsran_dl_sf_cfg_t* sf, srsran_
   }
   if (s.tb[0].enabled && s.tb[1].enabled) // srsran_ra_tb_t.cw_idx (dl_sniffer_pdsch.c:24): DCI 2/2A swap flag
     g.tb[0].cw_idx = (uint8_t)(s.tb[0].cw_idx & 1u), g.tb[1].cw_idx = (uint8_t)(s.tb[1].cw_idx & 1u);
+  // soft buffers of the enabled TBs (a disabled TB's pointer may be left over from an earlier grant, DL_Sniffer_PDSCH.cc:968-970)
+  const srsran_softbuffer_rx_t* sb[2] = {s.tb[0].enabled ? cfg->softbuffers.rx[0] : nullptr, s.tb[1].enabled ? cfg->softbuffers.rx[1] : nullptr};
+  if (sb[1] == sb[0]) sb[1] = nullptr; // one buffer cannot hold both TBs: the second decodes without combining
+  if ((sb[0] || sb[1]) && !p->harq_reserved) {
+    if (ltephy_harq_reserve(p->phy, p->harq_cap) != LTEPHY_SUCCESS) return SRSRAN_ERROR;
+    p->harq_reserved = true, p->clear_harq();
+  }
+  for (int t = 0; t < 2; t++) {
+    uint32_t slot = 0;
+    g.tb[t].harq_op = harq_slot_of(p, sb[t], &slot), g.tb[t].harq_slot = slot;
+  }
   if (ltephy_submit_grants(p->phy, &g, 1) != LTEPHY_SUCCESS) return SRSRAN_ERROR;
   ltephy_tb_result_t   r[2]{};
   std::vector<uint8_t> pl(2 * 16000);
@@ -219,7 +280,7 @@ int srsran_ue_dl_decode_pdsch(srsran_ue_dl_t* q, srsran_dl_sf_cfg_t* sf, srsran_
     if (!r[t].payload_len) continue;
     data[t].crc = r[t].crc != 0, data[t].avg_iterations_block = (float)r[t].avg_iters;
     if (data[t].payload) memcpy(data[t].payload, pl.data() + r[t].payload_off, r[t].payload_len);
-    if (cfg->softbuffers.rx[t]) cfg->softbuffers.rx[t]->tb_crc = data[t].crc;
+    if (sb[t]) cfg->softbuffers.rx[t]->tb_crc = data[t].crc;
   }
   return SRSRAN_SUCCESS;
 }
@@ -282,7 +343,7 @@ void srsran_enb_ul_fft(srsran_enb_ul_t* q)
   ltephy_get_ul(u->phy, &r, nullptr, nullptr, 0);
   ltephy_tap(u->phy, LTEPHY_TAP_UL_SYM, u->sym.data(), u->sym.size() * sizeof(cfx_t));
 }
-static int run_pusch(srsran_enb_ul_t* q, UlPriv* u, srsran_ul_sf_cfg_t* sf, srsran_pusch_cfg_t* cfg)
+static ltephy_ul_grant_t ul_grant_of(const srsran_pusch_cfg_t* cfg)
 {
   const srsran_pusch_grant_t& s = cfg->grant;
   static const uint8_t dmrs2_map[8] = {0, 6, 3, 4, 2, 8, 10, 9}; // 36.211 Table 5.5.2.1.1-1
@@ -291,13 +352,19 @@ static int run_pusch(srsran_enb_ul_t* q, UlPriv* u, srsran_ul_sf_cfg_t* sf, srsr
   g.L_prb = s.L_prb, g.n_prb = s.n_prb[0], g.n_prb_slot1 = s.n_prb[1], g.flags = LTEPHY_UL_FLAG_SLOT1, g.n_dmrs2 = dmrs2_map[s.n_dmrs & 7], g.tbs = s.tb.tbs;
   g.nof_ack = cfg->uci_cfg.ack[0].nof_acks, g.cqi_len = 0, g.ri_len = cfg->uci_cfg.cqi.ri_len;
   g.I_offset_ack = cfg->uci_offset.I_offset_ack, g.I_offset_cqi = cfg->uci_offset.I_offset_cqi, g.I_offset_ri = cfg->uci_offset.I_offset_ri;
-  if (cfg->uci_cfg.cqi.data_enable) g.cqi_len = (uint32_t)srsran_cqi_size(&cfg->uci_cfg.cqi);
-  const uint32_t tti = sf ? sf->tti : 0;
+  srsran_cqi_cfg_t cqi = cfg->uci_cfg.cqi;
+  if (cqi.data_enable) g.cqi_len = (uint32_t)srsran_cqi_size(&cqi);
+  return g;
+}
+static int run_pusch(srsran_enb_ul_t* q, UlPriv* u, srsran_ul_sf_cfg_t* sf, srsran_pusch_cfg_t* cfg)
+{
+  const ltephy_ul_grant_t g   = ul_grant_of(cfg);
+  const uint32_t          tti = sf ? sf->tti : 0;
   // the symbols of srsran_enb_ul_fft stay on the device: only the grant travels
   if (ltephy_submit_ul(u->phy, u->fft_done ? nullptr : reinterpret_cast<const float*>(q->in_buffer), &tti, 1, &g, 1) != LTEPHY_SUCCESS) return SRSRAN_ERROR;
   u->fft_done = true;
   if (ltephy_get_ul(u->phy, &u->res, &u->chest, u->payload.data(), u->payload.size()) != LTEPHY_SUCCESS) return SRSRAN_ERROR;
-  u->grant = g, u->have = true;
+  u->grant = g, u->tti = tti, u->have = true;
   return SRSRAN_SUCCESS;
 }
 // srsran_chest_ul_estimate_pusch (UL_Sniffer_PUSCH.cc:256): DMRS estimate of the grant; the GPU pass that produces it also decodes the
@@ -314,12 +381,12 @@ int srsran_chest_ul_estimate_pusch(srsran_chest_ul_t* c, srsran_ul_sf_cfg_t* sf,
   res->snr_db = u->chest.snr_db, res->snr = powf(10.0f, u->chest.snr_db / 10.0f), res->ta_us = u->chest.ta_us, res->nof_re = 12 * cfg->grant.L_prb * 12;
   return SRSRAN_SUCCESS;
 }
-static bool same_grant(const ltephy_ul_grant_t& a, const srsran_pusch_cfg_t* cfg)
+// the estimate's pass decoded exactly the grant run_pusch would build for cfg, in the same TTI
+static_assert(sizeof(ltephy_ul_grant_t) == 36, "ltephy_ul_grant_t has padding: same_grant cannot memcmp it");
+static bool same_grant(const UlPriv* u, const srsran_ul_sf_cfg_t* sf, const srsran_pusch_cfg_t* cfg)
 {
-  const srsran_pusch_grant_t& s = cfg->grant;
-  return a.rnti == cfg->rnti && a.L_prb == s.L_prb && a.n_prb == s.n_prb[0] && a.n_prb_slot1 == s.n_prb[1] && a.tbs == s.tb.tbs &&
-         a.qm == ((unsigned)s.tb.mod < 5 ? QM_OF[s.tb.mod] : 0) && a.nof_ack == cfg->uci_cfg.ack[0].nof_acks && a.ri_len == cfg->uci_cfg.cqi.ri_len &&
-         (a.cqi_len != 0) == cfg->uci_cfg.cqi.data_enable;
+  const ltephy_ul_grant_t g = ul_grant_of(cfg); // value-initialised and free of padding: memcmp compares every field
+  return u->tti == (sf ? sf->tti : 0) && memcmp(&g, &u->grant, sizeof(g)) == 0;
 }
 int srsran_pusch_decode(srsran_pusch_t* pq, srsran_ul_sf_cfg_t* sf, srsran_pusch_cfg_t* cfg, srsran_chest_ul_res_t* channel, cf_t* sf_symbols, srsran_pusch_res_t* data)
 {
@@ -328,7 +395,7 @@ int srsran_pusch_decode(srsran_pusch_t* pq, srsran_ul_sf_cfg_t* sf, srsran_pusch
   srsran_enb_ul_t* q = static_cast<srsran_enb_ul_t*>(pq->b200);
   UlPriv*          u = U(q);
   if (!u || !u->phy) return SRSRAN_ERROR_INVALID_INPUTS;
-  if (!u->have || !same_grant(u->grant, cfg))
+  if (!u->have || !same_grant(u, sf, cfg))
     if (run_pusch(q, u, sf, cfg) != SRSRAN_SUCCESS) return SRSRAN_ERROR;
   data->crc = u->res.crc != 0, data->avg_iterations_block = (float)u->res.avg_iters;
   if (data->data && u->res.payload_len) memcpy(data->data, u->payload.data() + u->res.payload_off, u->res.payload_len);
