@@ -21,9 +21,9 @@ oracle/liblteosync.so: oracle/lte_sync_oracle.c oracle/lte_sync_oracle.h oracle/
 oracle/liblteomib.so: oracle/lte_mib_oracle.c oracle/lte_mib_oracle.h oracle/lte_oracle.h oracle/liblteoracle.so
 	$(CC) $(CFLAGS) -shared -o $@ oracle/lte_mib_oracle.c -Loracle -llteoracle -Wl,-rpath,'$$ORIGIN' -lm
 
-# tracker oracle: stand-alone
-oracle_track/liblteotrack.so: oracle_track/lte_track_oracle.c oracle_track/lte_track_oracle.h
-	$(CC) $(CFLAGS) -shared -o $@ oracle_track/lte_track_oracle.c -lm
+# tracker oracle: its find state (LTEO_TRACK_REACQUIRE) is lteo_cell_search of liblteosync.so
+oracle_track/liblteotrack.so: oracle_track/lte_track_oracle.c oracle_track/lte_track_oracle.h oracle/lte_sync_oracle.h oracle/liblteosync.so
+	$(CC) $(CFLAGS) -shared -o $@ oracle_track/lte_track_oracle.c -Loracle -llteosync -Wl,-rpath,'$$ORIGIN/../oracle' -lm
 
 # C++ example of the C-ABI (needs ltesniffer_b200/libltephy_b200.so, built by ltesniffer_b200/build.py)
 examples/offline_decode: examples/offline_decode.cpp include/ltephy_b200.h include/ltephy_search.h include/ltephy_sinks.h

@@ -5,7 +5,12 @@
 // the MAC-LTE pcap and the DCI trace exactly as offline_decode does, and prints the cell and a lock summary.  Host code only; without a GPU
 // ltephy_sync_create fails.
 //
-//   decode_recording <iq.cf32> <symbol_sz> <nof_rx> <out.pcap> <out_dci.tsv> [subframes_per_push=500] [max_ppm=50] [no_cfo=0]
+//   decode_recording <iq.cf32> <symbol_sz> <nof_rx> <out.pcap> <out_dci.tsv> [subframes_per_push=500] [max_ppm=50] [no_cfo=0] [reacquire=0]
+//
+// With reacquire = 1 the tracker searches a lost cell again (LTEPHY_TRACK_REACQUIRE), and the example falls back as the reference does from
+// DECODE_PDSCH to DECODE_MIB (src/src/LTESniffer_Core.cc:506-524): from the re-acquired subframe on it decodes nothing and feeds every
+// subframe 0 of the cut to the MIB decoder until one passes, then adds (mib.sfn - tti / 10) mod 1024 frames to every later tti, because
+// after dropped samples the tracker's SFN, which continues by sample count, is wrong.
 //
 // File layout: antenna after antenna, each a continuous run of complex float32 samples at 15 kHz * symbol_sz (what cell_search reads).  The
 // file is read one push at a time (one seek per antenna), so its length is not limited by host memory.
@@ -30,13 +35,14 @@ static bool read_span(FILE* f, uint32_t A, uint64_t L, uint64_t s, uint64_t n, s
 int main(int argc, char** argv)
 {
   if (argc < 6) {
-    fprintf(stderr, "usage: %s <iq.cf32> <symbol_sz> <nof_rx> <out.pcap> <out_dci.tsv> [subframes_per_push=500] [max_ppm=50] [no_cfo=0]\n", argv[0]);
+    fprintf(stderr, "usage: %s <iq.cf32> <symbol_sz> <nof_rx> <out.pcap> <out_dci.tsv> [subframes_per_push=500] [max_ppm=50] [no_cfo=0] [reacquire=0]\n", argv[0]);
     return 2;
   }
   const uint32_t N = (uint32_t)atoi(argv[2]), A = (uint32_t)atoi(argv[3]), SF = 15 * N;
   const uint32_t B       = argc > 6 ? (uint32_t)atoi(argv[6]) : 500;
   const float    max_ppm = argc > 7 ? (float)atof(argv[7]) : 50.0f;
   const int      no_cfo  = argc > 8 ? atoi(argv[8]) : 0;
+  const int      reacq   = argc > 9 ? atoi(argv[9]) : 0;
   FILE*          in      = fopen(argv[1], "rb");
   if (!in || A < 1 || A > 2 || B < 1) {
     fprintf(stderr, "cannot open %s / bad nof_rx or subframes_per_push\n", argv[1]);
@@ -125,12 +131,25 @@ int main(int argc, char** argv)
   ltephy_search_t*   search = ltephy_search_create(phy, 5); // rnti_histogram_threshold default of the reference
   ltephy_track_cfg_t tcfg{};
   tcfg.symbol_sz = N, tcfg.nof_rx = A, tcfg.pci = c->pci, tcfg.first_tti = 10 * mib.sfn, tcfg.frame_offset = c->frame_offset, tcfg.cfo_hz = c->cfo_hz;
-  tcfg.max_ppm = max_ppm, tcfg.max_subframes = B, tcfg.flags = no_cfo ? LTEPHY_TRACK_NO_CFO : 0;
+  tcfg.max_ppm = max_ppm, tcfg.max_subframes = B, tcfg.flags = (no_cfo ? LTEPHY_TRACK_NO_CFO : 0) | (reacq ? LTEPHY_TRACK_REACQUIRE : 0);
   ltephy_track_t* tr = nullptr;
   if (!search || ltephy_track_create(&tcfg, &tr) != LTEPHY_SUCCESS) {
     fprintf(stderr, "search / tracker: %s\n", ltephy_last_error());
     return 1;
   }
+  // the MIB decoder of the fallback: the cell's bandwidth and ports are known, so no port search; the cut is already CFO-corrected
+  ltephy_t* mibh = nullptr;
+  if (reacq) {
+    ltephy_cfg_t rcfg{};
+    rcfg.nof_prb = mib.nof_prb, rcfg.nof_ports = mib.nof_ports, rcfg.cell_id = c->pci, rcfg.nof_rx = A, rcfg.max_subframes = 1, rcfg.symbol_sz = N;
+    if (ltephy_create(&rcfg, &mibh) != LTEPHY_SUCCESS) {
+      fprintf(stderr, "ltephy_create: %s\n", ltephy_last_error());
+      return 1;
+    }
+  }
+  bool               awaiting = false; // between a re-acquired subframe and the next MIB that passes: decode nothing
+  uint32_t           sfn_corr = 0;     // frames added to every tti after the MIB read again
+  unsigned long long n_finds = 0, n_reacq = 0, n_await = 0;
   ltephy_pcap_t* pcap = ltephy_pcap_open(argv[4]);
   FILE*          tsv  = fopen(argv[5], "w");
   if (!pcap || !tsv) {
@@ -166,7 +185,7 @@ int main(int argc, char** argv)
       return 1;
     }
     next = o.next_sample;
-    n_remeasured += o.remeasured, n_hf += o.nof_half_frames;
+    n_remeasured += o.remeasured, n_hf += o.nof_half_frames, n_finds += o.finds;
     for (uint32_t i = 0; i < o.nof_half_frames; i++) n_hf_locked += (o.hf[i].flags & LTEPHY_TRACK_LOCKED) != 0;
     const uint32_t got = o.nof_subframes;
     if (!got) {
@@ -174,38 +193,73 @@ int main(int argc, char** argv)
       continue;
     }
     for (uint32_t i = 0; i < got; i++) {
-      ttis[i] = o.sf[i].tti;
+      ttis[i] = (o.sf[i].tti + 10 * sfn_corr) % 10240;
       n_locked += (o.sf[i].flags & LTEPHY_TRACK_LOCKED) != 0, n_lost += (o.sf[i].flags & LTEPHY_TRACK_LOST) != 0;
     }
     last_start = o.sf[got - 1].start, last_cfo = o.sf[got - 1].cfo_hz;
-    uint32_t nd = 0;
-    if (ltephy_decode_subframes_device(phy, search, o.iq_dev, ttis.data(), got, LTEPHY_SEQ_NONE, info.data(), scratch.data(), dcis.data(), max_dcis, &nd,
-                                       tbs.data(), payload.data(), payload.size()) != LTEPHY_SUCCESS) {
-      fprintf(stderr, "ltephy_decode_subframes_device: %s\n", ltephy_last_error());
-      return 1;
+    // the push as runs of subframes to decode, split where the MIB fallback starts and ends
+    const size_t sf_bytes = (size_t)A * SF * 8;
+    for (uint32_t i0 = 0; i0 < got;) {
+      if (awaiting || (o.sf[i0].flags & LTEPHY_TRACK_REACQUIRED)) {
+        if (o.sf[i0].flags & LTEPHY_TRACK_REACQUIRED) {
+          if (ltephy_mib_reset(mibh) != LTEPHY_SUCCESS) {
+            fprintf(stderr, "ltephy_mib_reset: %s\n", ltephy_last_error());
+            return 1;
+          }
+          awaiting = true, n_reacq++;
+        }
+        n_await++;
+        if (o.sf[i0].tti % 10 == 0) {
+          ltephy_mib_comb_t mc{};
+          if (ltephy_submit_iq_device(mibh, static_cast<const char*>(o.iq_dev) + i0 * sf_bytes, &o.sf[i0].tti, 1) != LTEPHY_SUCCESS ||
+              ltephy_mib_decode_combined(mibh, 0, &mc) != LTEPHY_SUCCESS) {
+            fprintf(stderr, "MIB decode: %s\n", ltephy_last_error());
+            return 1;
+          }
+          if (mc.mib.found) {
+            sfn_corr = (mc.mib.sfn + 1024 - o.sf[i0].tti / 10 % 1024) % 1024, awaiting = false;
+            for (uint32_t i = i0 + 1; i < got; i++) ttis[i] = (o.sf[i].tti + 10 * sfn_corr) % 10240;
+          }
+        }
+        i0++;
+        continue;
+      }
+      uint32_t i1 = i0 + 1;
+      while (i1 < got && !(o.sf[i1].flags & LTEPHY_TRACK_REACQUIRED)) i1++;
+      const uint32_t m = i1 - i0, base = (uint32_t)(n_sf + i0);
+      uint32_t       nd = 0;
+      if (ltephy_decode_subframes_device(phy, search, static_cast<const char*>(o.iq_dev) + i0 * sf_bytes, ttis.data() + i0, m, LTEPHY_SEQ_NONE, info.data(),
+                                         scratch.data(), dcis.data(), max_dcis, &nd, tbs.data(), payload.data(), payload.size()) != LTEPHY_SUCCESS) {
+        fprintf(stderr, "ltephy_decode_subframes_device: %s\n", ltephy_last_error());
+        return 1;
+      }
+      // timestamps: capture time, 1 ms per subframe cut (as offline_decode)
+      for (uint32_t i = 0; i < nd; i++) {
+        const uint32_t t = ttis[i0 + dcis[i].sf];
+        const int      n = ltephy_dci_trace_line(search, &dcis[i], t, info[dcis[i].sf].cfi, tbs[2 * i].crc == 2 || tbs[2 * i + 1].crc == 2, (base + dcis[i].sf) / 1000,
+                                                 ((base + dcis[i].sf) % 1000) * 1000, line, sizeof(line));
+        if (n > 0) fwrite(line, 1, (size_t)n, tsv);
+        for (int k = 0; k < 2; k++) n_tb += tbs[2 * i + k].payload_len > 0, n_ok += tbs[2 * i + k].crc != 0;
+      }
+      if (ltephy_pcap_write_dl_batch(pcap, ttis.data() + i0, dcis.data(), nd, tbs.data(), payload.data(), 0, base / 1000, (base % 1000) * 1000) < 0) {
+        fprintf(stderr, "pcap write failed\n");
+        return 1;
+      }
+      n_dci += nd;
+      i0 = i1;
     }
-    // timestamps: capture time, 1 ms per subframe decoded (as offline_decode)
-    for (uint32_t i = 0; i < nd; i++) {
-      const uint32_t t = ttis[dcis[i].sf];
-      const int      n = ltephy_dci_trace_line(search, &dcis[i], t, info[dcis[i].sf].cfi, tbs[2 * i].crc == 2 || tbs[2 * i + 1].crc == 2, (uint32_t)((n_sf + dcis[i].sf) / 1000),
-                                               (uint32_t)(((n_sf + dcis[i].sf) % 1000) * 1000), line, sizeof(line));
-      if (n > 0) fwrite(line, 1, (size_t)n, tsv);
-      for (int k = 0; k < 2; k++) n_tb += tbs[2 * i + k].payload_len > 0, n_ok += tbs[2 * i + k].crc != 0;
-    }
-    if (ltephy_pcap_write_dl_batch(pcap, ttis.data(), dcis.data(), nd, tbs.data(), payload.data(), 0, (uint32_t)(n_sf / 1000), (uint32_t)((n_sf % 1000) * 1000)) < 0) {
-      fprintf(stderr, "pcap write failed\n");
-      return 1;
-    }
-    n_sf += got, n_dci += nd;
+    n_sf += got;
   }
   const long long drift = n_sf ? (long long)(last_start - (int64_t)c->frame_offset - (int64_t)(n_sf - 1) * SF) : 0;
   printf("tracking: subframes %llu locked %llu lost %llu  half-frames %llu locked %llu remeasured %llu  timing moved %lld samples  cfo_hz %.1f\n", n_sf,
          n_locked, n_lost, n_hf, n_hf_locked, n_remeasured, drift, last_cfo);
   printf("subframes %llu  dcis %llu  transport blocks %llu  crc ok %llu\n", n_sf, n_dci, n_tb, n_ok);
+  if (reacq) printf("reacquire: finds %llu reacquired %llu awaiting_mib %llu\n", n_finds, n_reacq, n_await);
   fclose(in), fclose(tsv);
   ltephy_pcap_close(pcap);
   ltephy_track_destroy(tr);
   ltephy_search_destroy(search);
   ltephy_destroy(phy);
+  if (mibh) ltephy_destroy(mibh);
   return 0;
 }

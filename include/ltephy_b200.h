@@ -300,7 +300,12 @@ int  ltephy_sync_tap(ltephy_sync_t* h, int what, void* dst, size_t bytes);
  * input ltephy_submit_iq_device / ltephy_decode_subframes_device take, with ltephy_set_cfo left at 0.  The rule and its summation orders are
  * DESIGN.md §2 ("tracking"); the CPU oracle lteo_track_* (oracle_track/) defines every record and cut sample bit for bit. */
 typedef struct ltephy_track ltephy_track_t;
-#define LTEPHY_TRACK_NO_CFO 1u /* keep cfo_hz at its initial value (the reference's disable_cfo) */
+#define LTEPHY_TRACK_NO_CFO    1u /* keep cfo_hz at its initial value (the reference's disable_cfo) */
+/* After 4 half-frames in a row without lock, search the cell again instead of cutting on: the find state of srsran_ue_sync_zerocopy.  The
+ * tracker steps through the recording one frame at a time (windows of 150 N + N samples, each searched once it has been fed) with the cell
+ * search of pci mod 3, cuts nothing meanwhile, and resumes at the first subframe boundary of the window where the cell is detected with this
+ * pci.  Subframe numbers come from the SSS; the SFN continues by sample count, so after dropped samples only the MIB gives it (DESIGN.md §2). */
+#define LTEPHY_TRACK_REACQUIRE 2u
 typedef struct {
   uint32_t symbol_sz;     /* N, as for ltephy_sync_cfg_t */
   uint32_t nof_rx;        /* 1 or 2 antennas */
@@ -316,11 +321,12 @@ typedef struct {
 } ltephy_track_cfg_t;
 #define LTEPHY_TRACK_LOCKED 1u /* subframe: the last half-frame measured before it was locked (or none was measured yet); half-frame: locked */
 #define LTEPHY_TRACK_LOST   2u /* 4 or more half-frames in a row were not locked */
+#define LTEPHY_TRACK_REACQUIRED 4u /* subframe: the first cut after the find state found the cell again (with LTEPHY_TRACK_LOCKED) */
 typedef struct {
   int64_t  start;  /* absolute first sample of the subframe as cut */
   uint32_t tti;
   float    cfo_hz; /* carrier offset it was corrected with */
-  uint32_t flags;  /* LTEPHY_TRACK_LOCKED / _LOST */
+  uint32_t flags;  /* LTEPHY_TRACK_LOCKED / _LOST / _REACQUIRED */
   uint32_t index;  /* subframe number since frame_offset */
 } ltephy_track_sf_t;
 typedef struct {
@@ -340,7 +346,7 @@ typedef struct {
   const void*              iq_dev;      /* cf32 [nof_subframes][nof_rx][15 N] in device memory, valid until the next push */
   uint64_t                 next_sample; /* the first absolute sample the next push must still include */
   uint32_t                 remeasured;  /* half-frames whose metric window had to be computed again (diagnostic) */
-  uint32_t                 reserved;
+  uint32_t                 finds;       /* find windows searched during this push (LTEPHY_TRACK_REACQUIRE) */
 } ltephy_track_out_t;
 int  ltephy_track_create(const ltephy_track_cfg_t* cfg, ltephy_track_t** h);
 void ltephy_track_destroy(ltephy_track_t* h);

@@ -797,8 +797,8 @@ class CellSearch:
 
 # ------------------------------------------------------------------------------------------------
 # tracking after acquisition (ltephy_track_*, include/ltephy_b200.h)
-TRACK_NO_CFO = 1
-TRACK_LOCKED, TRACK_LOST = 1, 2
+TRACK_NO_CFO, TRACK_REACQUIRE = 1, 2
+TRACK_LOCKED, TRACK_LOST, TRACK_REACQUIRED = 1, 2, 4
 
 
 class TrackCfg(C.Structure):
@@ -814,7 +814,7 @@ TRACK_HF_DTYPE = np.dtype([("tau", "<i8"), ("index", "<u4"), ("delta", "<i4"), (
 
 class TrackOut(C.Structure):
     _fields_ = [("nof_subframes", C.c_uint32), ("nof_half_frames", C.c_uint32), ("sf", C.c_void_p), ("hf", C.c_void_p), ("iq_dev", C.c_void_p),
-                ("next_sample", C.c_uint64), ("remeasured", C.c_uint32), ("reserved", C.c_uint32)]
+                ("next_sample", C.c_uint64), ("remeasured", C.c_uint32), ("finds", C.c_uint32)]
 
 
 class TrackUlCfg(C.Structure):
@@ -828,7 +828,8 @@ assert C.sizeof(TrackUlCfg) == 32
 class Tracker:
     """PSS tracking and subframe cutting of a recording after the cell search: push the recording part by part (antenna-major complex64
     [nof_rx][n] with its absolute first sample); each push returns the subframes that now lie wholly inside what was fed.  With ul=dict(cfo_ratio=..., ul_offset=...) the tracker also cuts the
-    uplink carrier of the same radio (ltephy_track_set_ul); push both carriers with push_ul / push_ul_device."""
+    uplink carrier of the same radio (ltephy_track_set_ul); push both carriers with push_ul / push_ul_device.  With flags=TRACK_REACQUIRE a
+    lost cell is searched again frame by frame; the first subframe cut after it is found carries TRACK_REACQUIRED."""
 
     def __init__(self, symbol_sz, nof_rx, pci, frame_offset, cfo_hz=0.0, first_tti=0, max_subframes=1000, max_ppm=50.0, flags=0, device=0, ul=None):
         self.L = load_library()
@@ -887,14 +888,14 @@ class Tracker:
             np.zeros(0, TRACK_HF_DTYPE)
         iq = self._view(o.iq_dev, (o.nof_subframes, self.cfg.nof_rx, 15 * self.cfg.symbol_sz))
         self.next_sample = o.next_sample
-        out = dict(sf=sf, hf=hf, iq=iq, next_sample=o.next_sample, remeasured=o.remeasured)
+        out = dict(sf=sf, hf=hf, iq=iq, next_sample=o.next_sample, remeasured=o.remeasured, finds=o.finds)
         if ul_ptr is not None:
             out["ul_iq"] = self._view(ul_ptr.value, (o.nof_subframes, 15 * self.cfg.symbol_sz))
         return out
 
     def push(self, iq, first_sample):
         """iq: complex64 [nof_rx][n] (host) of absolute samples first_sample ... -> dict(sf, hf: record arrays, iq: torch complex64
-        [k][nof_rx][15 N] on the device (a copy of the tracker's cut), next_sample, remeasured)"""
+        [k][nof_rx][15 N] on the device (a copy of the tracker's cut), next_sample, remeasured, finds)"""
         iq = np.ascontiguousarray(iq, np.complex64)
         assert iq.ndim == 2 and iq.shape[0] == self.cfg.nof_rx, iq.shape
         o = TrackOut()

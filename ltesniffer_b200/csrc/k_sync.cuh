@@ -2,6 +2,7 @@
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
+#include "../../include/ltephy_b200.h"
 
 #define SYNC_BINS 9600 // coarse bins per half-frame: 75 N / D
 
@@ -33,6 +34,9 @@ struct SyncSss {
 
 // host (sync.cu): d_u and the replica of N_ID_2 = u, returns E_p
 float sync_pss_replica(uint32_t N, uint32_t u, float2* d, float2* rep);
+// host (sync.cu): the cell search of the L samples x[a * lda + i] (device memory, i < L <= max_samples) on h's stream; blocks until out[3] is
+// written.  ltephy_cell_search_device is lda = L; the tracker's find state (track.cu) searches a window of its own buffer in place.
+int sync_run(ltephy_sync_t* h, const float2* x, uint64_t lda, uint64_t L, ltephy_cell_t* out);
 
 extern "C" int launch_sync_pss(const SyncArgs& g, float* m, float* fold, SyncPeak* pk, float* rm, float4* c12, float* refined, cudaStream_t st,
                                uint64_t* launches);

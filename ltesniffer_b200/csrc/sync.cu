@@ -148,12 +148,12 @@ static int sync_check(ltephy_sync_t* h, const void* iq, uint64_t L, ltephy_cell_
   return LTEPHY_SUCCESS;
 }
 
-static int sync_run(ltephy_sync_t* h, const float2* x, uint64_t L, ltephy_cell_t* out)
+int sync_run(ltephy_sync_t* h, const float2* x, uint64_t lda, uint64_t L, ltephy_cell_t* out)
 {
   const uint32_t N = h->N, D = h->D, CP6 = 9 * D;
   const uint64_t HF = 75ull * N, FR = 150ull * N;
   SyncArgs       g{};
-  g.x = x, g.lda = L, g.L = L, g.J = (L - N) / D + 1, g.N = N, g.D = D, g.A = h->A, g.nh = (uint32_t)((L - N) / HF + 1);
+  g.x = x, g.lda = lda, g.L = L, g.J = (L - N) / D + 1, g.N = N, g.D = D, g.A = h->A, g.nh = (uint32_t)((L - N) / HF + 1);
   g.rep = h->d_rep.p, g.W = h->d_W.p;
   for (int u = 0; u < 3; u++) g.ep[u] = h->ep[u];
   if (launch_sync_pss(g, h->d_m.p, h->d_fold.p, h->d_pk.p, h->d_rm.p, h->d_c12.p, h->d_ref.p, h->stream, &h->launches))
@@ -223,14 +223,14 @@ extern "C" int ltephy_cell_search(ltephy_sync_t* h, const float* iq, uint64_t no
   if (int r = sync_check(h, iq, nof_samples, out)) return r;
   CU(cudaSetDevice(h->cfg.device));
   CU(cudaMemcpyAsync(h->d_x.p, iq, (size_t)h->A * nof_samples * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
-  return sync_run(h, h->d_x.p, nof_samples, out);
+  return sync_run(h, h->d_x.p, nof_samples, nof_samples, out);
 }
 
 extern "C" int ltephy_cell_search_device(ltephy_sync_t* h, const void* iq_dev, uint64_t nof_samples, ltephy_cell_t out[3])
 {
   if (int r = sync_check(h, iq_dev, nof_samples, out)) return r;
   CU(cudaSetDevice(h->cfg.device));
-  return sync_run(h, static_cast<const float2*>(iq_dev), nof_samples, out);
+  return sync_run(h, static_cast<const float2*>(iq_dev), nof_samples, nof_samples, out);
 }
 
 extern "C" int ltephy_sync_tap(ltephy_sync_t* h, int what, void* dst, size_t bytes)

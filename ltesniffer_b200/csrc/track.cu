@@ -1,6 +1,7 @@
 // track.cu -- host side of the tracker (include/ltephy_b200.h, DESIGN.md §2 "tracking"): predicts the measurement windows of a push, runs the
 // metric kernel over them, replays the rule on its bit-exact results in the order lteo_track states it (measuring a window again when the
-// tracked position left the predicted one), then the CFO sums, the carrier-offset loop and the cut.
+// tracked position left the predicted one), then the CFO sums, the carrier-offset loop and the cut.  With LTEPHY_TRACK_REACQUIRE a loss
+// enters the find state: the cell search (sync.cu, k_sync.cu) on one frame of the push's own device buffer at a time.
 #include "../../include/ltephy_b200.h"
 #include "k_sync.cuh"
 #include "k_track.cuh"
@@ -30,6 +31,13 @@ struct ltephy_track {
   float    f = 0.0f, d = 0.0f, acc = 0.0f;
   uint32_t miss = 0, nhf = 0, ncor = 0, nl = 0;
   int64_t  sd = 0, sh = 0, shh = 0, shd = 0;
+  int64_t  base = 0; // start of subframe 0 of the drift estimate's grid: frame_offset, after a find s' - k' SF
+  // the find state (LTEPHY_TRACK_REACQUIRE): searching the window [f0, f0 + FR + N) predicted to start subframe kn
+  bool           find = false, reacq = false;
+  int64_t        f0 = 0;
+  uint32_t       kn = 0;
+  float          f_find = 0.0f; // the found carrier offset, installed at the re-acquired subframe in step 3
+  ltephy_sync_t* sync = nullptr;
   std::vector<ltephy_track_sf_t> sf;
   std::vector<ltephy_track_hf_t> hf;
   // the uplink carrier (ltephy_track_set_ul): one antenna cut at start + ul_off with its own rotation tables
@@ -41,7 +49,12 @@ struct ltephy_track {
 };
 
 // the lowest absolute sample the pending DL window, and with the uplink set its UL window, still needs
-static int64_t track_needed(const ltephy_track* h) { return h->ul && h->ul_off < 0 ? h->s + h->ul_off : h->s; }
+// in the find state, the window's first sample
+static int64_t track_needed(const ltephy_track* h)
+{
+  const int64_t s = h->find ? h->f0 : h->s;
+  return h->ul && h->ul_off < 0 ? s + h->ul_off : s;
+}
 
 // a subframe starting at s is cut only when its DL window, and with the uplink set its UL window, lie inside [first, end)
 static bool track_fits(const ltephy_track* h, int64_t s, uint64_t first, uint64_t end)
@@ -67,7 +80,7 @@ extern "C" int ltephy_track_create(const ltephy_track_cfg_t* cfg, ltephy_track_t
   if (!(std::fabs(cfg->cfo_hz) <= 7500.0f)) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_create: cfo_hz outside +-7500 Hz");
   if (!(cfg->max_ppm >= 0.0f && cfg->max_ppm <= 1000.0f)) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_create: max_ppm outside 0..1000");
   if (cfg->max_subframes < 1 || cfg->max_subframes > 20000) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_create: max_subframes outside 1..20000");
-  if (cfg->flags & ~LTEPHY_TRACK_NO_CFO) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_create: unknown flags 0x%x", cfg->flags);
+  if (cfg->flags & ~(LTEPHY_TRACK_NO_CFO | LTEPHY_TRACK_REACQUIRE)) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_create: unknown flags 0x%x", cfg->flags);
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail(LTEPHY_ERROR, "no CUDA device: this library has no CPU path");
   CU(cudaSetDevice(cfg->device));
@@ -83,8 +96,15 @@ extern "C" int ltephy_track_create(const ltephy_track_cfg_t* cfg, ltephy_track_t
   h->cfg = *cfg, h->N = N, h->A = cfg->nof_rx, h->W = 9 * N / 128, h->SF = 15 * N;
   h->max_ppm = cfg->max_ppm > 0.0f ? cfg->max_ppm : 50.0f;
   h->thr     = TRACK_LOCK_K / (float)N;
-  h->s = (int64_t)cfg->frame_offset, h->f = cfg->cfo_hz;
+  h->s = h->base = (int64_t)cfg->frame_offset, h->f = cfg->cfo_hz;
   CU(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
+  // the find's cell search: one window of a frame plus a symbol.  The handle's own sample buffer (A (150 N + N) samples, 4.9 MB at N = 2048
+  // with 2 antennas) stays unused: the find reads the push's samples in place through sync_run.
+  if (cfg->flags & LTEPHY_TRACK_REACQUIRE) {
+    ltephy_sync_cfg_t sc{};
+    sc.symbol_sz = N, sc.nof_rx = h->A, sc.max_samples = 151ull * N, sc.device = cfg->device;
+    if (int r = ltephy_sync_create(&sc, &h->sync)) return r;
+  }
   // the replica of N_ID_2 = pci mod 3 and its energy: the cell search's (sync.cu), as lteo_track_create computes them
   std::vector<float2> rep(N), d62(62);
   h->ep = sync_pss_replica(N, cfg->pci % 3, d62.data(), rep.data());
@@ -104,6 +124,7 @@ extern "C" void ltephy_track_destroy(ltephy_track_t* h)
   if (!h) return;
   cudaSetDevice(h->cfg.device);
   if (h->stream) cudaStreamSynchronize(h->stream);
+  ltephy_sync_destroy(h->sync);
   h->d_rep.release(), h->d_x.release(), h->d_cut.release(), h->d_tabA.release(), h->d_tabB.release(), h->d_c.release(), h->d_m.release();
   h->d_win.release(), h->d_pos.release(), h->d_start.release();
   h->d_xu.release(), h->d_cutu.release(), h->d_tabAu.release(), h->d_tabBu.release(), h->d_startu.release();
@@ -127,21 +148,52 @@ static int track_metrics(ltephy_track_t* h, const TrackArgs& g, const std::vecto
   return LTEPHY_SUCCESS;
 }
 
+// one find window (lteo_track's track_find): the cell search on the samples [f0, f0 + FR + N) of x, read in place; found: resume at the
+// window's first subframe boundary with the subframe number of its SSS, otherwise step one frame on
+static int track_find(ltephy_track_t* h, const float2* x, uint64_t first, uint64_t n, bool& found)
+{
+  const uint32_t N = h->N, SF = h->SF;
+  const uint64_t FR = 150ull * N;
+  CU(cudaStreamSynchronize(h->stream)); // the push's copy of x runs on the tracker's stream, the search on the sync handle's
+  ltephy_cell_t res[3];
+  if (int r = sync_run(h->sync, x + (h->f0 - (int64_t)first), n, FR + N, res)) return r;
+  const ltephy_cell_t* c = nullptr;
+  for (uint32_t i = 0; i < 3; i++)
+    if (res[i].n_id_2 == h->cfg.pci % 3) c = &res[i];
+  found = c->detected && c->pci == h->cfg.pci;
+  if (!found) {
+    h->f0 += (int64_t)FR, h->kn += 10;
+    return LTEPHY_SUCCESS;
+  }
+  const uint64_t fo   = c->frame_offset;
+  const uint32_t sfno = (uint32_t)((10 - fo / SF) % 10);
+  const uint32_t k    = h->kn + (sfno + 10 - (h->cfg.first_tti + h->kn) % 10) % 10;
+  h->s = h->f0 + (int64_t)(fo % SF), h->k = k, h->f_find = c->cfo_hz;
+  h->miss = 0, h->acc = 0.0f;
+  h->nl = 0, h->sd = h->sh = h->shh = h->shd = 0, h->ncor = 0;
+  h->base = h->s - (int64_t)k * SF, h->nhf = 0; // the drift d is kept: a clock does not change with a gap
+  h->find = false, h->reacq = true;
+  return LTEPHY_SUCCESS;
+}
+
 static int track_run(ltephy_track_t* h, const float2* x, const float2* xu, uint64_t first, uint64_t n, ltephy_track_out_t* out, const void** ul_iq_dev)
 {
   const uint32_t N = h->N, SF = h->SF, W = h->W, maxsf = h->cfg.max_subframes;
   const uint64_t end = first + n;
   TrackArgs      g{};
   g.x = x, g.lda = n, g.N = N, g.A = h->A, g.rep = h->d_rep.p, g.ep = h->ep;
-  // 1. predict: the subframes of this push from the state at its start, without corrections; each half-frame's window is the tracker's +-W
-  //    plus the distance a clock max_ppm off moves the start over the predicted span, clamped to the samples fed
+  // 1. predict: the subframes of this push from the state at its start (and again after a find), without corrections; each half-frame's
+  //    window is the tracker's +-W plus the distance a clock max_ppm off moves the start over the predicted span, clamped to the samples fed
   std::vector<TrackWin> win;
   std::vector<uint32_t> wk; // subframe number of each window
-  {
+  std::vector<float>    m;
+  uint32_t              stride = 0;
+  auto predict = [&]() -> int {
+    win.clear(), wk.clear();
     int64_t  ps  = h->s;
     float    pac = h->acc;
-    uint32_t pk = h->k, cnt = 0;
-    while (cnt < maxsf && track_fits(h, ps, first, end)) {
+    uint32_t pk = h->k, cnt = (uint32_t)h->sf.size();
+    while (!h->find && cnt < maxsf && track_fits(h, ps, first, end)) {
       if ((h->cfg.first_tti + pk) % 10240 % 5 == 0) {
         const int64_t tau = ps + 13 * N / 2 - (int64_t)first;
         const int64_t M   = (int64_t)std::ceil((double)h->max_ppm * 1e-6 * (double)(ps - h->s)) + 1; // half-width W + M
@@ -155,22 +207,36 @@ static int track_run(ltephy_track_t* h, const float2* x, const float2* xu, uint6
       ps            = ps + SF + (int64_t)r;
       pk++, cnt++;
     }
-  }
-  std::vector<float> m;
-  uint32_t           stride = 0;
-  if (int r = track_metrics(h, g, win, m, stride)) return r;
-  // 2. replay the timing rule (lteo_track_push) subframe by subframe; the carrier offset waits for the sums of step 3
+    return track_metrics(h, g, win, m, stride);
+  };
   h->sf.clear(), h->hf.clear();
+  if (int r = predict()) return r;
+  // 2. replay the timing rule (lteo_track_push) subframe by subframe; the carrier offset waits for the sums of step 3
   std::vector<uint64_t> spos, hpos;
-  uint32_t              remeasured = 0;
+  std::vector<float>    fre; // the found carrier offset of each re-acquired subframe
+  uint32_t              remeasured = 0, finds = 0;
   size_t                wi         = 0;
-  while (h->sf.size() < maxsf && track_fits(h, h->s, first, end)) {
+  while (h->sf.size() < maxsf) {
+    if (h->find) { // a window is searched once all of its samples have been fed
+      if ((uint64_t)h->f0 + 151ull * N > end) break;
+      bool found = false;
+      if (int r = track_find(h, x, first, n, found)) return r;
+      finds++;
+      if (found) {
+        if (int r = predict()) return r;
+        wi = 0;
+      }
+      continue;
+    }
+    if (!track_fits(h, h->s, first, end)) break;
     const uint32_t    tti = (h->cfg.first_tti + h->k) % 10240;
     ltephy_track_sf_t o{};
     o.start = h->s, o.tti = tti, o.index = h->k;
-    o.flags = (h->miss == 0 ? LTEPHY_TRACK_LOCKED : 0) | (h->miss >= TRACK_MISS ? LTEPHY_TRACK_LOST : 0);
+    o.flags = (h->miss == 0 ? LTEPHY_TRACK_LOCKED : 0) | (h->miss >= TRACK_MISS ? LTEPHY_TRACK_LOST : 0) | (h->reacq ? LTEPHY_TRACK_REACQUIRED : 0);
+    if (h->reacq) fre.push_back(h->f_find), h->reacq = false;
     h->sf.push_back(o);
     spos.push_back((uint64_t)(h->s - (int64_t)first));
+    bool lost_now = false;
     if (tti % 5 == 0) {
       ltephy_track_hf_t q{};
       q.tau = h->s + 13 * N / 2, q.index = h->k;
@@ -208,13 +274,13 @@ static int track_run(ltephy_track_t* h, const float2* x, const float2* xu, uint6
             const int64_t num = P * h->shd - h->sh * h->sd, den = P * h->shh - h->sh * h->sh;
             h->d = h->d + (float)num / (float)den;
           } else {
-            const int64_t moved = h->s - (int64_t)h->cfg.frame_offset - (int64_t)h->k * SF;
+            const int64_t moved = h->s - h->base - (int64_t)h->k * SF;
             h->d = (float)moved / ((float)h->nhf - 0.5f * (float)(P - 1));
           }
           h->nl = 0, h->sd = h->sh = h->shh = h->shd = 0;
         }
       } else
-        h->miss++;
+        lost_now = ++h->miss == TRACK_MISS;
       if (h->miss >= TRACK_MISS) q.flags |= LTEPHY_TRACK_LOST;
       h->hf.push_back(q);
       hpos.push_back(tau + best);
@@ -224,6 +290,7 @@ static int track_run(ltephy_track_t* h, const float2* x, const float2* xu, uint6
     h->acc        = h->acc - r;
     h->s          = h->s + SF + (int64_t)r;
     h->k++;
+    if (lost_now && (h->cfg.flags & LTEPHY_TRACK_REACQUIRE)) h->find = true, h->f0 = h->s, h->kn = h->k;
   }
   const uint32_t nsf = (uint32_t)h->sf.size(), nh = (uint32_t)h->hf.size();
   // 3. the CFO sums at the chosen positions, then the loop in subframe order: each subframe keeps the offset that held before its half-frame
@@ -244,9 +311,13 @@ static int track_run(ltephy_track_t* h, const float2* x, const float2* xu, uint6
   };
   std::vector<float2> tabA((size_t)nsf * (SF / 128)), tabB((size_t)nsf * 128), tabAu, tabBu;
   if (xu) tabAu.resize(tabA.size()), tabBu.resize(tabB.size());
-  for (uint32_t i = 0, j = 0; i < nsf; i++) {
+  for (uint32_t i = 0, j = 0, ri = 0; i < nsf; i++) {
     ltephy_track_sf_t& o = h->sf[i];
-    o.cfo_hz             = h->f;
+    if (o.flags & LTEPHY_TRACK_REACQUIRED) {
+      if (!(h->cfg.flags & LTEPHY_TRACK_NO_CFO)) h->f = fre[ri];
+      ri++;
+    }
+    o.cfo_hz = h->f;
     tables(tabA, tabB, i, h->f);
     if (xu) tables(tabAu, tabBu, i, (float)((double)h->f * h->ul_ratio)); // f_ul = (float)(cfo_hz cfo_ratio)
     if (j < nh && h->hf[j].index == o.index) {
@@ -286,7 +357,7 @@ static int track_run(ltephy_track_t* h, const float2* x, const float2* xu, uint6
   if (ul_iq_dev) *ul_iq_dev = h->d_cutu.p;
   out->nof_subframes = nsf, out->nof_half_frames = nh;
   out->sf = h->sf.data(), out->hf = h->hf.data(), out->iq_dev = h->d_cut.p;
-  out->next_sample = (uint64_t)track_needed(h), out->remeasured = remeasured, out->reserved = 0;
+  out->next_sample = (uint64_t)track_needed(h), out->remeasured = remeasured, out->finds = finds;
   return LTEPHY_SUCCESS;
 }
 

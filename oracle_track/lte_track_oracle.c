@@ -2,13 +2,13 @@
  * lte_track_oracle.c -- see lte_track_oracle.h.
  */
 #include "lte_track_oracle.h"
+#include "../oracle/lte_sync_oracle.h"
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
 
 struct lteo_track {
-  uint32_t    N, A, W, flags, first_tti;
-  uint64_t    s0;
+  uint32_t    N, A, W, flags, first_tti, pci;
   float       ep, thr;
   lteo_tcf_t* rep;   /* [N] replica of the PSS of N_ID_2 */
   lteo_tcf_t* tabA;  /* [15 N / 128] exp(-j theta 128 i) of the current subframe */
@@ -20,6 +20,14 @@ struct lteo_track {
   uint32_t miss, nhf, ncor;
   uint32_t nl;       /* locked half-frames since the last correction */
   int64_t  sd, sh, shh, shd; /* their sums of delta, h, h^2, h delta (h: half-frame number) */
+  int64_t  base;     /* start of subframe 0 of the drift estimate's grid: frame_offset, after a find s' - k' 15 N */
+  /* find state (LTEO_TRACK_REACQUIRE) */
+  int      find;     /* searching: no subframe is cut */
+  int64_t  f0;       /* first sample of the next find window */
+  uint32_t kn;       /* subframe number predicted at f0 */
+  int      reacq;    /* the next subframe cut is the first after a successful find */
+  uint32_t finds;    /* find windows searched */
+  lteo_tcf_t* win;   /* [A][150 N + N] copy of a find window */
   /* uplink carrier (lteo_track_set_ul) */
   int      pushed;   /* a push was accepted: the uplink can no longer be set */
   int      ul;       /* set: pushes go through lteo_track_push_ul */
@@ -36,11 +44,13 @@ static int track_symbol_ok(uint32_t N)
 lteo_track_t* lteo_track_create(uint32_t N, uint32_t A, uint32_t pci, uint32_t first_tti, uint64_t frame_offset, float cfo_hz, uint32_t flags)
 {
   if (!track_symbol_ok(N) || A < 1 || A > 2 || pci > 503 || first_tti > 10239 || !(fabsf(cfo_hz) <= 7500.0f)) return NULL;
+  if (flags & ~(LTEO_TRACK_NO_CFO | LTEO_TRACK_REACQUIRE)) return NULL;
   lteo_track_t* t = (lteo_track_t*)calloc(1, sizeof(*t));
-  t->N = N, t->A = A, t->W = 9 * N / 128, t->flags = flags, t->first_tti = first_tti, t->s0 = frame_offset;
+  t->N = N, t->A = A, t->W = 9 * N / 128, t->flags = flags, t->first_tti = first_tti, t->pci = pci, t->base = (int64_t)frame_offset;
   t->rep  = (lteo_tcf_t*)malloc(sizeof(lteo_tcf_t) * N);
   t->tabA = (lteo_tcf_t*)malloc(sizeof(lteo_tcf_t) * (15 * N / 128));
   t->tabB = (lteo_tcf_t*)malloc(sizeof(lteo_tcf_t) * 128);
+  if (flags & LTEO_TRACK_REACQUIRE) t->win = (lteo_tcf_t*)malloc(sizeof(lteo_tcf_t) * A * (151 * N));
   /* d_u(n) = exp(-j pi u m / 63) (36.211 6.11.1.1); p[k] = (1/sqrt N) sum_n d_u(n) exp(+j 2 pi f_n k / N); E_p = sum_k |p[k]|^2; all in double */
   static const uint32_t ROOT[3] = {25, 29, 34};
   double                dr[62], di[62];
@@ -73,7 +83,7 @@ lteo_track_t* lteo_track_create(uint32_t N, uint32_t A, uint32_t pci, uint32_t f
 void lteo_track_destroy(lteo_track_t* t)
 {
   if (!t) return;
-  free(t->rep), free(t->tabA), free(t->tabB), free(t);
+  free(t->rep), free(t->tabA), free(t->tabB), free(t->win), free(t);
 }
 
 /* the cell search's stride-1 metric: sum_a |c_a|^2 / (E_p sum_a E_a), every sum ascending from 0.0f; 0 when the denominator is 0 */
@@ -150,15 +160,46 @@ static void track_cut(lteo_track_t* t, const lteo_tcf_t* x, uint64_t lda, uint32
 int lteo_track_set_ul(lteo_track_t* t, double cfo_ratio, int32_t ul_offset)
 {
   if (!t || t->pushed || t->ul || !(cfo_ratio > 0.0 && cfo_ratio <= 2.0)) return -2;
-  if ((int64_t)(ul_offset < 0 ? -(int64_t)ul_offset : ul_offset) >= 15 * (int64_t)t->N || (int64_t)t->s0 + ul_offset < 0) return -2;
+  if ((int64_t)(ul_offset < 0 ? -(int64_t)ul_offset : ul_offset) >= 15 * (int64_t)t->N || t->base + ul_offset < 0) return -2;
   t->ul = 1, t->ul_ratio = cfo_ratio, t->ul_off = ul_offset;
   return 0;
 }
 
-/* the lowest absolute sample the pending DL window, and with the uplink set its UL window, still needs */
+/* the lowest absolute sample the pending DL window, and with the uplink set its UL window, still needs; in the find state the window's start */
 static int64_t track_needed(const lteo_track_t* t)
 {
-  return t->ul && t->ul_off < 0 ? t->s + t->ul_off : t->s;
+  const int64_t s = t->find ? t->f0 : t->s;
+  return t->ul && t->ul_off < 0 ? s + t->ul_off : s;
+}
+
+uint32_t lteo_track_finds(const lteo_track_t* t) { return t ? t->finds : 0; }
+
+/* one find window [f0, f0 + FR + N) (DESIGN.md §2, "tracking"): the cell search on exactly these samples, the result of N_ID_2 = pci mod 3.  Found:
+ * resume at the first subframe boundary of the window with the subframe number its SSS gives; otherwise step to the next frame. */
+static void track_find(lteo_track_t* t, const lteo_tcf_t* x, uint64_t first, uint64_t n)
+{
+  const uint32_t N = t->N, SF = 15 * N;
+  const uint64_t FR = 150ull * N, L = FR + N;
+  for (uint32_t a = 0; a < t->A; a++) memcpy(t->win + a * L, x + a * n + (uint64_t)(t->f0 - (int64_t)first), sizeof(lteo_tcf_t) * L);
+  lteo_cell_t res[3];
+  lteo_cell_search(N, t->A, (const cf_t*)t->win, L, res, NULL);
+  t->finds++;
+  const lteo_cell_t* c = NULL;
+  for (uint32_t i = 0; i < 3; i++)
+    if (res[i].n_id_2 == t->pci % 3) c = &res[i];
+  if (!c->detected || c->pci != t->pci) {
+    t->f0 += (int64_t)FR, t->kn += 10;
+    return;
+  }
+  const uint64_t fo   = c->frame_offset;
+  const uint32_t sfno = (uint32_t)((10 - fo / SF) % 10);
+  const uint32_t k    = t->kn + (sfno + 10 - (t->first_tti + t->kn) % 10) % 10;
+  t->s = t->f0 + (int64_t)(fo % SF), t->k = k;
+  if (!(t->flags & LTEO_TRACK_NO_CFO)) t->f = c->cfo_hz;
+  t->miss = 0, t->acc = 0.0f;
+  t->nl = 0, t->sd = t->sh = t->shh = t->shd = 0, t->ncor = 0;
+  t->base = t->s - (int64_t)k * SF, t->nhf = 0; /* the drift d is kept: a clock does not change with a gap */
+  t->find = 0, t->reacq = 1;
 }
 
 /* a subframe is processed only when its DL window (and its UL window) lie inside first .. first + n - 1 */
@@ -178,17 +219,25 @@ static int track_push(lteo_track_t* t, const lteo_tcf_t* x, const lteo_tcf_t* xu
   const uint32_t N = t->N, SF = 15 * N, P = LTEO_TRACK_P;
   uint32_t       ns = 0, nh = 0;
   t->pushed = 1;
-  while (ns < max_sf && track_fits(t, first, n)) {
+  while (ns < max_sf) {
+    if (t->find) { /* a window is searched once all of its samples have been fed */
+      if ((uint64_t)t->f0 + 151ull * N > first + n) break;
+      track_find(t, x, first, n);
+      continue;
+    }
+    if (!track_fits(t, first, n)) break;
     const uint64_t   s   = (uint64_t)t->s - first;
     const uint32_t   tti = (t->first_tti + t->k) % 10240;
     lteo_track_sf_t* o   = &sf[ns];
     memset(o, 0, sizeof(*o));
     o->start  = t->s, o->tti = tti, o->cfo_hz = t->f, o->index = t->k;
-    o->flags  = (t->miss == 0 ? LTEO_TRACK_LOCKED : 0) | (t->miss >= LTEO_TRACK_MISS ? LTEO_TRACK_LOST : 0);
+    o->flags  = (t->miss == 0 ? LTEO_TRACK_LOCKED : 0) | (t->miss >= LTEO_TRACK_MISS ? LTEO_TRACK_LOST : 0) | (t->reacq ? LTEO_TRACK_REACQUIRED : 0);
+    t->reacq  = 0;
     if (cut) track_cut(t, x, n, t->A, t->f, s, cut + (uint64_t)ns * t->A * SF);
     /* UL: one antenna at start + ul_offset, rotated by f_ul = (float)(f cfo_ratio) with the DL rule */
     if (xu && cut_ul) track_cut(t, xu, n, 1, (float)((double)t->f * t->ul_ratio), (uint64_t)(t->s + t->ul_off) - first, cut_ul + (uint64_t)ns * SF);
     ns++;
+    int lost_now = 0;
     if (tti % 5 == 0) {
       lteo_track_hf_t* h = &hf[nh++];
       memset(h, 0, sizeof(*h));
@@ -209,13 +258,13 @@ static int track_push(lteo_track_t* t, const lteo_tcf_t* x, const lteo_tcf_t* xu
             const int64_t num = (int64_t)P * t->shd - t->sh * t->sd, den = (int64_t)P * t->shh - t->sh * t->sh;
             t->d = t->d + (float)num / (float)den;
           } else { /* then: the whole movement of the start beyond the nominal grid over the half-frames seen, less half a correction period */
-            const int64_t moved = t->s - (int64_t)t->s0 - (int64_t)t->k * SF;
+            const int64_t moved = t->s - t->base - (int64_t)t->k * SF;
             t->d = (float)moved / ((float)t->nhf - 0.5f * (float)(P - 1));
           }
           t->nl = 0, t->sd = t->sh = t->shh = t->shd = 0;
         }
       } else
-        t->miss++;
+        lost_now = ++t->miss == LTEO_TRACK_MISS;
       if (t->miss >= LTEO_TRACK_MISS) h->flags |= LTEO_TRACK_LOST;
     }
     t->acc         = t->acc + t->d / 5.0f;
@@ -223,6 +272,7 @@ static int track_push(lteo_track_t* t, const lteo_tcf_t* x, const lteo_tcf_t* xu
     t->acc         = t->acc - r;
     t->s           = t->s + SF + (int64_t)r;
     t->k++;
+    if (lost_now && (t->flags & LTEO_TRACK_REACQUIRE)) t->find = 1, t->f0 = t->s, t->kn = t->k;
   }
   *nsf = ns, *nhf = nh, *next = (uint64_t)track_needed(t);
   return 0;
