@@ -21,14 +21,17 @@ static std::mutex  g_h2d_mtx;
 static cudaEvent_t g_h2d_last[64]; // per device: completion of the most recently issued sample upload (phase_a_common)
 
 thread_local std::string ltephy_g_err;
+// a constant table of the handle on the device; a failure is kept in h->table_err, which ltephy_create checks after the last upload
 template <typename T>
 static T* upload(ltephy* h, const T* src, size_t n)
 {
-  T* d = nullptr;
-  if (cudaMalloc(&d, n * sizeof(T)) != cudaSuccess) return nullptr;
-  cudaMemcpy(d, src, n * sizeof(T), cudaMemcpyHostToDevice);
-  h->tables.push_back(d);
-  return d;
+  if (h->table_err != cudaSuccess) return nullptr;
+  DevBuf<uint8_t>& b = h->tables.emplace_back();
+  if ((h->table_err = cudaMalloc(&b.p, n * sizeof(T))) != cudaSuccess ||
+      (h->table_err = cudaMemcpy(b.p, src, n * sizeof(T), cudaMemcpyHostToDevice)) != cudaSuccess)
+    return nullptr;
+  b.cap = n * sizeof(T);
+  return reinterpret_cast<T*>(b.p);
 }
 
 // Small host->device transfers do not use the copy engine: a DMA queued behind another pipeline's 0.5 GB IQ copy would
@@ -78,15 +81,8 @@ extern "C" int ltephy_create(const ltephy_cfg_t* cfg, ltephy_t** out)
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail(LTEPHY_ERROR, "no CUDA device: this library has no CPU path");
   CU(cudaSetDevice(cfg->device));
-  ltephy* h = new ltephy();
-  struct CreateGuard { // every failing return below releases what was created so far
-    ltephy* h;
-    bool    ok = false;
-    ~CreateGuard()
-    {
-      if (!ok) ltephy_destroy(h);
-    }
-  } guard{h};
+  std::unique_ptr<ltephy, decltype(&ltephy_destroy)> owner(new ltephy(), ltephy_destroy); // every failing return below destroys what was created so far
+  ltephy* const                                      h = owner.get();
   h->cfg    = *cfg;
   if (!h->cfg.turbo_max_iter) h->cfg.turbo_max_iter = 8;
   if (!h->cfg.max_grants) h->cfg.max_grants = 24 * cfg->max_subframes;
@@ -97,10 +93,10 @@ extern "C" int ltephy_create(const ltephy_cfg_t* cfg, ltephy_t** out)
   h->st = ltehost::dci_size_table(h->cell);
   memset(h->pi_fast, 0xFF, sizeof(h->pi_fast));
   h->segm_fast.assign(110000 / 8, ltehost::Segm{});
-  CU(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
-  for (auto& e : h->ev) CU(cudaEventCreate(&e));
-  CU(cudaEventCreateWithFlags(&h->ev_h2d, cudaEventDisableTiming));
-  for (auto& e : h->mark) CU(cudaEventCreate(&e));
+  CU(cudaStreamCreateWithFlags(&h->stream.raw, cudaStreamNonBlocking));
+  for (auto& e : h->ev) CU(cudaEventCreate(&e.raw));
+  CU(cudaEventCreateWithFlags(&h->ev_h2d.raw, cudaEventDisableTiming));
+  for (auto& e : h->mark) CU(cudaEventCreate(&e.raw));
 
   DevCell& c = h->dc;
   c.nof_prb = cfg->nof_prb, c.nof_ports = cfg->nof_ports, c.cell_id = cfg->cell_id, c.nof_rx = cfg->nof_rx;
@@ -242,38 +238,26 @@ extern "C" int ltephy_create(const ltephy_cfg_t* cfg, ltephy_t** out)
           }
     c.re_mask = upload(h, masks.data(), masks.size());
   }
+  if (h->table_err != cudaSuccess) return fail(LTEPHY_ERROR, "table upload failed: %s", cudaGetErrorString(h->table_err));
   const size_t S = cfg->max_subframes, g = (size_t)14 * c.nsc;
   if (h->d_iq.reserve(S * c.nof_rx * c.sf_len) || h->d_sym.reserve(S * c.nof_rx * g) || h->d_pil.reserve(S * c.nof_ports * c.nof_rx * 4 * 2 * c.nof_prb) ||
       h->d_llr.reserve(S * LLR_STRIDE) || h->d_info.reserve(S) || h->d_cands.reserve(S * LTEPHY_MAX_LOC * LTEPHY_MAX_SIZES) || h->d_vwork.reserve(S * (LTEPHY_MAX_LOC / 2) * LTEPHY_MAX_SIZES * 2 + 16) ||
       h->h_info.reserve(S) || h->d_compact.reserve(S) || h->h_compact.reserve(S) || h->d_rm.reserve((size_t)4 << 20) || h->d_pi.reserve((size_t)188 * 6144))
     return fail(LTEPHY_ERROR, "device allocation failed");
   CU(cudaMemset(h->d_cands.p, 0, h->d_cands.cap * sizeof(ltephy_cand_t)));
-  guard.ok = true;
-  *out     = h;
+  *out = owner.release();
   return LTEPHY_SUCCESS;
 }
 
 extern "C" void ltephy_destroy(ltephy_t* h)
 {
   if (!h) return;
+  cudaSetDevice(h->cfg.device);
   cudaDeviceSynchronize();
-  for (void* p : h->tables) cudaFree(p);
-  h->d_iq.release(), h->d_sym.release(), h->d_ce.release(), h->d_pil.release(), h->d_llr.release(), h->d_info.release(), h->d_cands.release();
-  h->h_info.release(), h->d_compact.release(), h->h_compact.release(), h->d_grants.release(), h->d_cbs.release(), h->d_pairs.release(), h->d_tbs.release(), h->d_pair_pi_off.release();
-  h->d_tscratch.release(), h->d_tqueue.release();
-  h->d_seq.release(), h->d_rm.release(), h->d_turbo.release(), h->d_pllr.release(), h->d_pi.release(), h->d_payload.release(), h->d_harq.release(), h->d_cfo.release(), h->d_ulcfo.release(), h->d_mib.release(), h->d_pbch.release(), h->d_vwork.release();
-  h->d_cb_iters.release(), h->d_cb_crc.release(), h->d_res.release(), h->h_res.release(), h->h_payload.release(), h->h_stage.release();
-  h->d_uliq.release(), h->d_ulsym.release(), h->d_ulpool.release(), h->d_ulgrants.release(), h->d_ulchest.release(), h->h_ulchest.release();
-  for (auto& e : h->ev)
-    if (e) cudaEventDestroy(e);
-  for (auto& e : h->mark)
-    if (e) cudaEventDestroy(e);
-  if (h->ev_h2d) {
-    std::lock_guard<std::mutex> lk(g_h2d_mtx);
+  {
+    std::lock_guard<std::mutex> lk(g_h2d_mtx); // no later upload may wait on the event once it is destroyed
     if (g_h2d_last[h->cfg.device & 63] == h->ev_h2d) g_h2d_last[h->cfg.device & 63] = nullptr;
-    cudaEventDestroy(h->ev_h2d);
   }
-  if (h->stream) cudaStreamDestroy(h->stream);
   delete h;
 }
 
@@ -430,14 +414,12 @@ static int64_t pool_append(ltephy* h, DevBuf<T>& pool, size_t& used, const T* sr
 {
   if (used + n > pool.cap) {
     const size_t want = 2 * pool.cap + n;
-    T*           np   = nullptr;
-    if (cudaStreamSynchronize(h->stream) != cudaSuccess || cudaMalloc(&np, want * sizeof(T)) != cudaSuccess) return -1;
-    if (cudaMemcpy(np, pool.p, used * sizeof(T), cudaMemcpyDeviceToDevice) != cudaSuccess) {
-      cudaFree(np);
+    DevBuf<T>    grown;
+    if (cudaStreamSynchronize(h->stream) != cudaSuccess || cudaMalloc(&grown.p, want * sizeof(T)) != cudaSuccess ||
+        cudaMemcpy(grown.p, pool.p, used * sizeof(T), cudaMemcpyDeviceToDevice) != cudaSuccess)
       return -1;
-    }
-    cudaFree(pool.p);
-    pool.p = np, pool.cap = want;
+    grown.cap = want;
+    pool      = std::move(grown);
   }
   if (cudaMemcpyAsync(pool.p + used, src, n * sizeof(T), cudaMemcpyHostToDevice, h->stream) != cudaSuccess) return -1;
   cudaStreamSynchronize(h->stream);

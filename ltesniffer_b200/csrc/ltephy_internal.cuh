@@ -9,8 +9,10 @@
 #include <cstdarg>
 #include <cstdio>
 #include <map>
+#include <memory>
 #include <string>
 #include <tuple>
+#include <utility>
 #include <vector>
 
 extern thread_local std::string ltephy_g_err;
@@ -30,11 +32,22 @@ static inline int fail(int code, const char* fmt, ...)
     if (e_ != cudaSuccess) return fail(LTEPHY_ERROR, "%s: %s", #x, cudaGetErrorString(e_));        \
   } while (0)
 
+// The owners below free what they hold when they die.  A handle declares its stream before its buffers, so the buffers go first.
 template <typename T>
 struct DevBuf { // growable device buffer
   T*     p   = nullptr;
   size_t cap = 0;
-  int    reserve(size_t n)
+  DevBuf()   = default;
+  DevBuf(const DevBuf&)            = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  DevBuf(DevBuf&& o) noexcept { *this = std::move(o); }
+  DevBuf& operator=(DevBuf&& o) noexcept // the buffer held before dies with o
+  {
+    std::swap(p, o.p), std::swap(cap, o.cap);
+    return *this;
+  }
+  ~DevBuf() { release(); }
+  int reserve(size_t n)
   {
     if (n <= cap) return 0;
     size_t want = n + n / 4 + 1024;
@@ -60,7 +73,17 @@ template <typename T>
 struct PinBuf { // growable pinned host buffer
   T*     p   = nullptr;
   size_t cap = 0;
-  int    reserve(size_t n)
+  PinBuf()   = default;
+  PinBuf(const PinBuf&)            = delete;
+  PinBuf& operator=(const PinBuf&) = delete;
+  PinBuf(PinBuf&& o) noexcept { *this = std::move(o); }
+  PinBuf& operator=(PinBuf&& o) noexcept
+  {
+    std::swap(p, o.p), std::swap(cap, o.cap);
+    return *this;
+  }
+  ~PinBuf() { release(); }
+  int reserve(size_t n)
   {
     if (n <= cap) return 0;
     size_t want = n + n / 4 + 1024;
@@ -79,6 +102,21 @@ struct PinBuf { // growable pinned host buffer
     p = nullptr, cap = 0;
   }
 };
+// a stream or an event: created into &raw while it is null, used wherever the CUDA type is
+template <typename H, cudaError_t (*destroy)(H)>
+struct CudaOwned {
+  H raw = nullptr;
+  CudaOwned() = default;
+  CudaOwned(const CudaOwned&)            = delete;
+  CudaOwned& operator=(const CudaOwned&) = delete;
+  ~CudaOwned()
+  {
+    if (raw) destroy(raw);
+  }
+  operator H() const { return raw; }
+};
+using Stream = CudaOwned<cudaStream_t, cudaStreamDestroy>;
+using Event  = CudaOwned<cudaEvent_t, cudaEventDestroy>;
 
 struct ltephy {
   ltephy_cfg_t       cfg{};
@@ -86,8 +124,8 @@ struct ltephy {
   ltehost::CtrlMap   cm;
   ltehost::SizeTable st;
   DevCell            dc{};
-  cudaStream_t       stream = nullptr;
-  cudaEvent_t        ev[6]{}, mark[2]{}, ev_h2d = nullptr;
+  Stream             stream;
+  Event              ev[6], mark[2], ev_h2d;
   DevBuf<float2>     d_cfo;                  // per-sample rotation of ltephy_set_cfo
   DevBuf<float2>     d_ulcfo;                // per-sample rotation of ltephy_set_ul_cfo
   DevBuf<uint32_t>   d_vwork;                // work list of the Viterbi kernel: count + two-word (subframe, locations, size) items
@@ -98,8 +136,9 @@ struct ltephy {
   uint32_t           pbch_frames  = 0;       // frames the last PBCH call wrote to rows 3.. of d_pbch (LTEPHY_TAP_PBCH_LLR)
   DevBuf<short>      d_harq;                 // HARQ store: harq_slots x LTEPHY_HARQ_SLOT_BYTES
   uint32_t           harq_slots = 0;
-  std::vector<void*> tables; // device tables freed at destroy
-  uint64_t           launches = 0;
+  std::vector<DevBuf<uint8_t>> tables;                 // the cell's constant tables (upload): dc, d_gold_* and d_xpow* point into them
+  cudaError_t                  table_err = cudaSuccess; // the first table upload that failed
+  uint64_t                     launches  = 0;
 
   // phase A
   DevBuf<float2>        d_iq, d_sym, d_pil, d_ce; // d_pil: smoothed CRS estimates [n][port][rx][4][2 nof_prb]; d_ce: interpolated grid, filled on demand (tap)

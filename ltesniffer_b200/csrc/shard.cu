@@ -180,19 +180,10 @@ struct Slot {
   PinBuf<uint32_t>   h_offs_all;
   DevBuf<uint8_t>    d_msg, d_g_msg;   // gather message of this rank / of every other rank (rank 0): GatherHdr, TbMeta[2 ng], ltephy_tb_result_t[ntb]
   PinBuf<uint8_t>    h_msg, h_g_msg;
-  cudaEvent_t        ev_pack = nullptr, ev_g = nullptr, ev_x = nullptr, ev_msg = nullptr;
+  Event              ev_pack, ev_g, ev_x, ev_msg; // created on first use
   std::vector<uint32_t>           tti_cfi, grant_dci;
   std::vector<ltephy_grant_t>     grants;
   std::vector<ltephy_tb_result_t> res;
-  void release()
-  {
-    d_pack.release(), d_pack_all.release(), d_full_all.release(), d_g_payload.release(), d_offs.release(), d_offs_all.release();
-    h_pack_all.release(), h_full_all.release(), h_offs_all.release(), d_msg.release(), d_g_msg.release(), h_msg.release(), h_g_msg.release();
-    for (cudaEvent_t* e : {&ev_pack, &ev_g, &ev_x, &ev_msg}) {
-      if (*e) cudaEventDestroy(*e);
-      *e = nullptr;
-    }
-  }
 };
 inline double now_ms() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
 } // namespace
@@ -201,20 +192,18 @@ struct ltephy_shard {
   uint32_t     rank = 0, world = 1;
   int          device = 0;
   ncclComm_t   comm_x = nullptr, comm_g = nullptr, comm_f = nullptr; // exchange / gather / full-table fetch: one communicator per ordered section
-  cudaStream_t st_x = nullptr, st_g = nullptr, st_f = nullptr;
+  Stream       st_x, st_g, st_f;
   Turn         turn_x, turn_f, turn_w, turn_g;
   uint32_t     gather_bytes_per_sf = 24576; // fixed payload capacity of one rank's gather message, per subframe of the batch
   std::mutex   slots_mtx;
-  std::map<ltephy_t*, Slot*> slots;
+  std::map<ltephy_t*, std::unique_ptr<Slot>> slots;
   std::atomic<bool> failed{false}; // set and read by the pipelines' threads
   Slot*        slot_of(ltephy_t* h)
   {
     std::lock_guard<std::mutex> lk(slots_mtx);
-    auto                        it = slots.find(h);
-    if (it != slots.end()) return it->second;
-    Slot* s   = new Slot();
-    slots[h]  = s;
-    return s;
+    std::unique_ptr<Slot>&      s = slots[h];
+    if (!s) s = std::make_unique<Slot>();
+    return s.get();
   }
 };
 
@@ -246,9 +235,9 @@ extern "C" int ltephy_shard_create(const uint8_t* id, uint32_t rank, uint32_t wo
   // the other pipelines -- without it an NCCL kernel waits behind whole grids of them
   int prio_lo = 0, prio_hi = 0;
   cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);
-  if (r != ncclSuccess || cudaStreamCreateWithPriority(&sh->st_x, cudaStreamNonBlocking, prio_hi) != cudaSuccess ||
-      cudaStreamCreateWithPriority(&sh->st_g, cudaStreamNonBlocking, prio_hi) != cudaSuccess ||
-      cudaStreamCreateWithPriority(&sh->st_f, cudaStreamNonBlocking, prio_hi) != cudaSuccess) {
+  if (r != ncclSuccess || cudaStreamCreateWithPriority(&sh->st_x.raw, cudaStreamNonBlocking, prio_hi) != cudaSuccess ||
+      cudaStreamCreateWithPriority(&sh->st_g.raw, cudaStreamNonBlocking, prio_hi) != cudaSuccess ||
+      cudaStreamCreateWithPriority(&sh->st_f.raw, cudaStreamNonBlocking, prio_hi) != cudaSuccess) {
     ltephy_shard_destroy(sh);
     return fail(LTEPHY_ERROR, "shard_create: %s", r != ncclSuccess ? g_nccl.GetErrorString(r) : "stream creation failed");
   }
@@ -266,16 +255,9 @@ extern "C" void ltephy_shard_destroy(ltephy_shard_t* sh)
   if (!sh) return;
   cudaSetDevice(sh->device);
   cudaDeviceSynchronize();
-  for (auto& kv : sh->slots) {
-    kv.second->release();
-    delete kv.second;
-  }
   if (sh->comm_x) g_nccl.CommDestroy(sh->comm_x);
   if (sh->comm_g) g_nccl.CommDestroy(sh->comm_g);
   if (sh->comm_f) g_nccl.CommDestroy(sh->comm_f);
-  if (sh->st_f) cudaStreamDestroy(sh->st_f);
-  if (sh->st_x) cudaStreamDestroy(sh->st_x);
-  if (sh->st_g) cudaStreamDestroy(sh->st_g);
   delete sh;
 }
 
@@ -285,7 +267,7 @@ static int pack_current(ltephy* h, Slot* sl)
   const uint32_t n = h->n_cur;
   if (sl->d_pack.reserve((size_t)h->cfg.max_subframes * PACK_MAX_BYTES) || sl->d_offs.reserve(h->cfg.max_subframes + 1))
     return fail(LTEPHY_ERROR, "device allocation failed");
-  if (!sl->ev_pack) CU(cudaEventCreateWithFlags(&sl->ev_pack, cudaEventDisableTiming));
+  if (!sl->ev_pack) CU(cudaEventCreateWithFlags(&sl->ev_pack.raw, cudaEventDisableTiming));
   pack_kernel<<<n, 256, 0, h->stream>>>(h->dc, h->d_info.p, h->d_compact.p, n, sl->d_pack.p, sl->d_offs.p);
   h->launches++;
   CU(cudaEventRecord(sl->ev_pack, h->stream));
@@ -309,7 +291,6 @@ extern "C" int ltephy_pack_phase_a(ltephy_t* h, uint8_t* out, size_t out_cap, ui
       r = fail(LTEPHY_ERROR, "pack_phase_a: copy failed");
   }
   cudaStreamSynchronize(h->stream);
-  sl.release();
   return r;
 }
 
@@ -350,8 +331,8 @@ extern "C" int ltephy_decode_subframes_sharded(ltephy_shard_t* sh, ltephy_t* h, 
     return fail(LTEPHY_ERROR, "allocation of the exchange buffers failed");
   // ---- exchange turn: the turn orders the two collectives of this batch among the batches in flight, nothing else.  Waiting for them
   // (= for the slowest rank) and the copies to the host happen outside it, so a straggler delays its own batch only.
-  for (cudaEvent_t* e : {&sl->ev_x, &sl->ev_g, &sl->ev_msg})
-    if (!*e) CU(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+  for (Event* e : {&sl->ev_x, &sl->ev_g, &sl->ev_msg})
+    if (!*e) CU(cudaEventCreateWithFlags(&e->raw, cudaEventDisableTiming));
   gx.take();
   CU(cudaStreamWaitEvent(sh->st_x, sl->ev_pack, 0));
   // offsets, then the records at their fixed per-rank capacity (4.6 MB per 1000 subframes, a third of it used: NVLink does not notice, and

@@ -15,7 +15,7 @@ struct ltephy_sync {
   ltephy_sync_cfg_t cfg{};
   uint32_t          N = 0, D = 0, A = 0, NR = 0, nhmax = 0;
   uint64_t          Jmax = 0;
-  cudaStream_t      stream = nullptr;
+  Stream            stream;
   float             ep[3]{};
   std::vector<float2> dpss; // [3][62]
   DevBuf<float2>    d_x, d_rep, d_W, d_dpss, d_Y;
@@ -90,19 +90,12 @@ extern "C" int ltephy_sync_create(const ltephy_sync_cfg_t* cfg, ltephy_sync_t** 
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail(LTEPHY_ERROR, "no CUDA device: this library has no CPU path");
   CU(cudaSetDevice(cfg->device));
-  ltephy_sync* h = new ltephy_sync();
-  struct Guard {
-    ltephy_sync* h;
-    bool         ok = false;
-    ~Guard()
-    {
-      if (!ok) ltephy_sync_destroy(h);
-    }
-  } guard{h};
+  std::unique_ptr<ltephy_sync, decltype(&ltephy_sync_destroy)> owner(new ltephy_sync(), ltephy_sync_destroy);
+  ltephy_sync* const                                           h = owner.get();
   h->cfg = *cfg, h->N = N, h->D = N / 128, h->A = cfg->nof_rx, h->NR = 2 * h->D - 1;
   h->Jmax  = (cfg->max_samples - N) / h->D + 1;
   h->nhmax = (uint32_t)((cfg->max_samples - N) / (75ull * N) + 1);
-  CU(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
+  CU(cudaStreamCreateWithFlags(&h->stream.raw, cudaStreamNonBlocking));
   // replicas p_u[k] = (1/sqrt N) sum_n d_u(n) exp(+j 2 pi f_n k / N) and E_p, in double, as lteo_cell_search computes them
   std::vector<float2> rep((size_t)3 * N), W(N);
   h->dpss.resize(3 * 62);
@@ -124,8 +117,7 @@ extern "C" int ltephy_sync_create(const ltephy_sync_cfg_t* cfg, ltephy_sync_t** 
   CU(cudaMemcpy(h->d_W.p, W.data(), W.size() * sizeof(float2), cudaMemcpyHostToDevice));
   CU(cudaMemcpy(h->d_dpss.p, h->dpss.data(), h->dpss.size() * sizeof(float2), cudaMemcpyHostToDevice));
   CU(cudaMemcpy(h->d_seq.p, seq.data(), seq.size() * sizeof(float), cudaMemcpyHostToDevice));
-  guard.ok = true;
-  *out     = h;
+  *out = owner.release();
   return LTEPHY_SUCCESS;
 }
 
@@ -134,9 +126,6 @@ extern "C" void ltephy_sync_destroy(ltephy_sync_t* h)
   if (!h) return;
   cudaSetDevice(h->cfg.device);
   if (h->stream) cudaStreamSynchronize(h->stream);
-  h->d_x.release(), h->d_rep.release(), h->d_W.release(), h->d_dpss.release(), h->d_Y.release(), h->d_seq.release(), h->d_m.release();
-  h->d_fold.release(), h->d_rm.release(), h->d_ref.release(), h->d_sss.release(), h->d_c12.release(), h->d_pk.release();
-  if (h->stream) cudaStreamDestroy(h->stream);
   delete h;
 }
 

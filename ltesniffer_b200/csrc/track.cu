@@ -20,7 +20,7 @@ struct ltephy_track {
   ltephy_track_cfg_t cfg{};
   uint32_t           N = 0, A = 0, W = 0, SF = 0;
   float              ep = 0.0f, thr = 0.0f, max_ppm = 50.0f;
-  cudaStream_t       stream = nullptr;
+  Stream             stream;
   DevBuf<float2>     d_rep, d_x, d_cut, d_tabA, d_tabB, d_c;
   DevBuf<float>      d_m;
   DevBuf<TrackWin>   d_win;
@@ -37,7 +37,7 @@ struct ltephy_track {
   int64_t        f0 = 0;
   uint32_t       kn = 0;
   float          f_find = 0.0f; // the found carrier offset, installed at the re-acquired subframe in step 3
-  ltephy_sync_t* sync = nullptr;
+  std::unique_ptr<ltephy_sync_t, decltype(&ltephy_sync_destroy)> sync{nullptr, ltephy_sync_destroy};
   std::vector<ltephy_track_sf_t> sf;
   std::vector<ltephy_track_hf_t> hf;
   // the uplink carrier (ltephy_track_set_ul): one antenna cut at start + ul_off with its own rotation tables
@@ -84,26 +84,21 @@ extern "C" int ltephy_track_create(const ltephy_track_cfg_t* cfg, ltephy_track_t
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail(LTEPHY_ERROR, "no CUDA device: this library has no CPU path");
   CU(cudaSetDevice(cfg->device));
-  ltephy_track* h = new ltephy_track();
-  struct Guard {
-    ltephy_track* h;
-    bool          ok = false;
-    ~Guard()
-    {
-      if (!ok) ltephy_track_destroy(h);
-    }
-  } guard{h};
+  std::unique_ptr<ltephy_track, decltype(&ltephy_track_destroy)> owner(new ltephy_track(), ltephy_track_destroy);
+  ltephy_track* const                                            h = owner.get();
   h->cfg = *cfg, h->N = N, h->A = cfg->nof_rx, h->W = 9 * N / 128, h->SF = 15 * N;
   h->max_ppm = cfg->max_ppm > 0.0f ? cfg->max_ppm : 50.0f;
   h->thr     = TRACK_LOCK_K / (float)N;
   h->s = h->base = (int64_t)cfg->frame_offset, h->f = cfg->cfo_hz;
-  CU(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
+  CU(cudaStreamCreateWithFlags(&h->stream.raw, cudaStreamNonBlocking));
   // the find's cell search: one window of a frame plus a symbol.  The handle's own sample buffer (A (150 N + N) samples, 4.9 MB at N = 2048
   // with 2 antennas) stays unused: the find reads the push's samples in place through sync_run.
   if (cfg->flags & LTEPHY_TRACK_REACQUIRE) {
     ltephy_sync_cfg_t sc{};
     sc.symbol_sz = N, sc.nof_rx = h->A, sc.max_samples = 151ull * N, sc.device = cfg->device;
-    if (int r = ltephy_sync_create(&sc, &h->sync)) return r;
+    ltephy_sync_t* sync = nullptr;
+    if (int r = ltephy_sync_create(&sc, &sync)) return r;
+    h->sync.reset(sync);
   }
   // the replica of N_ID_2 = pci mod 3 and its energy: the cell search's (sync.cu), as lteo_track_create computes them
   std::vector<float2> rep(N), d62(62);
@@ -114,8 +109,7 @@ extern "C" int ltephy_track_create(const ltephy_track_cfg_t* cfg, ltephy_track_t
     return fail(LTEPHY_ERROR, "track_create: device allocation failed");
   CU(cudaMemcpy(h->d_rep.p, rep.data(), N * sizeof(float2), cudaMemcpyHostToDevice));
   h->sf.reserve(nsf), h->hf.reserve(nsf / 5 + 1);
-  guard.ok = true;
-  *out     = h;
+  *out = owner.release();
   return LTEPHY_SUCCESS;
 }
 
@@ -124,11 +118,6 @@ extern "C" void ltephy_track_destroy(ltephy_track_t* h)
   if (!h) return;
   cudaSetDevice(h->cfg.device);
   if (h->stream) cudaStreamSynchronize(h->stream);
-  ltephy_sync_destroy(h->sync);
-  h->d_rep.release(), h->d_x.release(), h->d_cut.release(), h->d_tabA.release(), h->d_tabB.release(), h->d_c.release(), h->d_m.release();
-  h->d_win.release(), h->d_pos.release(), h->d_start.release();
-  h->d_xu.release(), h->d_cutu.release(), h->d_tabAu.release(), h->d_tabBu.release(), h->d_startu.release();
-  if (h->stream) cudaStreamDestroy(h->stream);
   delete h;
 }
 
@@ -156,7 +145,7 @@ static int track_find(ltephy_track_t* h, const float2* x, uint64_t first, uint64
   const uint64_t FR = 150ull * N;
   CU(cudaStreamSynchronize(h->stream)); // the push's copy of x runs on the tracker's stream, the search on the sync handle's
   ltephy_cell_t res[3];
-  if (int r = sync_run(h->sync, x + (h->f0 - (int64_t)first), n, FR + N, res)) return r;
+  if (int r = sync_run(h->sync.get(), x + (h->f0 - (int64_t)first), n, FR + N, res)) return r;
   const ltephy_cell_t* c = nullptr;
   for (uint32_t i = 0; i < 3; i++)
     if (res[i].n_id_2 == h->cfg.pci % 3) c = &res[i];
