@@ -71,12 +71,16 @@ struct DevGrant {          // one PDSCH grant
   uint32_t np[2];          // allocated PRBs per slot
   uint8_t  plist[2][112];  // allocated PRB indices per slot, ascending
   uint32_t qm[2];
-  uint32_t llr_off[2];     // offset (int16 elements) of codeword LLRs in the LLR pool
+  uint64_t llr_off[2];     // offset (int16 elements) of codeword LLRs in the LLR pool
   uint32_t scr_off[2];     // offset (words) of the scrambling sequence in the sequence pool
 };
 
+// The soft-bit, turbo-stream and HARQ pools of one batch pass 2^32 elements (8.6 GB of soft bits after ~24 000 subframes of a loaded
+// 20 MHz cell), so offsets into them are 64-bit.  Scrambling-word and payload-byte offsets (scr_off, DevPair.out_byte, DevTb.byte_off) stay
+// 32-bit: they would need ~2^37 soft bits or ~200 GB of turbo pool before they wrap, which no 80 GB card holds.
 struct DevCb {             // one code block
-  uint32_t llr_off;        // first soft bit of this code block in the LLR pool
+  uint64_t llr_off;        // first soft bit of this code block in the LLR pool
+  uint64_t harq_off;       // int16 offset of this code block's accumulators in the HARQ store
   uint32_t E;              // soft bits received
   uint32_t K, F;
   uint32_t rm_tab;         // offset into the rate-matching table pool: inverse table of (K, F), one uint16 per pair-buffer word
@@ -85,13 +89,12 @@ struct DevCb {             // one code block
   uint32_t shift;          // conditioning shift from Qm
   uint32_t pair, half;     // turbo job and 16-bit lane it occupies
   uint32_t harq_op;        // LTEPHY_HARQ_*: 0 none, 1 overwrite the store, 2 add to it
-  uint32_t harq_off;       // int16 offset of this code block's accumulators in the HARQ store
   uint32_t harq_gen;       // 0: first use of the slot in this batch, 1: second, ... (one rate-dematch launch per generation)
 };
 
 struct DevPair {           // turbo job: up to two code blocks of equal K decoded by one CTA
+  uint64_t buf_off;        // offset (uint32) of this pair's stream buffers in the turbo pool
   uint32_t K, NW, f1, f2;
-  uint32_t buf_off;        // offset (uint32) of this pair's stream buffers in the turbo pool
   uint32_t ncb;            // 1 or 2
   uint32_t crc_type[2];    // 0 none, 1 CRC24A, 2 CRC24B
   uint32_t out_byte[2];    // byte offset in the payload buffer where the CB's data bits go

@@ -470,7 +470,7 @@ static int pi_table_for(ltephy* h, uint32_t K, uint32_t& off)
 }
 
 // transport block -> code blocks (shared by the PDSCH and PUSCH paths); pair_code_blocks puts them into turbo pairs once the batch is complete
-static int add_transport_block(ltephy* h, uint32_t tbs, uint32_t G, uint32_t qm, uint32_t rv, uint32_t NL, uint32_t llr_off, uint32_t& tb_index,
+static int add_transport_block(ltephy* h, uint32_t tbs, uint32_t G, uint32_t qm, uint32_t rv, uint32_t NL, uint64_t llr_off, uint32_t& tb_index,
                                uint32_t harq_op = LTEPHY_HARQ_NONE, uint32_t harq_slot = 0)
 {
   if (tbs / 8 >= h->segm_fast.size() || (tbs & 7)) return fail(LTEPHY_ERROR_INVALID_INPUTS, "invalid TBS %u", tbs);
@@ -487,14 +487,15 @@ static int add_transport_block(ltephy* h, uint32_t tbs, uint32_t G, uint32_t qm,
   DevTb                tb{};
   tb.byte_off = (uint32_t)b.payload_bytes, tb.nbytes = tbs / 8, tb.cb_first = (uint32_t)b.cbs.size(), tb.ncb = s.C;
   b.payload_bytes += (tb.nbytes + 3 + 3) & ~3u;
-  uint32_t rp = llr_off, wbit = 0;
+  uint64_t rp   = llr_off;
+  uint32_t wbit = 0;
   for (uint32_t r = 0; r < s.C; r++) {
     DevCb cb{};
     cb.K = s.K(r), cb.F = r == 0 ? s.F : 0, cb.E = ltehost::rm_turbo_E(G, s.C, r, qm, NL);
     cb.llr_off = rp;
     rp += cb.E;
     cb.shift = qm == 2 ? 0 : qm == 4 ? 1 : 2;
-    cb.harq_op = harq_op, cb.harq_off = harq_op ? (uint32_t)((size_t)harq_slot * (LTEPHY_HARQ_SLOT_BYTES / 2) + (size_t)r * 18448u) : 0u, cb.harq_gen = harq_gen;
+    cb.harq_op = harq_op, cb.harq_off = harq_op ? (uint64_t)harq_slot * (LTEPHY_HARQ_SLOT_BYTES / 2) + (uint64_t)r * 18448u : 0u, cb.harq_gen = harq_gen;
     const ltephy::RmEntry* rm = rm_table_for(h, cb.K, cb.F);
     if (!rm) return fail(LTEPHY_ERROR, "rate-matching table upload failed");
     cb.rm_tab = (uint32_t)rm->off, cb.rm_nn = rm->nn, cb.rm_rot = rm->rot[rv & 3u];
@@ -510,12 +511,12 @@ static int add_transport_block(ltephy* h, uint32_t tbs, uint32_t G, uint32_t qm,
 }
 // LLR and scrambling space of one codeword: G soft bits, scrambled with the first `bits` bits of the Gold sequence (PDSCH: G, PUSCH: 12 M Qm);
 // false if the scrambling basis is shorter
-static bool alloc_codeword(ltephy* h, uint32_t bits, uint32_t G, uint32_t& llr_off, uint32_t& scr_off)
+static bool alloc_codeword(ltephy* h, uint32_t bits, uint32_t G, uint64_t& llr_off, uint32_t& scr_off)
 {
   ltephy::PhaseB& b = h->pb;
   const uint32_t  w = (bits + 31) / 32;
   if (w > h->gold_words) return false;
-  llr_off = (uint32_t)b.pllr_elems, scr_off = (uint32_t)b.seq_words;
+  llr_off = b.pllr_elems, scr_off = (uint32_t)b.seq_words;
   b.max_scr_words = std::max(b.max_scr_words, w);
   b.seq_words += w + 1; // +1: the demapper reads a 64-bit window
   b.pllr_elems += (G + 7) & ~7u;
@@ -590,7 +591,7 @@ static int pair_code_blocks(ltephy* h)
     DevPair& p = b.pairs[pi];
     p.NW = (p.K + 31) / 32;
     ltehost::qpp_params(p.K, p.f1, p.f2);
-    p.buf_off = (uint32_t)b.turbo_words;
+    p.buf_off = b.turbo_words;
     b.turbo_words += ltephy_pair_words(p.NW);
     if (pi_table_for(h, p.K, b.pair_pi_off[pi])) return fail(LTEPHY_ERROR, "interleaver table upload failed");
   }
@@ -1220,7 +1221,7 @@ extern "C" int ltephy_turbo_batch(ltephy_t* h, const int16_t* d, uint32_t K, uin
   const uint32_t        out_bytes = K / 8;
   for (uint32_t p = 0; p < npairs; p++) {
     DevPair pr{};
-    pr.K = K, pr.NW = NW, pr.f1 = f1, pr.f2 = f2, pr.buf_off = (uint32_t)(pw * p), pr.ncb = (2 * p + 1 < ncb) ? 2 : 1;
+    pr.K = K, pr.NW = NW, pr.f1 = f1, pr.f2 = f2, pr.buf_off = pw * p, pr.ncb = (2 * p + 1 < ncb) ? 2 : 1;
     for (uint32_t hh = 0; hh < pr.ncb; hh++) {
       const uint32_t cbi = 2 * p + hh;
       pr.crc_type[hh] = (uint32_t)crc_type, pr.out_skip[hh] = 0, pr.out_bits[hh] = K, pr.out_byte[hh] = cbi * out_bytes, pr.cb_index[hh] = cbi;
