@@ -5,7 +5,7 @@ CXX ?= g++
 CFLAGS = -O3 -g -fPIC -std=gnu11 -Wall -Wno-unused-function -ffp-contract=off -fno-fast-math
 CXXFLAGS = -O2 -g -fPIC -std=c++17 -Wall -ffp-contract=off -fno-fast-math
 
-all: sim/libltesim.so oracle/liblteoracle.so oracle/liblteosync.so oracle/liblteomib.so oracle_track/liblteotrack.so
+all: sim/libltesim.so oracle/liblteoracle.so oracle/liblteosync.so oracle/liblteomib.so oracle_track/liblteotrack.so oracle/liblteochan.so
 
 sim/libltesim.so: sim/lte_common.c sim/lte_sim.c sim/lte_common.h sim/lte_sim.h include/lte_tables.h
 	$(CC) $(CFLAGS) -shared -o $@ sim/lte_common.c sim/lte_sim.c -lm
@@ -25,6 +25,10 @@ oracle/liblteomib.so: oracle/lte_mib_oracle.c oracle/lte_mib_oracle.h oracle/lte
 oracle_track/liblteotrack.so: oracle_track/lte_track_oracle.c oracle_track/lte_track_oracle.h oracle/lte_sync_oracle.h oracle/liblteosync.so
 	$(CC) $(CFLAGS) -shared -o $@ oracle_track/lte_track_oracle.c -Loracle -llteosync -Wl,-rpath,'$$ORIGIN/../oracle' -lm
 
+# channeliser oracle: stands alone
+oracle/liblteochan.so: oracle/lte_chan_oracle.c oracle/lte_chan_oracle.h
+	$(CC) $(CFLAGS) -shared -o $@ oracle/lte_chan_oracle.c -lm
+
 # C++ example of the C-ABI (needs ltesniffer_b200/libltephy_b200.so, built by ltesniffer_b200/build.py)
 examples/offline_decode: examples/offline_decode.cpp include/ltephy_b200.h include/ltephy_search.h include/ltephy_sinks.h
 	$(CXX) -O2 -std=c++17 -Wall -Iinclude -o $@ examples/offline_decode.cpp -Lltesniffer_b200 -lltephy_b200 -Wl,-rpath,'$$ORIGIN/../ltesniffer_b200'
@@ -35,8 +39,11 @@ examples/offline_ul: examples/offline_ul.cpp include/ltephy_b200.h include/lteph
 examples/cell_search: examples/cell_search.cpp include/ltephy_b200.h
 	$(CXX) -O2 -std=c++17 -Wall -Iinclude -o $@ examples/cell_search.cpp -Lltesniffer_b200 -lltephy_b200 -Wl,-rpath,'$$ORIGIN/../ltesniffer_b200'
 
-examples/decode_recording: examples/decode_recording.cpp include/ltephy_b200.h include/ltephy_search.h include/ltephy_sinks.h
+examples/decode_recording: examples/decode_recording.cpp examples/cell_chain.h include/ltephy_b200.h include/ltephy_search.h include/ltephy_sinks.h
 	$(CXX) -O2 -std=c++17 -Wall -Iinclude -o $@ examples/decode_recording.cpp -Lltesniffer_b200 -lltephy_b200 -Wl,-rpath,'$$ORIGIN/../ltesniffer_b200'
+
+examples/decode_wideband: examples/decode_wideband.cpp examples/cell_chain.h include/ltephy_b200.h include/ltephy_search.h include/ltephy_sinks.h
+	$(CXX) -O2 -std=c++17 -Wall -Iinclude -o $@ examples/decode_wideband.cpp -Lltesniffer_b200 -lltephy_b200 -Wl,-rpath,'$$ORIGIN/../ltesniffer_b200'
 
 examples/decode_recording_ul: examples/decode_recording_ul.cpp include/ltephy_b200.h include/ltephy_search.h include/ltephy_sinks.h
 	$(CXX) -O2 -std=c++17 -Wall -Iinclude -o $@ examples/decode_recording_ul.cpp -Lltesniffer_b200 -lltephy_b200 -Wl,-rpath,'$$ORIGIN/../ltesniffer_b200'
@@ -48,4 +55,4 @@ examples/compat_ul_check: examples/compat_ul_check.cpp compat/srsran/srsran.h in
 	$(CXX) -O2 -std=c++17 -Wall -Iinclude -Icompat -o $@ examples/compat_ul_check.cpp -Lltesniffer_b200 -lltephy_srsran_compat -lltephy_b200 -Wl,-rpath,'$$ORIGIN/../ltesniffer_b200'
 
 clean:
-	rm -f sim/*.so oracle/*.so oracle_track/*.so examples/offline_decode examples/offline_ul examples/compat_check examples/compat_ul_check examples/cell_search examples/decode_recording examples/decode_recording_ul
+	rm -f sim/*.so oracle/*.so oracle_track/*.so examples/offline_decode examples/offline_ul examples/compat_check examples/compat_ul_check examples/cell_search examples/decode_recording examples/decode_recording_ul examples/decode_wideband

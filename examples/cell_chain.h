@@ -1,0 +1,210 @@
+// cell_chain.h -- the per-cell chain of the recording examples (decode_recording.cpp, decode_wideband.cpp), host code over the C-ABI of
+// libltephy_b200: the MIB soft-combined over the frames of a capture, then, for every push of a tracker, the decoder and the DCI search on the cut
+// subframes, written to a MAC-LTE pcap and a DCI trace, with the lock counts and the summary lines.
+#pragma once
+#include "ltephy_b200.h"
+#include "ltephy_search.h"
+#include "ltephy_sinks.h"
+#include <cstdio>
+#include <cstdlib>
+#include <vector>
+
+// samples [s, s + n) of every antenna, antenna-major, from a file holding L samples per antenna
+static inline bool read_span(FILE* f, uint32_t A, uint64_t L, uint64_t s, uint64_t n, std::vector<float>& out)
+{
+  out.resize((size_t)2 * A * n);
+  for (uint32_t a = 0; a < A; a++) {
+    if (fseeko(f, (off_t)(8 * ((uint64_t)a * L + s)), SEEK_SET) != 0) return false;
+    if (fread(out.data() + (size_t)2 * a * n, 8, n, f) != n) return false;
+  }
+  return true;
+}
+
+// the MIB, soft-combined over nframes subframes 0 (cf32 [nframes][A][15 N], host memory, subframe 0 of frame f at tti 10 f) with the carrier
+// offset cfo_hz corrected and the port count searched; mib->sfn is that of frame 0.  0, 1 on a library error, 3 when no MIB passed
+static inline int chain_mib_host(const float* sf0, uint32_t nframes, uint32_t pci, float cfo_hz, uint32_t N, uint32_t A, ltephy_mib_t* mib)
+{
+  std::vector<uint32_t> tti0(nframes);
+  for (uint32_t f = 0; f < nframes; f++) tti0[f] = 10 * f;
+  ltephy_cfg_t mcfg{};
+  mcfg.nof_prb = 15, mcfg.nof_ports = 2, mcfg.cell_id = pci, mcfg.nof_rx = A, mcfg.max_subframes = nframes, mcfg.symbol_sz = N;
+  ltephy_t*                      mphy = nullptr;
+  std::vector<ltephy_mib_comb_t> m(nframes);
+  if (ltephy_create(&mcfg, &mphy) != LTEPHY_SUCCESS || ltephy_set_cfo(mphy, cfo_hz) != LTEPHY_SUCCESS ||
+      ltephy_submit_iq(mphy, sf0, tti0.data(), nframes) != LTEPHY_SUCCESS ||
+      ltephy_mib_decode_combined(mphy, LTEPHY_MIB_SEARCH_PORTS, m.data()) != LTEPHY_SUCCESS) {
+    fprintf(stderr, "MIB decode: %s\n", ltephy_last_error());
+    return 1;
+  }
+  ltephy_destroy(mphy);
+  *mib = ltephy_mib_t{};
+  for (uint32_t f = 0; f < nframes && !mib->found; f++)
+    if (m[f].mib.found) {
+      *mib     = m[f].mib;
+      mib->sfn = (mib->sfn + 1024 - f % 1024) % 1024; // the SFN of the frame at frame_offset
+    }
+  if (!mib->found) {
+    fprintf(stderr, "cell %u found, MIB not decoded\n", pci);
+    return 3;
+  }
+  return 0;
+}
+
+static inline void chain_print_cell(const ltephy_cell_t& c, const ltephy_mib_t& mib)
+{
+  printf("pci %u frame_offset %llu cfo_hz %.9g nof_prb %u nof_ports %u phich_resources %u phich_length %u sfn %u\n", c.pci,
+         (unsigned long long)c.frame_offset, c.cfo_hz, mib.nof_prb, mib.nof_ports, mib.phich_resources, mib.phich_length, mib.sfn);
+}
+
+// decoder, DCI search and sinks of one cell, fed with the pushes of its tracker
+struct CellChain {
+  uint32_t           N = 0, A = 0, SF = 0, B = 0;
+  int                reacq = 0;
+  ltephy_cell_t      cell{};
+  ltephy_t*          phy    = nullptr;
+  ltephy_search_t*   search = nullptr;
+  ltephy_t*          mibh   = nullptr; // the MIB decoder of the fallback after a re-acquisition
+  ltephy_pcap_t*     pcap   = nullptr;
+  FILE*              tsv    = nullptr;
+  bool               awaiting = false; // between a re-acquired subframe and the next MIB that passes: decode nothing
+  uint32_t           sfn_corr = 0;     // frames added to every tti (after the MIB read again, or when the tracker started at tti 0)
+  unsigned long long n_finds = 0, n_reacq = 0, n_await = 0;
+  unsigned long long n_sf = 0, n_dci = 0, n_tb = 0, n_ok = 0, n_locked = 0, n_lost = 0, n_hf = 0, n_hf_locked = 0, n_remeasured = 0;
+  int64_t            last_start = 0;
+  float              last_cfo   = 0.0f;
+  uint32_t                        max_dcis = 0;
+  std::vector<uint32_t>           ttis;
+  std::vector<ltephy_sf_info_t>   info;
+  std::vector<ltephy_cand_t>      scratch;
+  std::vector<ltephy_dci_t>       dcis;
+  std::vector<ltephy_tb_result_t> tbs;
+  std::vector<uint8_t>            payload;
+
+  // the decoder and the DCI search for the cell of the MIB; batches of up to B subframes.  0 or 1 (error printed)
+  int open_decoder(const ltephy_cell_t& c, const ltephy_mib_t& mib, uint32_t N_, uint32_t A_, uint32_t B_)
+  {
+    N = N_, A = A_, SF = 15 * N_, B = B_, cell = c, last_start = (int64_t)c.frame_offset, last_cfo = c.cfo_hz;
+    ltephy_cfg_t cfg{};
+    cfg.nof_prb = mib.nof_prb, cfg.nof_ports = mib.nof_ports, cfg.cell_id = c.pci, cfg.nof_rx = A, cfg.max_subframes = B, cfg.turbo_max_iter = 8;
+    cfg.flags = LTEPHY_FLAG_SKIP_LOW_POWER, cfg.symbol_sz = N, cfg.phich_resources = mib.phich_resources, cfg.phich_length = mib.phich_length;
+    if (ltephy_create(&cfg, &phy) != LTEPHY_SUCCESS) {
+      fprintf(stderr, "ltephy_create: %s\n", ltephy_last_error());
+      return 1;
+    }
+    search = ltephy_search_create(phy, 5); // rnti_histogram_threshold default of the reference
+    return 0;
+  }
+
+  // the fallback's MIB decoder (with reacquire) and the sinks.  0 or 1 (error printed)
+  int open_sinks(const ltephy_mib_t& mib, int reacquire, const char* pcap_path, const char* tsv_path)
+  {
+    reacq = reacquire;
+    // the MIB decoder of the fallback: the cell's bandwidth and ports are known, so no port search; the cut is already CFO-corrected
+    if (reacq) {
+      ltephy_cfg_t rcfg{};
+      rcfg.nof_prb = mib.nof_prb, rcfg.nof_ports = mib.nof_ports, rcfg.cell_id = cell.pci, rcfg.nof_rx = A, rcfg.max_subframes = 1, rcfg.symbol_sz = N;
+      if (ltephy_create(&rcfg, &mibh) != LTEPHY_SUCCESS) {
+        fprintf(stderr, "ltephy_create: %s\n", ltephy_last_error());
+        return 1;
+      }
+    }
+    pcap = ltephy_pcap_open(pcap_path);
+    tsv  = fopen(tsv_path, "w");
+    if (!pcap || !tsv) {
+      fprintf(stderr, "cannot open outputs\n");
+      return 1;
+    }
+    max_dcis = 32 * B;
+    ttis.resize(B), info.resize(B), scratch.resize((size_t)B * LTEPHY_MAX_LOC * LTEPHY_MAX_SIZES), dcis.resize(max_dcis);
+    tbs.resize(2 * (size_t)max_dcis), payload.resize((size_t)B * 64 * 1024);
+    return 0;
+  }
+
+  // one push of the cell's tracker: lock counts, the MIB fallback after a re-acquisition, decode, pcap and trace.  0 or 1 (error printed)
+  int consume(const ltephy_track_out_t& o)
+  {
+    char line[256];
+    n_remeasured += o.remeasured, n_hf += o.nof_half_frames, n_finds += o.finds;
+    for (uint32_t i = 0; i < o.nof_half_frames; i++) n_hf_locked += (o.hf[i].flags & LTEPHY_TRACK_LOCKED) != 0;
+    const uint32_t got = o.nof_subframes;
+    if (!got) return 0;
+    for (uint32_t i = 0; i < got; i++) {
+      ttis[i] = (o.sf[i].tti + 10 * sfn_corr) % 10240;
+      n_locked += (o.sf[i].flags & LTEPHY_TRACK_LOCKED) != 0, n_lost += (o.sf[i].flags & LTEPHY_TRACK_LOST) != 0;
+    }
+    last_start = o.sf[got - 1].start, last_cfo = o.sf[got - 1].cfo_hz;
+    // the push as runs of subframes to decode, split where the MIB fallback starts and ends
+    const size_t sf_bytes = (size_t)A * SF * 8;
+    for (uint32_t i0 = 0; i0 < got;) {
+      if (awaiting || (o.sf[i0].flags & LTEPHY_TRACK_REACQUIRED)) {
+        if (o.sf[i0].flags & LTEPHY_TRACK_REACQUIRED) {
+          if (ltephy_mib_reset(mibh) != LTEPHY_SUCCESS) {
+            fprintf(stderr, "ltephy_mib_reset: %s\n", ltephy_last_error());
+            return 1;
+          }
+          awaiting = true, n_reacq++;
+        }
+        n_await++;
+        if (o.sf[i0].tti % 10 == 0) {
+          ltephy_mib_comb_t mc{};
+          if (ltephy_submit_iq_device(mibh, static_cast<const char*>(o.iq_dev) + i0 * sf_bytes, &o.sf[i0].tti, 1) != LTEPHY_SUCCESS ||
+              ltephy_mib_decode_combined(mibh, 0, &mc) != LTEPHY_SUCCESS) {
+            fprintf(stderr, "MIB decode: %s\n", ltephy_last_error());
+            return 1;
+          }
+          if (mc.mib.found) {
+            sfn_corr = (mc.mib.sfn + 1024 - o.sf[i0].tti / 10 % 1024) % 1024, awaiting = false;
+            for (uint32_t i = i0 + 1; i < got; i++) ttis[i] = (o.sf[i].tti + 10 * sfn_corr) % 10240;
+          }
+        }
+        i0++;
+        continue;
+      }
+      uint32_t i1 = i0 + 1;
+      while (i1 < got && !(o.sf[i1].flags & LTEPHY_TRACK_REACQUIRED)) i1++;
+      const uint32_t m = i1 - i0, base = (uint32_t)(n_sf + i0);
+      uint32_t       nd = 0;
+      if (ltephy_decode_subframes_device(phy, search, static_cast<const char*>(o.iq_dev) + i0 * sf_bytes, ttis.data() + i0, m, LTEPHY_SEQ_NONE, info.data(),
+                                         scratch.data(), dcis.data(), max_dcis, &nd, tbs.data(), payload.data(), payload.size()) != LTEPHY_SUCCESS) {
+        fprintf(stderr, "ltephy_decode_subframes_device: %s\n", ltephy_last_error());
+        return 1;
+      }
+      // timestamps: capture time, 1 ms per subframe cut (as offline_decode)
+      for (uint32_t i = 0; i < nd; i++) {
+        const uint32_t t = ttis[i0 + dcis[i].sf];
+        const int      n = ltephy_dci_trace_line(search, &dcis[i], t, info[dcis[i].sf].cfi, tbs[2 * i].crc == 2 || tbs[2 * i + 1].crc == 2, (base + dcis[i].sf) / 1000,
+                                                 ((base + dcis[i].sf) % 1000) * 1000, line, sizeof(line));
+        if (n > 0) fwrite(line, 1, (size_t)n, tsv);
+        for (int k = 0; k < 2; k++) n_tb += tbs[2 * i + k].payload_len > 0, n_ok += tbs[2 * i + k].crc != 0;
+      }
+      if (ltephy_pcap_write_dl_batch(pcap, ttis.data() + i0, dcis.data(), nd, tbs.data(), payload.data(), 0, base / 1000, (base % 1000) * 1000) < 0) {
+        fprintf(stderr, "pcap write failed\n");
+        return 1;
+      }
+      n_dci += nd;
+      i0 = i1;
+    }
+    n_sf += got;
+    return 0;
+  }
+
+  // the tracking and decode summary lines
+  void print_summary() const
+  {
+    const long long drift = n_sf ? (long long)(last_start - (int64_t)cell.frame_offset - (int64_t)(n_sf - 1) * SF) : 0;
+    printf("tracking: subframes %llu locked %llu lost %llu  half-frames %llu locked %llu remeasured %llu  timing moved %lld samples  cfo_hz %.1f\n", n_sf,
+           n_locked, n_lost, n_hf, n_hf_locked, n_remeasured, drift, last_cfo);
+    printf("subframes %llu  dcis %llu  transport blocks %llu  crc ok %llu\n", n_sf, n_dci, n_tb, n_ok);
+    if (reacq) printf("reacquire: finds %llu reacquired %llu awaiting_mib %llu\n", n_finds, n_reacq, n_await);
+  }
+
+  void close()
+  {
+    if (tsv) fclose(tsv);
+    if (pcap) ltephy_pcap_close(pcap);
+    if (search) ltephy_search_destroy(search);
+    if (phy) ltephy_destroy(phy);
+    if (mibh) ltephy_destroy(mibh);
+    tsv = nullptr, pcap = nullptr, search = nullptr, phy = nullptr, mibh = nullptr;
+  }
+};

@@ -1,0 +1,203 @@
+// decode_wideband.cpp -- one wideband recording in, one pcap per carrier out: a continuous antenna-major cf32 capture at fs_in that holds several
+// LTE carriers, decoded through the C-ABI of libltephy_b200.  The capture is read one span at a time and the channeliser (ltephy_chan_run) shifts,
+// filters and decimates every carrier of the span to 15 kHz * N in one call.  Per carrier the chain of decode_recording follows on the carrier
+// stream in device memory: cell search on its first 40 ms (ltephy_cell_search_device), the tracker (ltephy_track_push_device), the MIB
+// soft-combined over the subframes 0 of the tracker's first cut, then ltephy_decode_subframes_device (cell_chain.h).  Host code only; without a
+// GPU ltephy_chan_create fails.
+//
+//   decode_wideband <iq.cf32> <fs_in> <nof_rx> <out_prefix> <offset_hz>:<N> [<offset_hz>:<N> ...] [subframes_per_push=500]
+//
+// Carrier c writes <out_prefix>_<c>.pcap and <out_prefix>_<c>.tsv and prints, in carrier order, a "carrier" line, then the cell line and the
+// summary lines in decode_recording's format.  The tracker starts at tti 0 on the cell search's frame timing; the MIB read from its cut gives the
+// SFN, added to every tti from then on.  Subframes cut before the first push whose subframes 0 pass the MIB are not decoded.  Each span of the
+// capture starts at the lowest sample any carrier's tracker still needs, so every carrier's output starts at or before what its tracker needs.
+#include "cell_chain.h"
+#include <algorithm>
+#include <cstring>
+#include <string>
+
+struct Carrier {
+  int32_t         offset_hz = 0;
+  uint32_t        N = 0, D = 0, H = 0, SF = 0;
+  bool            found = false, mib_found = false;
+  ltephy_cell_t   cell{};
+  ltephy_mib_t    mib{};
+  ltephy_track_t* tr   = nullptr;
+  ltephy_t*       mibh = nullptr; // MIB decoder on the tracker's cut (no port count known yet: searched)
+  uint64_t        next = 0;       // the tracker's next_sample, in carrier samples
+  CellChain       chain;
+};
+
+int main(int argc, char** argv)
+{
+  if (argc < 6) {
+    fprintf(stderr, "usage: %s <iq.cf32> <fs_in> <nof_rx> <out_prefix> <offset_hz>:<N> [<offset_hz>:<N> ...] [subframes_per_push=500]\n", argv[0]);
+    return 2;
+  }
+  const uint32_t       fs = (uint32_t)strtoul(argv[2], nullptr, 10), A = (uint32_t)atoi(argv[3]);
+  const std::string    prefix = argv[4];
+  std::vector<Carrier> car;
+  uint32_t             B = 500;
+  for (int i = 5; i < argc; i++) {
+    const char* colon = strchr(argv[i], ':');
+    if (!colon) {
+      B = (uint32_t)atoi(argv[i]);
+      continue;
+    }
+    Carrier k;
+    k.offset_hz = (int32_t)strtol(argv[i], nullptr, 10), k.N = (uint32_t)atoi(colon + 1), k.SF = 15 * k.N;
+    car.push_back(std::move(k));
+  }
+  FILE* in = fopen(argv[1], "rb");
+  if (!in || A < 1 || A > 2 || B < 1 || car.empty() || car.size() > LTEPHY_CHAN_MAX_CARRIERS || fs % 1000) {
+    fprintf(stderr, "cannot open %s / bad nof_rx, carriers, fs_in or subframes_per_push\n", argv[1]);
+    return 2;
+  }
+  fseeko(in, 0, SEEK_END);
+  const uint64_t L  = (uint64_t)ftello(in) / (8ull * A);
+  const uint64_t MS = fs / 1000; // capture samples per ms
+  ltephy_chan_cfg_t ccfg{};
+  ccfg.fs_in = fs, ccfg.nof_rx = A, ccfg.nof_carriers = (uint32_t)car.size();
+  for (size_t c = 0; c < car.size(); c++) ccfg.carrier[c].offset_hz = car[c].offset_hz, ccfg.carrier[c].symbol_sz = car[c].N;
+  uint32_t Tmax = 0;
+  for (size_t c = 0; c < car.size(); c++) {
+    uint32_t T, P;
+    if (ltephy_chan_taps(&ccfg, (uint32_t)c, nullptr, nullptr, nullptr, &T, &car[c].D, &P) != LTEPHY_SUCCESS) {
+      fprintf(stderr, "carrier %zu: %s\n", c, ltephy_last_error());
+      return 2;
+    }
+    car[c].H = T / 2, Tmax = std::max(Tmax, T);
+  }
+  // 1. the first 40 ms of every carrier (and the filter's reach past them) in one call; cell search on each carrier stream
+  const uint64_t L0   = std::min<uint64_t>(L, 40 * MS + Tmax);
+  const uint64_t span = std::min<uint64_t>(L, std::max<uint64_t>(L0, (uint64_t)(B + 20) * MS));
+  ccfg.max_samples    = span;
+  ltephy_chan_t* ch   = nullptr;
+  if (ltephy_chan_create(&ccfg, &ch) != LTEPHY_SUCCESS) {
+    fprintf(stderr, "ltephy_chan_create: %s\n", ltephy_last_error());
+    return 1;
+  }
+  std::vector<float>             x;
+  std::vector<ltephy_chan_out_t> out(car.size());
+  uint64_t                       nx = 0;
+  if (!read_span(in, A, L, 0, L0, x)) {
+    fprintf(stderr, "short read\n");
+    return 1;
+  }
+  if (ltephy_chan_run(ch, x.data(), 0, L0, out.data(), &nx) != LTEPHY_SUCCESS) {
+    fprintf(stderr, "ltephy_chan_run: %s\n", ltephy_last_error());
+    return 1;
+  }
+  int status = 0;
+  for (size_t c = 0; c < car.size(); c++) {
+    Carrier&          k = car[c];
+    ltephy_sync_cfg_t scfg{};
+    scfg.symbol_sz = k.N, scfg.nof_rx = A, scfg.max_samples = out[c].count;
+    ltephy_sync_t* sync = nullptr;
+    ltephy_cell_t  cells[3];
+    if (out[c].count < 75ull * k.N + k.N) {
+      fprintf(stderr, "carrier %zu: capture shorter than a half-frame\n", c);
+      status = 3;
+      continue;
+    }
+    if (ltephy_sync_create(&scfg, &sync) != LTEPHY_SUCCESS || ltephy_cell_search_device(sync, out[c].iq_dev, out[c].count, cells) != LTEPHY_SUCCESS) {
+      fprintf(stderr, "cell search: %s\n", ltephy_last_error());
+      return 1;
+    }
+    ltephy_sync_destroy(sync);
+    for (auto& q : cells)
+      if (q.detected) {
+        k.cell = q, k.found = true;
+        break;
+      }
+    if (!k.found) {
+      fprintf(stderr, "carrier %zu: no cell found\n", c);
+      status = 3;
+      continue;
+    }
+    // 2. the tracker from tti 0 at the found timing, and a MIB decoder for the subframes 0 of its cut
+    ltephy_track_cfg_t tcfg{};
+    tcfg.symbol_sz = k.N, tcfg.nof_rx = A, tcfg.pci = k.cell.pci, tcfg.first_tti = 0, tcfg.frame_offset = k.cell.frame_offset, tcfg.cfo_hz = k.cell.cfo_hz;
+    tcfg.max_ppm = 50.0f, tcfg.max_subframes = B;
+    ltephy_cfg_t mcfg{};
+    mcfg.nof_prb = 15, mcfg.nof_ports = 2, mcfg.cell_id = k.cell.pci, mcfg.nof_rx = A, mcfg.max_subframes = 1, mcfg.symbol_sz = k.N;
+    if (ltephy_track_create(&tcfg, &k.tr) != LTEPHY_SUCCESS || ltephy_create(&mcfg, &k.mibh) != LTEPHY_SUCCESS) {
+      fprintf(stderr, "tracker / MIB decoder: %s\n", ltephy_last_error());
+      return 1;
+    }
+    k.next = k.cell.frame_offset;
+  }
+  // 3. the capture one span at a time, from the lowest sample any tracker still needs; every carrier's cut through its chain
+  uint64_t recv = 0;
+  for (;;) {
+    if (recv < L) recv = recv + (uint64_t)B * MS < L ? recv + (uint64_t)B * MS : L;
+    uint64_t first = UINT64_MAX;
+    for (auto& k : car)
+      if (k.tr) first = std::min(first, k.next * k.D > k.H ? k.next * k.D - k.H : 0);
+    if (first == UINT64_MAX) break;
+    if (first >= recv) {
+      if (recv == L) break;
+      continue;
+    }
+    const uint64_t end = std::min(recv, first + span);
+    if (!read_span(in, A, L, first, end - first, x)) {
+      fprintf(stderr, "short read\n");
+      return 1;
+    }
+    if (ltephy_chan_run(ch, x.data(), first, end - first, out.data(), &nx) != LTEPHY_SUCCESS) {
+      fprintf(stderr, "ltephy_chan_run: %s\n", ltephy_last_error());
+      return 1;
+    }
+    bool any = false;
+    for (size_t c = 0; c < car.size(); c++) {
+      Carrier& k = car[c];
+      if (!k.tr || !out[c].count) continue;
+      ltephy_track_out_t o{};
+      if (ltephy_track_push_device(k.tr, out[c].iq_dev, out[c].first, out[c].count, &o) != LTEPHY_SUCCESS) {
+        fprintf(stderr, "ltephy_track_push_device: %s\n", ltephy_last_error());
+        return 1;
+      }
+      k.next = o.next_sample;
+      any    = any || o.nof_subframes > 0;
+      if (!k.mib_found) {
+        const size_t sf_bytes = (size_t)A * k.SF * 8;
+        for (uint32_t i = 0; i < o.nof_subframes && !k.mib_found; i++) {
+          if (o.sf[i].tti % 10) continue;
+          ltephy_mib_comb_t mc{};
+          if (ltephy_submit_iq_device(k.mibh, static_cast<const char*>(o.iq_dev) + i * sf_bytes, &o.sf[i].tti, 1) != LTEPHY_SUCCESS ||
+              ltephy_mib_decode_combined(k.mibh, LTEPHY_MIB_SEARCH_PORTS, &mc) != LTEPHY_SUCCESS) {
+            fprintf(stderr, "MIB decode: %s\n", ltephy_last_error());
+            return 1;
+          }
+          if (!mc.mib.found) continue;
+          k.mib = mc.mib, k.mib_found = true;
+          k.mib.sfn = (mc.mib.sfn + 1024 - o.sf[i].tti / 10 % 1024) % 1024; // the SFN of the frame at frame_offset
+          const std::string base = prefix + "_" + std::to_string(c);
+          if (k.chain.open_decoder(k.cell, k.mib, k.N, A, B) || !k.chain.search || k.chain.open_sinks(k.mib, 0, (base + ".pcap").c_str(), (base + ".tsv").c_str()))
+            return 1;
+          k.chain.sfn_corr = k.mib.sfn;
+        }
+        if (!k.mib_found) continue;
+      }
+      if (k.chain.consume(o)) return 1;
+    }
+    if (!any && recv == L) break;
+  }
+  for (size_t c = 0; c < car.size(); c++) {
+    Carrier& k = car[c];
+    printf("carrier %zu offset_hz %d symbol_sz %u\n", c, k.offset_hz, k.N);
+    if (k.found && k.mib_found) {
+      chain_print_cell(k.cell, k.mib);
+      k.chain.print_summary();
+    } else {
+      printf(k.found ? "cell %u found, MIB not decoded\n" : "no cell found\n", k.cell.pci);
+      status = 3;
+    }
+    k.chain.close();
+    if (k.tr) ltephy_track_destroy(k.tr);
+    if (k.mibh) ltephy_destroy(k.mibh);
+  }
+  ltephy_chan_destroy(ch);
+  fclose(in);
+  return status;
+}

@@ -377,6 +377,50 @@ int  ltephy_track_push_ul(ltephy_track_t* h, const float* iq, const float* iq_ul
 int  ltephy_track_push_ul_device(ltephy_track_t* h, const void* iq_dev, const void* iq_ul_dev, uint64_t first_sample, uint64_t nof_samples,
                                  ltephy_track_out_t* out, const void** ul_iq_dev);
 
+/* Channeliser: several carriers from one wideband capture.  Each carrier is shifted to 0 Hz, low-pass filtered and decimated by an integer
+ * D = fs_in / (15 kHz * symbol_sz) to the rate the cell search and the tracker take.  The filter, its arithmetic and the output range of a call are
+ * DESIGN.md §2 ("channeliser"); the CPU oracle lteo_chan_run (oracle/lte_chan_oracle.h) defines every output sample bit for bit.  Output m of a
+ * carrier belongs to input time m D (zero group delay), so a cell's timing in a carrier stream is its timing in the capture divided by D.
+ * The handle keeps no state between calls: the outputs do not depend on how the capture is split. */
+#define LTEPHY_CHAN_MAX_CARRIERS 8
+#define LTEPHY_CHAN_MAX_FS 245760000u
+typedef struct ltephy_chan ltephy_chan_t;
+typedef struct {
+  int32_t  offset_hz; /* carrier centre minus capture centre, a multiple of 1000 */
+  uint32_t symbol_sz; /* N of the carrier: 128, 256, 384, 512, 768, 1024, 1536 or 2048; its rate is 15 kHz * N */
+} ltephy_chan_carrier_t;
+typedef struct {
+  uint32_t              fs_in;        /* capture rate in Hz, at most LTEPHY_CHAN_MAX_FS; fs_in / (15 kHz * N) must be an integer 2..128 */
+  uint32_t              nof_rx;       /* 1 or 2 antennas */
+  uint32_t              nof_carriers; /* 1..LTEPHY_CHAN_MAX_CARRIERS */
+  uint32_t              pad;
+  ltephy_chan_carrier_t carrier[LTEPHY_CHAN_MAX_CARRIERS];
+  uint64_t              max_samples;  /* longest call per antenna, 1..2^31 (device memory is sized for it) */
+  int32_t               device;       /* CUDA device ordinal */
+  uint32_t              reserved[5];
+} ltephy_chan_cfg_t;
+typedef struct {
+  uint64_t    first;  /* carrier sample index of the first output of this call */
+  uint64_t    count;  /* outputs per antenna */
+  const void* iq_dev; /* cf32 [nof_rx][count] in device memory (what ltephy_cell_search_device / ltephy_track_push_device take), valid until the next call */
+} ltephy_chan_out_t;
+/* INVALID_INPUTS, before any device is looked for, for: a carrier whose D is not an integer in 2..128, an offset off the 1 kHz grid, a carrier whose
+ * widest occupied band (|offset_hz| + 90 kHz * the largest PRB count of its N) reaches past fs_in / 2, an unknown N, 0 or more than 8 carriers,
+ * nof_rx other than 1 or 2, fs_in above LTEPHY_CHAN_MAX_FS, max_samples 0 or above 2^31. */
+int  ltephy_chan_create(const ltephy_chan_cfg_t* cfg, ltephy_chan_t** h);
+void ltephy_chan_destroy(ltephy_chan_t* h);
+/* iq: cf32 [nof_rx][nof_samples], antenna-major, host memory: capture samples first_sample .. first_sample + nof_samples - 1 (1 <= nof_samples <=
+ * max_samples).  out[nof_carriers]: every output m >= 0 of each carrier whose filter window [m D - H, m D + H] has all its non-negative samples
+ * inside the call (samples before 0 count as zero).  *next_sample: the lowest capture sample the next call must still include for every carrier
+ * to continue without a gap; a carrier's first output in that call may repeat outputs of this one.  Blocks until the outputs are complete. */
+int  ltephy_chan_run(ltephy_chan_t* h, const float* iq, uint64_t first_sample, uint64_t nof_samples, ltephy_chan_out_t* out, uint64_t* next_sample);
+/* same, with the samples already in device memory on the handle's device */
+int  ltephy_chan_run_device(ltephy_chan_t* h, const void* iq_dev, uint64_t first_sample, uint64_t nof_samples, ltephy_chan_out_t* out,
+                            uint64_t* next_sample);
+/* host only, needs no device: the tables of carrier c (< nof_carriers) as the kernel uses them.  h: f32 [T] prototype, g: cf32 [T] band-pass taps g[k] at index
+ * k + H, rot: cf32 [P] output rotation r[m mod P]; any of the three may be NULL.  *T (odd, H = (T - 1) / 2), *D and *P are always written. */
+int  ltephy_chan_taps(const ltephy_chan_cfg_t* cfg, uint32_t c, float* h, float* g, float* rot, uint32_t* T, uint32_t* D, uint32_t* P);
+
 /* nslots HARQ slots of LTEPHY_HARQ_SLOT_BYTES each (150 RNTIs x 8 processes x 2 TBs = 2400 slots = 1.4 GB); contents survive across batches */
 int ltephy_harq_reserve(ltephy_t* h, uint32_t nslots);
 

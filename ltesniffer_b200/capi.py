@@ -923,3 +923,121 @@ class Tracker:
         o, u = TrackOut(), C.c_void_p()
         return self._done(self.L.ltephy_track_push_ul_device(self.h, C.c_void_p(iq.data_ptr()), C.c_void_p(iq_ul.data_ptr()), first_sample, iq.shape[1],
                                                              C.byref(o), C.byref(u)), o, u)
+
+
+# ------------------------------------------------------------------------------------------------
+# channeliser (ltephy_chan_*, include/ltephy_b200.h)
+CHAN_MAX_CARRIERS = 8
+
+
+class ChanCarrier(C.Structure):
+    _fields_ = [("offset_hz", C.c_int32), ("symbol_sz", C.c_uint32)]
+
+
+class ChanCfg(C.Structure):
+    _fields_ = [("fs_in", C.c_uint32), ("nof_rx", C.c_uint32), ("nof_carriers", C.c_uint32), ("pad", C.c_uint32),
+                ("carrier", ChanCarrier * CHAN_MAX_CARRIERS), ("max_samples", C.c_uint64), ("device", C.c_int32), ("reserved", C.c_uint32 * 5)]
+
+
+class ChanOut(C.Structure):
+    _fields_ = [("first", C.c_uint64), ("count", C.c_uint64), ("iq_dev", C.c_void_p)]
+
+
+assert C.sizeof(ChanCfg) == 112 and C.sizeof(ChanOut) == 24
+
+
+def _bind_chan(L):
+    L.ltephy_chan_create.argtypes = [C.POINTER(ChanCfg), C.POINTER(C.c_void_p)]
+    L.ltephy_chan_destroy.argtypes = [C.c_void_p]
+    L.ltephy_chan_run.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p, C.POINTER(C.c_uint64)]
+    L.ltephy_chan_run_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p, C.POINTER(C.c_uint64)]
+    L.ltephy_chan_taps.argtypes = [C.POINTER(ChanCfg), C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32),
+                                   C.POINTER(C.c_uint32)]
+
+
+def chan_cfg(fs_in, carriers, nof_rx=1, max_samples=1, device=0):
+    """ChanCfg from carriers = [(offset_hz, symbol_sz), ...]"""
+    cfg = ChanCfg(fs_in=fs_in, nof_rx=nof_rx, nof_carriers=len(carriers), max_samples=max_samples, device=device)
+    for i, (off, n) in enumerate(carriers[:CHAN_MAX_CARRIERS]):
+        cfg.carrier[i] = ChanCarrier(off, n)
+    return cfg
+
+
+def chan_taps(fs_in, carriers, c):
+    """host-only tables of carrier c -> dict(h float32 [T], g complex64 [T], rot complex64 [P], T, D, P); RuntimeError when refused"""
+    L = load_library()
+    _bind_chan(L)
+    cfg = chan_cfg(fs_in, carriers)
+    T, D, P = C.c_uint32(), C.c_uint32(), C.c_uint32()
+    r = L.ltephy_chan_taps(C.byref(cfg), c, None, None, None, C.byref(T), C.byref(D), C.byref(P))
+    if r != 0:
+        raise RuntimeError("ltephy_chan_taps failed (%d): %s" % (r, L.ltephy_last_error().decode()))
+    h, g, rot = np.zeros(T.value, np.float32), np.zeros(T.value, np.complex64), np.zeros(P.value, np.complex64)
+    L.ltephy_chan_taps(C.byref(cfg), c, _p(h), _p(g), _p(rot), C.byref(T), C.byref(D), C.byref(P))
+    return dict(h=h, g=g, rot=rot, T=T.value, D=D.value, P=P.value)
+
+
+class Channelizer:
+    """Shift, filter and decimate the carriers [(offset_hz, symbol_sz), ...] of a capture at fs_in out of antenna-major complex64 [nof_rx][n]
+    spans of up to max_samples; each run returns every carrier's outputs that the span completes, and next_sample, the lowest capture sample the
+    next run must still include."""
+
+    def __init__(self, fs_in, carriers, nof_rx, max_samples, device=0):
+        self.L = load_library()
+        _bind_chan(self.L)
+        self.carriers = list(carriers)
+        self.cfg = chan_cfg(fs_in, self.carriers, nof_rx, max_samples, device)
+        self.h = C.c_void_p()
+        r = self.L.ltephy_chan_create(C.byref(self.cfg), C.byref(self.h))
+        if r != 0:
+            self.h = None
+            raise RuntimeError("ltephy_chan_create failed (%d): %s" % (r, self.L.ltephy_last_error().decode()))
+        self.next_sample = 0
+
+    def close(self):
+        if self.h:
+            self.L.ltephy_chan_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def taps(self, c):
+        return chan_taps(self.cfg.fs_in, self.carriers, c)
+
+    def _done(self, r, out, nxt, copy):
+        if r != 0:
+            raise RuntimeError("ltephy_chan_run failed (%d): %s" % (r, self.L.ltephy_last_error().decode()))
+        import torch
+        res = []
+        for c in range(len(self.carriers)):
+            o = out[c]
+            shape = (self.cfg.nof_rx, o.count)
+            if o.count:
+                view = type("_Chan", (), {"__cuda_array_interface__": dict(shape=shape, typestr="<c8", data=(o.iq_dev, False), version=2)})()
+                with torch.cuda.device(self.cfg.device):
+                    iq = torch.as_tensor(view, device="cuda:%d" % self.cfg.device)
+                    iq = iq.clone() if copy else iq
+            else:
+                iq = torch.empty(shape, dtype=torch.complex64, device="cuda:%d" % self.cfg.device)
+            res.append(dict(first=o.first, count=o.count, iq=iq))
+        self.next_sample = nxt.value
+        return res, nxt.value
+
+    def run(self, iq, first_sample, copy=True):
+        """iq: complex64 [nof_rx][n] (host) of capture samples first_sample ... -> ([dict(first, count, iq: torch complex64 [nof_rx][count] on the
+        device)] per carrier, next_sample).  With copy=False iq views the handle's buffer, valid until the next run."""
+        iq = np.ascontiguousarray(iq, np.complex64)
+        assert iq.ndim == 2 and iq.shape[0] == self.cfg.nof_rx, iq.shape
+        out, nxt = (ChanOut * CHAN_MAX_CARRIERS)(), C.c_uint64()
+        return self._done(self.L.ltephy_chan_run(self.h, _p(iq), first_sample, iq.shape[1], out, C.byref(nxt)), out, nxt, copy)
+
+    def run_device(self, iq, first_sample, copy=True):
+        """iq: torch complex64 [nof_rx][n], contiguous, on this handle's device"""
+        assert iq.is_cuda and iq.is_contiguous() and iq.dim() == 2 and iq.shape[0] == self.cfg.nof_rx
+        out, nxt = (ChanOut * CHAN_MAX_CARRIERS)(), C.c_uint64()
+        return self._done(self.L.ltephy_chan_run_device(self.h, C.c_void_p(iq.data_ptr()), first_sample, iq.shape[1], out, C.byref(nxt)), out, nxt,
+                          copy)

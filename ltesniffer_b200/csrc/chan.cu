@@ -1,0 +1,233 @@
+// chan.cu -- host side of the channeliser (include/ltephy_b200.h, DESIGN.md §2 "channeliser"): the per-carrier filter design in double precision,
+// the output range of a call, and one launch of k_chan.cu over every (carrier, antenna, tile).  The tables equal lteo_chan_design's bit for bit.
+#include "../../include/ltephy_b200.h"
+#include "k_chan.cuh"
+#include "ltephy_internal.cuh"
+#include <algorithm>
+#include <cmath>
+#include <cstdlib>
+#include <vector>
+
+#define CHAN_ATTEN 70.0 // stop-band target (dB) of Kaiser's formulas
+#define CHAN_SPAN 4096  // input samples a tile aims to stage: M = min(1024, max(64, (CHAN_SPAN - T) / D + 1)) outputs
+
+struct ltephy_chan {
+  ltephy_chan_cfg_t cfg{};
+  Stream            stream;
+  struct Carrier {
+    uint32_t       T = 0, D = 0, P = 0, M = 0, rows = 0;
+    uint64_t       cap = 0; // outputs per antenna the buffer holds
+    DevBuf<float2> g, rot, out;
+  } car[LTEPHY_CHAN_MAX_CARRIERS];
+  DevBuf<float2> d_x;
+  size_t         smem = 0;
+};
+
+static uint32_t chan_max_prb(uint32_t N)
+{
+  switch (N) {
+    case 128: return 6;
+    case 256: return 15;
+    case 384: case 512: return 25;
+    case 768: case 1024: return 50;
+    case 1536: case 2048: return 100;
+    default: return 0;
+  }
+}
+
+static double chan_i0(double x) // modified Bessel function I0, power series until the term no longer changes the sum
+{
+  double s = 1.0, t = 1.0, q = 0.25 * x * x;
+  for (int k = 1; k < 500; k++) {
+    t = t * q / ((double)k * (double)k);
+    s = s + t;
+    if (t < 1e-17 * s) break;
+  }
+  return s;
+}
+
+static int64_t chan_mod(int64_t a, int64_t fs) { return ((a % fs) + fs) % fs; }
+
+// decimation D, odd filter length T and rotation period P of one carrier; 0, or INVALID_INPUTS with the reason in the last error
+static int chan_geometry(uint32_t fs_in, int32_t offset_hz, uint32_t N, uint32_t* T, uint32_t* D, uint32_t* P)
+{
+  const uint32_t prb = chan_max_prb(N);
+  if (!prb) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: symbol size %u not supported", N);
+  if (fs_in == 0 || fs_in > LTEPHY_CHAN_MAX_FS) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: fs_in %u outside 1..245760000", fs_in);
+  if (offset_hz % 1000) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: offset %d Hz is not a multiple of 1 kHz", offset_hz);
+  const uint64_t fs_out = 15000ull * N;
+  if (fs_in % fs_out || fs_in / fs_out < 2 || fs_in / fs_out > 128)
+    return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: fs_in %u / %llu is not an integer decimation 2..128", fs_in, (unsigned long long)fs_out);
+  const uint64_t d = fs_in / fs_out, f_pass = 90000ull * prb, aoff = (uint64_t)std::llabs((long long)offset_hz);
+  if (2 * (aoff + f_pass) > fs_in)
+    return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: band of the carrier at %d Hz (N %u) reaches outside the capture", offset_hz, N);
+  // Kaiser's length for 70 dB over the transition band [f_pass, fs_out - f_pass], width relative to fs_in / 2 (scipy.signal.kaiserord), made odd
+  const double width = (double)(fs_out - 2 * f_pass) / (0.5 * (double)fs_in);
+  const double nt    = (CHAN_ATTEN - 7.95) / 2.285 / (M_PI * width) + 1.0;
+  *T = (uint32_t)std::ceil(nt) | 1u;
+  *D = (uint32_t)d;
+  int64_t a = chan_mod((int64_t)d * offset_hz, fs_in), b = fs_in; // P = fs_in / gcd(D offset mod fs_in, fs_in)
+  while (b) {
+    const int64_t t = a % b;
+    a = b, b = t;
+  }
+  *P = (uint32_t)(fs_in / a);
+  return LTEPHY_SUCCESS;
+}
+
+// the tables of one carrier, in the arithmetic of lteo_chan_design
+static int chan_design(uint32_t fs_in, int32_t offset_hz, uint32_t N, float* h, float* g, float* rot, uint32_t* T, uint32_t* D, uint32_t* P)
+{
+  if (int r = chan_geometry(fs_in, offset_hz, N, T, D, P)) return r;
+  const uint32_t t = *T, d = *D, p = *P;
+  const int64_t  H = (t - 1) / 2, fs = fs_in;
+  if (h || g) {
+    // windowed sinc with cutoff fs_out / 2 = fs_in / (2 D), scaled to DC gain 1 (scipy.signal.firwin)
+    std::vector<double> hd(t);
+    const double beta = 0.1102 * (CHAN_ATTEN - 8.7), a = 0.5 * (double)(t - 1), i0b = chan_i0(beta), c = 1.0 / (double)d;
+    double       s = 0.0;
+    for (int64_t j = 0; j < (int64_t)t; j++) {
+      const double m  = (double)(j - H) * c;
+      const double sn = m == 0.0 ? 1.0 : std::sin(M_PI * m) / (M_PI * m);
+      const double r  = ((double)j - a) / a;
+      const double w  = chan_i0(beta * std::sqrt(1.0 - r * r)) / i0b;
+      hd[j]           = c * sn * w;
+      s               = s + hd[j];
+    }
+    for (int64_t j = 0; j < (int64_t)t; j++) {
+      const double hn = hd[j] / s;
+      if (h) h[j] = (float)hn;
+      if (g) { // g[k] = h[k] e^{+j omega k}, omega = 2 pi offset / fs_in, the phase reduced in integers first
+        const double ph = 2.0 * M_PI * (double)chan_mod((int64_t)offset_hz * (j - H), fs) / (double)fs;
+        g[2 * j]        = (float)(hn * std::cos(ph));
+        g[2 * j + 1]    = (float)(hn * std::sin(ph));
+      }
+    }
+  }
+  if (rot) { // r[i] = e^{-j omega i D}
+    const int64_t step = chan_mod((int64_t)d * offset_hz, fs);
+    for (int64_t i = 0; i < (int64_t)p; i++) {
+      const double ph = -2.0 * M_PI * (double)((step * i) % fs) / (double)fs;
+      rot[2 * i]      = (float)std::cos(ph);
+      rot[2 * i + 1]  = (float)std::sin(ph);
+    }
+  }
+  return LTEPHY_SUCCESS;
+}
+
+static int chan_check_cfg(const ltephy_chan_cfg_t* cfg)
+{
+  if (!cfg) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: null configuration");
+  if (cfg->nof_rx < 1 || cfg->nof_rx > 2) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: %u antennas not supported", cfg->nof_rx);
+  if (cfg->nof_carriers < 1 || cfg->nof_carriers > LTEPHY_CHAN_MAX_CARRIERS)
+    return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: %u carriers, not 1..8", cfg->nof_carriers);
+  if (cfg->max_samples < 1 || cfg->max_samples > (1ull << 31)) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: max_samples outside 1..2^31");
+  for (uint32_t c = 0; c < cfg->nof_carriers; c++) {
+    uint32_t T, D, P;
+    if (int r = chan_geometry(cfg->fs_in, cfg->carrier[c].offset_hz, cfg->carrier[c].symbol_sz, &T, &D, &P)) return r;
+  }
+  return LTEPHY_SUCCESS;
+}
+
+extern "C" int ltephy_chan_taps(const ltephy_chan_cfg_t* cfg, uint32_t c, float* h, float* g, float* rot, uint32_t* T, uint32_t* D, uint32_t* P)
+{
+  if (!cfg || !T || !D || !P) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan_taps: null argument");
+  if (c >= cfg->nof_carriers || c >= LTEPHY_CHAN_MAX_CARRIERS)
+    return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan_taps: carrier %u of %u", c, cfg->nof_carriers);
+  return chan_design(cfg->fs_in, cfg->carrier[c].offset_hz, cfg->carrier[c].symbol_sz, h, g, rot, T, D, P);
+}
+
+extern "C" int ltephy_chan_create(const ltephy_chan_cfg_t* cfg, ltephy_chan_t** out)
+{
+  if (!out) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan_create: null argument");
+  if (int r = chan_check_cfg(cfg)) return r;
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail(LTEPHY_ERROR, "no CUDA device: this library has no CPU path");
+  CU(cudaSetDevice(cfg->device));
+  std::unique_ptr<ltephy_chan, decltype(&ltephy_chan_destroy)> owner(new ltephy_chan(), ltephy_chan_destroy);
+  ltephy_chan* const                                           h = owner.get();
+  h->cfg                                                         = *cfg;
+  CU(cudaStreamCreateWithFlags(&h->stream.raw, cudaStreamNonBlocking));
+  if (h->d_x.reserve((size_t)cfg->nof_rx * cfg->max_samples)) return fail(LTEPHY_ERROR, "chan_create: device allocation failed");
+  for (uint32_t c = 0; c < cfg->nof_carriers; c++) {
+    ltephy_chan::Carrier& k = h->car[c];
+    chan_design(cfg->fs_in, cfg->carrier[c].offset_hz, cfg->carrier[c].symbol_sz, nullptr, nullptr, nullptr, &k.T, &k.D, &k.P);
+    std::vector<float> g(2 * (size_t)k.T), rot(2 * (size_t)k.P);
+    chan_design(cfg->fs_in, cfg->carrier[c].offset_hz, cfg->carrier[c].symbol_sz, nullptr, g.data(), rot.data(), &k.T, &k.D, &k.P);
+    const int64_t fit = ((int64_t)CHAN_SPAN - (int64_t)k.T) / (int64_t)k.D + 1;
+    k.M    = (uint32_t)std::min<int64_t>(1024, std::max<int64_t>(64, fit));
+    k.rows = k.M - 1 + (k.T + k.D - 1) / k.D;
+    k.cap  = cfg->max_samples / k.D + 2;
+    h->smem = std::max(h->smem, ((size_t)k.T + (size_t)k.rows * k.D) * sizeof(float2));
+    if (k.g.reserve(k.T) || k.rot.reserve(k.P) || k.out.reserve((size_t)cfg->nof_rx * k.cap))
+      return fail(LTEPHY_ERROR, "chan_create: device allocation failed");
+    CU(cudaMemcpy(k.g.p, g.data(), g.size() * sizeof(float), cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(k.rot.p, rot.data(), rot.size() * sizeof(float), cudaMemcpyHostToDevice));
+  }
+  *out = owner.release();
+  return LTEPHY_SUCCESS;
+}
+
+extern "C" void ltephy_chan_destroy(ltephy_chan_t* h)
+{
+  if (!h) return;
+  cudaSetDevice(h->cfg.device);
+  if (h->stream) cudaStreamSynchronize(h->stream);
+  delete h;
+}
+
+static int chan_check(ltephy_chan_t* h, const void* iq, uint64_t first, uint64_t n, ltephy_chan_out_t* out, uint64_t* next)
+{
+  if (!h || !iq || !out || !next) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan_run: null argument");
+  if (n < 1 || n > h->cfg.max_samples) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan_run: %llu samples, not 1..max_samples", (unsigned long long)n);
+  if (first > UINT64_MAX / 2) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan_run: first_sample too large");
+  return LTEPHY_SUCCESS;
+}
+
+static int chan_run(ltephy_chan_t* h, const float2* x, uint64_t first, uint64_t n, ltephy_chan_out_t* out, uint64_t* next)
+{
+  const uint32_t A = h->cfg.nof_rx;
+  ChanArgs       g{};
+  g.x = x, g.lda = n, g.first = first;
+  uint32_t ntiles = 0;
+  uint64_t nx     = UINT64_MAX;
+  for (uint32_t c = 0; c < h->cfg.nof_carriers; c++) {
+    const ltephy_chan::Carrier& k = h->car[c];
+    // outputs m >= 0 whose window [m D - H, m D + H] has every non-negative sample inside [first, first + n)
+    const uint64_t H = k.T / 2, last = first + n - 1;
+    const uint64_t lo   = first == 0 ? 0 : (first + H + k.D - 1) / k.D;
+    const uint64_t hi_n = last >= H ? (last - H) / k.D + 1 : 0;
+    const uint64_t cnt  = hi_n > lo ? hi_n - lo : 0;
+    const uint64_t mn   = cnt ? hi_n : lo;
+    nx                  = std::min(nx, mn * k.D >= H ? mn * k.D - H : 0);
+    out[c].first = lo, out[c].count = cnt, out[c].iq_dev = k.out.p;
+    if (!cnt) continue;
+    const uint32_t tiles = (uint32_t)((cnt + k.M - 1) / k.M);
+    for (uint32_t a = 0; a < A; a++) {
+      ChanSeg& s = g.seg[g.nseg++];
+      s.g = k.g.p, s.rot = k.rot.p, s.out = k.out.p + (size_t)a * cnt, s.m0 = lo, s.count = (uint32_t)cnt;
+      s.D = k.D, s.T = k.T, s.P = k.P, s.M = k.M, s.rows = k.rows, s.tile0 = ntiles, s.a = a;
+      ntiles += tiles;
+    }
+  }
+  *next = nx;
+  if (launch_chan(g, ntiles, h->smem, h->stream)) return fail(LTEPHY_ERROR, "chan_run: kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
+  CU(cudaStreamSynchronize(h->stream));
+  return LTEPHY_SUCCESS;
+}
+
+extern "C" int ltephy_chan_run(ltephy_chan_t* h, const float* iq, uint64_t first_sample, uint64_t nof_samples, ltephy_chan_out_t* out, uint64_t* next_sample)
+{
+  if (int r = chan_check(h, iq, first_sample, nof_samples, out, next_sample)) return r;
+  CU(cudaSetDevice(h->cfg.device));
+  CU(cudaMemcpyAsync(h->d_x.p, iq, (size_t)h->cfg.nof_rx * nof_samples * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
+  return chan_run(h, h->d_x.p, first_sample, nof_samples, out, next_sample);
+}
+
+extern "C" int ltephy_chan_run_device(ltephy_chan_t* h, const void* iq_dev, uint64_t first_sample, uint64_t nof_samples, ltephy_chan_out_t* out,
+                                      uint64_t* next_sample)
+{
+  if (int r = chan_check(h, iq_dev, first_sample, nof_samples, out, next_sample)) return r;
+  CU(cudaSetDevice(h->cfg.device));
+  return chan_run(h, static_cast<const float2*>(iq_dev), first_sample, nof_samples, out, next_sample);
+}
