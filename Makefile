@@ -5,7 +5,7 @@ CXX ?= g++
 CFLAGS = -O3 -g -fPIC -std=gnu11 -Wall -Wno-unused-function -ffp-contract=off -fno-fast-math
 CXXFLAGS = -O2 -g -fPIC -std=c++17 -Wall -ffp-contract=off -fno-fast-math
 
-all: sim/libltesim.so oracle/liblteoracle.so oracle/liblteosync.so oracle/liblteomib.so oracle_track/liblteotrack.so oracle/liblteochan.so
+all: sim/libltesim.so oracle/liblteoracle.so oracle/liblteosync.so oracle/liblteomib.so oracle_track/liblteotrack.so oracle/liblteochan.so oracle/liblteochanpoly.so
 
 sim/libltesim.so: sim/lte_common.c sim/lte_sim.c sim/lte_common.h sim/lte_sim.h include/lte_tables.h
 	$(CC) $(CFLAGS) -shared -o $@ sim/lte_common.c sim/lte_sim.c -lm
@@ -28,6 +28,10 @@ oracle_track/liblteotrack.so: oracle_track/lte_track_oracle.c oracle_track/lte_t
 # channeliser oracle: stands alone
 oracle/liblteochan.so: oracle/lte_chan_oracle.c oracle/lte_chan_oracle.h
 	$(CC) $(CFLAGS) -shared -o $@ oracle/lte_chan_oracle.c -lm
+
+# rational carriers and integer samples: integer carriers are lteo_chan_design's, from liblteochan.so
+oracle/liblteochanpoly.so: oracle/lte_chan_poly_oracle.c oracle/lte_chan_poly_oracle.h oracle/lte_chan_oracle.h oracle/liblteochan.so
+	$(CC) $(CFLAGS) -shared -o $@ oracle/lte_chan_poly_oracle.c -Loracle -llteochan -Wl,-rpath,'$$ORIGIN' -lm
 
 # C++ example of the C-ABI (needs ltesniffer_b200/libltephy_b200.so, built by ltesniffer_b200/build.py)
 examples/offline_decode: examples/offline_decode.cpp include/ltephy_b200.h include/ltephy_search.h include/ltephy_sinks.h

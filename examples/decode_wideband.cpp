@@ -1,24 +1,38 @@
-// decode_wideband.cpp -- one wideband recording in, one pcap per carrier out: a continuous antenna-major cf32 capture at fs_in that holds several
-// LTE carriers, decoded through the C-ABI of libltephy_b200.  The capture is read one span at a time and the channeliser (ltephy_chan_run) shifts,
-// filters and decimates every carrier of the span to 15 kHz * N in one call.  Per carrier the chain of decode_recording follows on the carrier
+// decode_wideband.cpp -- one wideband recording in, one pcap per carrier out: a continuous antenna-major capture (cf32, sc16 or sc8) at any rate
+// fs_in that holds one or several LTE carriers, decoded through the C-ABI of libltephy_b200.  The capture is read one span at a time and the
+// channeliser (ltephy_chan_run, LTEPHY_CHAN_RATIONAL set) shifts, filters and resamples every carrier of the span to 15 kHz * N in one call.  Per carrier the chain of decode_recording follows on the carrier
 // stream in device memory: cell search on its first 40 ms (ltephy_cell_search_device), the tracker (ltephy_track_push_device), the MIB
 // soft-combined over the subframes 0 of the tracker's first cut, then ltephy_decode_subframes_device (cell_chain.h).  Host code only; without a
 // GPU ltephy_chan_create fails.
 //
-//   decode_wideband <iq.cf32> <fs_in> <nof_rx> <out_prefix> <offset_hz>:<N> [<offset_hz>:<N> ...] [subframes_per_push=500]
+//   decode_wideband <iq file> <fs_in> <nof_rx> <out_prefix> <offset_hz>:<N> [<offset_hz>:<N> ...] [subframes_per_push=500] [fmt=cf32|sc16|sc8]
 //
+// A single-carrier capture at any rate, e.g. a 20 Msps sc16 recording of a 20 MHz cell, decodes with the one carrier 0:2048.
 // Carrier c writes <out_prefix>_<c>.pcap and <out_prefix>_<c>.tsv and prints, in carrier order, a "carrier" line, then the cell line and the
 // summary lines in decode_recording's format.  The tracker starts at tti 0 on the cell search's frame timing; the MIB read from its cut gives the
 // SFN, added to every tti from then on.  Subframes cut before the first push whose subframes 0 pass the MIB are not decoded.  Each span of the
-// capture starts at the lowest sample any carrier's tracker still needs, so every carrier's output starts at or before what its tracker needs.
+// capture starts at the lowest sample any carrier's tracker still needs, so every carrier's output starts at or before what its tracker needs:
+// carrier sample s needs capture samples from floor(s M / L) - Ka (ltephy_chan_design).
 #include "cell_chain.h"
 #include <algorithm>
 #include <cstring>
 #include <string>
 
+// samples s .. s + n - 1 of every antenna of an antenna-major file of L samples per antenna, b bytes per complex sample, into out
+static bool read_span_fmt(FILE* f, uint32_t A, uint64_t L, uint32_t b, uint64_t s, uint64_t n, std::vector<uint8_t>& out)
+{
+  out.resize((size_t)b * A * n);
+  for (uint32_t a = 0; a < A; a++) {
+    if (fseeko(f, (off_t)(b * ((uint64_t)a * L + s)), SEEK_SET) != 0) return false;
+    if (fread(out.data() + (size_t)b * a * n, b, n, f) != n) return false;
+  }
+  return true;
+}
+
 struct Carrier {
   int32_t         offset_hz = 0;
-  uint32_t        N = 0, D = 0, H = 0, SF = 0;
+  uint32_t        N = 0, SF = 0;
+  uint32_t        Lr = 1, Mr = 1, Ka = 0; // output / capture rate L / M, and the taps before an output's own sample (ltephy_chan_design)
   bool            found = false, mib_found = false;
   ltephy_cell_t   cell{};
   ltephy_mib_t    mib{};
@@ -31,14 +45,26 @@ struct Carrier {
 int main(int argc, char** argv)
 {
   if (argc < 6) {
-    fprintf(stderr, "usage: %s <iq.cf32> <fs_in> <nof_rx> <out_prefix> <offset_hz>:<N> [<offset_hz>:<N> ...] [subframes_per_push=500]\n", argv[0]);
+    fprintf(stderr, "usage: %s <iq file> <fs_in> <nof_rx> <out_prefix> <offset_hz>:<N> [<offset_hz>:<N> ...] [subframes_per_push=500] [fmt=cf32|sc16|sc8]\n",
+            argv[0]);
     return 2;
   }
   const uint32_t       fs = (uint32_t)strtoul(argv[2], nullptr, 10), A = (uint32_t)atoi(argv[3]);
   const std::string    prefix = argv[4];
   std::vector<Carrier> car;
-  uint32_t             B = 500;
+  uint32_t             B = 500, fmt = LTEPHY_IQ_CF32;
   for (int i = 5; i < argc; i++) {
+    if (!strncmp(argv[i], "fmt=", 4)) {
+      const char* f = argv[i] + 4;
+      if (!strcmp(f, "cf32")) fmt = LTEPHY_IQ_CF32;
+      else if (!strcmp(f, "sc16")) fmt = LTEPHY_IQ_SC16;
+      else if (!strcmp(f, "sc8")) fmt = LTEPHY_IQ_SC8;
+      else {
+        fprintf(stderr, "unknown %s\n", argv[i]);
+        return 2;
+      }
+      continue;
+    }
     const char* colon = strchr(argv[i], ':');
     if (!colon) {
       B = (uint32_t)atoi(argv[i]);
@@ -53,23 +79,24 @@ int main(int argc, char** argv)
     fprintf(stderr, "cannot open %s / bad nof_rx, carriers, fs_in or subframes_per_push\n", argv[1]);
     return 2;
   }
+  const uint32_t bps = fmt == LTEPHY_IQ_SC16 ? 4 : fmt == LTEPHY_IQ_SC8 ? 2 : 8; // bytes per complex sample
   fseeko(in, 0, SEEK_END);
-  const uint64_t L  = (uint64_t)ftello(in) / (8ull * A);
+  const uint64_t L  = (uint64_t)ftello(in) / ((uint64_t)bps * A);
   const uint64_t MS = fs / 1000; // capture samples per ms
   ltephy_chan_cfg_t ccfg{};
-  ccfg.fs_in = fs, ccfg.nof_rx = A, ccfg.nof_carriers = (uint32_t)car.size();
+  ccfg.fs_in = fs, ccfg.nof_rx = A, ccfg.nof_carriers = (uint32_t)car.size(), ccfg.flags = LTEPHY_CHAN_RATIONAL, ccfg.iq_format = fmt;
   for (size_t c = 0; c < car.size(); c++) ccfg.carrier[c].offset_hz = car[c].offset_hz, ccfg.carrier[c].symbol_sz = car[c].N;
-  uint32_t Tmax = 0;
+  uint32_t reach = 0; // the longest filter window in capture samples (T of an integer carrier)
   for (size_t c = 0; c < car.size(); c++) {
-    uint32_t T, P;
-    if (ltephy_chan_taps(&ccfg, (uint32_t)c, nullptr, nullptr, nullptr, &T, &car[c].D, &P) != LTEPHY_SUCCESS) {
+    ltephy_chan_poly_t q;
+    if (ltephy_chan_design(&ccfg, (uint32_t)c, &q, nullptr, nullptr, nullptr) != LTEPHY_SUCCESS) {
       fprintf(stderr, "carrier %zu: %s\n", c, ltephy_last_error());
       return 2;
     }
-    car[c].H = T / 2, Tmax = std::max(Tmax, T);
+    car[c].Lr = q.L, car[c].Mr = q.M, car[c].Ka = q.Ka, reach = std::max(reach, q.Kp);
   }
   // 1. the first 40 ms of every carrier (and the filter's reach past them) in one call; cell search on each carrier stream
-  const uint64_t L0   = std::min<uint64_t>(L, 40 * MS + Tmax);
+  const uint64_t L0   = std::min<uint64_t>(L, 40 * MS + reach);
   const uint64_t span = std::min<uint64_t>(L, std::max<uint64_t>(L0, (uint64_t)(B + 20) * MS));
   ccfg.max_samples    = span;
   ltephy_chan_t* ch   = nullptr;
@@ -77,10 +104,10 @@ int main(int argc, char** argv)
     fprintf(stderr, "ltephy_chan_create: %s\n", ltephy_last_error());
     return 1;
   }
-  std::vector<float>             x;
+  std::vector<uint8_t>           x;
   std::vector<ltephy_chan_out_t> out(car.size());
   uint64_t                       nx = 0;
-  if (!read_span(in, A, L, 0, L0, x)) {
+  if (!read_span_fmt(in, A, L, bps, 0, L0, x)) {
     fprintf(stderr, "short read\n");
     return 1;
   }
@@ -133,14 +160,17 @@ int main(int argc, char** argv)
     if (recv < L) recv = recv + (uint64_t)B * MS < L ? recv + (uint64_t)B * MS : L;
     uint64_t first = UINT64_MAX;
     for (auto& k : car)
-      if (k.tr) first = std::min(first, k.next * k.D > k.H ? k.next * k.D - k.H : 0);
+      if (k.tr) {
+        const uint64_t n = (uint64_t)(((unsigned __int128)k.next * k.Mr) / k.Lr); // capture sample of carrier sample next
+        first            = std::min(first, n > k.Ka ? n - k.Ka : 0);
+      }
     if (first == UINT64_MAX) break;
     if (first >= recv) {
       if (recv == L) break;
       continue;
     }
     const uint64_t end = std::min(recv, first + span);
-    if (!read_span(in, A, L, first, end - first, x)) {
+    if (!read_span_fmt(in, A, L, bps, first, end - first, x)) {
       fprintf(stderr, "short read\n");
       return 1;
     }

@@ -379,47 +379,74 @@ int  ltephy_track_push_ul_device(ltephy_track_t* h, const void* iq_dev, const vo
 
 /* Channeliser: several carriers from one wideband capture.  Each carrier is shifted to 0 Hz, low-pass filtered and decimated by an integer
  * D = fs_in / (15 kHz * symbol_sz) to the rate the cell search and the tracker take.  The filter, its arithmetic and the output range of a call are
- * DESIGN.md §2 ("channeliser"); the CPU oracle lteo_chan_run (oracle/lte_chan_oracle.h) defines every output sample bit for bit.  Output m of a
+ * DESIGN.md §2 ("channeliser"); the CPU oracles lteo_chan_run (oracle/lte_chan_oracle.h) and lteo_chan_run_poly (oracle/lte_chan_poly_oracle.h,
+ * rational carriers and integer samples) define every output sample bit for bit.  Output m of a
  * carrier belongs to input time m D (zero group delay), so a cell's timing in a carrier stream is its timing in the capture divided by D.
  * The handle keeps no state between calls: the outputs do not depend on how the capture is split. */
 #define LTEPHY_CHAN_MAX_CARRIERS 8
 #define LTEPHY_CHAN_MAX_FS 245760000u
+/* Rational carriers (opt-in).  With LTEPHY_CHAN_RATIONAL, a carrier whose 15 kHz * N / fs_in = L / M in lowest terms is not an integer decimation
+ * 2..128 is resampled by L / M through a polyphase filter (DESIGN.md §2): accepted when L <= 1024, M <= 128 L (output at least fs_in / 128),
+ * L <= 2 M (upsampling at most 2x) and its phase table L * Kp has at most 2^15 taps.  Output m belongs to capture time m M / L and needs capture
+ * samples floor(m M / L) - Ka .. floor(m M / L) + Kb (ltephy_chan_design).  A carrier of integer ratio keeps the integer rule, flag or not. */
+#define LTEPHY_CHAN_RATIONAL 1u
+/* Sample formats of the input: interleaved I/Q, complex sample i of antenna a at index a * nof_samples + i */
+#define LTEPHY_IQ_CF32 0u /* float32 */
+#define LTEPHY_IQ_SC16 1u /* int16, value * 2^-15 */
+#define LTEPHY_IQ_SC8 2u  /* int8, value * 2^-7 */
 typedef struct ltephy_chan ltephy_chan_t;
 typedef struct {
   int32_t  offset_hz; /* carrier centre minus capture centre, a multiple of 1000 */
   uint32_t symbol_sz; /* N of the carrier: 128, 256, 384, 512, 768, 1024, 1536 or 2048; its rate is 15 kHz * N */
 } ltephy_chan_carrier_t;
 typedef struct {
-  uint32_t              fs_in;        /* capture rate in Hz, at most LTEPHY_CHAN_MAX_FS; fs_in / (15 kHz * N) must be an integer 2..128 */
+  uint32_t              fs_in;        /* capture rate in Hz, at most LTEPHY_CHAN_MAX_FS; fs_in / (15 kHz * N) an integer 2..128, or any ratio the
+                                         rational rule accepts when flags has LTEPHY_CHAN_RATIONAL */
   uint32_t              nof_rx;       /* 1 or 2 antennas */
   uint32_t              nof_carriers; /* 1..LTEPHY_CHAN_MAX_CARRIERS */
   uint32_t              pad;
   ltephy_chan_carrier_t carrier[LTEPHY_CHAN_MAX_CARRIERS];
   uint64_t              max_samples;  /* longest call per antenna, 1..2^31 (device memory is sized for it) */
   int32_t               device;       /* CUDA device ordinal */
-  uint32_t              reserved[5];
+  uint32_t              flags;        /* 0 or LTEPHY_CHAN_RATIONAL */
+  uint32_t              iq_format;    /* LTEPHY_IQ_CF32 (0), LTEPHY_IQ_SC16 or LTEPHY_IQ_SC8: the sample type of the input */
+  uint32_t              reserved[3];
 } ltephy_chan_cfg_t;
 typedef struct {
   uint64_t    first;  /* carrier sample index of the first output of this call */
   uint64_t    count;  /* outputs per antenna */
   const void* iq_dev; /* cf32 [nof_rx][count] in device memory (what ltephy_cell_search_device / ltephy_track_push_device take), valid until the next call */
 } ltephy_chan_out_t;
-/* INVALID_INPUTS, before any device is looked for, for: a carrier whose D is not an integer in 2..128, an offset off the 1 kHz grid, a carrier whose
- * widest occupied band (|offset_hz| + 90 kHz * the largest PRB count of its N) reaches past fs_in / 2, an unknown N, 0 or more than 8 carriers,
- * nof_rx other than 1 or 2, fs_in above LTEPHY_CHAN_MAX_FS, max_samples 0 or above 2^31. */
+/* INVALID_INPUTS, before any device is looked for, for: a carrier whose D is not an integer in 2..128 (without LTEPHY_CHAN_RATIONAL) or that
+ * breaks the rational limits (with it), an offset off the 1 kHz grid, a carrier whose widest occupied band (|offset_hz| + 90 kHz * the largest PRB
+ * count of its N) reaches past fs_in / 2, an unknown N, 0 or more than 8 carriers, nof_rx other than 1 or 2, fs_in above LTEPHY_CHAN_MAX_FS,
+ * max_samples 0 or above 2^31, unknown flag bits or an unknown iq_format. */
 int  ltephy_chan_create(const ltephy_chan_cfg_t* cfg, ltephy_chan_t** h);
 void ltephy_chan_destroy(ltephy_chan_t* h);
-/* iq: cf32 [nof_rx][nof_samples], antenna-major, host memory: capture samples first_sample .. first_sample + nof_samples - 1 (1 <= nof_samples <=
- * max_samples).  out[nof_carriers]: every output m >= 0 of each carrier whose filter window [m D - H, m D + H] has all its non-negative samples
- * inside the call (samples before 0 count as zero).  *next_sample: the lowest capture sample the next call must still include for every carrier
- * to continue without a gap; a carrier's first output in that call may repeat outputs of this one.  Blocks until the outputs are complete. */
-int  ltephy_chan_run(ltephy_chan_t* h, const float* iq, uint64_t first_sample, uint64_t nof_samples, ltephy_chan_out_t* out, uint64_t* next_sample);
+/* iq: [nof_rx][nof_samples] complex samples in the plan's iq_format, antenna-major, host memory: capture samples first_sample .. first_sample +
+ * nof_samples - 1 (1 <= nof_samples <= max_samples).  out[nof_carriers]: every output m >= 0 of each carrier whose filter window [m D - H, m D + H]
+ * ([n - Ka, n + Kb], n = floor(m M / L), for a rational carrier) has all its non-negative samples inside the call (samples before 0 count as zero).
+ * *next_sample: the lowest capture sample the next call must still include for every carrier to continue without a gap; a carrier's first output
+ * in that call may repeat outputs of this one.  Blocks until the outputs are complete. */
+int  ltephy_chan_run(ltephy_chan_t* h, const void* iq, uint64_t first_sample, uint64_t nof_samples, ltephy_chan_out_t* out, uint64_t* next_sample);
 /* same, with the samples already in device memory on the handle's device */
 int  ltephy_chan_run_device(ltephy_chan_t* h, const void* iq_dev, uint64_t first_sample, uint64_t nof_samples, ltephy_chan_out_t* out,
                             uint64_t* next_sample);
 /* host only, needs no device: the tables of carrier c (< nof_carriers) as the kernel uses them.  h: f32 [T] prototype, g: cf32 [T] band-pass taps g[k] at index
- * k + H, rot: cf32 [P] output rotation r[m mod P]; any of the three may be NULL.  *T (odd, H = (T - 1) / 2), *D and *P are always written. */
+ * k + H, rot: cf32 [P] output rotation r[m mod P]; any of the three may be NULL.  *T (odd, H = (T - 1) / 2), *D and *P are always written.
+ * A rational carrier is refused: its tables come from ltephy_chan_design. */
 int  ltephy_chan_taps(const ltephy_chan_cfg_t* cfg, uint32_t c, float* h, float* g, float* rot, uint32_t* T, uint32_t* D, uint32_t* P);
+typedef struct {
+  uint32_t L, M; /* output rate / capture rate in lowest terms (L = 1, M = D for an integer carrier) */
+  uint32_t Tp;   /* odd prototype length at rate L fs_in (T for an integer carrier), Hp = (Tp - 1) / 2 */
+  uint32_t Kp;   /* taps per phase, Ka + Kb + 1 */
+  uint32_t Ka, Kb; /* floor(Hp / L), ceil(Hp / L): output m reads capture samples floor(m M / L) - Ka .. floor(m M / L) + Kb */
+  uint32_t P;    /* period of the output rotation */
+} ltephy_chan_poly_t;
+/* host only, needs no device: the geometry and tables of carrier c under the plan's flags, integer or rational.  hp: f32 [Tp] prototype (DC gain
+ * L), g: cf32 [L][Kp] phase taps, g_phi[k] at [phi][k + Kb], rot: cf32 [P]; any of the three may be NULL.  For an integer carrier they equal
+ * ltephy_chan_taps's h, g and rot. */
+int  ltephy_chan_design(const ltephy_chan_cfg_t* cfg, uint32_t c, ltephy_chan_poly_t* out, float* hp, float* g, float* rot);
 
 /* nslots HARQ slots of LTEPHY_HARQ_SLOT_BYTES each (150 RNTIs x 8 processes x 2 TBs = 2400 slots = 1.4 GB); contents survive across batches */
 int ltephy_harq_reserve(ltephy_t* h, uint32_t nslots);

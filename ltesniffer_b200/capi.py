@@ -928,6 +928,9 @@ class Tracker:
 # ------------------------------------------------------------------------------------------------
 # channeliser (ltephy_chan_*, include/ltephy_b200.h)
 CHAN_MAX_CARRIERS = 8
+CHAN_RATIONAL = 1
+IQ_FORMATS = {"cf32": 0, "sc16": 1, "sc8": 2}
+_IQ_DTYPES = {"cf32": np.complex64, "sc16": np.int16, "sc8": np.int8}
 
 
 class ChanCarrier(C.Structure):
@@ -936,11 +939,16 @@ class ChanCarrier(C.Structure):
 
 class ChanCfg(C.Structure):
     _fields_ = [("fs_in", C.c_uint32), ("nof_rx", C.c_uint32), ("nof_carriers", C.c_uint32), ("pad", C.c_uint32),
-                ("carrier", ChanCarrier * CHAN_MAX_CARRIERS), ("max_samples", C.c_uint64), ("device", C.c_int32), ("reserved", C.c_uint32 * 5)]
+                ("carrier", ChanCarrier * CHAN_MAX_CARRIERS), ("max_samples", C.c_uint64), ("device", C.c_int32), ("flags", C.c_uint32), ("iq_format", C.c_uint32),
+                ("reserved", C.c_uint32 * 3)]
 
 
 class ChanOut(C.Structure):
     _fields_ = [("first", C.c_uint64), ("count", C.c_uint64), ("iq_dev", C.c_void_p)]
+
+
+class ChanPoly(C.Structure):
+    _fields_ = [(k, C.c_uint32) for k in ("L", "M", "Tp", "Kp", "Ka", "Kb", "P")]
 
 
 assert C.sizeof(ChanCfg) == 112 and C.sizeof(ChanOut) == 24
@@ -953,11 +961,12 @@ def _bind_chan(L):
     L.ltephy_chan_run_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p, C.POINTER(C.c_uint64)]
     L.ltephy_chan_taps.argtypes = [C.POINTER(ChanCfg), C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32),
                                    C.POINTER(C.c_uint32)]
+    L.ltephy_chan_design.argtypes = [C.POINTER(ChanCfg), C.c_uint32, C.POINTER(ChanPoly), C.c_void_p, C.c_void_p, C.c_void_p]
 
 
-def chan_cfg(fs_in, carriers, nof_rx=1, max_samples=1, device=0):
+def chan_cfg(fs_in, carriers, nof_rx=1, max_samples=1, device=0, flags=0, iq_format=0):
     """ChanCfg from carriers = [(offset_hz, symbol_sz), ...]"""
-    cfg = ChanCfg(fs_in=fs_in, nof_rx=nof_rx, nof_carriers=len(carriers), max_samples=max_samples, device=device)
+    cfg = ChanCfg(fs_in=fs_in, nof_rx=nof_rx, nof_carriers=len(carriers), max_samples=max_samples, device=device, flags=flags, iq_format=iq_format)
     for i, (off, n) in enumerate(carriers[:CHAN_MAX_CARRIERS]):
         cfg.carrier[i] = ChanCarrier(off, n)
     return cfg
@@ -977,16 +986,35 @@ def chan_taps(fs_in, carriers, c):
     return dict(h=h, g=g, rot=rot, T=T.value, D=D.value, P=P.value)
 
 
-class Channelizer:
-    """Shift, filter and decimate the carriers [(offset_hz, symbol_sz), ...] of a capture at fs_in out of antenna-major complex64 [nof_rx][n]
-    spans of up to max_samples; each run returns every carrier's outputs that the span completes, and next_sample, the lowest capture sample the
-    next run must still include."""
+def chan_design(fs_in, carriers, c, rational=True):
+    """host-only geometry and tables of carrier c under the plan's flags -> dict(L, M, Tp, Kp, Ka, Kb, P, hp float32 [Tp], g complex64 [L][Kp],
+    rot complex64 [P]); RuntimeError when refused"""
+    L = load_library()
+    _bind_chan(L)
+    cfg = chan_cfg(fs_in, carriers, flags=CHAN_RATIONAL if rational else 0)
+    q = ChanPoly()
+    r = L.ltephy_chan_design(C.byref(cfg), c, C.byref(q), None, None, None)
+    if r != 0:
+        raise RuntimeError("ltephy_chan_design failed (%d): %s" % (r, L.ltephy_last_error().decode()))
+    hp, g, rot = np.zeros(q.Tp, np.float32), np.zeros((q.L, q.Kp), np.complex64), np.zeros(q.P, np.complex64)
+    L.ltephy_chan_design(C.byref(cfg), c, C.byref(q), _p(hp), _p(g), _p(rot))
+    d = {k: getattr(q, k) for k, _ in ChanPoly._fields_}
+    d.update(hp=hp, g=g, rot=rot)
+    return d
 
-    def __init__(self, fs_in, carriers, nof_rx, max_samples, device=0):
+
+class Channelizer:
+    """Shift, filter and resample the carriers [(offset_hz, symbol_sz), ...] of a capture at fs_in out of antenna-major [nof_rx][n] spans of up
+    to max_samples; each run returns every carrier's outputs that the span completes, and next_sample, the lowest capture sample the next run must
+    still include.  rational=True sets LTEPHY_CHAN_RATIONAL (any ratio the rational rule accepts); iq_format "cf32" takes complex64 [nof_rx][n],
+    "sc16" / "sc8" take interleaved int16 / int8 [nof_rx][2n]."""
+
+    def __init__(self, fs_in, carriers, nof_rx, max_samples, device=0, rational=False, iq_format="cf32"):
         self.L = load_library()
         _bind_chan(self.L)
         self.carriers = list(carriers)
-        self.cfg = chan_cfg(fs_in, self.carriers, nof_rx, max_samples, device)
+        self.rational, self.iq_format = rational, iq_format
+        self.cfg = chan_cfg(fs_in, self.carriers, nof_rx, max_samples, device, CHAN_RATIONAL if rational else 0, IQ_FORMATS[iq_format])
         self.h = C.c_void_p()
         r = self.L.ltephy_chan_create(C.byref(self.cfg), C.byref(self.h))
         if r != 0:
@@ -1008,6 +1036,17 @@ class Channelizer:
     def taps(self, c):
         return chan_taps(self.cfg.fs_in, self.carriers, c)
 
+    def design(self, c):
+        return chan_design(self.cfg.fs_in, self.carriers, c, self.rational)
+
+    def _samples(self, iq):
+        """the number of complex samples per antenna of iq in the handle's format"""
+        assert iq.ndim == 2 and iq.shape[0] == self.cfg.nof_rx, iq.shape
+        if self.iq_format == "cf32":
+            return iq.shape[1]
+        assert iq.shape[1] % 2 == 0, iq.shape
+        return iq.shape[1] // 2
+
     def _done(self, r, out, nxt, copy):
         if r != 0:
             raise RuntimeError("ltephy_chan_run failed (%d): %s" % (r, self.L.ltephy_last_error().decode()))
@@ -1028,16 +1067,19 @@ class Channelizer:
         return res, nxt.value
 
     def run(self, iq, first_sample, copy=True):
-        """iq: complex64 [nof_rx][n] (host) of capture samples first_sample ... -> ([dict(first, count, iq: torch complex64 [nof_rx][count] on the
-        device)] per carrier, next_sample).  With copy=False iq views the handle's buffer, valid until the next run."""
-        iq = np.ascontiguousarray(iq, np.complex64)
-        assert iq.ndim == 2 and iq.shape[0] == self.cfg.nof_rx, iq.shape
+        """iq: complex64 [nof_rx][n] (host; int16 / int8 [nof_rx][2n] for sc16 / sc8) of capture samples first_sample ... -> ([dict(first,
+        count, iq: torch complex64 [nof_rx][count] on the device)] per carrier, next_sample).  With copy=False iq views the handle's buffer, valid
+        until the next run."""
+        iq = np.ascontiguousarray(iq, _IQ_DTYPES[self.iq_format])
+        n = self._samples(iq)
         out, nxt = (ChanOut * CHAN_MAX_CARRIERS)(), C.c_uint64()
-        return self._done(self.L.ltephy_chan_run(self.h, _p(iq), first_sample, iq.shape[1], out, C.byref(nxt)), out, nxt, copy)
+        return self._done(self.L.ltephy_chan_run(self.h, _p(iq), first_sample, n, out, C.byref(nxt)), out, nxt, copy)
 
     def run_device(self, iq, first_sample, copy=True):
-        """iq: torch complex64 [nof_rx][n], contiguous, on this handle's device"""
-        assert iq.is_cuda and iq.is_contiguous() and iq.dim() == 2 and iq.shape[0] == self.cfg.nof_rx
+        """iq: torch complex64 [nof_rx][n] (int16 / int8 [nof_rx][2n] for sc16 / sc8), contiguous, on this handle's device"""
+        import torch
+        want = {"cf32": torch.complex64, "sc16": torch.int16, "sc8": torch.int8}[self.iq_format]
+        assert iq.is_cuda and iq.is_contiguous() and iq.dim() == 2 and iq.dtype == want, (iq.dtype, want)
+        n = self._samples(iq)
         out, nxt = (ChanOut * CHAN_MAX_CARRIERS)(), C.c_uint64()
-        return self._done(self.L.ltephy_chan_run_device(self.h, C.c_void_p(iq.data_ptr()), first_sample, iq.shape[1], out, C.byref(nxt)), out, nxt,
-                          copy)
+        return self._done(self.L.ltephy_chan_run_device(self.h, C.c_void_p(iq.data_ptr()), first_sample, n, out, C.byref(nxt)), out, nxt, copy)

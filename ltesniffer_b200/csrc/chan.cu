@@ -1,5 +1,6 @@
 // chan.cu -- host side of the channeliser (include/ltephy_b200.h, DESIGN.md §2 "channeliser"): the per-carrier filter design in double precision,
-// the output range of a call, and one launch of k_chan.cu over every (carrier, antenna, tile).  The tables equal lteo_chan_design's bit for bit.
+// the output range of a call, and one launch of k_chan.cu over every (carrier, antenna, tile) per kind of carrier (integer, rational).  The tables
+// equal lteo_chan_design's and lteo_chan_design_poly's bit for bit.
 #include "../../include/ltephy_b200.h"
 #include "k_chan.cuh"
 #include "ltephy_internal.cuh"
@@ -10,18 +11,26 @@
 
 #define CHAN_ATTEN 70.0 // stop-band target (dB) of Kaiser's formulas
 #define CHAN_SPAN 4096  // input samples a tile aims to stage: M = min(1024, max(64, (CHAN_SPAN - T) / D + 1)) outputs
+#define CHAN_PSPAN 12288 // input samples a rational tile may stage: R = (CHAN_PSPAN - Kp) / M rows per phase class, at least 1
+#define CHAN_MAX_L 1024u
+#define CHAN_MAX_TABLE 32768u
 
 struct ltephy_chan {
   ltephy_chan_cfg_t cfg{};
   Stream            stream;
   struct Carrier {
     uint32_t       T = 0, D = 0, P = 0, M = 0, rows = 0;
-    uint64_t       cap = 0; // outputs per antenna the buffer holds
+    uint64_t       cap = 0;      // outputs per antenna the buffer holds
+    bool           poly = false; // rational: L, M (= pq.M), Kp, Ka, Kb in pq, R rows per phase class in a tile
+    ltephy_chan_poly_t pq{};
+    uint32_t       R = 0;
     DevBuf<float2> g, rot, out;
   } car[LTEPHY_CHAN_MAX_CARRIERS];
   DevBuf<float2> d_x;
-  size_t         smem = 0;
+  size_t         smem = 0, psmem = 0;
 };
+
+static size_t chan_sample_bytes(uint32_t fmt) { return fmt == LTEPHY_IQ_SC16 ? 4 : fmt == LTEPHY_IQ_SC8 ? 2 : 8; }
 
 static uint32_t chan_max_prb(uint32_t N)
 {
@@ -115,6 +124,100 @@ static int chan_design(uint32_t fs_in, int32_t offset_hz, uint32_t N, float* h, 
   return LTEPHY_SUCCESS;
 }
 
+static int64_t chan_gcd(int64_t a, int64_t b)
+{
+  while (b) {
+    const int64_t t = a % b;
+    a = b, b = t;
+  }
+  return a;
+}
+
+// geometry of a carrier under the plan's flags: an integer carrier keeps chan_geometry (L = 1, M = D, Ka = Kb = H, *poly false); with
+// LTEPHY_CHAN_RATIONAL any other ratio L / M within the limits of DESIGN.md §2.  0, or INVALID_INPUTS with the reason in the last error
+static int chan_poly_geometry(uint32_t fs_in, int32_t offset_hz, uint32_t N, uint32_t flags, ltephy_chan_poly_t* q, bool* poly)
+{
+  const uint32_t prb = chan_max_prb(N);
+  if (!prb) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: symbol size %u not supported", N);
+  if (fs_in == 0 || fs_in > LTEPHY_CHAN_MAX_FS) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: fs_in %u outside 1..245760000", fs_in);
+  if (offset_hz % 1000) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: offset %d Hz is not a multiple of 1 kHz", offset_hz);
+  const int64_t fs_out = 15000ll * N, gg = chan_gcd(fs_out, fs_in), L = fs_out / gg, M = fs_in / gg;
+  *poly = !(L == 1 && M >= 2 && M <= 128);
+  if (!*poly || !(flags & LTEPHY_CHAN_RATIONAL)) {
+    uint32_t T, D, P;
+    if (int r = chan_geometry(fs_in, offset_hz, N, &T, &D, &P)) return r;
+    q->L = 1, q->M = D, q->Tp = T, q->Kp = T, q->Ka = T / 2, q->Kb = T / 2, q->P = P;
+    return LTEPHY_SUCCESS;
+  }
+  if (L > CHAN_MAX_L) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: fs_out / fs_in = %lld / %lld, L above 1024", (long long)L, (long long)M);
+  if (M > 128 * L) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: fs_out / fs_in = %lld / %lld is below 1 / 128", (long long)L, (long long)M);
+  if (L > 2 * M) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: fs_out / fs_in = %lld / %lld upsamples more than 2x", (long long)L, (long long)M);
+  const int64_t f_pass = 90000ll * prb, aoff = std::llabs((long long)offset_hz), mn = std::min<int64_t>(fs_out, fs_in);
+  if (2 * (aoff + f_pass) > (int64_t)fs_in)
+    return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: band of the carrier at %d Hz (N %u) reaches outside the capture", offset_hz, N);
+  // Kaiser's length for 70 dB over [f_pass, min(fs_in, fs_out) - f_pass] at the prototype's rate L fs_in, made odd
+  const double  width = (double)(mn - 2 * f_pass) / (0.5 * (double)(L * (int64_t)fs_in));
+  const double  nt    = (CHAN_ATTEN - 7.95) / 2.285 / (M_PI * width) + 1.0;
+  const int64_t tp = (int64_t)std::ceil(nt) | 1, hp = (tp - 1) / 2, ka = hp / L, kb = (hp + L - 1) / L;
+  if (L * (ka + kb + 1) > CHAN_MAX_TABLE)
+    return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: phase table of %lld taps (L %lld x Kp %lld) above 2^15", (long long)(L * (ka + kb + 1)), (long long)L,
+                (long long)(ka + kb + 1));
+  q->L = (uint32_t)L, q->M = (uint32_t)M, q->Tp = (uint32_t)tp, q->Ka = (uint32_t)ka, q->Kb = (uint32_t)kb, q->Kp = (uint32_t)(ka + kb + 1);
+  q->P = (uint32_t)(fs_out / chan_gcd(chan_mod(offset_hz, fs_out), fs_out));
+  return LTEPHY_SUCCESS;
+}
+
+// the tables of a carrier under the plan's flags, in the arithmetic of lteo_chan_design_poly: an integer carrier's are chan_design's
+static int chan_design_poly(uint32_t fs_in, int32_t offset_hz, uint32_t N, uint32_t flags, ltephy_chan_poly_t* out, float* hp, float* g, float* rot)
+{
+  ltephy_chan_poly_t q;
+  bool               poly;
+  if (int r = chan_poly_geometry(fs_in, offset_hz, N, flags, &q, &poly)) return r;
+  if (out) *out = q;
+  if (!poly) {
+    uint32_t T, D, P;
+    return chan_design(fs_in, offset_hz, N, hp, g, rot, &T, &D, &P);
+  }
+  const int64_t L = q.L, Hp = (q.Tp - 1) / 2, Lfs = L * (int64_t)fs_in, fs_out = 15000ll * N;
+  if (hp || g) {
+    // windowed sinc with cutoff min(fs_in, fs_out) / 2 at rate L fs_in, scaled to DC gain L
+    std::vector<double> hd(q.Tp);
+    const double        beta = 0.1102 * (CHAN_ATTEN - 8.7), a = 0.5 * (double)(q.Tp - 1), i0b = chan_i0(beta), c = 1.0 / (double)std::max(q.L, q.M);
+    double              s = 0.0;
+    for (int64_t j = 0; j < (int64_t)q.Tp; j++) {
+      const double m  = (double)(j - Hp) * c;
+      const double sn = m == 0.0 ? 1.0 : std::sin(M_PI * m) / (M_PI * m);
+      const double r  = ((double)j - a) / a;
+      const double w  = chan_i0(beta * std::sqrt(1.0 - r * r)) / i0b;
+      hd[j]           = c * sn * w;
+      s               = s + hd[j];
+    }
+    const double sl = s / (double)L;
+    for (int64_t j = 0; j < (int64_t)q.Tp; j++) hd[j] = hd[j] / sl;
+    if (hp)
+      for (int64_t j = 0; j < (int64_t)q.Tp; j++) hp[j] = (float)hd[j];
+    if (g) // g_phi[k] at [phi][k + Kb]: hp[Hp + phi + L k] e^{+j 2 pi offset (phi + L k) / (L fs_in)}, zero outside the prototype
+      for (int64_t ph = 0; ph < L; ph++)
+        for (int64_t k = -(int64_t)q.Kb; k <= (int64_t)q.Ka; k++) {
+          const int64_t idx = Hp + ph + L * k;
+          const double  tap = idx >= 0 && idx < (int64_t)q.Tp ? hd[idx] : 0.0;
+          const double  a2  = 2.0 * M_PI * (double)chan_mod((int64_t)offset_hz * (ph + L * k), Lfs) / (double)Lfs;
+          float*        o   = g + 2 * ((size_t)ph * q.Kp + (size_t)(k + q.Kb));
+          o[0]              = (float)(tap * std::cos(a2));
+          o[1]              = (float)(tap * std::sin(a2));
+        }
+  }
+  if (rot) { // r[i] = e^{-j 2 pi offset i / fs_out}
+    const int64_t step = chan_mod(offset_hz, fs_out);
+    for (int64_t i = 0; i < (int64_t)q.P; i++) {
+      const double ph = -2.0 * M_PI * (double)((step * i) % fs_out) / (double)fs_out;
+      rot[2 * i]      = (float)std::cos(ph);
+      rot[2 * i + 1]  = (float)std::sin(ph);
+    }
+  }
+  return LTEPHY_SUCCESS;
+}
+
 static int chan_check_cfg(const ltephy_chan_cfg_t* cfg)
 {
   if (!cfg) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: null configuration");
@@ -122,9 +225,12 @@ static int chan_check_cfg(const ltephy_chan_cfg_t* cfg)
   if (cfg->nof_carriers < 1 || cfg->nof_carriers > LTEPHY_CHAN_MAX_CARRIERS)
     return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: %u carriers, not 1..8", cfg->nof_carriers);
   if (cfg->max_samples < 1 || cfg->max_samples > (1ull << 31)) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: max_samples outside 1..2^31");
+  if (cfg->flags & ~LTEPHY_CHAN_RATIONAL) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: unknown flags 0x%x", cfg->flags);
+  if (cfg->iq_format > LTEPHY_IQ_SC8) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: unknown iq_format %u", cfg->iq_format);
   for (uint32_t c = 0; c < cfg->nof_carriers; c++) {
-    uint32_t T, D, P;
-    if (int r = chan_geometry(cfg->fs_in, cfg->carrier[c].offset_hz, cfg->carrier[c].symbol_sz, &T, &D, &P)) return r;
+    ltephy_chan_poly_t q;
+    bool               poly;
+    if (int r = chan_poly_geometry(cfg->fs_in, cfg->carrier[c].offset_hz, cfg->carrier[c].symbol_sz, cfg->flags, &q, &poly)) return r;
   }
   return LTEPHY_SUCCESS;
 }
@@ -134,7 +240,22 @@ extern "C" int ltephy_chan_taps(const ltephy_chan_cfg_t* cfg, uint32_t c, float*
   if (!cfg || !T || !D || !P) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan_taps: null argument");
   if (c >= cfg->nof_carriers || c >= LTEPHY_CHAN_MAX_CARRIERS)
     return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan_taps: carrier %u of %u", c, cfg->nof_carriers);
+  if (cfg->flags & LTEPHY_CHAN_RATIONAL) {
+    ltephy_chan_poly_t q;
+    bool               poly;
+    if (chan_poly_geometry(cfg->fs_in, cfg->carrier[c].offset_hz, cfg->carrier[c].symbol_sz, cfg->flags, &q, &poly) == LTEPHY_SUCCESS && poly)
+      return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan_taps: carrier %u is rational (L %u / M %u): its tables come from ltephy_chan_design", c, q.L, q.M);
+  }
   return chan_design(cfg->fs_in, cfg->carrier[c].offset_hz, cfg->carrier[c].symbol_sz, h, g, rot, T, D, P);
+}
+
+extern "C" int ltephy_chan_design(const ltephy_chan_cfg_t* cfg, uint32_t c, ltephy_chan_poly_t* out, float* hp, float* g, float* rot)
+{
+  if (!cfg || !out) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan_design: null argument");
+  if (c >= cfg->nof_carriers || c >= LTEPHY_CHAN_MAX_CARRIERS)
+    return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan_design: carrier %u of %u", c, cfg->nof_carriers);
+  if (cfg->flags & ~LTEPHY_CHAN_RATIONAL) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan_design: unknown flags 0x%x", cfg->flags);
+  return chan_design_poly(cfg->fs_in, cfg->carrier[c].offset_hz, cfg->carrier[c].symbol_sz, cfg->flags, out, hp, g, rot);
 }
 
 extern "C" int ltephy_chan_create(const ltephy_chan_cfg_t* cfg, ltephy_chan_t** out)
@@ -148,9 +269,28 @@ extern "C" int ltephy_chan_create(const ltephy_chan_cfg_t* cfg, ltephy_chan_t** 
   ltephy_chan* const                                           h = owner.get();
   h->cfg                                                         = *cfg;
   CU(cudaStreamCreateWithFlags(&h->stream.raw, cudaStreamNonBlocking));
-  if (h->d_x.reserve((size_t)cfg->nof_rx * cfg->max_samples)) return fail(LTEPHY_ERROR, "chan_create: device allocation failed");
+  const size_t xbytes = (size_t)cfg->nof_rx * cfg->max_samples * chan_sample_bytes(cfg->iq_format);
+  if (h->d_x.reserve((xbytes + sizeof(float2) - 1) / sizeof(float2))) return fail(LTEPHY_ERROR, "chan_create: device allocation failed");
   for (uint32_t c = 0; c < cfg->nof_carriers; c++) {
     ltephy_chan::Carrier& k = h->car[c];
+    chan_poly_geometry(cfg->fs_in, cfg->carrier[c].offset_hz, cfg->carrier[c].symbol_sz, cfg->flags, &k.pq, &k.poly);
+    if (k.poly) {
+      const ltephy_chan_poly_t& q = k.pq;
+      std::vector<float>        g(2 * (size_t)q.L * q.Kp), rot(2 * (size_t)q.P);
+      chan_design_poly(cfg->fs_in, cfg->carrier[c].offset_hz, cfg->carrier[c].symbol_sz, cfg->flags, nullptr, nullptr, g.data(), rot.data());
+      // rows per phase class: the span R M + Kp within CHAN_PSPAN; from 32 rows up, whole warps per class and about 4096 outputs a tile
+      uint32_t R = std::max<int64_t>(1, ((int64_t)CHAN_PSPAN - (int64_t)q.Kp) / (int64_t)q.M);
+      if (R >= 32) R = std::max<uint32_t>(32, std::min<uint32_t>(R, 4096 / q.L) / 32 * 32);
+      k.R   = R, k.P = q.P;
+      k.cap = (uint64_t)(((unsigned __int128)cfg->max_samples * q.L) / q.M) + 2;
+      const uint64_t span = ((uint64_t)(q.L - 1) + ((uint64_t)q.L * R - 1) * q.M) / q.L + q.Kp;
+      h->psmem            = std::max(h->psmem, (size_t)span * sizeof(float2));
+      if (k.g.reserve(g.size() / 2) || k.rot.reserve(q.P) || k.out.reserve((size_t)cfg->nof_rx * k.cap))
+        return fail(LTEPHY_ERROR, "chan_create: device allocation failed");
+      CU(cudaMemcpy(k.g.p, g.data(), g.size() * sizeof(float), cudaMemcpyHostToDevice));
+      CU(cudaMemcpy(k.rot.p, rot.data(), rot.size() * sizeof(float), cudaMemcpyHostToDevice));
+      continue;
+    }
     chan_design(cfg->fs_in, cfg->carrier[c].offset_hz, cfg->carrier[c].symbol_sz, nullptr, nullptr, nullptr, &k.T, &k.D, &k.P);
     std::vector<float> g(2 * (size_t)k.T), rot(2 * (size_t)k.P);
     chan_design(cfg->fs_in, cfg->carrier[c].offset_hz, cfg->carrier[c].symbol_sz, nullptr, g.data(), rot.data(), &k.T, &k.D, &k.P);
@@ -184,15 +324,39 @@ static int chan_check(ltephy_chan_t* h, const void* iq, uint64_t first, uint64_t
   return LTEPHY_SUCCESS;
 }
 
-static int chan_run(ltephy_chan_t* h, const float2* x, uint64_t first, uint64_t n, ltephy_chan_out_t* out, uint64_t* next)
+static int chan_run(ltephy_chan_t* h, const void* x, uint64_t first, uint64_t n, ltephy_chan_out_t* out, uint64_t* next)
 {
   const uint32_t A = h->cfg.nof_rx;
   ChanArgs       g{};
+  ChanPolyArgs   pg{};
   g.x = x, g.lda = n, g.first = first;
-  uint32_t ntiles = 0;
+  pg.x = x, pg.lda = n, pg.first = first;
+  uint32_t ntiles = 0, nptiles = 0;
   uint64_t nx     = UINT64_MAX;
   for (uint32_t c = 0; c < h->cfg.nof_carriers; c++) {
     const ltephy_chan::Carrier& k = h->car[c];
+    if (k.poly) {
+      // outputs m >= 0 whose window [n - Ka, n + Kb], n = floor(m M / L), has every non-negative sample inside [first, first + n)
+      const ltephy_chan_poly_t& q = k.pq;
+      const unsigned __int128   L = q.L, M = q.M, last = first + n - 1;
+      const uint64_t lo   = first == 0 ? 0 : (uint64_t)(((first + q.Ka) * L + M - 1) / M);
+      const uint64_t hi_n = last >= q.Kb ? (uint64_t)(((last - q.Kb + 1) * L - 1) / M + 1) : 0;
+      const uint64_t cnt  = hi_n > lo ? hi_n - lo : 0;
+      const uint64_t mn = cnt ? hi_n : lo, nn = (uint64_t)(mn * M / L);
+      nx                = std::min<uint64_t>(nx, nn >= q.Ka ? nn - q.Ka : 0);
+      out[c].first = lo, out[c].count = cnt, out[c].iq_dev = k.out.p;
+      if (!cnt) continue;
+      const uint64_t per   = (uint64_t)q.L * k.R;
+      const uint32_t tiles = (uint32_t)((cnt + per - 1) / per);
+      for (uint32_t a = 0; a < A; a++) {
+        ChanPolySeg& s = pg.seg[pg.nseg++];
+        s.g = k.g.p, s.rot = k.rot.p, s.out = k.out.p + (size_t)a * cnt, s.n0 = (uint64_t)(lo * M / L), s.count = cnt;
+        s.phi0 = (uint32_t)(lo * M % L), s.r0 = (uint32_t)(lo % q.P), s.L = q.L, s.M = q.M, s.Kp = q.Kp, s.Ka = q.Ka, s.P = q.P, s.R = k.R;
+        s.tile0 = nptiles, s.a = a;
+        nptiles += tiles;
+      }
+      continue;
+    }
     // outputs m >= 0 whose window [m D - H, m D + H] has every non-negative sample inside [first, first + n)
     const uint64_t H = k.T / 2, last = first + n - 1;
     const uint64_t lo   = first == 0 ? 0 : (first + H + k.D - 1) / k.D;
@@ -211,16 +375,19 @@ static int chan_run(ltephy_chan_t* h, const float2* x, uint64_t first, uint64_t 
     }
   }
   *next = nx;
-  if (launch_chan(g, ntiles, h->smem, h->stream)) return fail(LTEPHY_ERROR, "chan_run: kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
+  if (launch_chan(g, ntiles, h->smem, h->cfg.iq_format, h->stream))
+    return fail(LTEPHY_ERROR, "chan_run: kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
+  if (launch_chan_poly(pg, nptiles, h->psmem, h->cfg.iq_format, h->stream))
+    return fail(LTEPHY_ERROR, "chan_run: polyphase kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
   CU(cudaStreamSynchronize(h->stream));
   return LTEPHY_SUCCESS;
 }
 
-extern "C" int ltephy_chan_run(ltephy_chan_t* h, const float* iq, uint64_t first_sample, uint64_t nof_samples, ltephy_chan_out_t* out, uint64_t* next_sample)
+extern "C" int ltephy_chan_run(ltephy_chan_t* h, const void* iq, uint64_t first_sample, uint64_t nof_samples, ltephy_chan_out_t* out, uint64_t* next_sample)
 {
   if (int r = chan_check(h, iq, first_sample, nof_samples, out, next_sample)) return r;
   CU(cudaSetDevice(h->cfg.device));
-  CU(cudaMemcpyAsync(h->d_x.p, iq, (size_t)h->cfg.nof_rx * nof_samples * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
+  CU(cudaMemcpyAsync(h->d_x.p, iq, (size_t)h->cfg.nof_rx * nof_samples * chan_sample_bytes(h->cfg.iq_format), cudaMemcpyHostToDevice, h->stream));
   return chan_run(h, h->d_x.p, first_sample, nof_samples, out, next_sample);
 }
 
@@ -228,6 +395,8 @@ extern "C" int ltephy_chan_run_device(ltephy_chan_t* h, const void* iq_dev, uint
                                       uint64_t* next_sample)
 {
   if (int r = chan_check(h, iq_dev, first_sample, nof_samples, out, next_sample)) return r;
+  if (h->cfg.iq_format != LTEPHY_IQ_CF32 && (uintptr_t)iq_dev % chan_sample_bytes(h->cfg.iq_format))
+    return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan_run_device: iq_dev not aligned to its %zu-byte samples", chan_sample_bytes(h->cfg.iq_format));
   CU(cudaSetDevice(h->cfg.device));
-  return chan_run(h, static_cast<const float2*>(iq_dev), first_sample, nof_samples, out, next_sample);
+  return chan_run(h, iq_dev, first_sample, nof_samples, out, next_sample);
 }
