@@ -1,6 +1,6 @@
 // chan.cu -- host side of the channeliser (include/ltephy_b200.h, DESIGN.md §2 "channeliser"): the per-carrier filter design in double precision,
-// the output range of a call, and one launch of k_chan.cu over every (carrier, antenna, tile) per kind of carrier (integer, rational).  The tables
-// equal lteo_chan_design's and lteo_chan_design_poly's bit for bit.
+// the output range of a call, and one launch of k_chan.cu over every (carrier, antenna, tile).  An integer carrier is computed as the rational
+// one at L = 1, M = D; the tables equal lteo_chan_design's and lteo_chan_design_poly's bit for bit.
 #include "../../include/ltephy_b200.h"
 #include "k_chan.cuh"
 #include "ltephy_internal.cuh"
@@ -9,8 +9,8 @@
 #include <cstdlib>
 #include <vector>
 
-#define CHAN_ATTEN 70.0 // stop-band target (dB) of Kaiser's formulas
-#define CHAN_SPAN 4096  // input samples a tile aims to stage: M = min(1024, max(64, (CHAN_SPAN - T) / D + 1)) outputs
+#define CHAN_ATTEN 70.0  // stop-band target (dB) of Kaiser's formulas
+#define CHAN_SPAN 4096   // input samples an integer tile aims to stage: R = min(1024, max(64, (CHAN_SPAN - T) / D + 1)) outputs
 #define CHAN_PSPAN 12288 // input samples a rational tile may stage: R = (CHAN_PSPAN - Kp) / M rows per phase class, at least 1
 #define CHAN_MAX_L 1024u
 #define CHAN_MAX_TABLE 32768u
@@ -19,15 +19,13 @@ struct ltephy_chan {
   ltephy_chan_cfg_t cfg{};
   Stream            stream;
   struct Carrier {
-    uint32_t       T = 0, D = 0, P = 0, M = 0, rows = 0;
-    uint64_t       cap = 0;      // outputs per antenna the buffer holds
-    bool           poly = false; // rational: L, M (= pq.M), Kp, Ka, Kb in pq, R rows per phase class in a tile
-    ltephy_chan_poly_t pq{};
-    uint32_t       R = 0;
-    DevBuf<float2> g, rot, out;
+    ltephy_chan_poly_t q{};
+    uint32_t           R = 0, Q = 0, rows = 0; // tiles of L R outputs, their span staged in Q phases of rows samples (ChanSeg)
+    uint64_t           cap = 0;                // outputs per antenna the buffer holds
+    DevBuf<float2>     g, rot, out;
   } car[LTEPHY_CHAN_MAX_CARRIERS];
   DevBuf<float2> d_x;
-  size_t         smem = 0, psmem = 0;
+  size_t         smem = 0;
 };
 
 static size_t chan_sample_bytes(uint32_t fmt) { return fmt == LTEPHY_IQ_SC16 ? 4 : fmt == LTEPHY_IQ_SC8 ? 2 : 8; }
@@ -57,73 +55,6 @@ static double chan_i0(double x) // modified Bessel function I0, power series unt
 
 static int64_t chan_mod(int64_t a, int64_t fs) { return ((a % fs) + fs) % fs; }
 
-// decimation D, odd filter length T and rotation period P of one carrier; 0, or INVALID_INPUTS with the reason in the last error
-static int chan_geometry(uint32_t fs_in, int32_t offset_hz, uint32_t N, uint32_t* T, uint32_t* D, uint32_t* P)
-{
-  const uint32_t prb = chan_max_prb(N);
-  if (!prb) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: symbol size %u not supported", N);
-  if (fs_in == 0 || fs_in > LTEPHY_CHAN_MAX_FS) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: fs_in %u outside 1..245760000", fs_in);
-  if (offset_hz % 1000) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: offset %d Hz is not a multiple of 1 kHz", offset_hz);
-  const uint64_t fs_out = 15000ull * N;
-  if (fs_in % fs_out || fs_in / fs_out < 2 || fs_in / fs_out > 128)
-    return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: fs_in %u / %llu is not an integer decimation 2..128", fs_in, (unsigned long long)fs_out);
-  const uint64_t d = fs_in / fs_out, f_pass = 90000ull * prb, aoff = (uint64_t)std::llabs((long long)offset_hz);
-  if (2 * (aoff + f_pass) > fs_in)
-    return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: band of the carrier at %d Hz (N %u) reaches outside the capture", offset_hz, N);
-  // Kaiser's length for 70 dB over the transition band [f_pass, fs_out - f_pass], width relative to fs_in / 2 (scipy.signal.kaiserord), made odd
-  const double width = (double)(fs_out - 2 * f_pass) / (0.5 * (double)fs_in);
-  const double nt    = (CHAN_ATTEN - 7.95) / 2.285 / (M_PI * width) + 1.0;
-  *T = (uint32_t)std::ceil(nt) | 1u;
-  *D = (uint32_t)d;
-  int64_t a = chan_mod((int64_t)d * offset_hz, fs_in), b = fs_in; // P = fs_in / gcd(D offset mod fs_in, fs_in)
-  while (b) {
-    const int64_t t = a % b;
-    a = b, b = t;
-  }
-  *P = (uint32_t)(fs_in / a);
-  return LTEPHY_SUCCESS;
-}
-
-// the tables of one carrier, in the arithmetic of lteo_chan_design
-static int chan_design(uint32_t fs_in, int32_t offset_hz, uint32_t N, float* h, float* g, float* rot, uint32_t* T, uint32_t* D, uint32_t* P)
-{
-  if (int r = chan_geometry(fs_in, offset_hz, N, T, D, P)) return r;
-  const uint32_t t = *T, d = *D, p = *P;
-  const int64_t  H = (t - 1) / 2, fs = fs_in;
-  if (h || g) {
-    // windowed sinc with cutoff fs_out / 2 = fs_in / (2 D), scaled to DC gain 1 (scipy.signal.firwin)
-    std::vector<double> hd(t);
-    const double beta = 0.1102 * (CHAN_ATTEN - 8.7), a = 0.5 * (double)(t - 1), i0b = chan_i0(beta), c = 1.0 / (double)d;
-    double       s = 0.0;
-    for (int64_t j = 0; j < (int64_t)t; j++) {
-      const double m  = (double)(j - H) * c;
-      const double sn = m == 0.0 ? 1.0 : std::sin(M_PI * m) / (M_PI * m);
-      const double r  = ((double)j - a) / a;
-      const double w  = chan_i0(beta * std::sqrt(1.0 - r * r)) / i0b;
-      hd[j]           = c * sn * w;
-      s               = s + hd[j];
-    }
-    for (int64_t j = 0; j < (int64_t)t; j++) {
-      const double hn = hd[j] / s;
-      if (h) h[j] = (float)hn;
-      if (g) { // g[k] = h[k] e^{+j omega k}, omega = 2 pi offset / fs_in, the phase reduced in integers first
-        const double ph = 2.0 * M_PI * (double)chan_mod((int64_t)offset_hz * (j - H), fs) / (double)fs;
-        g[2 * j]        = (float)(hn * std::cos(ph));
-        g[2 * j + 1]    = (float)(hn * std::sin(ph));
-      }
-    }
-  }
-  if (rot) { // r[i] = e^{-j omega i D}
-    const int64_t step = chan_mod((int64_t)d * offset_hz, fs);
-    for (int64_t i = 0; i < (int64_t)p; i++) {
-      const double ph = -2.0 * M_PI * (double)((step * i) % fs) / (double)fs;
-      rot[2 * i]      = (float)std::cos(ph);
-      rot[2 * i + 1]  = (float)std::sin(ph);
-    }
-  }
-  return LTEPHY_SUCCESS;
-}
-
 static int64_t chan_gcd(int64_t a, int64_t b)
 {
   while (b) {
@@ -133,29 +64,27 @@ static int64_t chan_gcd(int64_t a, int64_t b)
   return a;
 }
 
-// geometry of a carrier under the plan's flags: an integer carrier keeps chan_geometry (L = 1, M = D, Ka = Kb = H, *poly false); with
-// LTEPHY_CHAN_RATIONAL any other ratio L / M within the limits of DESIGN.md §2.  0, or INVALID_INPUTS with the reason in the last error
-static int chan_poly_geometry(uint32_t fs_in, int32_t offset_hz, uint32_t N, uint32_t flags, ltephy_chan_poly_t* q, bool* poly)
+// geometry of a carrier under the plan's flags (DESIGN.md §2): fs_out / fs_in = L / M in lowest terms; an integer decimation D = 2..128 is L = 1,
+// M = D, Tp = Kp = T, Ka = Kb = H, flag or not, and with LTEPHY_CHAN_RATIONAL any other ratio within the limits is accepted.  0, or
+// INVALID_INPUTS with the reason in the last error
+static int chan_geometry(uint32_t fs_in, int32_t offset_hz, uint32_t N, uint32_t flags, ltephy_chan_poly_t* q)
 {
   const uint32_t prb = chan_max_prb(N);
   if (!prb) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: symbol size %u not supported", N);
   if (fs_in == 0 || fs_in > LTEPHY_CHAN_MAX_FS) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: fs_in %u outside 1..245760000", fs_in);
   if (offset_hz % 1000) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: offset %d Hz is not a multiple of 1 kHz", offset_hz);
   const int64_t fs_out = 15000ll * N, gg = chan_gcd(fs_out, fs_in), L = fs_out / gg, M = fs_in / gg;
-  *poly = !(L == 1 && M >= 2 && M <= 128);
-  if (!*poly || !(flags & LTEPHY_CHAN_RATIONAL)) {
-    uint32_t T, D, P;
-    if (int r = chan_geometry(fs_in, offset_hz, N, &T, &D, &P)) return r;
-    q->L = 1, q->M = D, q->Tp = T, q->Kp = T, q->Ka = T / 2, q->Kb = T / 2, q->P = P;
-    return LTEPHY_SUCCESS;
+  if (!(L == 1 && M >= 2 && M <= 128)) {
+    if (!(flags & LTEPHY_CHAN_RATIONAL))
+      return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: fs_in %u / %lld is not an integer decimation 2..128", fs_in, (long long)fs_out);
+    if (L > CHAN_MAX_L) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: fs_out / fs_in = %lld / %lld, L above 1024", (long long)L, (long long)M);
+    if (M > 128 * L) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: fs_out / fs_in = %lld / %lld is below 1 / 128", (long long)L, (long long)M);
+    if (L > 2 * M) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: fs_out / fs_in = %lld / %lld upsamples more than 2x", (long long)L, (long long)M);
   }
-  if (L > CHAN_MAX_L) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: fs_out / fs_in = %lld / %lld, L above 1024", (long long)L, (long long)M);
-  if (M > 128 * L) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: fs_out / fs_in = %lld / %lld is below 1 / 128", (long long)L, (long long)M);
-  if (L > 2 * M) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: fs_out / fs_in = %lld / %lld upsamples more than 2x", (long long)L, (long long)M);
   const int64_t f_pass = 90000ll * prb, aoff = std::llabs((long long)offset_hz), mn = std::min<int64_t>(fs_out, fs_in);
   if (2 * (aoff + f_pass) > (int64_t)fs_in)
     return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: band of the carrier at %d Hz (N %u) reaches outside the capture", offset_hz, N);
-  // Kaiser's length for 70 dB over [f_pass, min(fs_in, fs_out) - f_pass] at the prototype's rate L fs_in, made odd
+  // Kaiser's length for 70 dB over [f_pass, min(fs_in, fs_out) - f_pass] at the prototype's rate L fs_in (scipy.signal.kaiserord), made odd
   const double  width = (double)(mn - 2 * f_pass) / (0.5 * (double)(L * (int64_t)fs_in));
   const double  nt    = (CHAN_ATTEN - 7.95) / 2.285 / (M_PI * width) + 1.0;
   const int64_t tp = (int64_t)std::ceil(nt) | 1, hp = (tp - 1) / 2, ka = hp / L, kb = (hp + L - 1) / L;
@@ -167,20 +96,15 @@ static int chan_poly_geometry(uint32_t fs_in, int32_t offset_hz, uint32_t N, uin
   return LTEPHY_SUCCESS;
 }
 
-// the tables of a carrier under the plan's flags, in the arithmetic of lteo_chan_design_poly: an integer carrier's are chan_design's
-static int chan_design_poly(uint32_t fs_in, int32_t offset_hz, uint32_t N, uint32_t flags, ltephy_chan_poly_t* out, float* hp, float* g, float* rot)
+// the tables of a carrier under the plan's flags, in the arithmetic of lteo_chan_design_poly, and at L = 1 of lteo_chan_design
+static int chan_design(uint32_t fs_in, int32_t offset_hz, uint32_t N, uint32_t flags, ltephy_chan_poly_t* out, float* hp, float* g, float* rot)
 {
   ltephy_chan_poly_t q;
-  bool               poly;
-  if (int r = chan_poly_geometry(fs_in, offset_hz, N, flags, &q, &poly)) return r;
+  if (int r = chan_geometry(fs_in, offset_hz, N, flags, &q)) return r;
   if (out) *out = q;
-  if (!poly) {
-    uint32_t T, D, P;
-    return chan_design(fs_in, offset_hz, N, hp, g, rot, &T, &D, &P);
-  }
   const int64_t L = q.L, Hp = (q.Tp - 1) / 2, Lfs = L * (int64_t)fs_in, fs_out = 15000ll * N;
   if (hp || g) {
-    // windowed sinc with cutoff min(fs_in, fs_out) / 2 at rate L fs_in, scaled to DC gain L
+    // windowed sinc with cutoff min(fs_in, fs_out) / 2 at rate L fs_in, scaled to DC gain L (scipy.signal.firwin, times L)
     std::vector<double> hd(q.Tp);
     const double        beta = 0.1102 * (CHAN_ATTEN - 8.7), a = 0.5 * (double)(q.Tp - 1), i0b = chan_i0(beta), c = 1.0 / (double)std::max(q.L, q.M);
     double              s = 0.0;
@@ -207,10 +131,12 @@ static int chan_design_poly(uint32_t fs_in, int32_t offset_hz, uint32_t N, uint3
           o[1]              = (float)(tap * std::sin(a2));
         }
   }
-  if (rot) { // r[i] = e^{-j 2 pi offset i / fs_out}
-    const int64_t step = chan_mod(offset_hz, fs_out);
+  if (rot) {
+    // r[i] = e^{-j 2 pi offset i / fs_out}, the angle reduced in int64 over F before it is divided: at L = 1 over fs_in, as (D offset i) mod fs_in
+    // (DESIGN.md §2 "channeliser"; the same angle as over fs_out, but not the same last bit when D is not a power of 2), else over fs_out
+    const int64_t F = L == 1 ? (int64_t)fs_in : fs_out, step = chan_mod((int64_t)offset_hz * (F / fs_out), F);
     for (int64_t i = 0; i < (int64_t)q.P; i++) {
-      const double ph = -2.0 * M_PI * (double)((step * i) % fs_out) / (double)fs_out;
+      const double ph = -2.0 * M_PI * (double)((step * i) % F) / (double)F;
       rot[2 * i]      = (float)std::cos(ph);
       rot[2 * i + 1]  = (float)std::sin(ph);
     }
@@ -229,8 +155,7 @@ static int chan_check_cfg(const ltephy_chan_cfg_t* cfg)
   if (cfg->iq_format > LTEPHY_IQ_SC8) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: unknown iq_format %u", cfg->iq_format);
   for (uint32_t c = 0; c < cfg->nof_carriers; c++) {
     ltephy_chan_poly_t q;
-    bool               poly;
-    if (int r = chan_poly_geometry(cfg->fs_in, cfg->carrier[c].offset_hz, cfg->carrier[c].symbol_sz, cfg->flags, &q, &poly)) return r;
+    if (int r = chan_geometry(cfg->fs_in, cfg->carrier[c].offset_hz, cfg->carrier[c].symbol_sz, cfg->flags, &q)) return r;
   }
   return LTEPHY_SUCCESS;
 }
@@ -240,13 +165,14 @@ extern "C" int ltephy_chan_taps(const ltephy_chan_cfg_t* cfg, uint32_t c, float*
   if (!cfg || !T || !D || !P) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan_taps: null argument");
   if (c >= cfg->nof_carriers || c >= LTEPHY_CHAN_MAX_CARRIERS)
     return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan_taps: carrier %u of %u", c, cfg->nof_carriers);
-  if (cfg->flags & LTEPHY_CHAN_RATIONAL) {
-    ltephy_chan_poly_t q;
-    bool               poly;
-    if (chan_poly_geometry(cfg->fs_in, cfg->carrier[c].offset_hz, cfg->carrier[c].symbol_sz, cfg->flags, &q, &poly) == LTEPHY_SUCCESS && poly)
-      return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan_taps: carrier %u is rational (L %u / M %u): its tables come from ltephy_chan_design", c, q.L, q.M);
-  }
-  return chan_design(cfg->fs_in, cfg->carrier[c].offset_hz, cfg->carrier[c].symbol_sz, h, g, rot, T, D, P);
+  const ltephy_chan_carrier_t& k = cfg->carrier[c];
+  ltephy_chan_poly_t           q;
+  if ((cfg->flags & LTEPHY_CHAN_RATIONAL) && chan_geometry(cfg->fs_in, k.offset_hz, k.symbol_sz, cfg->flags, &q) == LTEPHY_SUCCESS &&
+      !(q.L == 1 && q.M > 1))
+    return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan_taps: carrier %u is rational (L %u / M %u): its tables come from ltephy_chan_design", c, q.L, q.M);
+  if (int r = chan_design(cfg->fs_in, k.offset_hz, k.symbol_sz, 0, &q, h, g, rot)) return r; // without the flag: L = 1, M = D = 2..128
+  *T = q.Tp, *D = q.M, *P = q.P;
+  return LTEPHY_SUCCESS;
 }
 
 extern "C" int ltephy_chan_design(const ltephy_chan_cfg_t* cfg, uint32_t c, ltephy_chan_poly_t* out, float* hp, float* g, float* rot)
@@ -255,7 +181,7 @@ extern "C" int ltephy_chan_design(const ltephy_chan_cfg_t* cfg, uint32_t c, ltep
   if (c >= cfg->nof_carriers || c >= LTEPHY_CHAN_MAX_CARRIERS)
     return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan_design: carrier %u of %u", c, cfg->nof_carriers);
   if (cfg->flags & ~LTEPHY_CHAN_RATIONAL) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan_design: unknown flags 0x%x", cfg->flags);
-  return chan_design_poly(cfg->fs_in, cfg->carrier[c].offset_hz, cfg->carrier[c].symbol_sz, cfg->flags, out, hp, g, rot);
+  return chan_design(cfg->fs_in, cfg->carrier[c].offset_hz, cfg->carrier[c].symbol_sz, cfg->flags, out, hp, g, rot);
 }
 
 extern "C" int ltephy_chan_create(const ltephy_chan_cfg_t* cfg, ltephy_chan_t** out)
@@ -273,33 +199,22 @@ extern "C" int ltephy_chan_create(const ltephy_chan_cfg_t* cfg, ltephy_chan_t** 
   if (h->d_x.reserve((xbytes + sizeof(float2) - 1) / sizeof(float2))) return fail(LTEPHY_ERROR, "chan_create: device allocation failed");
   for (uint32_t c = 0; c < cfg->nof_carriers; c++) {
     ltephy_chan::Carrier& k = h->car[c];
-    chan_poly_geometry(cfg->fs_in, cfg->carrier[c].offset_hz, cfg->carrier[c].symbol_sz, cfg->flags, &k.pq, &k.poly);
-    if (k.poly) {
-      const ltephy_chan_poly_t& q = k.pq;
-      std::vector<float>        g(2 * (size_t)q.L * q.Kp), rot(2 * (size_t)q.P);
-      chan_design_poly(cfg->fs_in, cfg->carrier[c].offset_hz, cfg->carrier[c].symbol_sz, cfg->flags, nullptr, nullptr, g.data(), rot.data());
-      // rows per phase class: the span R M + Kp within CHAN_PSPAN; from 32 rows up, whole warps per class and about 4096 outputs a tile
-      uint32_t R = std::max<int64_t>(1, ((int64_t)CHAN_PSPAN - (int64_t)q.Kp) / (int64_t)q.M);
-      if (R >= 32) R = std::max<uint32_t>(32, std::min<uint32_t>(R, 4096 / q.L) / 32 * 32);
-      k.R   = R, k.P = q.P;
-      k.cap = (uint64_t)(((unsigned __int128)cfg->max_samples * q.L) / q.M) + 2;
-      const uint64_t span = ((uint64_t)(q.L - 1) + ((uint64_t)q.L * R - 1) * q.M) / q.L + q.Kp;
-      h->psmem            = std::max(h->psmem, (size_t)span * sizeof(float2));
-      if (k.g.reserve(g.size() / 2) || k.rot.reserve(q.P) || k.out.reserve((size_t)cfg->nof_rx * k.cap))
-        return fail(LTEPHY_ERROR, "chan_create: device allocation failed");
-      CU(cudaMemcpy(k.g.p, g.data(), g.size() * sizeof(float), cudaMemcpyHostToDevice));
-      CU(cudaMemcpy(k.rot.p, rot.data(), rot.size() * sizeof(float), cudaMemcpyHostToDevice));
-      continue;
+    ltephy_chan_poly_t&   q = k.q;
+    chan_geometry(cfg->fs_in, cfg->carrier[c].offset_hz, cfg->carrier[c].symbol_sz, cfg->flags, &q);
+    std::vector<float> g(2 * (size_t)q.L * q.Kp), rot(2 * (size_t)q.P);
+    chan_design(cfg->fs_in, cfg->carrier[c].offset_hz, cfg->carrier[c].symbol_sz, cfg->flags, nullptr, nullptr, g.data(), rot.data());
+    k.Q = q.L == 1 ? q.M : 1;
+    if (k.Q > 1) { // an integer carrier: R = min(1024, max(64, (CHAN_SPAN - T) / D + 1)) outputs, the span split into its D phases
+      k.R = (uint32_t)std::min<int64_t>(1024, std::max<int64_t>(64, ((int64_t)CHAN_SPAN - (int64_t)q.Kp) / (int64_t)q.M + 1));
+    } else { // rows per phase class: the span R M + Kp within CHAN_PSPAN; from 32 rows up, whole warps per class and about 4096 outputs a tile
+      k.R = (uint32_t)std::max<int64_t>(1, ((int64_t)CHAN_PSPAN - (int64_t)q.Kp) / (int64_t)q.M);
+      if (k.R >= 32) k.R = std::max<uint32_t>(32, std::min<uint32_t>(k.R, 4096 / q.L) / 32 * 32);
     }
-    chan_design(cfg->fs_in, cfg->carrier[c].offset_hz, cfg->carrier[c].symbol_sz, nullptr, nullptr, nullptr, &k.T, &k.D, &k.P);
-    std::vector<float> g(2 * (size_t)k.T), rot(2 * (size_t)k.P);
-    chan_design(cfg->fs_in, cfg->carrier[c].offset_hz, cfg->carrier[c].symbol_sz, nullptr, g.data(), rot.data(), &k.T, &k.D, &k.P);
-    const int64_t fit = ((int64_t)CHAN_SPAN - (int64_t)k.T) / (int64_t)k.D + 1;
-    k.M    = (uint32_t)std::min<int64_t>(1024, std::max<int64_t>(64, fit));
-    k.rows = k.M - 1 + (k.T + k.D - 1) / k.D;
-    k.cap  = cfg->max_samples / k.D + 2;
-    h->smem = std::max(h->smem, ((size_t)k.T + (size_t)k.rows * k.D) * sizeof(float2));
-    if (k.g.reserve(k.T) || k.rot.reserve(k.P) || k.out.reserve((size_t)cfg->nof_rx * k.cap))
+    const uint64_t span = ((uint64_t)(q.L - 1) + ((uint64_t)q.L * k.R - 1) * q.M) / q.L + q.Kp; // the longest span of a tile
+    k.rows              = (uint32_t)((span + k.Q - 1) / k.Q);
+    k.cap               = (uint64_t)(((unsigned __int128)cfg->max_samples * q.L) / q.M) + 2;
+    h->smem             = std::max(h->smem, ((q.L == 1 ? q.Kp : 0) + (size_t)k.Q * k.rows) * sizeof(float2)); // taps at L = 1, and the span
+    if (k.g.reserve(g.size() / 2) || k.rot.reserve(q.P) || k.out.reserve((size_t)cfg->nof_rx * k.cap))
       return fail(LTEPHY_ERROR, "chan_create: device allocation failed");
     CU(cudaMemcpy(k.g.p, g.data(), g.size() * sizeof(float), cudaMemcpyHostToDevice));
     CU(cudaMemcpy(k.rot.p, rot.data(), rot.size() * sizeof(float), cudaMemcpyHostToDevice));
@@ -328,57 +243,34 @@ static int chan_run(ltephy_chan_t* h, const void* x, uint64_t first, uint64_t n,
 {
   const uint32_t A = h->cfg.nof_rx;
   ChanArgs       g{};
-  ChanPolyArgs   pg{};
   g.x = x, g.lda = n, g.first = first;
-  pg.x = x, pg.lda = n, pg.first = first;
-  uint32_t ntiles = 0, nptiles = 0;
+  uint32_t ntiles = 0;
   uint64_t nx     = UINT64_MAX;
   for (uint32_t c = 0; c < h->cfg.nof_carriers; c++) {
     const ltephy_chan::Carrier& k = h->car[c];
-    if (k.poly) {
-      // outputs m >= 0 whose window [n - Ka, n + Kb], n = floor(m M / L), has every non-negative sample inside [first, first + n)
-      const ltephy_chan_poly_t& q = k.pq;
-      const unsigned __int128   L = q.L, M = q.M, last = first + n - 1;
-      const uint64_t lo   = first == 0 ? 0 : (uint64_t)(((first + q.Ka) * L + M - 1) / M);
-      const uint64_t hi_n = last >= q.Kb ? (uint64_t)(((last - q.Kb + 1) * L - 1) / M + 1) : 0;
-      const uint64_t cnt  = hi_n > lo ? hi_n - lo : 0;
-      const uint64_t mn = cnt ? hi_n : lo, nn = (uint64_t)(mn * M / L);
-      nx                = std::min<uint64_t>(nx, nn >= q.Ka ? nn - q.Ka : 0);
-      out[c].first = lo, out[c].count = cnt, out[c].iq_dev = k.out.p;
-      if (!cnt) continue;
-      const uint64_t per   = (uint64_t)q.L * k.R;
-      const uint32_t tiles = (uint32_t)((cnt + per - 1) / per);
-      for (uint32_t a = 0; a < A; a++) {
-        ChanPolySeg& s = pg.seg[pg.nseg++];
-        s.g = k.g.p, s.rot = k.rot.p, s.out = k.out.p + (size_t)a * cnt, s.n0 = (uint64_t)(lo * M / L), s.count = cnt;
-        s.phi0 = (uint32_t)(lo * M % L), s.r0 = (uint32_t)(lo % q.P), s.L = q.L, s.M = q.M, s.Kp = q.Kp, s.Ka = q.Ka, s.P = q.P, s.R = k.R;
-        s.tile0 = nptiles, s.a = a;
-        nptiles += tiles;
-      }
-      continue;
-    }
-    // outputs m >= 0 whose window [m D - H, m D + H] has every non-negative sample inside [first, first + n)
-    const uint64_t H = k.T / 2, last = first + n - 1;
-    const uint64_t lo   = first == 0 ? 0 : (first + H + k.D - 1) / k.D;
-    const uint64_t hi_n = last >= H ? (last - H) / k.D + 1 : 0;
-    const uint64_t cnt  = hi_n > lo ? hi_n - lo : 0;
-    const uint64_t mn   = cnt ? hi_n : lo;
-    nx                  = std::min(nx, mn * k.D >= H ? mn * k.D - H : 0);
+    const ltephy_chan_poly_t&   q = k.q;
+    // outputs m >= 0 whose window [n - Ka, n + Kb], n = floor(m M / L), has every non-negative sample inside [first, first + n)
+    const unsigned __int128 L = q.L, M = q.M, last = first + n - 1;
+    const uint64_t          lo   = first == 0 ? 0 : (uint64_t)(((first + q.Ka) * L + M - 1) / M);
+    const uint64_t          hi_n = last >= q.Kb ? (uint64_t)(((last - q.Kb + 1) * L - 1) / M + 1) : 0;
+    const uint64_t          cnt  = hi_n > lo ? hi_n - lo : 0;
+    const uint64_t          mn = cnt ? hi_n : lo, nn = (uint64_t)(mn * M / L);
+    nx                         = std::min<uint64_t>(nx, nn >= q.Ka ? nn - q.Ka : 0);
     out[c].first = lo, out[c].count = cnt, out[c].iq_dev = k.out.p;
     if (!cnt) continue;
-    const uint32_t tiles = (uint32_t)((cnt + k.M - 1) / k.M);
+    const uint64_t per   = (uint64_t)q.L * k.R;
+    const uint32_t tiles = (uint32_t)((cnt + per - 1) / per);
     for (uint32_t a = 0; a < A; a++) {
       ChanSeg& s = g.seg[g.nseg++];
-      s.g = k.g.p, s.rot = k.rot.p, s.out = k.out.p + (size_t)a * cnt, s.m0 = lo, s.count = (uint32_t)cnt;
-      s.D = k.D, s.T = k.T, s.P = k.P, s.M = k.M, s.rows = k.rows, s.tile0 = ntiles, s.a = a;
+      s.g = k.g.p, s.rot = k.rot.p, s.out = k.out.p + (size_t)a * cnt, s.n0 = (uint64_t)(lo * M / L), s.count = cnt;
+      s.phi0 = (uint32_t)(lo * M % L), s.r0 = (uint32_t)(lo % q.P), s.L = q.L, s.M = q.M, s.Kp = q.Kp, s.Ka = q.Ka, s.P = q.P, s.R = k.R;
+      s.Q = k.Q, s.rows = k.rows, s.tile0 = ntiles, s.a = a;
       ntiles += tiles;
     }
   }
   *next = nx;
   if (launch_chan(g, ntiles, h->smem, h->cfg.iq_format, h->stream))
     return fail(LTEPHY_ERROR, "chan_run: kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
-  if (launch_chan_poly(pg, nptiles, h->psmem, h->cfg.iq_format, h->stream))
-    return fail(LTEPHY_ERROR, "chan_run: polyphase kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
   CU(cudaStreamSynchronize(h->stream));
   return LTEPHY_SUCCESS;
 }

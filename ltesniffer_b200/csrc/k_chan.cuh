@@ -1,4 +1,4 @@
-// k_chan.cuh -- arguments shared by the channeliser kernels (k_chan.cu) and its host code (chan.cu).  Private to libltephy_b200.
+// k_chan.cuh -- arguments shared by the channeliser kernel (k_chan.cu) and its host code (chan.cu).  Private to libltephy_b200.
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -6,14 +6,18 @@
 #define CHAN_THREADS 256
 #define CHAN_MAX_SEGS 16 // 8 carriers x 2 antennas
 
-struct ChanSeg {       // one (carrier, antenna) of a call: outputs m0 .. m0 + count - 1, in tiles of M
-  const float2* g;     // [T] taps g[k] at k + H
+struct ChanSeg {       // one (carrier, antenna) of a call: outputs m0 .. m0 + count - 1, in tiles of L R (an integer carrier: L = 1, M = D)
+  const float2* g;     // [L][Kp] phase taps g_phi[k] at [phi][k + Kb]
   const float2* rot;   // [P] r[m mod P]
   float2*       out;   // [count] this antenna's row of the carrier's output
-  uint64_t      m0;    // first output index
-  uint32_t      count, D, T, P;
-  uint32_t      M;     // outputs per tile
-  uint32_t      rows;  // rows of the tile's polyphase input in shared memory: M - 1 + ceil(T / D)
+  uint64_t      n0;    // floor(m0 M / L): the capture sample of output m0
+  uint64_t      count;
+  uint32_t      phi0;  // m0 M mod L
+  uint32_t      r0;    // m0 mod P
+  uint32_t      L, M, Kp, Ka, P;
+  uint32_t      R;     // outputs per phase class in a tile: a tile holds outputs m0 + i0 + c + L r, c < L, r < R
+  uint32_t      Q;     // phases of the tile's span in shared memory: position s at row s / Q of phase s mod Q (M at L = 1, else 1)
+  uint32_t      rows;  // rows per phase: ceil(longest span / Q)
   uint32_t      tile0; // first tile of this segment in the grid
   uint32_t      a;     // antenna
 };
@@ -25,27 +29,5 @@ struct ChanArgs {
   ChanSeg       seg[CHAN_MAX_SEGS];
 };
 
-struct ChanPolySeg {   // one (rational carrier, antenna) of a call: outputs m0 .. m0 + count - 1, in tiles of L R
-  const float2* g;     // [L][Kp] phase taps g_phi[k] at [phi][k + Kb]
-  const float2* rot;   // [P] r[m mod P]
-  float2*       out;   // [count] this antenna's row of the carrier's output
-  uint64_t      n0;    // floor(m0 M / L): the capture sample of output m0
-  uint64_t      count;
-  uint32_t      phi0;  // m0 M mod L
-  uint32_t      r0;    // m0 mod P
-  uint32_t      L, M, Kp, Ka, P;
-  uint32_t      R;     // outputs per phase class in a tile: a tile holds outputs m0 + i0 + c + L r, c < L, r < R
-  uint32_t      tile0; // first tile of this segment in the grid
-  uint32_t      a;     // antenna
-};
-
-struct ChanPolyArgs {
-  const void*   x;     // as ChanArgs
-  uint64_t      lda, first;
-  uint32_t      nseg, pad;
-  ChanPolySeg   seg[CHAN_MAX_SEGS];
-};
-
 // every tile of every segment in one launch: ntiles CTAs of CHAN_THREADS, smem bytes of dynamic shared memory; fmt is the plan's iq_format
 extern "C" int launch_chan(const ChanArgs& g, uint32_t ntiles, size_t smem, uint32_t fmt, cudaStream_t st);
-extern "C" int launch_chan_poly(const ChanPolyArgs& g, uint32_t ntiles, size_t smem, uint32_t fmt, cudaStream_t st);
