@@ -84,6 +84,9 @@ static int chan_geometry(uint32_t fs_in, int32_t offset_hz, uint32_t N, uint32_t
   const int64_t f_pass = 90000ll * prb, aoff = std::llabs((long long)offset_hz), mn = std::min<int64_t>(fs_out, fs_in);
   if (2 * (aoff + f_pass) > (int64_t)fs_in)
     return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: band of the carrier at %d Hz (N %u) reaches outside the capture", offset_hz, N);
+  if (mn <= 2 * f_pass) // the transition band [f_pass, min(fs_in, fs_out) - f_pass] would be empty, and Kaiser's length infinite
+    return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: carrier at %d Hz (N %u) leaves no transition band: min(fs_in, fs_out) %lld <= 2 f_pass %lld", offset_hz,
+                N, (long long)mn, (long long)(2 * f_pass));
   // Kaiser's length for 70 dB over [f_pass, min(fs_in, fs_out) - f_pass] at the prototype's rate L fs_in (scipy.signal.kaiserord), made odd
   const double  width = (double)(mn - 2 * f_pass) / (0.5 * (double)(L * (int64_t)fs_in));
   const double  nt    = (CHAN_ATTEN - 7.95) / 2.285 / (M_PI * width) + 1.0;

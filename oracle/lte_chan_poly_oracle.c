@@ -56,6 +56,7 @@ static int poly_geometry(uint32_t fs_in, int32_t offset_hz, uint32_t N, lteo_cha
   if (L > CHAN_MAX_L || M > 128 * L || L > 2 * M) return -2;
   const int64_t f_pass = 90000ll * prb, aoff = llabs((long long)offset_hz), mn = fs_out < (int64_t)fs_in ? fs_out : (int64_t)fs_in;
   if (2 * (aoff + f_pass) > (int64_t)fs_in) return -2;
+  if (mn <= 2 * f_pass) return -2; /* no transition band [f_pass, min(fs_in, fs_out) - f_pass] */
   /* Kaiser's length for 70 dB over [f_pass, min(fs_in, fs_out) - f_pass] at the prototype's rate L fs_in, made odd */
   const double width = (double)(mn - 2 * f_pass) / (0.5 * (double)(L * (int64_t)fs_in));
   const double nt    = (CHAN_ATTEN - 7.95) / 2.285 / (M_PI * width) + 1.0;

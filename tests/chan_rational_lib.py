@@ -101,6 +101,8 @@ def geometry(fs_in, offset_hz, N):
     f_pass = 90000 * CH.MAX_PRB[N]
     if L > MAX_L or M > 128 * L or L > 2 * M or abs(offset_hz) + f_pass > fs_in / 2:
         return None
+    if min(fs_in, fs_out) <= 2 * f_pass:     # no transition band
+        return None
     w = (min(fs_in, fs_out) - 2 * f_pass) / (L * fs_in / 2)
     Tp = ss.kaiserord(CH.ATTEN, w)[0] | 1
     Hp = (Tp - 1) // 2
@@ -109,6 +111,33 @@ def geometry(fs_in, offset_hz, N):
         return None
     P = fs_out // math.gcd(offset_hz % fs_out, fs_out)
     return dict(L=L, M=M, Tp=Tp, Kp=Ka + Kb + 1, Ka=Ka, Kb=Kb, P=P, f_pass=f_pass, w=w)
+
+
+def tile_rows(L, M, Kp):
+    """R of a carrier's tiles of L R outputs (DESIGN.md §4 C1): min(1024, max(64, (4096 - T) / D + 1)) at L = 1, else (12288 - Kp) / M rows per
+    phase class, at least 1, and from 32 up a multiple of 32 with about 4096 outputs a tile"""
+    if L == 1:
+        return min(1024, max(64, (4096 - Kp) // M + 1))
+    R = max(1, (12288 - Kp) // M)
+    return max(32, min(R, 4096 // L) // 32 * 32) if R >= 32 else R
+
+
+def plan_space(step=1000):
+    """every (fs_in, N) with fs_in on the step-Hz grid up to 245.76 MHz that the rational rule accepts at offset 0 -> [dict(fs, N, L, M, Tp,
+    Kp, Ka, Kb, P, R)], in N then fs_in order.  The ratio limits are checked in integers first, so only plausible plans reach geometry()."""
+    plans = []
+    for N in CH.SYMBOL_SIZES:
+        fs_out, f2 = 15000 * N, 2 * 90000 * CH.MAX_PRB[N]
+        for fs in range(step, 245760000 + 1, step):
+            g = math.gcd(fs_out, fs)
+            L, M = fs_out // g, fs // g
+            if fs < f2 or L > MAX_L or M > 128 * L or L > 2 * M:
+                continue
+            d = geometry(fs, 0, N)
+            if d is not None:
+                d.update(fs=fs, N=N, R=tile_rows(d["L"], d["M"], d["Kp"]))
+                plans.append(d)
+    return plans
 
 
 def reference(fs_in, offset_hz, N, x, ms):

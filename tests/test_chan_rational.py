@@ -191,6 +191,9 @@ REFUSED = [
     (25000000, [(10000000, 1024)], 1, 0, "band outside the capture", b"outside the capture"),
     (25000000, [(0, 1024)], 3, 0, "unknown flag bits", b"flags"),
     (25000000, [(0, 1024)], 1, 3, "unknown format", b"iq_format"),
+] + [  # fs_in = 2 f_pass < fs_out: the band check holds with equality, and the transition band [f_pass, fs_in - f_pass] is empty
+    (fs, [(0, N)], 1, 0, "no transition band at %g Msps, N %d" % (fs / 1e6, N), b"no transition band")
+    for fs, N in ((18000000, 1536), (18000000, 2048), (9000000, 768), (9000000, 1024), (4500000, 384), (4500000, 512), (2700000, 256), (1080000, 128))
 ]
 
 
