@@ -204,8 +204,8 @@ int ltephy_ul_grants_from_dcis(const ltephy_search_t* s, const ltephy_sf_info_t*
 /* Whole batch: IQ in host memory -> accepted DCIs + transport blocks.  seq orders concurrent calls on
  * different PHY handles that share one search object (the search runs strictly in seq order, starting
  * at 0); pass LTEPHY_SEQ_NONE for a single pipeline.  A call that fails, argument checks included, still passes its turn on.  A seq
- * whose turn is over (reused, or a restart from 0 on a search that has walked) returns LTEPHY_ERROR_INVALID_INPUTS at once and
- * consumes no turn.
+ * whose turn is over (reused, or a restart from 0 on a search that has walked), or that another call on this search object is decoding,
+ * returns LTEPHY_ERROR_INVALID_INPUTS at once and consumes no turn.
  *   info[n], cand_scratch[n*LTEPHY_MAX_LOC*LTEPHY_MAX_SIZES] (caller-owned, pinned if possible),
  *   dcis[max_dcis], tbs[2*max_dcis] (tbs[2*i+t] belongs to dcis[i]), payload. */
 int ltephy_decode_subframes(ltephy_t* h, ltephy_search_t* s, const float* iq, const uint32_t* tti, uint32_t n, uint64_t seq, ltephy_sf_info_t* info,

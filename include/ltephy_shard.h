@@ -84,7 +84,9 @@ typedef struct {
 /* One batch: this rank's n subframes (global subframe g = i * world + rank; every rank passes the same n and seq).
  *   iq: host memory (pinned makes the copy asynchronous), or device memory when iq_on_device != 0
  *   seq: 0, 1, 2, ... -- batch number, the same on every rank; calls for different seq may run concurrently on different
- *        handles h of the same rank (h must not be shared between concurrent calls)
+ *        handles h of the same rank (h must not be shared between concurrent calls).  A seq whose turn is over (reused, or a restart
+ *        from 0 on a shard that has decoded), a seq another call of this rank is decoding, and LTEPHY_SEQ_NONE return
+ *        LTEPHY_ERROR_INVALID_INPUTS at once: no section is taken and the rank does not count as failed
  *   info[n]: this rank's subframes
  *   dcis[max_dcis], *n_dcis: accepted DCIs of ALL n * world subframes in the order the walk produced them (sf = g)
  *   tbs[2 * max_dcis]: tbs[2 * i + t] belongs to dcis[i].  Rank 0 receives the transport blocks of every rank; other

@@ -11,10 +11,10 @@
 #include "../../include/lte_tables.h"
 #include "lte_host.hpp"
 #include "tb_merge.hpp"
+#include "turn.hpp"
 #include <algorithm>
 #include <chrono>
 #include <cmath>
-#include <condition_variable>
 #include <cstddef>
 #include <cstdio>
 #include <cstring>
@@ -117,8 +117,7 @@ struct RntiManager {
     remaining[f]--;
   }
   uint32_t n_rar = 0;        // RNTIs currently active with reason RAR (they make the walk look at every format-0 candidate)
-  bool     rar_seen = false; // sticky: some RNTI has been RAR-activated since creation (a superset of n_rar > 0 that does not
-                             // depend on how far the walk has progressed, so that all ranks of a sharded run decide alike)
+  bool     rar_seen = false; // sticky: some RNTI has been RAR-activated since creation (ltephy_search::may_need_full_table)
   void     activate(uint16_t r, uint8_t why)
   {
     if (!rec[r].active) rec[r].active = 1, rec[r].reason = why, n_rar += why == ACT_RAR, rar_seen |= why == ACT_RAR;
@@ -295,10 +294,7 @@ struct ltephy_search {
   std::vector<TempDci0> temp_dci0;
   ltephy_dci_t*        out = nullptr;
   uint32_t             out_cap = 0, out_n = 0;
-  // batch ordering for concurrent pipelines
-  std::mutex              mtx;
-  std::condition_variable cv;
-  uint64_t                next_seq = 0;
+  Turn turn; // the walks of concurrent ltephy_decode_subframes calls, in seq order; its lock also keeps RNTI updates out of a walk
 
   void update_formats()
   {
@@ -542,6 +538,47 @@ struct ltephy_search {
     stats.nof_subframes++;
     if (n) *n = out_n;
     return out_n > cap ? LTEPHY_ERROR_INVALID_INPUTS : (ret < 0 ? 0 : ret);
+  }
+  // One subframe of a batch: what the walk reads, and the subframe's full table when the caller gave full tables (else nullptr)
+  struct WalkSf {
+    WalkIn               in;
+    const ltephy_cand_t* full;
+  };
+  // The walk over a batch: at(i) -> WalkSf of subframe i, for i = 0 .. n - 1 in order; dci.sf = i.  A subframe whose survivor form
+  // cannot serve is walked over its full table instead.
+  template <class At>
+  int search_batch(uint32_t n, At at, ltephy_dci_t* dcis, uint32_t max_dcis, uint32_t* n_dcis)
+  {
+    uint32_t nd = 0;
+    for (uint32_t i = 0; i < n; i++) {
+      WalkSf   sf = at(i);
+      uint32_t k  = 0;
+      int      r  = search_subframe(sf.in, i, dcis + nd, max_dcis - nd, &k);
+      if (r == LTEPHY_NEED_FULL_TABLE && sf.full) {
+        sf.in.table = sf.full, sf.in.loc = nullptr, sf.in.list = nullptr;
+        r = search_subframe(sf.in, i, dcis + nd, max_dcis - nd, &k);
+      }
+      if (r < 0) return r;
+      nd += std::min(k, max_dcis - nd);
+    }
+    *n_dcis = nd;
+    return LTEPHY_SUCCESS;
+  }
+  // Whether a walk over n survivor forms may need the full tables: some subframe overflows its survivor list (count(i) survivors), or
+  // RAR-activated RNTIs make the walk look at every format-0 candidate.  The RAR test depends on the use:
+  //   FOR_WALK        a walk given no full tables refuses such a batch before it consumes anything.  It asks for RNTIs active with reason
+  //                   RAR now (n_rar), which is exact: RAR activations only arrive between batches.
+  //   FOR_COLLECTIVE  the ranks of a sharded run decide on a collective fetch of the full tables before they walk.  They ask whether any
+  //                   RNTI was ever RAR-activated (rar_seen), a superset of n_rar > 0 that does not depend on how far the walk has progressed,
+  //                   so that every rank decides alike.
+  enum FullTableUse { FOR_WALK, FOR_COLLECTIVE };
+  template <class Count>
+  bool may_need_full_table(FullTableUse use, uint32_t n, Count count) const
+  {
+    if (use == FOR_WALK ? rm.n_rar != 0 : rm.rar_seen) return true;
+    for (uint32_t i = 0; i < n; i++)
+      if (count(i) > LTEPHY_COMPACT_CAP) return true;
+    return false;
   }
 };
 
@@ -1105,17 +1142,17 @@ void ltephy_search_config(ltephy_search_t* s, int shortcut, int skip_secondary, 
 }
 void ltephy_search_add_evergreen(ltephy_search_t* s, uint16_t a, uint16_t b, uint32_t f)
 {
-  std::lock_guard<std::mutex> lk(s->mtx);
+  std::lock_guard<std::mutex> lk(s->turn.m);
   if (f < NF && a <= b) s->rm.add_evergreen(a, b, f);
 }
 void ltephy_search_add_forbidden(ltephy_search_t* s, uint16_t a, uint16_t b, uint32_t f)
 {
-  std::lock_guard<std::mutex> lk(s->mtx);
+  std::lock_guard<std::mutex> lk(s->turn.m);
   if (f < NF && a <= b) s->rm.add_forbidden(a, b, f);
 }
 void ltephy_search_activate(ltephy_search_t* s, uint16_t rnti, uint32_t format_idx, int reason)
 {
-  std::lock_guard<std::mutex> lk(s->mtx); // another pipeline thread may be inside the walk
+  std::lock_guard<std::mutex> lk(s->turn.m); // another pipeline thread may be inside the walk
   s->rm.activate_and_refresh(rnti, format_idx, (uint8_t)reason);
 }
 int  ltephy_search_subframe(ltephy_search_t* s, const ltephy_sf_info_t* info, const ltephy_cand_t* cands, uint32_t sf_in_batch, ltephy_dci_t* out,
@@ -1198,59 +1235,41 @@ int      ltephy_search_rnti_is_forbidden(const ltephy_search_t* s, uint16_t r, u
 int      ltephy_search_rnti_is_evergreen(const ltephy_search_t* s, uint16_t r, uint32_t f) { return s->rm.is_evergreen(r, f); }
 
 // ===================================================================================================
-// Batch helpers.  ltephy_search_batch: FALCON walk over n subframes in order (dci.sf = index in the batch).
+// Batch helpers: the FALCON walk over n subframes in order (dci.sf = index in the batch), over full tables or survivor forms.
 int ltephy_search_batch(ltephy_search_t* s, const ltephy_sf_info_t* info, const ltephy_cand_t* cands, uint32_t n, ltephy_dci_t* dcis, uint32_t max_dcis,
                         uint32_t* n_dcis)
 {
   if (!s || !info || !cands || !dcis || !n_dcis) return LTEPHY_ERROR_INVALID_INPUTS;
-  uint32_t nd = 0;
-  for (uint32_t i = 0; i < n; i++) {
-    uint32_t k = 0;
-    int      r = s->search_subframe(info[i], cands + (size_t)i * LTEPHY_MAX_LOC * LTEPHY_MAX_SIZES, nullptr, i, dcis + nd, max_dcis - nd, &k);
-    if (r < 0) return r;
-    nd += std::min(k, max_dcis - nd);
-  }
-  *n_dcis = nd;
-  return LTEPHY_SUCCESS;
+  return s->search_batch(
+      n, [&](uint32_t i) { return ltephy_search::WalkSf{s->walk_in(info[i], cands + (size_t)i * LTEPHY_MAX_LOC * LTEPHY_MAX_SIZES, nullptr), nullptr}; },
+      dcis, max_dcis, n_dcis);
 }
 // Same walk over the survivor form.  full (optional) is the full table of the same batch; it is consulted for the
-// subframes the survivor form cannot serve.  Without it such a batch is refused up front, before anything is consumed
-// (RAR activations only arrive between batches, so the check is exact).
+// subframes the survivor form cannot serve.  Without it such a batch is refused up front, before anything is consumed.
 int ltephy_search_batch_compact(ltephy_search_t* s, const ltephy_sf_info_t* info, const ltephy_compact_t* comp, const ltephy_cand_t* full, uint32_t n,
                                 ltephy_dci_t* dcis, uint32_t max_dcis, uint32_t* n_dcis)
 {
   if (!s || !info || !comp || !dcis || !n_dcis) return LTEPHY_ERROR_INVALID_INPUTS;
-  if (!full) {
-    if (s->rm.n_rar) return LTEPHY_NEED_FULL_TABLE;
-    for (uint32_t i = 0; i < n; i++)
-      if (comp[i].count > LTEPHY_COMPACT_CAP) return LTEPHY_NEED_FULL_TABLE;
-  }
-  uint32_t nd = 0;
-  for (uint32_t i = 0; i < n; i++) {
-    uint32_t k = 0;
-    if (i + 2 < n) __builtin_prefetch(&comp[i + 2], 0, 3), __builtin_prefetch(&info[i + 2], 0, 3);
-    if (i + 1 < n) { // the inputs stream through once: have the next subframe's records in cache when its walk starts
-      const char*    c  = reinterpret_cast<const char*>(&comp[i + 1]);
-      const uint32_t nb = (uint32_t)offsetof(ltephy_compact_t, list) + 16u * std::min<uint32_t>(comp[i + 1].count, LTEPHY_COMPACT_CAP);
-      for (uint32_t o = 64; o < nb; o += 64) __builtin_prefetch(c + o, 0, 3);
-      const char* f = reinterpret_cast<const char*>(&info[i + 1]);
-      for (uint32_t o = 0; o < sizeof(ltephy_sf_info_t); o += 64) __builtin_prefetch(f + o, 0, 3);
-    }
-    int      r = s->search_subframe(info[i], nullptr, &comp[i], i, dcis + nd, max_dcis - nd, &k);
-    if (r == LTEPHY_NEED_FULL_TABLE) r = s->search_subframe(info[i], full + (size_t)i * LTEPHY_MAX_LOC * LTEPHY_MAX_SIZES, nullptr, i, dcis + nd, max_dcis - nd, &k);
-    if (r < 0) return r;
-    nd += std::min(k, max_dcis - nd);
-  }
-  *n_dcis = nd;
-  return LTEPHY_SUCCESS;
+  if (!full && s->may_need_full_table(ltephy_search::FOR_WALK, n, [&](uint32_t i) { return comp[i].count; })) return LTEPHY_NEED_FULL_TABLE;
+  return s->search_batch(
+      n,
+      [&](uint32_t i) {
+        if (i + 2 < n) __builtin_prefetch(&comp[i + 2], 0, 3), __builtin_prefetch(&info[i + 2], 0, 3);
+        if (i + 1 < n) { // the inputs stream through once: have the next subframe's records in cache when its walk starts
+          const char*    c  = reinterpret_cast<const char*>(&comp[i + 1]);
+          const uint32_t nb = (uint32_t)offsetof(ltephy_compact_t, list) + 16u * std::min<uint32_t>(comp[i + 1].count, LTEPHY_COMPACT_CAP);
+          for (uint32_t o = 64; o < nb; o += 64) __builtin_prefetch(c + o, 0, 3);
+          const char* f = reinterpret_cast<const char*>(&info[i + 1]);
+          for (uint32_t o = 0; o < sizeof(ltephy_sf_info_t); o += 64) __builtin_prefetch(f + o, 0, 3);
+        }
+        return ltephy_search::WalkSf{s->walk_in(info[i], nullptr, &comp[i]), full ? full + (size_t)i * LTEPHY_MAX_LOC * LTEPHY_MAX_SIZES : nullptr};
+      },
+      dcis, max_dcis, n_dcis);
 }
 int ltephy_search_needs_full_table(const ltephy_search_t* s, const ltephy_compact_t* comp, uint32_t n)
 {
   if (!s || !comp) return LTEPHY_ERROR_INVALID_INPUTS;
-  if (s->rm.rar_seen) return 1;
-  for (uint32_t i = 0; i < n; i++)
-    if (comp[i].count > LTEPHY_COMPACT_CAP) return 1;
-  return 0;
+  return s->may_need_full_table(ltephy_search::FOR_COLLECTIVE, n, [&](uint32_t i) { return comp[i].count; });
 }
 // Accepted DL DCIs -> PDSCH grants, applying decode_dl_mode's skip rule (src/src/DL_Sniffer_PDSCH.cc:887-889).
 // Only subframes with sf % mod == rem are taken (multi-GPU sharding); grant.sf = sf / mod (local index).
@@ -1435,60 +1454,48 @@ int ltephy_pack_subframes(const ltephy_search_t* s, const ltephy_sf_info_t* info
   offs[n] = (uint32_t)pos;
   return LTEPHY_SUCCESS;
 }
-static inline ltephy_search::WalkIn walk_in_packed(const ltephy_search_t* s, const uint8_t* rec, const ltephy_cand_t* full)
+// record i of rank r = global subframe g = i * world + r
+static inline const ltephy_packed_hdr_t* packed_hdr(const uint8_t* const* bufs, const uint32_t* const* offs, uint32_t world, uint32_t g)
 {
-  const ltephy_packed_hdr_t* hd = reinterpret_cast<const ltephy_packed_hdr_t*>(rec);
+  return reinterpret_cast<const ltephy_packed_hdr_t*>(bufs[g % world] + offs[g % world][g / world]);
+}
+static inline ltephy_search::WalkIn walk_in_packed(const ltephy_search_t* s, const ltephy_packed_hdr_t* hd)
+{
   // snr_db exactly as ltephy_finalize_info evaluates it (DESIGN.md section 2: log10f on the host from bit-exact device sums)
   const uint32_t P = s->cell.nof_ports, A = s->cell.nof_rx;
   float          ns = 0.0f, ps = 0.0f;
   for (uint32_t p = 0; p < P; p++)
     for (uint32_t a = 0; a < A; a++) ns = ns + hd->noise[p][a], ps = ps + hd->rsrp[p][a];
   const float npa = (float)(P * A), snr = 10.0f * log10f((ps / npa) / (ns / npa));
-  const ltephy_cloc_t* loc = reinterpret_cast<const ltephy_cloc_t*>(rec + sizeof(*hd));
-  ltephy_search::WalkIn w{hd->tti, hd->cfi, snr, {hd->low[0], hd->low[1]}, hd->count, full, nullptr, nullptr};
-  if (!full) w.loc = loc, w.list = reinterpret_cast<const ltephy_cand_t*>(loc + ((hd->nloc + 3u) & ~3u));
-  return w;
+  const ltephy_cloc_t* loc = reinterpret_cast<const ltephy_cloc_t*>(hd + 1);
+  return ltephy_search::WalkIn{hd->tti, hd->cfi, snr, {hd->low[0], hd->low[1]}, hd->count, nullptr, loc, reinterpret_cast<const ltephy_cand_t*>(loc + ((hd->nloc + 3u) & ~3u))};
 }
 int ltephy_packed_needs_full_table(const ltephy_search_t* s, const uint8_t* const* bufs, const uint32_t* const* offs, uint32_t world, uint32_t n)
 {
   if (!s || !bufs || !offs) return LTEPHY_ERROR_INVALID_INPUTS;
-  if (s->rm.rar_seen) return 1;
-  for (uint32_t r = 0; r < world; r++)
-    for (uint32_t i = 0; i < n; i++)
-      if (reinterpret_cast<const ltephy_packed_hdr_t*>(bufs[r] + offs[r][i])->count > LTEPHY_COMPACT_CAP) return 1;
-  return 0;
+  return s->may_need_full_table(ltephy_search::FOR_COLLECTIVE, n * world, [&](uint32_t g) { return packed_hdr(bufs, offs, world, g)->count; });
 }
 int ltephy_search_batch_packed(ltephy_search_t* s, const uint8_t* const* bufs, const uint32_t* const* offs, const ltephy_cand_t* const* full,
                                uint32_t world, uint32_t n, ltephy_dci_t* dcis, uint32_t max_dcis, uint32_t* n_dcis, uint32_t* tti_cfi)
 {
   if (!s || !bufs || !offs || !dcis || !n_dcis || world == 0) return LTEPHY_ERROR_INVALID_INPUTS;
-  if (!full) {
-    if (s->rm.n_rar) return LTEPHY_NEED_FULL_TABLE;
-    for (uint32_t r = 0; r < world; r++)
-      for (uint32_t i = 0; i < n; i++)
-        if (reinterpret_cast<const ltephy_packed_hdr_t*>(bufs[r] + offs[r][i])->count > LTEPHY_COMPACT_CAP) return LTEPHY_NEED_FULL_TABLE;
-  }
-  uint32_t nd = 0;
   const uint32_t total = n * world;
-  for (uint32_t g = 0; g < total; g++) {
-    const uint32_t r = g % world, i = g / world;
-    if (g + 1 < total) { // the records stream through once: pull the next one towards the core while this one is walked
-      const uint32_t r2 = (g + 1) % world, i2 = (g + 1) / world;
-      const uint8_t* nx = bufs[r2] + offs[r2][i2];
-      const uint32_t nb = offs[r2][i2 + 1] - offs[r2][i2];
-      for (uint32_t o = 0; o < nb; o += 64) __builtin_prefetch(nx + o, 0, 3);
-    }
-    const uint8_t* rec = bufs[r] + offs[r][i];
-    if (tti_cfi) tti_cfi[2 * g] = reinterpret_cast<const ltephy_packed_hdr_t*>(rec)->tti, tti_cfi[2 * g + 1] = reinterpret_cast<const ltephy_packed_hdr_t*>(rec)->cfi;
-    uint32_t k   = 0;
-    int      ret = s->search_subframe(walk_in_packed(s, rec, nullptr), g, dcis + nd, max_dcis - nd, &k);
-    if (ret == LTEPHY_NEED_FULL_TABLE) // only reachable with full != NULL (checked above)
-      ret = s->search_subframe(walk_in_packed(s, rec, full[r] + (size_t)i * LTEPHY_MAX_LOC * LTEPHY_MAX_SIZES), g, dcis + nd, max_dcis - nd, &k);
-    if (ret < 0) return ret;
-    nd += std::min(k, max_dcis - nd);
-  }
-  *n_dcis = nd;
-  return LTEPHY_SUCCESS;
+  if (!full && s->may_need_full_table(ltephy_search::FOR_WALK, total, [&](uint32_t g) { return packed_hdr(bufs, offs, world, g)->count; }))
+    return LTEPHY_NEED_FULL_TABLE;
+  return s->search_batch(
+      total,
+      [&](uint32_t g) {
+        if (g + 1 < total) { // the records stream through once: pull the next one towards the core while this one is walked
+          const uint32_t r2 = (g + 1) % world, i2 = (g + 1) / world;
+          const uint8_t* nx = bufs[r2] + offs[r2][i2];
+          const uint32_t nb = offs[r2][i2 + 1] - offs[r2][i2];
+          for (uint32_t o = 0; o < nb; o += 64) __builtin_prefetch(nx + o, 0, 3);
+        }
+        const ltephy_packed_hdr_t* hd = packed_hdr(bufs, offs, world, g);
+        if (tti_cfi) tti_cfi[2 * g] = hd->tti, tti_cfi[2 * g + 1] = hd->cfi;
+        return ltephy_search::WalkSf{walk_in_packed(s, hd), full ? full[g % world] + (size_t)(g / world) * LTEPHY_MAX_LOC * LTEPHY_MAX_SIZES : nullptr};
+      },
+      dcis, max_dcis, n_dcis);
 }
 
 // One call = what SubframeWorker::work does for every subframe of the batch (src/src/SubframeWorker.cc:142-207):
@@ -1508,31 +1515,10 @@ static int decode_common(ltephy_t* h, ltephy_search_t* s, const void* iq, bool i
 {
   if (!s) return LTEPHY_ERROR_INVALID_INPUTS;
   double t0 = now_ms();
-  // A seq whose turn is over would wait forever: refuse it without touching the turn.  A second call with the same seq that gets past
-  // this check while the first still waits is refused at the walk (both waits below wake once next_seq reaches or passes seq).
-  if (seq != LTEPHY_SEQ_NONE) {
-    std::lock_guard<std::mutex> lk(s->mtx);
-    if (seq < s->next_seq) return LTEPHY_ERROR_INVALID_INPUTS;
-  }
-  // Whatever happens before this batch's turn in the walk, the argument check included, the turn is taken and passed on: a failing
+  if (!s->turn.claim(seq)) return LTEPHY_ERROR_INVALID_INPUTS;
+  // Whatever happens before this batch's turn in the walk, the argument check included, the turn is passed on: a failing
   // batch must not leave the other pipelines of this search object waiting for a sequence number that never comes.
-  struct SeqGuard {
-    ltephy_search_t* s;
-    uint64_t         seq;
-    bool             done = false;
-    void             pass()
-    {
-      if (done || seq == LTEPHY_SEQ_NONE) return;
-      {
-        std::unique_lock<std::mutex> lk(s->mtx);
-        s->cv.wait(lk, [&] { return s->next_seq >= seq; });
-        if (s->next_seq == seq) s->next_seq = seq + 1;
-      }
-      s->cv.notify_all();
-      done = true;
-    }
-    ~SeqGuard() { pass(); }
-  } guard{s, seq};
+  TurnGuard turn(s->turn, seq);
   if (!h || !iq || !tti || !info || !cand_scratch || !dcis || !n_dcis || !tbs) return LTEPHY_ERROR_INVALID_INPUTS;
   int r = iq_on_device ? ltephy_submit_iq_device(h, iq, tti, n) : ltephy_submit_iq(h, (const float*)iq, tti, n);
   if (r) return r;
@@ -1542,23 +1528,13 @@ static int decode_common(ltephy_t* h, ltephy_search_t* s, const void* iq, bool i
   const ltephy_compact_t* comp = ltephy_phase_a_compact_buffer(h);
   double t2 = now_ms();
   uint32_t nd = 0;
-  {
-    std::unique_lock<std::mutex> lk(s->mtx);
-    s->cv.wait(lk, [&] { return seq == LTEPHY_SEQ_NONE || s->next_seq >= seq; });
-    if (seq != LTEPHY_SEQ_NONE && s->next_seq != seq) { // a duplicate seq whose turn another call has taken meanwhile
-      guard.done = true;
-      return LTEPHY_ERROR_INVALID_INPUTS;
-    }
-    r = ltephy_search_batch_compact(s, info, comp, nullptr, n, dcis, max_dcis, &nd);
-    if (r == LTEPHY_NEED_FULL_TABLE) { // RAR-activated RNTIs or an overfull subframe: fetch the 20 KB / subframe table after all
-      r = ltephy_get_phase_a(h, nullptr, cand_scratch);
-      if (r == LTEPHY_SUCCESS) r = ltephy_search_batch_compact(s, info, comp, cand_scratch, n, dcis, max_dcis, &nd);
-    }
-    if (seq != LTEPHY_SEQ_NONE) s->next_seq = seq + 1;
-    guard.done = true;
-    lk.unlock();
-    s->cv.notify_all();
+  turn.take();
+  r = ltephy_search_batch_compact(s, info, comp, nullptr, n, dcis, max_dcis, &nd);
+  if (r == LTEPHY_NEED_FULL_TABLE) { // RAR-activated RNTIs or an overfull subframe: fetch the 20 KB / subframe table after all
+    r = ltephy_get_phase_a(h, nullptr, cand_scratch);
+    if (r == LTEPHY_SUCCESS) r = ltephy_search_batch_compact(s, info, comp, cand_scratch, n, dcis, max_dcis, &nd);
   }
+  turn.pass();
   if (r < 0) return r;
   double t3 = now_ms();
   *n_dcis = nd;

@@ -6,9 +6,9 @@
 #include "../../include/ltephy_shard.h"
 #include "ltephy_internal.cuh"
 #include "tb_merge.hpp"
+#include "turn.hpp"
 #include <atomic>
 #include <chrono>
-#include <condition_variable>
 #include <dlfcn.h>
 #include <mutex>
 #include <nccl.h>
@@ -123,43 +123,6 @@ int        nccl_load()
     ncclResult_t r_ = (x);                                                                         \
     if (r_ != ncclSuccess) return fail(LTEPHY_ERROR, "%s: %s", #x, g_nccl.GetErrorString(r_));     \
   } while (0)
-
-struct Turn { // sections entered strictly in batch order
-  std::mutex              m;
-  std::condition_variable cv;
-  uint64_t                next = 0;
-  void                    take(uint64_t seq)
-  {
-    std::unique_lock<std::mutex> lk(m);
-    cv.wait(lk, [&] { return next == seq; });
-  }
-  void give()
-  {
-    {
-      std::lock_guard<std::mutex> lk(m);
-      next++;
-    }
-    cv.notify_all();
-  }
-};
-struct TurnGuard { // a turn is always taken and given back exactly once, also on an error path, so later batches of this rank never wait forever
-  Turn&    t;
-  uint64_t seq;
-  int      state = 0; // 0 not taken yet, 1 held, 2 given back
-  TurnGuard(Turn& t_, uint64_t s) : t(t_), seq(s) {}
-  void take()
-  {
-    t.take(seq);
-    state = 1;
-  }
-  void give() // a section this batch skips (the gather at world size 1) still has to pass its turn on
-  {
-    if (state == 0) take();
-    if (state == 1) t.give();
-    state = 2;
-  }
-  ~TurnGuard() { give(); }
-};
 
 struct TbMeta { // one per result slot (2 per grant) of the sending rank
   uint32_t grant_dci; // global DCI index | LTEPHY_GRANT_ALT_TABLE
@@ -300,6 +263,9 @@ extern "C" int ltephy_decode_subframes_sharded(ltephy_shard_t* sh, ltephy_t* h, 
                                                ltephy_tb_result_t* tbs, uint8_t* payload, size_t payload_cap, ltephy_shard_stats_t* stats)
 {
   if (!sh) return fail(LTEPHY_ERROR_INVALID_INPUTS, "decode_subframes_sharded: bad arguments");
+  // every batch takes the exchange turn first, so owning seq there makes it the one call of its batch in every section
+  if (seq == LTEPHY_SEQ_NONE || !sh->turn_x.claim(seq))
+    return fail(LTEPHY_ERROR_INVALID_INPUTS, "decode_subframes_sharded: seq %llu is not the number of a batch still to come", (unsigned long long)seq);
   const uint32_t W = sh->world, R = sh->rank;
   // the ordered sections of this batch; the guards keep the order intact on every exit path, a refused argument list included
   TurnGuard gx(sh->turn_x, seq), gf(sh->turn_f, seq), gw(sh->turn_w, seq), gg(sh->turn_g, seq);
@@ -340,7 +306,7 @@ extern "C" int ltephy_decode_subframes_sharded(ltephy_shard_t* sh, ltephy_t* h, 
   NC(g_nccl.AllGather(sl->d_offs.p, sl->d_offs_all.p, n + 1, ncclUint32, sh->comm_x, sh->st_x));
   NC(g_nccl.AllGather(sl->d_pack.p, sl->d_pack_all.p, cap_rank, ncclUint8, sh->comm_x, sh->st_x));
   CU(cudaEventRecord(sl->ev_x, sh->st_x));
-  gx.give();
+  gx.pass();
   CU(cudaStreamWaitEvent(h->stream, sl->ev_x, 0)); // the handle's stream is idle between phase A and phase B
   CU(cudaMemcpyAsync(sl->h_offs_all.p, sl->d_offs_all.p, (size_t)W * (n + 1) * 4, cudaMemcpyDeviceToHost, h->stream));
   CU(cudaStreamSynchronize(h->stream));
@@ -370,7 +336,7 @@ extern "C" int ltephy_decode_subframes_sharded(ltephy_shard_t* sh, ltephy_t* h, 
     full.resize(W);
     for (uint32_t q = 0; q < W; q++) full[q] = reinterpret_cast<const ltephy_cand_t*>(sl->h_full_all.p + q * fb);
   }
-  gf.give();
+  gf.pass();
   t[3] = now_ms();
   // ---- walk turn -----------------------------------------------------------------------------------------
   gw.take();
@@ -378,7 +344,7 @@ extern "C" int ltephy_decode_subframes_sharded(ltephy_shard_t* sh, ltephy_t* h, 
   sl->tti_cfi.resize((size_t)2 * n * W);
   uint32_t nd = 0;
   r = ltephy_search_batch_packed(s, bufs.data(), offs.data(), need_full ? full.data() : nullptr, W, n, dcis, max_dcis, &nd, sl->tti_cfi.data());
-  gw.give();
+  gw.pass();
   if (r) return fail(r, "walk over the exchanged tables failed (%d)", r);
   *n_dcis = nd;
   t[5]    = now_ms();
@@ -429,7 +395,7 @@ extern "C" int ltephy_decode_subframes_sharded(ltephy_shard_t* sh, ltephy_t* h, 
       NC(g_nccl.Send(h->d_payload.p, cap_p, ncclUint8, 0, sh->comm_g, sh->st_g));
       NC(g_nccl.GroupEnd());
       CU(cudaEventRecord(sl->ev_g, sh->st_g));
-      gg.give();
+      gg.pass();
       CU(cudaEventSynchronize(sl->ev_g)); // the handle's buffers are free for its next batch when this call returns
     } else {
       if (sl->d_g_msg.reserve((W - 1) * cap_m) || sl->h_g_msg.reserve((W - 1) * cap_m) || sl->d_g_payload.reserve((W - 1) * cap_p + 16))
@@ -442,7 +408,7 @@ extern "C" int ltephy_decode_subframes_sharded(ltephy_shard_t* sh, ltephy_t* h, 
       }
       NC(g_nccl.GroupEnd());
       CU(cudaEventRecord(sl->ev_g, sh->st_g));
-      gg.give();
+      gg.pass();
       // host side, outside the turn: headers first, then exactly the used part of every rank's records and bytes
       CU(cudaStreamWaitEvent(h->stream, sl->ev_g, 0));
       CU(cudaMemcpy2DAsync(sl->h_g_msg.p, cap_m, sl->d_g_msg.p, cap_m, 64, W - 1, cudaMemcpyDeviceToHost, h->stream));
@@ -483,7 +449,7 @@ extern "C" int ltephy_decode_subframes_sharded(ltephy_shard_t* sh, ltephy_t* h, 
       }
     }
   }
-  gg.give();
+  gg.pass();
   t[8] = now_ms();
   if (stats) {
     stats->host_ms[0] = t[1] - t[0], stats->host_ms[1] = t[2] - t[1], stats->host_ms[2] = t[3] - t[2], stats->host_ms[3] = t[4] - t[3];

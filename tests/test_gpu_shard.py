@@ -169,6 +169,25 @@ def test_sharded_one_rank_three_threads_and_a_refused_batch(infra, phylib):
     phy.close()
 
 
+def test_sharded_one_rank_refuses_a_seq_whose_turn_is_over(infra, phylib):
+    """batch 0, then batch 0 again: the second call returns LTEPHY_ERROR_INVALID_INPUTS at once instead of waiting for a turn that has
+    passed, and consumes nothing -- batch 1 then decodes as the unsharded pipeline does"""
+    n = 16
+    capi, cell, iq, tti, phy, ref_info, ref_dcis, ref_table, sh, srch = _one_rank_setup(n)
+    info, dcis, tbs, pl, st = _sharded_decode(capi, sh, phy, srch, iq[:8], tti[:8], 0, 32 * n, 1)
+    out = []
+    th = threading.Thread(target=lambda: out.append(_sharded_call(capi, sh, phy, srch, iq[:8], tti[:8], 0, 32 * n, 1)), daemon=True)
+    th.start()
+    _join_all([th], 30.0)
+    assert out[0][0] == -2, out[0][:2]                                       # LTEPHY_ERROR_INVALID_INPUTS
+    info2, dcis2, tbs2, pl2, st2 = _sharded_decode(capi, sh, phy, srch, iq[8:], tti[8:], 1, 32 * n, 1)
+    got = [_key(d) for d in dcis] + [(k[0] + 8,) + k[1:] for k in (_key(d) for d in dcis2)]
+    assert got == [_key(d) for d in ref_dcis]
+    assert _tb_table(dcis, tbs, pl) + _tb_table(dcis2, tbs2, pl2) == ref_table
+    sh.close()
+    phy.close()
+
+
 def _rank_main(rank, world, uid, q):
     sys.path.insert(0, ROOT)
     sys.path.insert(0, os.path.join(ROOT, "tests"))
