@@ -37,10 +37,10 @@ oracle/liblteochanpoly.so: oracle/lte_chan_poly_oracle.c oracle/lte_chan_poly_or
 examples/offline_decode: examples/offline_decode.cpp include/ltephy_b200.h include/ltephy_search.h include/ltephy_sinks.h
 	$(CXX) -O2 -std=c++17 -Wall -Iinclude -o $@ examples/offline_decode.cpp -Lltesniffer_b200 -lltephy_b200 -Wl,-rpath,'$$ORIGIN/../ltesniffer_b200'
 
-examples/offline_ul: examples/offline_ul.cpp include/ltephy_b200.h include/ltephy_search.h include/ltephy_sinks.h
+examples/offline_ul: examples/offline_ul.cpp examples/cell_chain.h include/ltephy_b200.h include/ltephy_search.h include/ltephy_sinks.h
 	$(CXX) -O2 -std=c++17 -Wall -Iinclude -o $@ examples/offline_ul.cpp -Lltesniffer_b200 -lltephy_b200 -Wl,-rpath,'$$ORIGIN/../ltesniffer_b200'
 
-examples/cell_search: examples/cell_search.cpp include/ltephy_b200.h
+examples/cell_search: examples/cell_search.cpp examples/cell_chain.h include/ltephy_b200.h include/ltephy_search.h include/ltephy_sinks.h
 	$(CXX) -O2 -std=c++17 -Wall -Iinclude -o $@ examples/cell_search.cpp -Lltesniffer_b200 -lltephy_b200 -Wl,-rpath,'$$ORIGIN/../ltesniffer_b200'
 
 examples/decode_recording: examples/decode_recording.cpp examples/cell_chain.h include/ltephy_b200.h include/ltephy_search.h include/ltephy_sinks.h
@@ -49,7 +49,7 @@ examples/decode_recording: examples/decode_recording.cpp examples/cell_chain.h i
 examples/decode_wideband: examples/decode_wideband.cpp examples/cell_chain.h include/ltephy_b200.h include/ltephy_search.h include/ltephy_sinks.h
 	$(CXX) -O2 -std=c++17 -Wall -Iinclude -o $@ examples/decode_wideband.cpp -Lltesniffer_b200 -lltephy_b200 -Wl,-rpath,'$$ORIGIN/../ltesniffer_b200'
 
-examples/decode_recording_ul: examples/decode_recording_ul.cpp include/ltephy_b200.h include/ltephy_search.h include/ltephy_sinks.h
+examples/decode_recording_ul: examples/decode_recording_ul.cpp examples/cell_chain.h include/ltephy_b200.h include/ltephy_search.h include/ltephy_sinks.h
 	$(CXX) -O2 -std=c++17 -Wall -Iinclude -o $@ examples/decode_recording_ul.cpp -Lltesniffer_b200 -lltephy_b200 -Wl,-rpath,'$$ORIGIN/../ltesniffer_b200'
 
 examples/compat_check: examples/compat_check.cpp compat/srsran/srsran.h compat/ltephy_compat_ext.h include/ltephy_b200.h

@@ -1,10 +1,16 @@
-// cell_chain.h -- the per-cell chain of the recording examples (decode_recording.cpp, decode_wideband.cpp), host code over the C-ABI of
-// libltephy_b200: the MIB soft-combined over the frames of a capture, then, for every push of a tracker, the decoder and the DCI search on the cut
-// subframes, written to a MAC-LTE pcap and a DCI trace, with the lock counts and the summary lines.
+// cell_chain.h -- the steps the C++ examples share, host code over the C-ABI of libltephy_b200:
+//   chain_acquire (cell_search.cpp, decode_recording.cpp, decode_recording_ul.cpp): the cell search on the start of a file, then the MIB
+//     soft-combined over its frames (chain_mib_host);
+//   chain_print_cell (decode_recording.cpp, decode_recording_ul.cpp, decode_wideband.cpp): the cell line;
+//   CellChain (decode_recording.cpp, decode_wideband.cpp): for every push of a tracker, the decoder and the DCI search on the cut subframes,
+//     written to a MAC-LTE pcap and a DCI trace, with the lock counts and the summary lines;
+//   UlChain (offline_ul.cpp, decode_recording_ul.cpp): the UL mode, batch by batch: the downlink's RARs and DCI-0s turned into PUSCH grants on the
+//     uplink, both directions written to a MAC-LTE pcap.
 #pragma once
 #include "ltephy_b200.h"
 #include "ltephy_search.h"
 #include "ltephy_sinks.h"
+#include <algorithm>
 #include <cstdio>
 #include <cstdlib>
 #include <vector>
@@ -43,11 +49,54 @@ static inline int chain_mib_host(const float* sf0, uint32_t nframes, uint32_t pc
       *mib     = m[f].mib;
       mib->sfn = (mib->sfn + 1024 - f % 1024) % 1024; // the SFN of the frame at frame_offset
     }
-  if (!mib->found) {
+  if (!mib->found) { // no window of any frame passed its CRC (too weak even combined, or a cell with four CRS ports)
     fprintf(stderr, "cell %u found, MIB not decoded\n", pci);
     return 3;
   }
   return 0;
+}
+
+// the cell of samples [0, L0) of an antenna-major file of L samples per antenna: the cell search there, the first cell it detects, and that cell's
+// MIB soft-combined over the subframes 0 of every whole frame in those samples (chain_mib_host).  0, 1 on a read or library error, 3 when no cell
+// is found, no whole frame follows its first subframe 0 or no MIB passed (message printed)
+static inline int chain_acquire(FILE* f, uint32_t N, uint32_t A, uint64_t L, uint64_t L0, ltephy_cell_t* cell, ltephy_mib_t* mib)
+{
+  const uint32_t     SF = 15 * N;
+  std::vector<float> x;
+  if (!read_span(f, A, L, 0, L0, x)) {
+    fprintf(stderr, "short read\n");
+    return 1;
+  }
+  ltephy_sync_cfg_t scfg{};
+  scfg.symbol_sz = N, scfg.nof_rx = A, scfg.max_samples = L0;
+  ltephy_sync_t* sync = nullptr;
+  ltephy_cell_t  cells[3];
+  if (ltephy_sync_create(&scfg, &sync) != LTEPHY_SUCCESS) {
+    fprintf(stderr, "ltephy_sync_create: %s\n", ltephy_last_error());
+    return 1;
+  }
+  if (ltephy_cell_search(sync, x.data(), L0, cells) != LTEPHY_SUCCESS) {
+    fprintf(stderr, "ltephy_cell_search: %s\n", ltephy_last_error());
+    return 1;
+  }
+  ltephy_sync_destroy(sync);
+  const ltephy_cell_t* c = std::find_if(cells, cells + 3, [](const ltephy_cell_t& q) { return q.detected; });
+  if (c == cells + 3) {
+    fprintf(stderr, "no cell found\n");
+    return 3;
+  }
+  *cell = *c;
+  // the PBCH and the centre CRS do not depend on the bandwidth: chain_mib_host's 15-PRB handle reads the MIB of any cell
+  const uint32_t nframes = (uint32_t)((L0 - c->frame_offset) / (10ull * SF));
+  if (!nframes) {
+    fprintf(stderr, "no whole frame after the first subframe 0\n");
+    return 3;
+  }
+  std::vector<float> sf0((size_t)2 * A * SF * nframes); // subframe 0 of each frame, antenna after antenna
+  for (uint32_t f = 0; f < nframes; f++)
+    for (uint32_t a = 0; a < A; a++)
+      std::copy_n(x.data() + 2 * (a * L0 + c->frame_offset + (uint64_t)f * 10 * SF), 2 * SF, sf0.data() + 2 * ((size_t)f * A + a) * SF);
+  return chain_mib_host(sf0.data(), nframes, c->pci, c->cfo_hz, N, A, mib);
 }
 
 static inline void chain_print_cell(const ltephy_cell_t& c, const ltephy_mib_t& mib)
@@ -206,5 +255,137 @@ struct CellChain {
     if (phy) ltephy_destroy(phy);
     if (mibh) ltephy_destroy(mibh);
     tsv = nullptr, pcap = nullptr, search = nullptr, phy = nullptr, mibh = nullptr;
+  }
+};
+
+// the UL mode of one cell (the reference's -m 1: SubframeWorker's UL branch with PDSCH_Decoder::decode_ul_mode and PUSCH_Decoder::decode), fed one
+// batch at a time with the downlink and the uplink of the same ttis: the downlink decoded in UL mode (RARs and format 1 / 1A), the msg-3 grants of
+// the RARs (6 subframes later) and the grants of the DCI-0s (4 later) decoded on the uplink, both directions written to a MAC-LTE pcap.  A grant
+// that lands past its batch is carried into the next one, and stays carried while it lies past that one too (a short last batch).
+struct UlChain {
+  ltephy_t *                      dl = nullptr, *ul = nullptr;
+  ltephy_search_t*                search = nullptr;
+  ltephy_pcap_t*                  pcap   = nullptr;
+  uint32_t                        max_dcis = 0, max_ul = 0;
+  unsigned long long              n_sf = 0, n_dl_ok = 0, n_dci0 = 0, n_rar = 0, n_ul_ok = 0;
+  std::vector<uint32_t>           ttis; // the caller writes the batch's ttis here before step()
+  std::vector<ltephy_sf_info_t>   info;
+  std::vector<ltephy_cand_t>      scratch;
+  std::vector<ltephy_dci_t>       dcis;
+  std::vector<ltephy_tb_result_t> tbs, ures;
+  std::vector<uint8_t>            payload, upayload, reading;
+  std::vector<ltephy_ul_grant_t>  grants, now, carry; // carry: grants whose subframe lies past the batch, indexed into the next one
+  std::vector<uint32_t>           grant_dci;
+  std::vector<ltephy_ul_chest_t>  chest;
+
+  // the downlink and uplink decoders of cfg (batches of up to cfg.max_subframes), the UL configuration and hopping offset of SIB2, the DCI
+  // search in UL mode and the pcap.  0 or 1 (error printed)
+  int open(const ltephy_cfg_t& cfg, const ltephy_ul_cfg_t& ucfg, uint32_t hopping_offset, const char* pcap_path)
+  {
+    if (ltephy_create(&cfg, &dl) != LTEPHY_SUCCESS || ltephy_create(&cfg, &ul) != LTEPHY_SUCCESS) {
+      fprintf(stderr, "ltephy_create: %s\n", ltephy_last_error());
+      return 1;
+    }
+    if (ltephy_set_ul_cfg(ul, &ucfg) != LTEPHY_SUCCESS || !(search = ltephy_search_create(dl, 5))) {
+      fprintf(stderr, "UL config / search: %s\n", ltephy_last_error());
+      return 1;
+    }
+    ltephy_search_set_ul_hopping(search, hopping_offset);
+    ltephy_search_set_ul_mode(search, 1, 0); // the downlink side decodes RARs and format 1 / 1A only (decode_ul_mode)
+    if (!(pcap = ltephy_pcap_open(pcap_path))) {
+      fprintf(stderr, "cannot open %s\n", pcap_path);
+      return 1;
+    }
+    const uint32_t B = cfg.max_subframes;
+    max_dcis = 32 * B, max_ul = 3 * max_dcis + 64;
+    ttis.resize(B), info.resize(B), scratch.resize((size_t)B * LTEPHY_MAX_LOC * LTEPHY_MAX_SIZES), dcis.resize(max_dcis);
+    tbs.resize(2 * (size_t)max_dcis), ures.resize(max_ul), payload.resize((size_t)B * 64 * 1024), upayload.resize((size_t)B * 64 * 1024);
+    grants.resize(max_ul), grant_dci.resize(max_ul), reading.resize(max_ul), chest.resize(max_ul);
+    return 0;
+  }
+
+  // one batch of got subframes at ttis[0, got): downlink and uplink cf32 [got][15 N], one antenna, in host memory or, with on_device, in device
+  // memory (a tracker's cuts).  0 or 1 (error printed)
+  int step(const void* dl_iq, const void* ul_iq, bool on_device, uint32_t got)
+  {
+    uint32_t  nd = 0;
+    const int rd = on_device ? ltephy_decode_subframes_device(dl, search, dl_iq, ttis.data(), got, LTEPHY_SEQ_NONE, info.data(), scratch.data(), dcis.data(),
+                                                              max_dcis, &nd, tbs.data(), payload.data(), payload.size())
+                             : ltephy_decode_subframes(dl, search, static_cast<const float*>(dl_iq), ttis.data(), got, LTEPHY_SEQ_NONE, info.data(),
+                                                       scratch.data(), dcis.data(), max_dcis, &nd, tbs.data(), payload.data(), payload.size());
+    if (rd != LTEPHY_SUCCESS) {
+      fprintf(stderr, "%s: %s\n", on_device ? "ltephy_decode_subframes_device" : "ltephy_decode_subframes", ltephy_last_error());
+      return 1;
+    }
+    const uint32_t ts_s = (uint32_t)(n_sf / 1000), ts_us = (uint32_t)((n_sf % 1000) * 1000);
+    const int      wd   = ltephy_pcap_write_dl_batch(pcap, ttis.data(), dcis.data(), nd, tbs.data(), payload.data(), 0, ts_s, ts_us);
+    if (wd < 0) {
+      fprintf(stderr, "pcap write failed\n");
+      return 1;
+    }
+    n_dl_ok += (unsigned)wd;
+    // grants of this batch's uplink: what the previous batch left over, the msg-3 grants of the RARs (6 subframes later), the DCI-0s (4 later)
+    now.swap(carry), carry.clear();
+    const auto past = std::stable_partition(now.begin(), now.end(), [&](const ltephy_ul_grant_t& g) { return g.sf < got; });
+    carry.assign(past, now.end()), now.erase(past, now.end());
+    auto place = [&](const ltephy_ul_grant_t& g) { (g.sf < got ? now : carry).push_back(g); };
+    for (uint32_t i = 0; i < nd; i++) {
+      const ltephy_tb_result_t& r = tbs[2 * i];
+      if (dcis[i].rnti < 1 || dcis[i].rnti > 10 || !r.crc || !r.payload_len) continue; // RA-RNTI with a decoded block (unpack_rar_response_ul_mode)
+      ltephy_rar_t rars[16];
+      uint32_t     nr = 0;
+      if (ltephy_rar_unpack(search, payload.data() + r.payload_off, r.payload_len, rars, 16, &nr, nullptr) != LTEPHY_SUCCESS) continue;
+      for (uint32_t k = 0; k < nr; k++) {
+        ltephy_search_activate(search, rars[k].t_crnti, 0, LTEPHY_ACT_RAR); // rntiManager.activateAndRefresh, DL_Sniffer_PDSCH.cc:659
+        n_rar++;
+        if (!rars[k].valid) continue;
+        rars[k].grant.sf = dcis[i].sf + 6; // ULSchedule::get_rar_ul_tti
+        place(rars[k].grant);
+      }
+    }
+    uint32_t ng = 0;
+    if (ltephy_ul_grants_from_dcis(search, info.data(), dcis.data(), nd, nullptr, 0, grants.data(), grant_dci.data(), reading.data(), max_ul, &ng) !=
+        LTEPHY_SUCCESS) {
+      fprintf(stderr, "ltephy_ul_grants_from_dcis: %s\n", ltephy_last_error());
+      return 1;
+    }
+    for (uint32_t k = 0; k < ng; k++) {
+      n_dci0 += k == 0 || grant_dci[k] != grant_dci[k - 1];
+      place(grants[k]);
+    }
+    for (ltephy_ul_grant_t& g : carry) g.sf -= got; // index into the next batch's uplink
+    if (!now.empty()) {
+      if (now.size() > max_ul) now.resize(max_ul);
+      const int ru = on_device ? ltephy_submit_ul_device(ul, ul_iq, ttis.data(), got, now.data(), (uint32_t)now.size())
+                               : ltephy_submit_ul(ul, static_cast<const float*>(ul_iq), ttis.data(), got, now.data(), (uint32_t)now.size());
+      if (ru != LTEPHY_SUCCESS || ltephy_get_ul(ul, ures.data(), chest.data(), upayload.data(), upayload.size()) != LTEPHY_SUCCESS) {
+        fprintf(stderr, "uplink decode: %s\n", ltephy_last_error());
+        return 1;
+      }
+      // the attempts of one DCI-0 are adjacent and in the reference's order: keep the first that passed (PUSCH_Decoder::decode stops there)
+      bool passed = false;
+      for (size_t k = 0; k < now.size(); k++) {
+        if (k == 0 || now[k - 1].rnti != now[k].rnti || now[k - 1].sf != now[k].sf) passed = false;
+        if (ures[k].crc && passed) ures[k].crc = 0;
+        passed = passed || ures[k].crc != 0;
+      }
+      const int wu = ltephy_pcap_write_ul_batch(pcap, ttis.data(), now.data(), (uint32_t)now.size(), ures.data(), upayload.data(), 0, ts_s, ts_us);
+      if (wu < 0) {
+        fprintf(stderr, "pcap write failed\n");
+        return 1;
+      }
+      n_ul_ok += (unsigned)wu;
+    }
+    n_sf += got;
+    return 0;
+  }
+
+  void close()
+  {
+    if (pcap) ltephy_pcap_close(pcap);
+    if (search) ltephy_search_destroy(search);
+    if (dl) ltephy_destroy(dl);
+    if (ul) ltephy_destroy(ul);
+    pcap = nullptr, search = nullptr, dl = nullptr, ul = nullptr;
   }
 };

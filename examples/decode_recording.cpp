@@ -35,56 +35,17 @@ int main(int argc, char** argv)
   fseeko(in, 0, SEEK_END);
   const uint64_t L = (uint64_t)ftello(in) / (8ull * A);
 
-  // 1. cell search on the first 40 ms
-  const uint64_t     L0 = L < 40ull * SF ? L : 40ull * SF;
-  std::vector<float> x;
-  ltephy_sync_cfg_t  scfg{};
-  scfg.symbol_sz = N, scfg.nof_rx = A, scfg.max_samples = L0;
-  ltephy_sync_t* sync = nullptr;
-  ltephy_cell_t  cells[3];
-  if (!read_span(in, A, L, 0, L0, x)) {
-    fprintf(stderr, "short read\n");
-    return 1;
-  }
-  if (ltephy_sync_create(&scfg, &sync) != LTEPHY_SUCCESS || ltephy_cell_search(sync, x.data(), L0, cells) != LTEPHY_SUCCESS) {
-    fprintf(stderr, "cell search: %s\n", ltephy_last_error());
-    return 1;
-  }
-  ltephy_sync_destroy(sync);
-  const ltephy_cell_t* c = nullptr;
-  for (auto& q : cells)
-    if (q.detected) {
-      c = &q;
-      break;
-    }
-  if (!c) {
-    fprintf(stderr, "no cell found\n");
-    return 3;
-  }
+  // 1. cell search on the first 40 ms, and the MIB soft-combined over the frames there at the found timing, with the found carrier offset
+  ltephy_cell_t c{};
+  ltephy_mib_t  mib{};
+  if (int r = chain_acquire(in, N, A, L, L < 40ull * SF ? L : 40ull * SF, &c, &mib)) return r;
+  chain_print_cell(c, mib);
 
-  // 2. the MIB, soft-combined over the frames of those 40 ms at the found timing, with the found carrier offset (as cell_search does)
-  const uint32_t nframes = (uint32_t)((L0 - c->frame_offset) / (10ull * SF));
-  if (!nframes) {
-    fprintf(stderr, "no whole frame after the first subframe 0\n");
-    return 3;
-  }
-  std::vector<float> sf0((size_t)2 * A * SF * nframes);
-  for (uint32_t f = 0; f < nframes; f++)
-    for (uint32_t a = 0; a < A; a++)
-      for (uint32_t n = 0; n < SF; n++) {
-        const uint64_t s = c->frame_offset + (uint64_t)f * 10 * SF + n;
-        const size_t   d = ((size_t)f * A + a) * SF + n;
-        sf0[2 * d] = x[2 * (a * L0 + s)], sf0[2 * d + 1] = x[2 * (a * L0 + s) + 1];
-      }
-  ltephy_mib_t mib{};
-  if (int r = chain_mib_host(sf0.data(), nframes, c->pci, c->cfo_hz, N, A, &mib)) return r;
-  chain_print_cell(*c, mib);
-
-  // 3. decoder, DCI search and tracker for the cell
+  // 2. decoder, DCI search and tracker for the cell
   CellChain chain;
-  if (chain.open_decoder(*c, mib, N, A, B)) return 1;
+  if (chain.open_decoder(c, mib, N, A, B)) return 1;
   ltephy_track_cfg_t tcfg{};
-  tcfg.symbol_sz = N, tcfg.nof_rx = A, tcfg.pci = c->pci, tcfg.first_tti = 10 * mib.sfn, tcfg.frame_offset = c->frame_offset, tcfg.cfo_hz = c->cfo_hz;
+  tcfg.symbol_sz = N, tcfg.nof_rx = A, tcfg.pci = c.pci, tcfg.first_tti = 10 * mib.sfn, tcfg.frame_offset = c.frame_offset, tcfg.cfo_hz = c.cfo_hz;
   tcfg.max_ppm = max_ppm, tcfg.max_subframes = B, tcfg.flags = (no_cfo ? LTEPHY_TRACK_NO_CFO : 0) | (reacq ? LTEPHY_TRACK_REACQUIRE : 0);
   ltephy_track_t* tr = nullptr;
   if (!chain.search || ltephy_track_create(&tcfg, &tr) != LTEPHY_SUCCESS) {
@@ -92,8 +53,9 @@ int main(int argc, char** argv)
     return 1;
   }
   if (chain.open_sinks(mib, reacq, argv[4], argv[5])) return 1;
-  // 4. the recording arrives B subframes at a time; each push re-feeds from the tracker's next_sample
-  uint64_t recv = 0, next = c->frame_offset;
+  // 3. the recording arrives B subframes at a time; each push re-feeds from the tracker's next_sample
+  std::vector<float> x;
+  uint64_t           recv = 0, next = c.frame_offset;
   for (;;) {
     if (recv < L) recv = recv + (uint64_t)B * SF < L ? recv + (uint64_t)B * SF : L;
     if (next >= recv) {

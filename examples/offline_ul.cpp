@@ -1,7 +1,8 @@
 // offline_ul.cpp -- the reference's UL mode (LTESniffer -m 1: SubframeWorker's UL branch, src/src/SubframeWorker.cc:236-345, with PDSCH_Decoder::decode_ul_mode
 // and PUSCH_Decoder::decode) written against the C-ABI of libltephy_b200 from C++, for two recorded carriers: the downlink capture is searched for DCI-0s and
-// Random Access Responses, the uplink capture is decoded with the grants they carry -- 4 subframes after a DCI-0, 6 after a RAR.  Host code only; every
-// computation happens in the library (no CPU fallback: without a GPU ltephy_create fails).
+// Random Access Responses, the uplink capture is decoded with the grants they carry -- 4 subframes after a DCI-0, 6 after a RAR (UlChain of cell_chain.h,
+// batch by batch; a grant past a batch is carried into a later one).  Host code only; every computation happens in the library (no CPU fallback: without a
+// GPU ltephy_create fails).
 //
 //   offline_ul <dl.cf32> <ul.cf32> <nof_prb> <nof_ports> <cell_id> <out.pcap> [batch=200] [first_tti=0] [cyclic_shift=0] [group_assignment=0] [hopping_offset=0]
 //              [phich_resources=0]
@@ -9,12 +10,7 @@
 // dl.cf32: subframe after subframe, one antenna (the UL mode gives the downlink one antenna, README.md:57-58); ul.cf32: the uplink carrier, same framing and
 // the same first tti.  cyclic_shift / group_assignment / hopping_offset are SIB2's values (ULSchedule::set_config, src/src/ULSchedule.cc:140-158), which the
 // reference reads from the air before it starts; here they are arguments.
-#include "ltephy_b200.h"
-#include "ltephy_search.h"
-#include "ltephy_sinks.h"
-#include <cstdio>
-#include <cstdlib>
-#include <vector>
+#include "cell_chain.h"
 
 int main(int argc, char** argv)
 {
@@ -29,100 +25,24 @@ int main(int argc, char** argv)
   ltephy_cfg_t   cfg{};
   cfg.nof_prb = (uint32_t)atoi(argv[3]), cfg.nof_ports = (uint32_t)atoi(argv[4]), cfg.cell_id = (uint32_t)atoi(argv[5]), cfg.nof_rx = 1;
   cfg.max_subframes = B, cfg.turbo_max_iter = 8, cfg.flags = LTEPHY_FLAG_SKIP_LOW_POWER, cfg.phich_resources = arg(12, 0);
-  ltephy_t *dl = nullptr, *ul = nullptr;
-  if (ltephy_create(&cfg, &dl) != LTEPHY_SUCCESS || ltephy_create(&cfg, &ul) != LTEPHY_SUCCESS) {
-    fprintf(stderr, "ltephy_create: %s\n", ltephy_last_error());
+  UlChain u;
+  if (u.open(cfg, ltephy_ul_cfg_t{arg(9, 0), arg(10, 0), 0, 0}, arg(11, 0), argv[6])) return 1;
+  FILE *fd = fopen(argv[1], "rb"), *fu = fopen(argv[2], "rb");
+  if (!fd || !fu) {
+    fprintf(stderr, "cannot open %s / %s\n", argv[1], argv[2]);
     return 1;
   }
-  const ltephy_ul_cfg_t ucfg{arg(9, 0), arg(10, 0), 0, 0};
-  if (ltephy_set_ul_cfg(ul, &ucfg) != LTEPHY_SUCCESS) {
-    fprintf(stderr, "ltephy_set_ul_cfg: %s\n", ltephy_last_error());
-    return 1;
-  }
-  ltephy_search_t* search = ltephy_search_create(dl, 5);
-  ltephy_search_set_ul_hopping(search, arg(11, 0));
-  ltephy_search_set_ul_mode(search, 1, 0); // the downlink side decodes RARs and format 1 / 1A only (decode_ul_mode)
-  ltephy_pcap_t* pcap = ltephy_pcap_open(argv[6]);
-  FILE *         fd = fopen(argv[1], "rb"), *fu = fopen(argv[2], "rb");
-  if (!search || !pcap || !fd || !fu) {
-    fprintf(stderr, "cannot open inputs / outputs\n");
-    return 1;
-  }
-  const size_t                    sf_floats = (size_t)2 * ltephy_sf_len(dl);
-  const uint32_t                  max_dcis = 32 * B, max_ul = 3 * max_dcis + 64;
-  std::vector<float>              iq_d(sf_floats * B), iq_u(sf_floats * B);
-  std::vector<uint32_t>           ttis(B);
-  std::vector<ltephy_sf_info_t>   info(B);
-  std::vector<ltephy_cand_t>      scratch((size_t)B * LTEPHY_MAX_LOC * LTEPHY_MAX_SIZES);
-  std::vector<ltephy_dci_t>       dcis(max_dcis);
-  std::vector<ltephy_tb_result_t> tbs(2 * (size_t)max_dcis), ures(max_ul);
-  std::vector<uint8_t>            payload((size_t)B * 64 * 1024), upayload((size_t)B * 64 * 1024);
-  std::vector<ltephy_ul_grant_t>  grants(max_ul), now, carry; // carry: grants whose subframe lies in the next batch
-  std::vector<uint32_t>           grant_dci(max_ul);
-  std::vector<uint8_t>            reading(max_ul);
-  std::vector<ltephy_ul_chest_t>  chest(max_ul);
-  unsigned long long              n_sf = 0, n_dci0 = 0, n_rar = 0, n_ul_ok = 0, n_dl_ok = 0;
+  const size_t       sf_floats = (size_t)2 * ltephy_sf_len(u.dl);
+  std::vector<float> iq_d(sf_floats * B), iq_u(sf_floats * B);
   for (;;) {
-    const size_t got = fread(iq_d.data(), sizeof(float) * sf_floats, B, fd);
+    const uint32_t got = (uint32_t)fread(iq_d.data(), sizeof(float) * sf_floats, B, fd);
     if (!got || fread(iq_u.data(), sizeof(float) * sf_floats, got, fu) != got) break;
-    for (size_t i = 0; i < got; i++) ttis[i] = (tti0 + (uint32_t)i) % 10240;
-    uint32_t nd = 0;
-    if (ltephy_decode_subframes(dl, search, iq_d.data(), ttis.data(), (uint32_t)got, LTEPHY_SEQ_NONE, info.data(), scratch.data(), dcis.data(), max_dcis, &nd, tbs.data(),
-                                payload.data(), payload.size()) != LTEPHY_SUCCESS) {
-      fprintf(stderr, "ltephy_decode_subframes: %s\n", ltephy_last_error());
-      return 1;
-    }
-    const uint32_t ts_s = (uint32_t)(n_sf / 1000), ts_us = (uint32_t)((n_sf % 1000) * 1000);
-    const int      wd = ltephy_pcap_write_dl_batch(pcap, ttis.data(), dcis.data(), nd, tbs.data(), payload.data(), 0, ts_s, ts_us);
-    if (wd < 0) return 1;
-    n_dl_ok += (unsigned)wd;
-    // grants of this uplink batch: what the previous batch left over, the msg-3 grants of the RARs (6 subframes later), the DCI-0s (4 subframes later)
-    now.swap(carry), carry.clear();
-    for (uint32_t i = 0; i < nd; i++) {
-      const ltephy_tb_result_t& r = tbs[2 * i];
-      if (dcis[i].rnti < 1 || dcis[i].rnti > 10 || !r.crc || !r.payload_len) continue; // RA-RNTI with a decoded block (unpack_rar_response_ul_mode)
-      ltephy_rar_t rars[16];
-      uint32_t     nr = 0;
-      if (ltephy_rar_unpack(search, payload.data() + r.payload_off, r.payload_len, rars, 16, &nr, nullptr) != LTEPHY_SUCCESS) continue;
-      for (uint32_t k = 0; k < nr; k++) {
-        ltephy_search_activate(search, rars[k].t_crnti, 0, LTEPHY_ACT_RAR); // rntiManager.activateAndRefresh, DL_Sniffer_PDSCH.cc:659
-        n_rar++;
-        if (!rars[k].valid) continue;
-        rars[k].grant.sf = dcis[i].sf + 6; // ULSchedule::get_rar_ul_tti
-        (rars[k].grant.sf < got ? now : carry).push_back(rars[k].grant);
-      }
-    }
-    uint32_t ng = 0;
-    if (ltephy_ul_grants_from_dcis(search, info.data(), dcis.data(), nd, nullptr, 0, grants.data(), grant_dci.data(), reading.data(), max_ul, &ng) != LTEPHY_SUCCESS) return 1;
-    for (uint32_t k = 0; k < ng; k++) {
-      n_dci0 += k == 0 || grant_dci[k] != grant_dci[k - 1];
-      (grants[k].sf < got ? now : carry).push_back(grants[k]);
-    }
-    for (ltephy_ul_grant_t& g : carry) g.sf -= (uint32_t)got; // index into the next uplink batch
-    if (!now.empty()) {
-      if (now.size() > max_ul) now.resize(max_ul);
-      if (ltephy_submit_ul(ul, iq_u.data(), ttis.data(), (uint32_t)got, now.data(), (uint32_t)now.size()) != LTEPHY_SUCCESS ||
-          ltephy_get_ul(ul, ures.data(), chest.data(), upayload.data(), upayload.size()) != LTEPHY_SUCCESS) {
-        fprintf(stderr, "uplink decode: %s\n", ltephy_last_error());
-        return 1;
-      }
-      // the attempts of one DCI-0 are adjacent and in the reference's order: keep the first that passed (PUSCH_Decoder::decode stops there)
-      bool passed = false;
-      for (size_t k = 0; k < now.size(); k++) {
-        if (k == 0 || now[k - 1].rnti != now[k].rnti || now[k - 1].sf != now[k].sf) passed = false;
-        if (ures[k].crc && passed) ures[k].crc = 0;
-        passed = passed || ures[k].crc != 0;
-      }
-      const int wu = ltephy_pcap_write_ul_batch(pcap, ttis.data(), now.data(), (uint32_t)now.size(), ures.data(), upayload.data(), 0, ts_s, ts_us);
-      if (wu < 0) return 1;
-      n_ul_ok += (unsigned)wu;
-    }
-    n_sf += got, tti0 = (tti0 + (uint32_t)got) % 10240;
+    for (uint32_t i = 0; i < got; i++) u.ttis[i] = (tti0 + i) % 10240;
+    if (u.step(iq_d.data(), iq_u.data(), false, got)) return 1;
+    tti0 = (tti0 + got) % 10240;
   }
-  printf("subframes %llu  dl blocks %llu  dci0 %llu  rar %llu  ul blocks %llu\n", n_sf, n_dl_ok, n_dci0, n_rar, n_ul_ok);
+  printf("subframes %llu  dl blocks %llu  dci0 %llu  rar %llu  ul blocks %llu\n", u.n_sf, u.n_dl_ok, u.n_dci0, u.n_rar, u.n_ul_ok);
   fclose(fd), fclose(fu);
-  ltephy_pcap_close(pcap);
-  ltephy_search_destroy(search);
-  ltephy_destroy(dl), ltephy_destroy(ul);
+  u.close();
   return 0;
 }
