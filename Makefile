@@ -5,7 +5,7 @@ CXX ?= g++
 CFLAGS = -O3 -g -fPIC -std=gnu11 -Wall -Wno-unused-function -ffp-contract=off -fno-fast-math
 CXXFLAGS = -O2 -g -fPIC -std=c++17 -Wall -ffp-contract=off -fno-fast-math
 
-all: sim/libltesim.so oracle/liblteoracle.so oracle/liblteosync.so oracle/liblteomib.so oracle_track/liblteotrack.so oracle/liblteochan.so oracle/liblteochanpoly.so
+all: sim/libltesim.so oracle/liblteoracle.so oracle/liblteosync.so oracle/liblteomib.so oracle_track/liblteotrack.so oracle/liblteochan.so oracle/liblteochanpoly.so oracle_ul/liblteopuschrx.so
 
 sim/libltesim.so: sim/lte_common.c sim/lte_sim.c sim/lte_common.h sim/lte_sim.h include/lte_tables.h
 	$(CC) $(CFLAGS) -shared -o $@ sim/lte_common.c sim/lte_sim.c -lm
@@ -24,6 +24,10 @@ oracle/liblteomib.so: oracle/lte_mib_oracle.c oracle/lte_mib_oracle.h oracle/lte
 # tracker oracle: its find state (LTEO_TRACK_REACQUIRE) is lteo_cell_search of liblteosync.so
 oracle_track/liblteotrack.so: oracle_track/lte_track_oracle.c oracle_track/lte_track_oracle.h oracle/lte_sync_oracle.h oracle/liblteosync.so
 	$(CC) $(CFLAGS) -shared -o $@ oracle_track/lte_track_oracle.c -Loracle -llteosync -Wl,-rpath,'$$ORIGIN/../oracle' -lm
+
+# PUSCH with one or two receive antennas: lteo_det_sum, lteo_idft, lteo_dlsch_decode and the shared primitives come from liblteoracle.so
+oracle_ul/liblteopuschrx.so: oracle_ul/lte_pusch_rx_oracle.c oracle_ul/lte_pusch_rx_oracle.h oracle/lte_oracle.h oracle/liblteoracle.so
+	$(CC) $(CFLAGS) -shared -o $@ oracle_ul/lte_pusch_rx_oracle.c -Loracle -llteoracle -Wl,-rpath,'$$ORIGIN/../oracle' -lm
 
 # channeliser oracle: stands alone
 oracle/liblteochan.so: oracle/lte_chan_oracle.c oracle/lte_chan_oracle.h
@@ -59,4 +63,4 @@ examples/compat_ul_check: examples/compat_ul_check.cpp compat/srsran/srsran.h in
 	$(CXX) -O2 -std=c++17 -Wall -Iinclude -Icompat -o $@ examples/compat_ul_check.cpp -Lltesniffer_b200 -lltephy_srsran_compat -lltephy_b200 -Wl,-rpath,'$$ORIGIN/../ltesniffer_b200'
 
 clean:
-	rm -f sim/*.so oracle/*.so oracle_track/*.so examples/offline_decode examples/offline_ul examples/compat_check examples/compat_ul_check examples/cell_search examples/decode_recording examples/decode_recording_ul examples/decode_wideband
+	rm -f sim/*.so oracle/*.so oracle_track/*.so oracle_ul/*.so examples/offline_decode examples/offline_ul examples/compat_check examples/compat_ul_check examples/cell_search examples/decode_recording examples/decode_recording_ul examples/decode_wideband

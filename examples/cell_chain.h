@@ -278,7 +278,7 @@ struct UlChain {
   std::vector<uint32_t>           grant_dci;
   std::vector<ltephy_ul_chest_t>  chest;
 
-  // the downlink and uplink decoders of cfg (batches of up to cfg.max_subframes), the UL configuration and hopping offset of SIB2, the DCI
+  // the downlink and uplink decoders of cfg (batches of up to cfg.max_subframes, cfg.ul_nof_rx uplink antennas), the UL configuration and hopping offset of SIB2, the DCI
   // search in UL mode and the pcap.  0 or 1 (error printed)
   int open(const ltephy_cfg_t& cfg, const ltephy_ul_cfg_t& ucfg, uint32_t hopping_offset, const char* pcap_path)
   {
@@ -304,8 +304,8 @@ struct UlChain {
     return 0;
   }
 
-  // one batch of got subframes at ttis[0, got): downlink and uplink cf32 [got][15 N], one antenna, in host memory or, with on_device, in device
-  // memory (a tracker's cuts).  0 or 1 (error printed)
+  // one batch of got subframes at ttis[0, got): downlink cf32 [got][15 N] of one antenna and uplink cf32 [got][A][15 N] of A = cfg.ul_nof_rx
+  // antennas (one when 0), in host memory or, with on_device, in device memory (a tracker's cuts).  0 or 1 (error printed)
   int step(const void* dl_iq, const void* ul_iq, bool on_device, uint32_t got)
   {
     uint32_t  nd = 0;

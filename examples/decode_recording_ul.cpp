@@ -1,5 +1,7 @@
 // decode_recording_ul.cpp -- the reference's UL mode (LTESniffer -m 1) on two raw recordings of one radio: channel 0 on the downlink, channel 1 on
-// the uplink (src/src/LTESniffer_Core.cc:174-181), one antenna each, the same sample clock and the same first sample.  Both carriers are cut at the
+// the uplink (src/src/LTESniffer_Core.cc:174-181), the same sample clock and the same first sample.  The downlink file holds one antenna; the uplink
+// file holds ul_rx antennas, antenna-major (all of antenna 0, then all of antenna 1), and with ul_rx = 2 the PUSCH is combined over both (DESIGN.md
+// §2, "uplink receive diversity").  Both carriers are cut at the
 // timing the tracker follows on the downlink PSS (ltephy_track_push_ul: what srsran_ue_sync_zerocopy does to both channels, :365), so a sampling
 // clock a few ppm off and a carrier offset do not lose the uplink.  In order:
 //   1. cell search and the combined MIB on the first 40 ms of the downlink, as decode_recording does;
@@ -10,10 +12,11 @@
 // and one summary line.  Writes a MAC-LTE pcap with both directions.  Host code only; without a GPU ltephy_sync_create fails.
 //
 //   decode_recording_ul <dl.cf32> <ul.cf32> <symbol_sz> <out.pcap> [cfo_ratio=1] [ul_offset=0] [cyclic_shift=0] [group_assignment=0]
-//                       [hopping_offset=0]
+//                       [hopping_offset=0] [ul_rx=1]
 //
 // cfo_ratio = f_UL / f_DL scales the tracked carrier offset for the uplink (1 applies the downlink's, as srsRAN does); ul_offset is the number of
 // samples the uplink subframe starts after the downlink one.  cyclic_shift / group_assignment / hopping_offset are SIB2's values, as for offline_ul.
+// ul_rx (1 or 2) is the number of uplink antennas in <ul.cf32>.
 #include "cell_chain.h"
 
 static const uint32_t B = 200; // subframes per push
@@ -21,7 +24,7 @@ static const uint32_t B = 200; // subframes per push
 int main(int argc, char** argv)
 {
   if (argc < 5) {
-    fprintf(stderr, "usage: %s <dl.cf32> <ul.cf32> <symbol_sz> <out.pcap> [cfo_ratio=1] [ul_offset=0] [cyclic_shift] [group_assignment] [hopping_offset]\n",
+    fprintf(stderr, "usage: %s <dl.cf32> <ul.cf32> <symbol_sz> <out.pcap> [cfo_ratio=1] [ul_offset=0] [cyclic_shift] [group_assignment] [hopping_offset] [ul_rx=1]\n",
             argv[0]);
     return 2;
   }
@@ -29,13 +32,18 @@ int main(int argc, char** argv)
   const uint32_t N = (uint32_t)atoi(argv[3]), SF = 15 * N;
   const double   cfo_ratio = argc > 5 ? atof(argv[5]) : 1.0;
   const int32_t  ul_offset = argc > 6 ? atoi(argv[6]) : 0;
+  const uint32_t ul_rx     = arg(10, 1);
+  if (ul_rx < 1 || ul_rx > 2) {
+    fprintf(stderr, "ul_rx %u: 1 or 2 uplink antennas\n", ul_rx);
+    return 2;
+  }
   FILE *         fd = fopen(argv[1], "rb"), *fu = fopen(argv[2], "rb");
   if (!fd || !fu) {
     fprintf(stderr, "cannot open %s / %s\n", argv[1], argv[2]);
     return 2;
   }
   fseeko(fd, 0, SEEK_END), fseeko(fu, 0, SEEK_END);
-  const uint64_t Ld = (uint64_t)ftello(fd) / 8, Lu = (uint64_t)ftello(fu) / 8, L = Ld < Lu ? Ld : Lu;
+  const uint64_t Ld = (uint64_t)ftello(fd) / 8, Lu = (uint64_t)ftello(fu) / 8 / ul_rx, L = Ld < Lu ? Ld : Lu; // Lu: samples per UL antenna
 
   // 1. cell search and the MIB on the first 40 ms of the downlink
   ltephy_cell_t c{};
@@ -47,6 +55,7 @@ int main(int argc, char** argv)
   ltephy_cfg_t cfg{};
   cfg.nof_prb = mib.nof_prb, cfg.nof_ports = mib.nof_ports, cfg.cell_id = c.pci, cfg.nof_rx = 1, cfg.max_subframes = B, cfg.turbo_max_iter = 8;
   cfg.flags = LTEPHY_FLAG_SKIP_LOW_POWER, cfg.symbol_sz = N, cfg.phich_resources = mib.phich_resources, cfg.phich_length = mib.phich_length;
+  cfg.ul_nof_rx = ul_rx;
   UlChain u;
   if (u.open(cfg, ltephy_ul_cfg_t{arg(7, 0), arg(8, 0), 0, 0}, arg(9, 0), argv[4])) return 1;
   uint64_t fo  = c.frame_offset;
@@ -56,7 +65,7 @@ int main(int argc, char** argv)
   tcfg.symbol_sz = N, tcfg.nof_rx = 1, tcfg.pci = c.pci, tcfg.first_tti = tti, tcfg.frame_offset = fo, tcfg.cfo_hz = c.cfo_hz;
   tcfg.max_ppm = 50.0f, tcfg.max_subframes = B;
   ltephy_track_ul_cfg_t tul{};
-  tul.cfo_ratio = cfo_ratio, tul.ul_offset = ul_offset;
+  tul.cfo_ratio = cfo_ratio, tul.ul_offset = ul_offset, tul.nof_rx = ul_rx; // the UL cut is [got][ul_rx][15 N], what the UL decoder of cfg takes
   ltephy_track_t* tr = nullptr;
   if (ltephy_track_create(&tcfg, &tr) != LTEPHY_SUCCESS || ltephy_track_set_ul(tr, &tul) != LTEPHY_SUCCESS) {
     fprintf(stderr, "tracker: %s\n", ltephy_last_error());
@@ -72,7 +81,7 @@ int main(int argc, char** argv)
       if (recv == L) break;
       continue;
     }
-    if (!read_span(fd, 1, Ld, next, recv - next, x) || !read_span(fu, 1, Lu, next, recv - next, xu)) {
+    if (!read_span(fd, 1, Ld, next, recv - next, x) || !read_span(fu, ul_rx, Lu, next, recv - next, xu)) {
       fprintf(stderr, "short read\n");
       return 1;
     }

@@ -61,7 +61,10 @@ typedef struct {
                                mode, src/src/LTESniffer_Core.cc:242-247), 1 = 1/2, 2 = 1, 3 = 2.  Sets the PHICH groups of symbol 0 and with them the
                                CCE grid of the PDCCH. */
   uint32_t phich_length;    /* phich-Duration of the MIB (srsran_cell_t.phich_length): 0 normal, 1 extended (PHICH REGs in symbols 0, 1 and 2) */
-  uint32_t reserved[4];
+  uint32_t ul_nof_rx;       /* receive antennas of the uplink carrier: 0 or 1 one antenna, 2 two (PUSCH combined over both, DESIGN.md §2 "uplink
+                               receive diversity"); any other value is INVALID_INPUTS.  Sets the shape of ltephy_submit_ul / _device and
+                               LTEPHY_TAP_UL_SYM. */
+  uint32_t reserved[3];
 } ltephy_cfg_t;
 
 #define LTEPHY_FLAG_SKIP_LOW_POWER 1u /* do not decode locations covering a CCE with mean|LLR| < 0.7 (they are never consulted) */
@@ -365,12 +368,14 @@ int  ltephy_track_push_device(ltephy_track_t* h, const void* iq_dev, uint64_t fi
 typedef struct {
   double   cfo_ratio; /* f_UL / f_DL, in (0, 2] */
   int32_t  ul_offset; /* whole samples the UL subframe starts after the DL one, |ul_offset| < 15 N */
-  uint32_t reserved[5];
+  uint32_t nof_rx;    /* UL receive antennas: 0 or 1 one antenna, 2 two (every antenna cut at the same start with the same rotation); else INVALID_INPUTS */
+  uint32_t reserved[4];
 } ltephy_track_ul_cfg_t;
 int  ltephy_track_set_ul(ltephy_track_t* h, const ltephy_track_ul_cfg_t* cfg);
-/* iq as ltephy_track_push; iq_ul: cf32 [nof_samples] of one UL antenna, the same absolute samples.  A subframe is cut only when its DL window and
- * its UL window both lie inside what has been fed; out->next_sample is the lowest sample either pending window still needs.  The DL records and
- * cut equal those of a tracker without the uplink.  *ul_iq_dev: cf32 [nof_subframes][15 N] in device memory, valid until the next push. */
+/* iq as ltephy_track_push; iq_ul: cf32 [ul nof_rx][nof_samples], antenna-major like iq, the same absolute samples.  A subframe is cut only when its
+ * DL window and its UL window both lie inside what has been fed; out->next_sample is the lowest sample either pending window still needs.  The DL
+ * records and cut equal those of a tracker without the uplink.  *ul_iq_dev: cf32 [nof_subframes][ul nof_rx][15 N] in device memory, valid until the
+ * next push: the input ltephy_submit_ul_device takes with ltephy_cfg_t.ul_nof_rx = the same antenna count. */
 int  ltephy_track_push_ul(ltephy_track_t* h, const float* iq, const float* iq_ul, uint64_t first_sample, uint64_t nof_samples, ltephy_track_out_t* out,
                           const void** ul_iq_dev);
 /* same, with both carriers already in device memory */
@@ -482,16 +487,17 @@ typedef struct {
   float ta_us;            /* .ta_us    timing offset from the phase slope of the DMRS estimates (meas_ta_en, UL_Sniffer_PUSCH.cc:424,574) */
 } ltephy_ul_chest_t;
 int ltephy_set_ul_cfg(ltephy_t* h, const ltephy_ul_cfg_t* cfg);
-/* iq_ul: n * sf_len cf32 of the UL carrier (one antenna: the reference uses antenna buffer 1); host memory.  iq_ul may be NULL when the previous
- * call demodulated the same n subframes: their symbols are decoded again with the new grants (srsran_enb_ul_fft once, decode_run per grant).
- * L_prb >= 3: the 1- and 2-PRB DMRS base sequences (36.211 Tables 5.5.1.2-1 / -2) are not carried. */
+/* iq_ul: cf32 [n][A][sf_len] of the UL carrier, A = ltephy_cfg_t.ul_nof_rx antennas (one antenna, A = 1, is what the reference decodes: antenna
+ * buffer 1); host memory.  With A = 2 the PUSCH is estimated per antenna and equalised over both (DESIGN.md §2 "uplink receive diversity").
+ * iq_ul may be NULL when the previous call demodulated the same n subframes: their symbols are decoded again with the new grants
+ * (srsran_enb_ul_fft once, decode_run per grant).  L_prb >= 3: the 1- and 2-PRB DMRS base sequences (36.211 Tables 5.5.1.2-1 / -2) are not carried. */
 int ltephy_submit_ul(ltephy_t* h, const float* iq_ul, const uint32_t* tti, uint32_t n, const ltephy_ul_grant_t* grants, uint32_t ngrants);
-/* same, with iq_ul_dev cf32 [n][sf_len] already in device memory on the handle's device (e.g. ltephy_track_push_ul's cut), read in place: the
+/* same, with iq_ul_dev cf32 [n][A][sf_len] already in device memory on the handle's device (e.g. ltephy_track_push_ul's cut), read in place: the
  * caller keeps it alive until ltephy_get_ul returns.  NULL re-decodes the previous call's symbols, as above. */
 int ltephy_submit_ul_device(ltephy_t* h, const void* iq_ul_dev, const uint32_t* tti, uint32_t n, const ltephy_ul_grant_t* grants, uint32_t ngrants);
 /* the uplink twin of ltephy_set_cfo: a constant carrier-offset correction of every UL subframe (phase restarting at each subframe, the table of
  * ltephy_set_cfo), applied before the 7.5 kHz half-subcarrier rotation -- lteo_cfo_correct then lteo_ul_ofdm.  0 switches it off.  Kept apart
- * from ltephy_set_cfo's value.  For pre-aligned captures; the tracked cut of ltephy_track_push_ul is already rotated. */
+ * from ltephy_set_cfo's value; applies to every UL antenna.  For pre-aligned captures; the tracked cut of ltephy_track_push_ul is already rotated. */
 int ltephy_set_ul_cfo(ltephy_t* h, float cfo_hz);
 /* results[ngrants], chest[ngrants]; payload receives the TB bytes back to back */
 int ltephy_get_ul(ltephy_t* h, ltephy_tb_result_t* results, ltephy_ul_chest_t* chest, uint8_t* payload, size_t payload_cap);
@@ -511,7 +517,7 @@ enum {
   LTEPHY_TAP_LLR = 2, /* f32  [n][72*LTEPHY_MAX_CCE]           q->pdcch.llr */
   LTEPHY_TAP_PDSCH_LLR = 3, /* int16, all codewords of the submitted grants back to back */
   LTEPHY_TAP_TURBO_IN = 4,  /* int16 conditioned streams (debug) */
-  LTEPHY_TAP_UL_SYM = 5,    /* cf32 [n][14][12*nof_prb]  UL grid after srsran_enb_ul_fft */
+  LTEPHY_TAP_UL_SYM = 5,    /* cf32 [n][ul_nof_rx][14][12*nof_prb]  UL grid after srsran_enb_ul_fft */
   LTEPHY_TAP_PBCH_LLR = 6   /* f32  [frames][2][480]     PBCH soft bits (not descrambled) of the subframes 0 of the last ltephy_mib_decode or
                                ltephy_mib_decode_combined, in batch order, row [port count - 1]; ltephy_mib_decode writes only its handle's port count */
 };

@@ -17,7 +17,8 @@ FLAG_SKIP_LOW_POWER = 1
 class Cfg(C.Structure):
     _fields_ = [("nof_prb", C.c_uint32), ("nof_ports", C.c_uint32), ("cell_id", C.c_uint32), ("nof_rx", C.c_uint32),
                 ("max_subframes", C.c_uint32), ("max_grants", C.c_uint32), ("turbo_max_iter", C.c_uint32), ("device", C.c_int32),
-                ("flags", C.c_uint32), ("symbol_sz", C.c_uint32), ("phich_resources", C.c_uint32), ("phich_length", C.c_uint32), ("reserved", C.c_uint32 * 4)]
+                ("flags", C.c_uint32), ("symbol_sz", C.c_uint32), ("phich_resources", C.c_uint32), ("phich_length", C.c_uint32),
+                ("ul_nof_rx", C.c_uint32), ("reserved", C.c_uint32 * 3)]
 
 
 class SfInfo(C.Structure):
@@ -158,10 +159,13 @@ def _p(a):
 class LtePhy:
     """One PHY context (cell + batch capacity) on one GPU."""
 
-    def __init__(self, nof_prb, nof_ports, cell_id, nof_rx, max_subframes=16, turbo_max_iter=8, device=0, flags=0, symbol_sz=0, phich_resources=0, phich_length=0):
+    def __init__(self, nof_prb, nof_ports, cell_id, nof_rx, max_subframes=16, turbo_max_iter=8, device=0, flags=0, symbol_sz=0, phich_resources=0, phich_length=0,
+                 ul_nof_rx=1):
+        """ul_nof_rx: receive antennas of the uplink carrier (1 or 2): decode_ul / decode_ul_device then take [n][ul_nof_rx][sf_len]"""
         self.L = load_library()
         cfg = Cfg(nof_prb=nof_prb, nof_ports=nof_ports, cell_id=cell_id, nof_rx=nof_rx, max_subframes=max_subframes,
-                  turbo_max_iter=turbo_max_iter, device=device, flags=flags, symbol_sz=symbol_sz, phich_resources=phich_resources, phich_length=phich_length)
+                  turbo_max_iter=turbo_max_iter, device=device, flags=flags, symbol_sz=symbol_sz, phich_resources=phich_resources, phich_length=phich_length,
+                  ul_nof_rx=ul_nof_rx)
         self.cfg = cfg
         self.h = C.c_void_p()
         r = self.L.ltephy_create(C.byref(cfg), C.byref(self.h))
@@ -169,6 +173,7 @@ class LtePhy:
             raise RuntimeError("ltephy_create failed (%d): %s" % (r, self.L.ltephy_last_error().decode()))
         self.sf_len = self.L.ltephy_sf_len(self.h)
         self.nsc = 12 * nof_prb
+        self.ul_nof_rx = max(1, ul_nof_rx)
         self.n = 0
 
     def close(self):
@@ -274,9 +279,11 @@ class LtePhy:
         self._chk(self.L.ltephy_set_ul_cfg(self.h, C.byref(cfg)), "set_ul_cfg")
 
     def decode_ul(self, iq_ul, tti, grants):
-        """iq_ul complex64 [n][sf_len] (None: decode the subframes of the previous call again); grants: list of UlGrant -> (results, chest, payload)"""
+        """iq_ul complex64 [n][sf_len] with one UL antenna, [n][ul_nof_rx][sf_len] with two (None: decode the subframes of the previous call
+        again); grants: list of UlGrant -> (results, chest, payload)"""
         iq_ul = None if iq_ul is None else np.ascontiguousarray(iq_ul, np.complex64)
         tti = np.ascontiguousarray(tti, np.uint32)
+        assert iq_ul is None or iq_ul.size == len(tti) * self.ul_nof_rx * self.sf_len, (iq_ul.shape, self.ul_nof_rx)
         arr = (UlGrant * max(1, len(grants)))(*grants)
         self._chk(self.L.ltephy_submit_ul(self.h, None if iq_ul is None else _p(iq_ul), _p(tti), len(tti), arr, len(grants)), "submit_ul")
         res = (TbResult * max(1, len(grants)))()
@@ -287,12 +294,13 @@ class LtePhy:
         return res, ch, pl
 
     def decode_ul_device(self, iq_dev, tti, grants):
-        """ltephy_submit_ul_device: iq_dev a torch complex64 tensor [n][sf_len], contiguous, on this handle's device (None: decode the subframes
-        of the previous call again), read in place -> (results, chest, payload) as decode_ul"""
+        """ltephy_submit_ul_device: iq_dev a torch complex64 tensor [n][sf_len] ([n][ul_nof_rx][sf_len] with two UL antennas), contiguous, on this
+        handle's device (None: decode the subframes of the previous call again), read in place -> (results, chest, payload) as decode_ul"""
         self.L.ltephy_submit_ul_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32]
         tti = np.ascontiguousarray(tti, np.uint32)
         if iq_dev is not None:
-            assert iq_dev.is_cuda and iq_dev.is_contiguous() and tuple(iq_dev.shape) == (len(tti), self.sf_len), tuple(iq_dev.shape)
+            want = (len(tti), self.sf_len) if self.ul_nof_rx == 1 else (len(tti), self.ul_nof_rx, self.sf_len)
+            assert iq_dev.is_cuda and iq_dev.is_contiguous() and tuple(iq_dev.shape) == want, tuple(iq_dev.shape)
         arr = (UlGrant * max(1, len(grants)))(*grants)
         ptr = None if iq_dev is None else C.c_void_p(iq_dev.data_ptr())
         self._chk(self.L.ltephy_submit_ul_device(self.h, ptr, _p(tti), len(tti), arr, len(grants)), "submit_ul_device")
@@ -818,7 +826,7 @@ class TrackOut(C.Structure):
 
 
 class TrackUlCfg(C.Structure):
-    _fields_ = [("cfo_ratio", C.c_double), ("ul_offset", C.c_int32), ("reserved", C.c_uint32 * 5)]
+    _fields_ = [("cfo_ratio", C.c_double), ("ul_offset", C.c_int32), ("nof_rx", C.c_uint32), ("reserved", C.c_uint32 * 4)]
 
 
 assert C.sizeof(TrackCfg) == 64 and C.sizeof(TrackOut) == 48 and TRACK_SF_DTYPE.itemsize == 24 and TRACK_HF_DTYPE.itemsize == 40
@@ -828,7 +836,8 @@ assert C.sizeof(TrackUlCfg) == 32
 class Tracker:
     """PSS tracking and subframe cutting of a recording after the cell search: push the recording part by part (antenna-major complex64
     [nof_rx][n] with its absolute first sample); each push returns the subframes that now lie wholly inside what was fed.  With ul=dict(cfo_ratio=..., ul_offset=...) the tracker also cuts the
-    uplink carrier of the same radio (ltephy_track_set_ul); push both carriers with push_ul / push_ul_device.  With flags=TRACK_REACQUIRE a
+    uplink carrier of the same radio (ltephy_track_set_ul); push both carriers with push_ul / push_ul_device.  ul=dict(..., nof_rx=2) cuts two UL
+    antennas: push_ul then takes iq_ul [2][n] and ul_iq is [k][2][15 N] (one antenna: [n] and [k][15 N]).  With flags=TRACK_REACQUIRE a
     lost cell is searched again frame by frame; the first subframe cut after it is found carries TRACK_REACQUIRED."""
 
     def __init__(self, symbol_sz, nof_rx, pci, frame_offset, cfo_hz=0.0, first_tti=0, max_subframes=1000, max_ppm=50.0, flags=0, device=0, ul=None):
@@ -851,7 +860,7 @@ class Tracker:
         self.next_sample = frame_offset
         self.ul = None
         if ul is not None:
-            u = TrackUlCfg(cfo_ratio=float(ul.get("cfo_ratio", 1.0)), ul_offset=int(ul.get("ul_offset", 0)))
+            u = TrackUlCfg(cfo_ratio=float(ul.get("cfo_ratio", 1.0)), ul_offset=int(ul.get("ul_offset", 0)), nof_rx=int(ul.get("nof_rx", 1)))
             r = L.ltephy_track_set_ul(self.h, C.byref(u))
             if r != 0:
                 self.close()
@@ -890,7 +899,8 @@ class Tracker:
         self.next_sample = o.next_sample
         out = dict(sf=sf, hf=hf, iq=iq, next_sample=o.next_sample, remeasured=o.remeasured, finds=o.finds)
         if ul_ptr is not None:
-            out["ul_iq"] = self._view(ul_ptr.value, (o.nof_subframes, 15 * self.cfg.symbol_sz))
+            A = max(1, self.ul.nof_rx)
+            out["ul_iq"] = self._view(ul_ptr.value, (o.nof_subframes, 15 * self.cfg.symbol_sz) if A == 1 else (o.nof_subframes, A, 15 * self.cfg.symbol_sz))
         return out
 
     def push(self, iq, first_sample):
@@ -908,18 +918,18 @@ class Tracker:
         return self._done(self.L.ltephy_track_push_device(self.h, C.c_void_p(iq.data_ptr()), first_sample, iq.shape[1], C.byref(o)), o)
 
     def push_ul(self, iq, iq_ul, first_sample):
-        """iq as push, iq_ul: complex64 [n] of the uplink antenna, the same absolute samples -> push's dict plus ul_iq: torch complex64 [k][15 N]
-        on the device (a copy of the tracker's UL cut)"""
+        """iq as push, iq_ul: complex64 [n] of the uplink antenna ([A][n] with A = 2 UL antennas), the same absolute samples -> push's dict plus
+        ul_iq: torch complex64 [k][15 N] ([k][A][15 N]) on the device (a copy of the tracker's UL cut)"""
         iq = np.ascontiguousarray(iq, np.complex64)
         iq_ul = np.ascontiguousarray(iq_ul, np.complex64).reshape(-1)
-        assert iq.ndim == 2 and iq.shape[0] == self.cfg.nof_rx and iq_ul.shape[0] == iq.shape[1], (iq.shape, iq_ul.shape)
+        assert iq.ndim == 2 and iq.shape[0] == self.cfg.nof_rx and iq_ul.shape[0] == max(1, self.ul.nof_rx) * iq.shape[1], (iq.shape, iq_ul.shape)
         o, u = TrackOut(), C.c_void_p()
         return self._done(self.L.ltephy_track_push_ul(self.h, _p(iq), _p(iq_ul), first_sample, iq.shape[1], C.byref(o), C.byref(u)), o, u)
 
     def push_ul_device(self, iq, iq_ul, first_sample):
-        """iq: torch complex64 [nof_rx][n], iq_ul: torch complex64 [n], both contiguous on this handle's device"""
+        """iq: torch complex64 [nof_rx][n], iq_ul: torch complex64 [n] ([A][n] with A = 2 UL antennas), both contiguous on this handle's device"""
         assert iq.is_cuda and iq.is_contiguous() and iq.dim() == 2 and iq.shape[0] == self.cfg.nof_rx
-        assert iq_ul.is_cuda and iq_ul.is_contiguous() and iq_ul.numel() == iq.shape[1]
+        assert iq_ul.is_cuda and iq_ul.is_contiguous() and iq_ul.numel() == max(1, self.ul.nof_rx) * iq.shape[1]
         o, u = TrackOut(), C.c_void_p()
         return self._done(self.L.ltephy_track_push_ul_device(self.h, C.c_void_p(iq.data_ptr()), C.c_void_p(iq_ul.data_ptr()), first_sample, iq.shape[1],
                                                              C.byref(o), C.byref(u)), o, u)

@@ -9,6 +9,7 @@
 
 struct DevCell {
   uint32_t nof_prb, nof_ports, cell_id, nof_rx, fft, log2n, nsc, sf_len;
+  uint32_t ul_nof_rx;             // antennas of the uplink carrier, 1 or 2 (ltephy_cfg_t.ul_nof_rx)
   uint32_t sub;                   // power-of-two transform length: fft, or fft / 3 for a 3 * 2^k symbol size (log2n = log2(sub))
   uint32_t sym_off[14];
   uint32_t nof_cce[3], nloc[3];

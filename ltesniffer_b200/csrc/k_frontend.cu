@@ -65,7 +65,7 @@ __global__ void __launch_bounds__(256) ofdm_rx_kernel(const __grid_constant__ De
   const uint32_t l = blockIdx.x, a = blockIdx.y, sf = blockIdx.z, n = c.fft, M = c.sub, L = c.log2n, q8 = M >> 3;
   const uint32_t nt = R3 ? blockDim.x / 3 : blockDim.x, r = R3 ? threadIdx.x / nt : 0u, tid = R3 ? threadIdx.x % nt : threadIdx.x;
   float2*        work = reinterpret_cast<float2*>(smem_raw) + r * M; // [3][M] or [fft], swizzled
-  const uint32_t nant = UL ? 1u : c.nof_rx; // the UL carrier is decoded from one antenna (UL_Sniffer_PUSCH.cc:391-392)
+  const uint32_t nant = gridDim.y; // c.nof_rx, or c.ul_nof_rx on the UL carrier
   const float2*  src = iq + ((size_t)sf * nant + a) * c.sf_len + c.sym_off[l];
   const float2*  tw_st = c.tw_st;
 
@@ -360,7 +360,7 @@ extern "C" void launch_frontend(const DevCell& c, const float2* iq, float2* sym,
 extern "C" void launch_ul_ofdm(const DevCell& c, const float2* iq, float2* sym, uint32_t n, cudaStream_t st, uint64_t* launches)
 {
   const size_t smem_fft = (size_t)c.fft * sizeof(float2);
-  const dim3   grid(14, 1, n);
+  const dim3   grid(14, c.ul_nof_rx, n);
   const uint32_t nt2 = c.fft / 8 < 32 ? 32 : c.fft / 8, nt3 = 3 * (c.sub / 8);
   if (c.sub == c.fft) {
     if (c.ul_cfo_rot)

@@ -5,6 +5,8 @@
 // Restates srsran_chest_ul_estimate_pusch + the front half of srsran_pusch_decode as called from PUSCH_Decoder::decode_run
 // (reference src/src/UL_Sniffer_PUSCH.cc:250-263) with the configuration of :421-450; the UL OFDM demodulation (srsran_enb_ul_fft, :392)
 // is ofdm_rx_kernel in UL mode.  L_prb >= 3 (the 1- and 2-PRB DMRS base sequences are table-defined, 36.211 Tables 5.5.1.2-1/2).
+// With NA = 2 receive antennas (DESIGN.md §2 "uplink receive diversity") each antenna is estimated alone and the equaliser combines them as
+// eq_port0 does: sum_a conj(h_a) y_a / sum_a |h_a|^2; NA = 1 compiles to the one-antenna arithmetic.
 // The IDFT is a Stockham autosort with radices 5.., 3.., 4.., 2 whose butterflies are plain sums in index order, the same expression tree
 // as the oracle's, so the soft bits are bit-identical for every 2^a 3^b 5^c size.
 #include "dev_common.cuh"
@@ -115,7 +117,8 @@ template <uint32_t R> __device__ __forceinline__ void idft_butterfly(const float
 
 #define PUSCH_PASS_CAP 2400u // float2 per ping-pong buffer: S = min(12, PUSCH_PASS_CAP / M) data symbols are transformed together
 
-// grid (grants)
+// grid (grants); ulsym [n][NA][14][nsc]
+template <uint32_t NA>
 __global__ void __launch_bounds__(256) pusch_kernel(const __grid_constant__ DevCell c, const DevUlGrant* __restrict__ grants,
                                                     const float2* __restrict__ ulsym, const float2* __restrict__ dmrs_pool,
                                                     const float2* __restrict__ idft_pool, const uint32_t* __restrict__ seq_pool,
@@ -124,37 +127,41 @@ __global__ void __launch_bounds__(256) pusch_kernel(const __grid_constant__ DevC
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const DevUlGrant g = grants[blockIdx.x];
   const uint32_t   M = g.M, tid = threadIdx.x, nt = blockDim.x, nsc = c.nsc;
-  float2*          ls = reinterpret_cast<float2*>(smem_raw); // [2][M]
-  float2*          sm = ls + 2 * max_M;                      // [2][M]
-  float2*          W  = sm + 2 * max_M;                      // [M]
+  float2*          ls = reinterpret_cast<float2*>(smem_raw); // [2][M], one antenna at a time
+  float2*          sm = ls + 2 * max_M;                      // [NA][2][M]
+  float2*          W  = sm + 2 * NA * max_M;                 // [M]
   float2*          bufA = W + max_M;                         // [S][M]
   float2*          bufB = bufA + PUSCH_PASS_CAP;
-  __shared__ float red[2][4];
-  const float2*    y  = ulsym + (size_t)g.sf * 14 * nsc;
+  __shared__ float red[NA][2][4];
+  const float2*    y  = ulsym + (size_t)g.sf * NA * 14 * nsc; // antenna a at y + a 14 nsc
 
-  for (uint32_t i = tid; i < 2 * M; i += nt) {
-    const uint32_t sl = i / M, n = i % M;
-    const float2   v = y[(7 * sl + 3) * nsc + g.k0[sl] + n], r = dmrs_pool[g.dmrs_off[sl] + n];
-    ls[i]            = make_float2(v.x * r.x + v.y * r.y, v.y * r.x - v.x * r.y);
-  }
   for (uint32_t i = tid; i < M; i += nt) W[i] = idft_pool[g.idft_off + i];
-  __syncthreads();
   const float f0 = 0.3333f, f1 = 1.0f - 2.0f * 0.3333f, f2 = 0.3333f;
-  for (uint32_t i = tid; i < 2 * M; i += nt) {
-    const uint32_t sl = i / M, n = i % M;
-    float          ar = 0.0f, ai = 0.0f, ws = 0.0f;
-    if (n > 0) ar = ar + f0 * ls[sl * M + n - 1].x, ai = ai + f0 * ls[sl * M + n - 1].y, ws = ws + f0;
-    ar = ar + f1 * ls[i].x, ai = ai + f1 * ls[i].y, ws = ws + f1;
-    if (n + 1 < M) ar = ar + f2 * ls[sl * M + n + 1].x, ai = ai + f2 * ls[sl * M + n + 1].y, ws = ws + f2;
-    sm[i] = make_float2(ar / ws, ai / ws);
-  }
-  __syncthreads();
-  {
+#pragma unroll
+  for (uint32_t a = 0; a < NA; a++) {
+    const float2* ya  = y + a * 14 * nsc;
+    float2*       sma = sm + a * 2 * M;
+    if (a) __syncthreads(); // the previous antenna's sums have read ls
+    for (uint32_t i = tid; i < 2 * M; i += nt) {
+      const uint32_t sl = i / M, n = i % M;
+      const float2   v = ya[(7 * sl + 3) * nsc + g.k0[sl] + n], r = dmrs_pool[g.dmrs_off[sl] + n];
+      ls[i]            = make_float2(v.x * r.x + v.y * r.y, v.y * r.x - v.x * r.y);
+    }
+    __syncthreads();
+    for (uint32_t i = tid; i < 2 * M; i += nt) {
+      const uint32_t sl = i / M, n = i % M;
+      float          ar = 0.0f, ai = 0.0f, ws = 0.0f;
+      if (n > 0) ar = ar + f0 * ls[sl * M + n - 1].x, ai = ai + f0 * ls[sl * M + n - 1].y, ws = ws + f0;
+      ar = ar + f1 * ls[i].x, ai = ai + f1 * ls[i].y, ws = ws + f1;
+      if (n + 1 < M) ar = ar + f2 * ls[sl * M + n + 1].x, ai = ai + f2 * ls[sl * M + n + 1].y, ws = ws + f2;
+      sma[i] = make_float2(ar / ws, ai / ws);
+    }
+    __syncthreads();
     const uint32_t warp = tid >> 5, lane = tid & 31;
     if (warp < 2) { // one warp per slot: noise, power and the lag-1 correlation of the LS estimates (timing offset)
       float pn = 0.0f, pp = 0.0f, cr = 0.0f, ci = 0.0f;
       for (uint32_t n = lane; n < M; n += 32) {
-        const float2 s = sm[warp * M + n], r = ls[warp * M + n];
+        const float2 s = sma[warp * M + n], r = ls[warp * M + n];
         const float  dr = r.x - s.x, di = r.y - s.y;
         pn = pn + (dr * dr + di * di);
         pp = pp + (s.x * s.x + s.y * s.y);
@@ -165,20 +172,22 @@ __global__ void __launch_bounds__(256) pusch_kernel(const __grid_constant__ DevC
         }
       }
       pn = warp_tree_sum(pn), pp = warp_tree_sum(pp), cr = warp_tree_sum(cr), ci = warp_tree_sum(ci);
-      if (lane == 0) red[warp][0] = pn, red[warp][1] = pp, red[warp][2] = cr, red[warp][3] = ci;
+      if (lane == 0) red[a][warp][0] = pn, red[a][warp][1] = pp, red[a][warp][2] = cr, red[a][warp][3] = ci;
     }
-    __syncthreads();
-    if (tid == 0) {
-      float nsum = 0.0f, psum = 0.0f;
-      nsum = nsum + red[0][0], nsum = nsum + red[1][0];
-      psum = psum + red[0][1], psum = psum + red[1][1];
-      const float ncorr = (1.0f - 2.0f * f1) + (f0 * f0 + f1 * f1 + f2 * f2);
-      DevUlChest  o;
-      o.noise = (nsum / (float)(2 * M)) / ncorr;
-      o.rsrp  = psum / (float)(2 * M);
-      o.cr[0] = red[0][2], o.ci[0] = red[0][3], o.cr[1] = red[1][2], o.ci[1] = red[1][3];
-      chest[blockIdx.x] = o;
-    }
+  }
+  __syncthreads();
+  if (tid == 0) { // antenna-major, then slot; cr / ci per slot summed over the antennas
+    float nsum = 0.0f, psum = 0.0f;
+    for (uint32_t a = 0; a < NA; a++) nsum = nsum + red[a][0][0], nsum = nsum + red[a][1][0];
+    for (uint32_t a = 0; a < NA; a++) psum = psum + red[a][0][1], psum = psum + red[a][1][1];
+    const float ncorr = (1.0f - 2.0f * f1) + (f0 * f0 + f1 * f1 + f2 * f2);
+    DevUlChest  o;
+    o.noise = (nsum / (float)(2 * M * NA)) / ncorr;
+    o.rsrp  = psum / (float)(2 * M * NA);
+    o.cr[0] = red[0][0][2], o.ci[0] = red[0][0][3], o.cr[1] = red[0][1][2], o.ci[1] = red[0][1][3];
+    for (uint32_t a = 1; a < NA; a++)
+      o.cr[0] = o.cr[0] + red[a][0][2], o.ci[0] = o.ci[0] + red[a][0][3], o.cr[1] = o.cr[1] + red[a][1][2], o.ci[1] = o.ci[1] + red[a][1][3];
+    chest[blockIdx.x] = o;
   }
   // ---- data symbols, S at a time: equalise, IDFT, demap, descramble, de-multiplex, de-interleave --------------------
   const uint32_t  S = min(12u, PUSCH_PASS_CAP / M);
@@ -192,11 +201,17 @@ __global__ void __launch_bounds__(256) pusch_kernel(const __grid_constant__ DevC
     for (uint32_t i = tid; i < ns * M; i += nt) {
       const uint32_t s = i / M, n = i % M, cc = c0 + s, l = cc + (cc >= 3) + (cc >= 9), sl = cc / 6; // data symbols 0,1,2,4,5,6,7,8,9,11,12,13
       const float    t = (float)((int)l - 3) / 7.0f;
-      const float2   A = sm[n], B = sm[M + n];
-      const float2   h = hop ? sm[sl * M + n] : make_float2(A.x + (B.x - A.x) * t, A.y + (B.y - A.y) * t);
-      const float2   v = y[l * nsc + g.k0[sl] + n];
-      const float    den = h.x * h.x + h.y * h.y;
-      bufA[i]            = make_float2(eq_div(v.x * h.x + v.y * h.y, den), eq_div(v.y * h.x - v.x * h.y, den)); // no channel: 0, not NaN
+      float          nr = 0.0f, ni = 0.0f, den = 0.0f;
+#pragma unroll
+      for (uint32_t a = 0; a < NA; a++) { // antenna 0's terms start the sums: one antenna is the one-antenna expression
+        const float2* sma = sm + a * 2 * M;
+        const float2  A = sma[n], B = sma[M + n];
+        const float2  h = hop ? sma[sl * M + n] : make_float2(A.x + (B.x - A.x) * t, A.y + (B.y - A.y) * t);
+        const float2  v = y[(a * 14 + l) * nsc + g.k0[sl] + n];
+        const float   tr = v.x * h.x + v.y * h.y, ti = v.y * h.x - v.x * h.y, td = h.x * h.x + h.y * h.y;
+        nr = a ? nr + tr : tr, ni = a ? ni + ti : ti, den = a ? den + td : td;
+      }
+      bufA[i] = make_float2(eq_div(nr, den), eq_div(ni, den)); // no channel: 0, not NaN
     }
     __syncthreads();
     float2 * src = bufA, *dst = bufB;
@@ -242,8 +257,15 @@ extern "C" void launch_pusch(const DevCell& c, const DevUlGrant* grants, uint32_
 {
   if (!ngrants) return;
   scr_seq_ul_kernel<<<dim3(ngrants, (max_words + 255) / 256), 256, 0, st>>>(grants, x1, basis, basis_words, c.cell_id, seq_pool);
-  const size_t smem = ((size_t)5 * max_M + 2 * PUSCH_PASS_CAP) * sizeof(float2);
-  cudaFuncSetAttribute(pusch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (5 * 1200 + 2 * (int)PUSCH_PASS_CAP) * (int)sizeof(float2)); // per device / context
-  pusch_kernel<<<ngrants, 256, smem, st>>>(c, grants, ulsym, dmrs_pool, idft_pool, seq_pool, llr_pool, chest, max_M);
+  // ls [2][M], sm [A][2][M], W [M] and the two IDFT buffers: 86 KB at M = 1200 with one antenna, 106 KB with two (two CTAs per SM either way)
+  const size_t smem = ((size_t)(3 + 2 * c.ul_nof_rx) * max_M + 2 * PUSCH_PASS_CAP) * sizeof(float2);
+  const int    cap  = (int)(((3 + 2 * c.ul_nof_rx) * 1200 + 2 * PUSCH_PASS_CAP) * sizeof(float2));
+  if (c.ul_nof_rx == 2) {
+    cudaFuncSetAttribute(pusch_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap); // per device / context
+    pusch_kernel<2><<<ngrants, 256, smem, st>>>(c, grants, ulsym, dmrs_pool, idft_pool, seq_pool, llr_pool, chest, max_M);
+  } else {
+    cudaFuncSetAttribute(pusch_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap);
+    pusch_kernel<1><<<ngrants, 256, smem, st>>>(c, grants, ulsym, dmrs_pool, idft_pool, seq_pool, llr_pool, chest, max_M);
+  }
   *launches += 2;
 }

@@ -68,6 +68,7 @@ extern "C" int ltephy_create(const ltephy_cfg_t* cfg, ltephy_t** out)
   if (cfg->nof_prb <= 10 || cfg->nof_prb > 100 || cfg->nof_ports < 1 || cfg->nof_ports > 2 || cfg->nof_rx < 1 || cfg->nof_rx > 2 ||
       cfg->max_subframes == 0)
     return fail(LTEPHY_ERROR_INVALID_INPUTS, "unsupported cell/batch configuration");
+  if (cfg->ul_nof_rx > 2) return fail(LTEPHY_ERROR_INVALID_INPUTS, "ul_nof_rx %u: 0 or 1 (one uplink antenna) or 2", cfg->ul_nof_rx);
   // the front end puts the subframe index on gridDim.y / gridDim.z (k_frontend.cu), which stop at 65 535
   if (cfg->max_subframes > LTEPHY_MAX_BATCH_SUBFRAMES)
     return fail(LTEPHY_ERROR_INVALID_INPUTS, "max_subframes %u: at most %u subframes per batch", cfg->max_subframes, (uint32_t)LTEPHY_MAX_BATCH_SUBFRAMES);
@@ -86,6 +87,7 @@ extern "C" int ltephy_create(const ltephy_cfg_t* cfg, ltephy_t** out)
   h->cfg    = *cfg;
   if (!h->cfg.turbo_max_iter) h->cfg.turbo_max_iter = 8;
   if (!h->cfg.max_grants) h->cfg.max_grants = 24 * cfg->max_subframes;
+  if (!h->cfg.ul_nof_rx) h->cfg.ul_nof_rx = 1;
   if (cfg->phich_resources > 3 || cfg->phich_length > 1)
     return fail(LTEPHY_ERROR_INVALID_INPUTS, "phich_resources %u / phich_length %u: 0 (Ng = 1/6), 1 (1/2), 2 (1) or 3 (2); 0 normal or 1 extended", cfg->phich_resources, cfg->phich_length);
   h->cell = {cfg->nof_prb, cfg->nof_ports, cfg->cell_id, cfg->nof_rx, cfg->phich_resources, cfg->phich_length};
@@ -99,7 +101,7 @@ extern "C" int ltephy_create(const ltephy_cfg_t* cfg, ltephy_t** out)
   for (auto& e : h->mark) CU(cudaEventCreate(&e.raw));
 
   DevCell& c = h->dc;
-  c.nof_prb = cfg->nof_prb, c.nof_ports = cfg->nof_ports, c.cell_id = cfg->cell_id, c.nof_rx = cfg->nof_rx;
+  c.nof_prb = cfg->nof_prb, c.nof_ports = cfg->nof_ports, c.cell_id = cfg->cell_id, c.nof_rx = cfg->nof_rx, c.ul_nof_rx = h->cfg.ul_nof_rx;
   c.fft = cfg->symbol_sz ? cfg->symbol_sz : ltehost::fft_size(cfg->nof_prb), c.nsc = 12 * cfg->nof_prb, c.sf_len = 15 * c.fft;
   c.sub = c.fft % 3 ? c.fft : c.fft / 3; // length of the power-of-two transforms: the whole symbol, or a third of a 3 * 2^k one
   for (c.log2n = 0; (1u << c.log2n) < c.sub; c.log2n++) {
@@ -1085,13 +1087,14 @@ static int submit_ul_common(ltephy_t* h, const float2* iq_host, const float2* iq
   if (!have_iq && h->n_ul != n) return fail(LTEPHY_ERROR_INVALID_INPUTS, "submit_ul: no IQ given and the previous call demodulated %u subframes, not %u", h->n_ul, n);
   CU(cudaSetDevice(h->cfg.device));
   const DevCell& c = h->dc;
-  if ((iq_host && h->d_uliq.reserve((size_t)h->cfg.max_subframes * c.sf_len)) || h->d_ulsym.reserve((size_t)h->cfg.max_subframes * 14 * c.nsc) ||
+  const size_t   A = c.ul_nof_rx; // samples and symbols are [n][A][..]: their offsets stay 64-bit (65 535 x 2 x 14 x 1200 x 8 bytes > 2^32)
+  if ((iq_host && h->d_uliq.reserve((size_t)h->cfg.max_subframes * A * c.sf_len)) || h->d_ulsym.reserve((size_t)h->cfg.max_subframes * A * 14 * c.nsc) ||
       h->d_ulpool.reserve((size_t)1 << 20))
     return fail(LTEPHY_ERROR, "device allocation failed");
   CU(cudaEventRecord(h->ev[2], h->stream));
   if (have_iq) { // NULL: the demodulated symbols of the previous call stay (srsran_enb_ul_fft once, then one decode per grant)
     if (iq_host) {
-      CU(cudaMemcpyAsync(h->d_uliq.p, iq_host, (size_t)n * c.sf_len * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
+      CU(cudaMemcpyAsync(h->d_uliq.p, iq_host, (size_t)n * A * c.sf_len * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
       iq_dev = h->d_uliq.p;
     }
     launch_ul_ofdm(c, iq_dev, h->d_ulsym.p, n, h->stream, &h->launches);
@@ -1308,7 +1311,7 @@ extern "C" int ltephy_tap(ltephy_t* h, int what, void* dst, size_t bytes)
     case LTEPHY_TAP_LLR: src = h->d_llr.p, avail = n * LLR_STRIDE * sizeof(float); break;
     case LTEPHY_TAP_PDSCH_LLR: src = h->d_pllr.p, avail = h->pb.pllr_elems * sizeof(short); break;
     case LTEPHY_TAP_TURBO_IN: src = h->d_turbo.p, avail = h->d_turbo.cap * 4; break;
-    case LTEPHY_TAP_UL_SYM: src = h->d_ulsym.p, avail = (size_t)h->n_ul * 14 * h->dc.nsc * sizeof(float2); break;
+    case LTEPHY_TAP_UL_SYM: src = h->d_ulsym.p, avail = (size_t)h->n_ul * h->dc.ul_nof_rx * 14 * h->dc.nsc * sizeof(float2); break;
     case LTEPHY_TAP_PBCH_LLR: src = h->pbch_frames ? h->d_pbch.p + 3 * 960 : nullptr, avail = (size_t)h->pbch_frames * 960 * sizeof(float); break;
     default: return fail(LTEPHY_ERROR_INVALID_INPUTS, "tap: unknown buffer");
   }

@@ -40,10 +40,11 @@ struct ltephy_track {
   std::unique_ptr<ltephy_sync_t, decltype(&ltephy_sync_destroy)> sync{nullptr, ltephy_sync_destroy};
   std::vector<ltephy_track_sf_t> sf;
   std::vector<ltephy_track_hf_t> hf;
-  // the uplink carrier (ltephy_track_set_ul): one antenna cut at start + ul_off with its own rotation tables
+  // the uplink carrier (ltephy_track_set_ul): ul_A antennas cut at start + ul_off with their own rotation tables
   bool             pushed = false, ul = false;
   double           ul_ratio = 1.0;
   int32_t          ul_off   = 0;
+  uint32_t         ul_A     = 1;
   DevBuf<float2>   d_xu, d_cutu, d_tabAu, d_tabBu;
   DevBuf<uint64_t> d_startu;
 };
@@ -330,11 +331,11 @@ static int track_run(ltephy_track_t* h, const float2* x, const float2* xu, uint6
     CU(cudaMemcpyAsync(h->d_tabB.p, tabB.data(), tabB.size() * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
     if (launch_track_cut(g, h->d_start.p, h->d_tabA.p, h->d_tabB.p, nsf, h->d_cut.p, h->stream))
       return fail(LTEPHY_ERROR, "track_push: cut kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
-    if (xu) { // the same kernel on the UL carrier: one antenna, start + ul_offset, the UL tables
+    if (xu) { // the same kernel on the UL carrier: its antennas, start + ul_offset, the UL tables
       std::vector<uint64_t> upos(nsf);
       for (uint32_t i = 0; i < nsf; i++) upos[i] = (uint64_t)((int64_t)spos[i] + h->ul_off);
       TrackArgs gu = g;
-      gu.x = xu, gu.A = 1;
+      gu.x = xu, gu.A = h->ul_A;
       CU(cudaMemcpyAsync(h->d_startu.p, upos.data(), nsf * sizeof(uint64_t), cudaMemcpyHostToDevice, h->stream));
       CU(cudaMemcpyAsync(h->d_tabAu.p, tabAu.data(), tabAu.size() * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
       CU(cudaMemcpyAsync(h->d_tabBu.p, tabBu.data(), tabBu.size() * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
@@ -389,11 +390,13 @@ extern "C" int ltephy_track_set_ul(ltephy_track_t* h, const ltephy_track_ul_cfg_
   if ((off < 0 ? -off : off) >= (int64_t)h->SF) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_set_ul: |ul_offset| %lld >= 15 N", (long long)off);
   if ((int64_t)h->cfg.frame_offset + off < 0)
     return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_set_ul: the first UL subframe would start before sample 0 (frame_offset + ul_offset < 0)");
+  if (cfg->nof_rx > 2) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_set_ul: nof_rx %u: 0 or 1 (one UL antenna) or 2", cfg->nof_rx);
+  const uint32_t A = cfg->nof_rx ? cfg->nof_rx : 1;
   CU(cudaSetDevice(h->cfg.device));
   const size_t nsf = h->cfg.max_subframes;
-  if (h->d_cutu.reserve(nsf * h->SF) || h->d_tabAu.reserve(nsf * (h->SF / 128)) || h->d_tabBu.reserve(nsf * 128) || h->d_startu.reserve(nsf))
+  if (h->d_cutu.reserve(nsf * A * h->SF) || h->d_tabAu.reserve(nsf * (h->SF / 128)) || h->d_tabBu.reserve(nsf * 128) || h->d_startu.reserve(nsf))
     return fail(LTEPHY_ERROR, "track_set_ul: device allocation failed");
-  h->ul = true, h->ul_ratio = cfg->cfo_ratio, h->ul_off = cfg->ul_offset;
+  h->ul = true, h->ul_ratio = cfg->cfo_ratio, h->ul_off = cfg->ul_offset, h->ul_A = A;
   return LTEPHY_SUCCESS;
 }
 
@@ -404,9 +407,10 @@ extern "C" int ltephy_track_push_ul(ltephy_track_t* h, const float* iq, const fl
   if (int r = track_check(h, iq, first_sample, nof_samples, out, true)) return r;
   CU(cudaSetDevice(h->cfg.device));
   if (nof_samples) {
-    if (h->d_x.reserve((size_t)h->A * nof_samples) || h->d_xu.reserve(nof_samples)) return fail(LTEPHY_ERROR, "track_push_ul: device allocation failed");
+    if (h->d_x.reserve((size_t)h->A * nof_samples) || h->d_xu.reserve((size_t)h->ul_A * nof_samples))
+      return fail(LTEPHY_ERROR, "track_push_ul: device allocation failed");
     CU(cudaMemcpyAsync(h->d_x.p, iq, (size_t)h->A * nof_samples * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
-    CU(cudaMemcpyAsync(h->d_xu.p, iq_ul, nof_samples * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
+    CU(cudaMemcpyAsync(h->d_xu.p, iq_ul, (size_t)h->ul_A * nof_samples * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
   }
   return track_run(h, h->d_x.p, h->d_xu.p, first_sample, nof_samples, out, ul_iq_dev);
 }

@@ -33,6 +33,7 @@ struct lteo_track {
   int      ul;       /* set: pushes go through lteo_track_push_ul */
   double   ul_ratio; /* f_UL / f_DL */
   int32_t  ul_off;   /* UL subframe start - DL subframe start */
+  uint32_t ul_A;     /* UL antennas */
 };
 
 static int track_symbol_ok(uint32_t N)
@@ -157,13 +158,14 @@ static void track_cut(lteo_track_t* t, const lteo_tcf_t* x, uint64_t lda, uint32
   }
 }
 
-int lteo_track_set_ul(lteo_track_t* t, double cfo_ratio, int32_t ul_offset)
+int lteo_track_set_ul_rx(lteo_track_t* t, double cfo_ratio, int32_t ul_offset, uint32_t nof_rx)
 {
-  if (!t || t->pushed || t->ul || !(cfo_ratio > 0.0 && cfo_ratio <= 2.0)) return -2;
+  if (!t || t->pushed || t->ul || !(cfo_ratio > 0.0 && cfo_ratio <= 2.0) || nof_rx > 2) return -2;
   if ((int64_t)(ul_offset < 0 ? -(int64_t)ul_offset : ul_offset) >= 15 * (int64_t)t->N || t->base + ul_offset < 0) return -2;
-  t->ul = 1, t->ul_ratio = cfo_ratio, t->ul_off = ul_offset;
+  t->ul = 1, t->ul_ratio = cfo_ratio, t->ul_off = ul_offset, t->ul_A = nof_rx ? nof_rx : 1;
   return 0;
 }
+int lteo_track_set_ul(lteo_track_t* t, double cfo_ratio, int32_t ul_offset) { return lteo_track_set_ul_rx(t, cfo_ratio, ul_offset, 1); }
 
 /* the lowest absolute sample the pending DL window, and with the uplink set its UL window, still needs; in the find state the window's start */
 static int64_t track_needed(const lteo_track_t* t)
@@ -234,8 +236,9 @@ static int track_push(lteo_track_t* t, const lteo_tcf_t* x, const lteo_tcf_t* xu
     o->flags  = (t->miss == 0 ? LTEO_TRACK_LOCKED : 0) | (t->miss >= LTEO_TRACK_MISS ? LTEO_TRACK_LOST : 0) | (t->reacq ? LTEO_TRACK_REACQUIRED : 0);
     t->reacq  = 0;
     if (cut) track_cut(t, x, n, t->A, t->f, s, cut + (uint64_t)ns * t->A * SF);
-    /* UL: one antenna at start + ul_offset, rotated by f_ul = (float)(f cfo_ratio) with the DL rule */
-    if (xu && cut_ul) track_cut(t, xu, n, 1, (float)((double)t->f * t->ul_ratio), (uint64_t)(t->s + t->ul_off) - first, cut_ul + (uint64_t)ns * SF);
+    /* UL: every UL antenna at start + ul_offset, rotated by f_ul = (float)(f cfo_ratio) with the DL rule */
+    if (xu && cut_ul)
+      track_cut(t, xu, n, t->ul_A, (float)((double)t->f * t->ul_ratio), (uint64_t)(t->s + t->ul_off) - first, cut_ul + (uint64_t)ns * t->ul_A * SF);
     ns++;
     int lost_now = 0;
     if (tti % 5 == 0) {

@@ -61,9 +61,13 @@ uint32_t lteo_track_finds(const lteo_track_t* t);
 /* the uplink carrier (ltephy_track_set_ul): before the first push, 0 < cfo_ratio <= 2, |ul_offset| < 15 N, frame_offset + ul_offset >= 0; 0 or -2.
  * After it lteo_track_push is refused and lteo_track_push_ul takes both carriers. */
 int lteo_track_set_ul(lteo_track_t* t, double cfo_ratio, int32_t ul_offset);
+/* the same with nof_rx UL antennas (0 or 1: one, 2: two; else -2): lteo_track_push_ul then takes x_ul [nof_rx][n] and writes cut_ul
+ * [k][nof_rx][15 N], every antenna cut and rotated as the one antenna is */
+int lteo_track_set_ul_rx(lteo_track_t* t, double cfo_ratio, int32_t ul_offset, uint32_t nof_rx);
 /* lteo_track_push with x_ul [n] (one antenna, the same absolute samples): a subframe is processed only when its DL window start .. start + 15 N - 1
  * and its UL window start + ul_offset .. start + ul_offset + 15 N - 1 both lie inside what was fed.  UL subframe k is x_ul from start_k + ul_offset,
- * rotated as the DL cut with f_ul = (float)(cfo_hz_k * cfo_ratio), into cut_ul [k][15 N] (may be NULL).  *next is the lower of start and
+ * rotated as the DL cut with f_ul = (float)(cfo_hz_k * cfo_ratio), into cut_ul [k][15 N] (may be NULL).  After lteo_track_set_ul_rx with nof_rx = 2,
+ * x_ul is [nof_rx][n], antenna-major, and cut_ul [k][nof_rx][15 N], every antenna cut and rotated as above.  *next is the lower of start and
  * start + ul_offset of the next subframe. */
 int lteo_track_push_ul(lteo_track_t* t, const lteo_tcf_t* x, const lteo_tcf_t* x_ul, uint64_t first, uint64_t n, uint32_t max_sf, lteo_track_sf_t* sf,
                        uint32_t* nsf, lteo_track_hf_t* hf, uint32_t* nhf, lteo_tcf_t* cut, lteo_tcf_t* cut_ul, uint64_t* next);

@@ -616,6 +616,13 @@ int lte_sim_subframe(lte_sim_t* s, uint32_t tti, cf_t* iq, lte_sim_truth_t* trut
 int lte_sim_ul_subframe(lte_sim_t* s, uint32_t tti, const lte_ul_cfg_t* ucfg, const lte_ul_grant_t* grants, uint32_t n, cf_t* iq, uint8_t* payload,
                         uint32_t* payload_off, uint32_t payload_cap)
 {
+  return lte_sim_ul_subframe_rx(s, tti, ucfg, grants, n, 1, iq, payload, payload_off, payload_cap);
+}
+
+int lte_sim_ul_subframe_rx(lte_sim_t* s, uint32_t tti, const lte_ul_cfg_t* ucfg, const lte_ul_grant_t* grants, uint32_t n, uint32_t nof_rx, cf_t* iq,
+                           uint8_t* payload, uint32_t* payload_off, uint32_t payload_cap)
+{
+  if (nof_rx < 1 || nof_rx > LTE_MAX_ANT) return -5;
   const lte_cell_t* cell = &s->cfg.cell;
   const uint32_t    sf_idx = tti % 10, nsc = s->nsc, N = s->fft;
   lte_rng_t         rng;
@@ -750,17 +757,21 @@ int lte_sim_ul_subframe(lte_sim_t* s, uint32_t tti, const lte_ul_cfg_t* ucfg, co
       s->td[0][pos++] = (cf_t){(float)(re * scl), (float)(im * scl)};
     }
   }
+  /* antenna a: port 0's gain and delay towards it, and its own noise, drawn after antenna a - 1's */
   double sigma = pow(10.0, -s->cfg.snr_db / 20.0) * M_SQRT1_2;
-  float  hr = s->h_re[0][0], hi = s->h_im[0][0];
-  uint32_t dl = s->delay[0][0];
-  for (uint32_t i = 0; i < s->sf_len; i++) {
-    double re = sigma * lte_rng_gauss(&rng), im = sigma * lte_rng_gauss(&rng);
-    if (i >= dl) {
-      cf_t x = s->td[0][i - dl];
-      re += (double)hr * x.re - (double)hi * x.im;
-      im += (double)hr * x.im + (double)hi * x.re;
+  for (uint32_t a = 0; a < nof_rx; a++) {
+    const float    hr = s->h_re[a][0], hi = s->h_im[a][0];
+    const uint32_t dl = s->delay[a][0];
+    cf_t*          out = iq + (size_t)a * s->sf_len;
+    for (uint32_t i = 0; i < s->sf_len; i++) {
+      double re = sigma * lte_rng_gauss(&rng), im = sigma * lte_rng_gauss(&rng);
+      if (i >= dl) {
+        cf_t x = s->td[0][i - dl];
+        re += (double)hr * x.re - (double)hi * x.im;
+        im += (double)hr * x.im + (double)hi * x.re;
+      }
+      out[i] = (cf_t){(float)re, (float)im};
     }
-    iq[i] = (cf_t){(float)re, (float)im};
   }
   return 0;
 }

@@ -85,6 +85,10 @@ extern "C" {
 #endif
 int lte_sim_ul_subframe(lte_sim_t* s, uint32_t tti, const lte_ul_cfg_t* ucfg, const lte_ul_grant_t* grants, uint32_t n, cf_t* iq /* [sf_len] */,
                         uint8_t* payload, uint32_t* payload_off, uint32_t payload_cap);
+/* the same subframe received on nof_rx (1..LTE_MAX_ANT) antennas, iq [nof_rx][sf_len]: antenna a sees port 0's channel towards it (gain
+ * h[a][0], delay[a][0]) and its own noise, drawn after antenna a - 1's, so antenna 0 equals lte_sim_ul_subframe's output */
+int lte_sim_ul_subframe_rx(lte_sim_t* s, uint32_t tti, const lte_ul_cfg_t* ucfg, const lte_ul_grant_t* grants, uint32_t n, uint32_t nof_rx,
+                           cf_t* iq /* [nof_rx][sf_len] */, uint8_t* payload, uint32_t* payload_off, uint32_t payload_cap);
 #ifdef __cplusplus
 }
 #endif
