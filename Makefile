@@ -38,7 +38,7 @@ oracle/liblteochanpoly.so: oracle/lte_chan_poly_oracle.c oracle/lte_chan_poly_or
 	$(CC) $(CFLAGS) -shared -o $@ oracle/lte_chan_poly_oracle.c -Loracle -llteochan -Wl,-rpath,'$$ORIGIN' -lm
 
 # C++ example of the C-ABI (needs ltesniffer_b200/libltephy_b200.so, built by ltesniffer_b200/build.py)
-examples/offline_decode: examples/offline_decode.cpp include/ltephy_b200.h include/ltephy_search.h include/ltephy_sinks.h
+examples/offline_decode: examples/offline_decode.cpp examples/cell_chain.h include/ltephy_b200.h include/ltephy_search.h include/ltephy_sinks.h
 	$(CXX) -O2 -std=c++17 -Wall -Iinclude -o $@ examples/offline_decode.cpp -Lltesniffer_b200 -lltephy_b200 -Wl,-rpath,'$$ORIGIN/../ltesniffer_b200'
 
 examples/offline_ul: examples/offline_ul.cpp examples/cell_chain.h include/ltephy_b200.h include/ltephy_search.h include/ltephy_sinks.h

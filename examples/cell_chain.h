@@ -13,27 +13,55 @@
 #include <algorithm>
 #include <cstdio>
 #include <cstdlib>
+#include <cstring>
 #include <vector>
 
-// samples [s, s + n) of every antenna, antenna-major, from a file holding L samples per antenna
-static inline bool read_span(FILE* f, uint32_t A, uint64_t L, uint64_t s, uint64_t n, std::vector<float>& out)
+// bytes of one complex sample of an LTEPHY_IQ_* format
+static inline uint32_t chain_sample_bytes(uint32_t fmt) { return fmt == LTEPHY_IQ_SC16 ? 4 : fmt == LTEPHY_IQ_SC8 ? 2 : 8; }
+
+// removes every "fmt=cf32|sc16|sc8" argument from argv (the sample format of the input files, LTEPHY_IQ_*; cf32 without one), so that the
+// positional arguments keep their places.  0, or 2 for an unknown format (message printed)
+static inline int chain_take_fmt(int& argc, char** argv, uint32_t* fmt)
 {
-  out.resize((size_t)2 * A * n);
+  *fmt  = LTEPHY_IQ_CF32;
+  int o = 1;
+  for (int i = 1; i < argc; i++) {
+    if (strncmp(argv[i], "fmt=", 4)) {
+      argv[o++] = argv[i];
+      continue;
+    }
+    const char* f = argv[i] + 4;
+    if (!strcmp(f, "cf32")) *fmt = LTEPHY_IQ_CF32;
+    else if (!strcmp(f, "sc16")) *fmt = LTEPHY_IQ_SC16;
+    else if (!strcmp(f, "sc8")) *fmt = LTEPHY_IQ_SC8;
+    else {
+      fprintf(stderr, "unknown %s (fmt=cf32, sc16 or sc8)\n", argv[i]);
+      return 2;
+    }
+  }
+  argc = o;
+  return 0;
+}
+
+// samples [s, s + n) of every antenna, antenna-major, b bytes per complex sample, from a file holding L samples per antenna
+static inline bool read_span(FILE* f, uint32_t A, uint64_t L, uint32_t b, uint64_t s, uint64_t n, std::vector<uint8_t>& out)
+{
+  out.resize((size_t)b * A * n);
   for (uint32_t a = 0; a < A; a++) {
-    if (fseeko(f, (off_t)(8 * ((uint64_t)a * L + s)), SEEK_SET) != 0) return false;
-    if (fread(out.data() + (size_t)2 * a * n, 8, n, f) != n) return false;
+    if (fseeko(f, (off_t)(b * ((uint64_t)a * L + s)), SEEK_SET) != 0) return false;
+    if (fread(out.data() + (size_t)b * a * n, b, n, f) != n) return false;
   }
   return true;
 }
 
-// the MIB, soft-combined over nframes subframes 0 (cf32 [nframes][A][15 N], host memory, subframe 0 of frame f at tti 10 f) with the carrier
-// offset cfo_hz corrected and the port count searched; mib->sfn is that of frame 0.  0, 1 on a library error, 3 when no MIB passed
-static inline int chain_mib_host(const float* sf0, uint32_t nframes, uint32_t pci, float cfo_hz, uint32_t N, uint32_t A, ltephy_mib_t* mib)
+// the MIB, soft-combined over nframes subframes 0 ([nframes][A][15 N] samples of format fmt, host memory, subframe 0 of frame f at tti 10 f) with
+// the carrier offset cfo_hz corrected and the port count searched; mib->sfn is that of frame 0.  0, 1 on a library error, 3 when no MIB passed
+static inline int chain_mib_host(const void* sf0, uint32_t nframes, uint32_t pci, float cfo_hz, uint32_t N, uint32_t A, uint32_t fmt, ltephy_mib_t* mib)
 {
   std::vector<uint32_t> tti0(nframes);
   for (uint32_t f = 0; f < nframes; f++) tti0[f] = 10 * f;
   ltephy_cfg_t mcfg{};
-  mcfg.nof_prb = 15, mcfg.nof_ports = 2, mcfg.cell_id = pci, mcfg.nof_rx = A, mcfg.max_subframes = nframes, mcfg.symbol_sz = N;
+  mcfg.nof_prb = 15, mcfg.nof_ports = 2, mcfg.cell_id = pci, mcfg.nof_rx = A, mcfg.max_subframes = nframes, mcfg.symbol_sz = N, mcfg.iq_format = fmt;
   ltephy_t*                      mphy = nullptr;
   std::vector<ltephy_mib_comb_t> m(nframes);
   if (ltephy_create(&mcfg, &mphy) != LTEPHY_SUCCESS || ltephy_set_cfo(mphy, cfo_hz) != LTEPHY_SUCCESS ||
@@ -56,19 +84,19 @@ static inline int chain_mib_host(const float* sf0, uint32_t nframes, uint32_t pc
   return 0;
 }
 
-// the cell of samples [0, L0) of an antenna-major file of L samples per antenna: the cell search there, the first cell it detects, and that cell's
-// MIB soft-combined over the subframes 0 of every whole frame in those samples (chain_mib_host).  0, 1 on a read or library error, 3 when no cell
-// is found, no whole frame follows its first subframe 0 or no MIB passed (message printed)
-static inline int chain_acquire(FILE* f, uint32_t N, uint32_t A, uint64_t L, uint64_t L0, ltephy_cell_t* cell, ltephy_mib_t* mib)
+// the cell of samples [0, L0) of an antenna-major file of L samples per antenna in format fmt: the cell search there, the first cell it detects, and
+// that cell's MIB soft-combined over the subframes 0 of every whole frame in those samples (chain_mib_host).  0, 1 on a read or library error, 3 when
+// no cell is found, no whole frame follows its first subframe 0 or no MIB passed (message printed)
+static inline int chain_acquire(FILE* f, uint32_t N, uint32_t A, uint64_t L, uint64_t L0, uint32_t fmt, ltephy_cell_t* cell, ltephy_mib_t* mib)
 {
-  const uint32_t     SF = 15 * N;
-  std::vector<float> x;
-  if (!read_span(f, A, L, 0, L0, x)) {
+  const uint32_t       SF = 15 * N, b = chain_sample_bytes(fmt);
+  std::vector<uint8_t> x;
+  if (!read_span(f, A, L, b, 0, L0, x)) {
     fprintf(stderr, "short read\n");
     return 1;
   }
   ltephy_sync_cfg_t scfg{};
-  scfg.symbol_sz = N, scfg.nof_rx = A, scfg.max_samples = L0;
+  scfg.symbol_sz = N, scfg.nof_rx = A, scfg.max_samples = L0, scfg.iq_format = fmt;
   ltephy_sync_t* sync = nullptr;
   ltephy_cell_t  cells[3];
   if (ltephy_sync_create(&scfg, &sync) != LTEPHY_SUCCESS) {
@@ -92,11 +120,11 @@ static inline int chain_acquire(FILE* f, uint32_t N, uint32_t A, uint64_t L, uin
     fprintf(stderr, "no whole frame after the first subframe 0\n");
     return 3;
   }
-  std::vector<float> sf0((size_t)2 * A * SF * nframes); // subframe 0 of each frame, antenna after antenna
+  std::vector<uint8_t> sf0((size_t)b * A * SF * nframes); // subframe 0 of each frame, antenna after antenna
   for (uint32_t f = 0; f < nframes; f++)
     for (uint32_t a = 0; a < A; a++)
-      std::copy_n(x.data() + 2 * (a * L0 + c->frame_offset + (uint64_t)f * 10 * SF), 2 * SF, sf0.data() + 2 * ((size_t)f * A + a) * SF);
-  return chain_mib_host(sf0.data(), nframes, c->pci, c->cfo_hz, N, A, mib);
+      std::copy_n(x.data() + b * (a * L0 + c->frame_offset + (uint64_t)f * 10 * SF), (size_t)b * SF, sf0.data() + (size_t)b * ((size_t)f * A + a) * SF);
+  return chain_mib_host(sf0.data(), nframes, c->pci, c->cfo_hz, N, A, fmt, mib);
 }
 
 static inline void chain_print_cell(const ltephy_cell_t& c, const ltephy_mib_t& mib)
@@ -304,15 +332,15 @@ struct UlChain {
     return 0;
   }
 
-  // one batch of got subframes at ttis[0, got): downlink cf32 [got][15 N] of one antenna and uplink cf32 [got][A][15 N] of A = cfg.ul_nof_rx
-  // antennas (one when 0), in host memory or, with on_device, in device memory (a tracker's cuts).  0 or 1 (error printed)
+  // one batch of got subframes at ttis[0, got): downlink [got][15 N] of one antenna and uplink [got][A][15 N] of A = cfg.ul_nof_rx antennas (one
+  // when 0), samples of cfg.iq_format, in host memory or, with on_device, in device memory (a tracker's cuts, cf32).  0 or 1 (error printed)
   int step(const void* dl_iq, const void* ul_iq, bool on_device, uint32_t got)
   {
     uint32_t  nd = 0;
     const int rd = on_device ? ltephy_decode_subframes_device(dl, search, dl_iq, ttis.data(), got, LTEPHY_SEQ_NONE, info.data(), scratch.data(), dcis.data(),
                                                               max_dcis, &nd, tbs.data(), payload.data(), payload.size())
-                             : ltephy_decode_subframes(dl, search, static_cast<const float*>(dl_iq), ttis.data(), got, LTEPHY_SEQ_NONE, info.data(),
-                                                       scratch.data(), dcis.data(), max_dcis, &nd, tbs.data(), payload.data(), payload.size());
+                             : ltephy_decode_subframes(dl, search, dl_iq, ttis.data(), got, LTEPHY_SEQ_NONE, info.data(), scratch.data(), dcis.data(),
+                                                       max_dcis, &nd, tbs.data(), payload.data(), payload.size());
     if (rd != LTEPHY_SUCCESS) {
       fprintf(stderr, "%s: %s\n", on_device ? "ltephy_decode_subframes_device" : "ltephy_decode_subframes", ltephy_last_error());
       return 1;
@@ -357,7 +385,7 @@ struct UlChain {
     if (!now.empty()) {
       if (now.size() > max_ul) now.resize(max_ul);
       const int ru = on_device ? ltephy_submit_ul_device(ul, ul_iq, ttis.data(), got, now.data(), (uint32_t)now.size())
-                               : ltephy_submit_ul(ul, static_cast<const float*>(ul_iq), ttis.data(), got, now.data(), (uint32_t)now.size());
+                               : ltephy_submit_ul(ul, ul_iq, ttis.data(), got, now.data(), (uint32_t)now.size());
       if (ru != LTEPHY_SUCCESS || ltephy_get_ul(ul, ures.data(), chest.data(), upayload.data(), upayload.size()) != LTEPHY_SUCCESS) {
         fprintf(stderr, "uplink decode: %s\n", ltephy_last_error());
         return 1;

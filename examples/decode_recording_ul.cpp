@@ -11,20 +11,23 @@
 //   5. those grants decoded with ltephy_submit_ul_device on the uplink cut (3 to 5: UlChain of cell_chain.h, as in offline_ul);
 // and one summary line.  Writes a MAC-LTE pcap with both directions.  Host code only; without a GPU ltephy_sync_create fails.
 //
-//   decode_recording_ul <dl.cf32> <ul.cf32> <symbol_sz> <out.pcap> [cfo_ratio=1] [ul_offset=0] [cyclic_shift=0] [group_assignment=0]
-//                       [hopping_offset=0] [ul_rx=1]
+//   decode_recording_ul <dl file> <ul file> <symbol_sz> <out.pcap> [cfo_ratio=1] [ul_offset=0] [cyclic_shift=0] [group_assignment=0]
+//                       [hopping_offset=0] [ul_rx=1] [fmt=cf32|sc16|sc8]
 //
 // cfo_ratio = f_UL / f_DL scales the tracked carrier offset for the uplink (1 applies the downlink's, as srsRAN does); ul_offset is the number of
 // samples the uplink subframe starts after the downlink one.  cyclic_shift / group_assignment / hopping_offset are SIB2's values, as for offline_ul.
-// ul_rx (1 or 2) is the number of uplink antennas in <ul.cf32>.
+// ul_rx (1 or 2) is the number of uplink antennas in <ul file>.  fmt is the sample format of both files: complex float32 (the default) or int16 /
+// int8 I/Q pairs, which the search and the tracker take as they are (the cuts the decoders read are cf32).
 #include "cell_chain.h"
 
 static const uint32_t B = 200; // subframes per push
 
 int main(int argc, char** argv)
 {
+  uint32_t fmt = LTEPHY_IQ_CF32;
+  if (int r = chain_take_fmt(argc, argv, &fmt)) return r;
   if (argc < 5) {
-    fprintf(stderr, "usage: %s <dl.cf32> <ul.cf32> <symbol_sz> <out.pcap> [cfo_ratio=1] [ul_offset=0] [cyclic_shift] [group_assignment] [hopping_offset] [ul_rx=1]\n",
+    fprintf(stderr, "usage: %s <dl file> <ul file> <symbol_sz> <out.pcap> [cfo_ratio=1] [ul_offset=0] [cyclic_shift] [group_assignment] [hopping_offset] [ul_rx=1] [fmt=cf32|sc16|sc8]\n",
             argv[0]);
     return 2;
   }
@@ -43,12 +46,13 @@ int main(int argc, char** argv)
     return 2;
   }
   fseeko(fd, 0, SEEK_END), fseeko(fu, 0, SEEK_END);
-  const uint64_t Ld = (uint64_t)ftello(fd) / 8, Lu = (uint64_t)ftello(fu) / 8 / ul_rx, L = Ld < Lu ? Ld : Lu; // Lu: samples per UL antenna
+  const uint32_t b  = chain_sample_bytes(fmt);
+  const uint64_t Ld = (uint64_t)ftello(fd) / b, Lu = (uint64_t)ftello(fu) / b / ul_rx, L = Ld < Lu ? Ld : Lu; // Lu: samples per UL antenna
 
   // 1. cell search and the MIB on the first 40 ms of the downlink
   ltephy_cell_t c{};
   ltephy_mib_t  mib{};
-  if (int r = chain_acquire(fd, N, 1, Ld, L < 40ull * SF ? L : 40ull * SF, &c, &mib)) return r;
+  if (int r = chain_acquire(fd, N, 1, Ld, L < 40ull * SF ? L : 40ull * SF, fmt, &c, &mib)) return r;
   chain_print_cell(c, mib);
 
   // 2. decoders, DCI search in UL mode and the tracker with the uplink; the tracking starts at the first subframe whose UL window is recorded
@@ -63,7 +67,7 @@ int main(int argc, char** argv)
   while ((int64_t)fo + ul_offset < 0) fo += SF, tti = (tti + 1) % 10240;
   ltephy_track_cfg_t tcfg{};
   tcfg.symbol_sz = N, tcfg.nof_rx = 1, tcfg.pci = c.pci, tcfg.first_tti = tti, tcfg.frame_offset = fo, tcfg.cfo_hz = c.cfo_hz;
-  tcfg.max_ppm = 50.0f, tcfg.max_subframes = B;
+  tcfg.max_ppm = 50.0f, tcfg.max_subframes = B, tcfg.iq_format = fmt;
   ltephy_track_ul_cfg_t tul{};
   tul.cfo_ratio = cfo_ratio, tul.ul_offset = ul_offset, tul.nof_rx = ul_rx; // the UL cut is [got][ul_rx][15 N], what the UL decoder of cfg takes
   ltephy_track_t* tr = nullptr;
@@ -72,16 +76,16 @@ int main(int argc, char** argv)
     return 1;
   }
   // 3. the recordings arrive B subframes at a time; each push re-feeds both from the tracker's next_sample
-  std::vector<float> x, xu;
-  unsigned long long n_lost = 0;
-  uint64_t           recv = 0, next = (int64_t)fo + ul_offset < (int64_t)fo ? fo + ul_offset : fo;
+  std::vector<uint8_t> x, xu;
+  unsigned long long   n_lost = 0;
+  uint64_t             recv = 0, next = (int64_t)fo + ul_offset < (int64_t)fo ? fo + ul_offset : fo;
   for (;;) {
     if (recv < L) recv = recv + (uint64_t)B * SF < L ? recv + (uint64_t)B * SF : L;
     if (next >= recv) {
       if (recv == L) break;
       continue;
     }
-    if (!read_span(fd, 1, Ld, next, recv - next, x) || !read_span(fu, ul_rx, Lu, next, recv - next, xu)) {
+    if (!read_span(fd, 1, Ld, b, next, recv - next, x) || !read_span(fu, ul_rx, Lu, b, next, recv - next, xu)) {
       fprintf(stderr, "short read\n");
       return 1;
     }

@@ -18,17 +18,6 @@
 #include <cstring>
 #include <string>
 
-// samples s .. s + n - 1 of every antenna of an antenna-major file of L samples per antenna, b bytes per complex sample, into out
-static bool read_span_fmt(FILE* f, uint32_t A, uint64_t L, uint32_t b, uint64_t s, uint64_t n, std::vector<uint8_t>& out)
-{
-  out.resize((size_t)b * A * n);
-  for (uint32_t a = 0; a < A; a++) {
-    if (fseeko(f, (off_t)(b * ((uint64_t)a * L + s)), SEEK_SET) != 0) return false;
-    if (fread(out.data() + (size_t)b * a * n, b, n, f) != n) return false;
-  }
-  return true;
-}
-
 struct Carrier {
   int32_t         offset_hz = 0;
   uint32_t        N = 0, SF = 0;
@@ -44,6 +33,8 @@ struct Carrier {
 
 int main(int argc, char** argv)
 {
+  uint32_t fmt = LTEPHY_IQ_CF32;
+  if (int r = chain_take_fmt(argc, argv, &fmt)) return r;
   if (argc < 6) {
     fprintf(stderr, "usage: %s <iq file> <fs_in> <nof_rx> <out_prefix> <offset_hz>:<N> [<offset_hz>:<N> ...] [subframes_per_push=500] [fmt=cf32|sc16|sc8]\n",
             argv[0]);
@@ -52,19 +43,8 @@ int main(int argc, char** argv)
   const uint32_t       fs = (uint32_t)strtoul(argv[2], nullptr, 10), A = (uint32_t)atoi(argv[3]);
   const std::string    prefix = argv[4];
   std::vector<Carrier> car;
-  uint32_t             B = 500, fmt = LTEPHY_IQ_CF32;
+  uint32_t             B = 500;
   for (int i = 5; i < argc; i++) {
-    if (!strncmp(argv[i], "fmt=", 4)) {
-      const char* f = argv[i] + 4;
-      if (!strcmp(f, "cf32")) fmt = LTEPHY_IQ_CF32;
-      else if (!strcmp(f, "sc16")) fmt = LTEPHY_IQ_SC16;
-      else if (!strcmp(f, "sc8")) fmt = LTEPHY_IQ_SC8;
-      else {
-        fprintf(stderr, "unknown %s\n", argv[i]);
-        return 2;
-      }
-      continue;
-    }
     const char* colon = strchr(argv[i], ':');
     if (!colon) {
       B = (uint32_t)atoi(argv[i]);
@@ -79,7 +59,7 @@ int main(int argc, char** argv)
     fprintf(stderr, "cannot open %s / bad nof_rx, carriers, fs_in or subframes_per_push\n", argv[1]);
     return 2;
   }
-  const uint32_t bps = fmt == LTEPHY_IQ_SC16 ? 4 : fmt == LTEPHY_IQ_SC8 ? 2 : 8; // bytes per complex sample
+  const uint32_t bps = chain_sample_bytes(fmt);
   fseeko(in, 0, SEEK_END);
   const uint64_t L  = (uint64_t)ftello(in) / ((uint64_t)bps * A);
   const uint64_t MS = fs / 1000; // capture samples per ms
@@ -107,7 +87,7 @@ int main(int argc, char** argv)
   std::vector<uint8_t>           x;
   std::vector<ltephy_chan_out_t> out(car.size());
   uint64_t                       nx = 0;
-  if (!read_span_fmt(in, A, L, bps, 0, L0, x)) {
+  if (!read_span(in, A, L, bps, 0, L0, x)) {
     fprintf(stderr, "short read\n");
     return 1;
   }
@@ -170,7 +150,7 @@ int main(int argc, char** argv)
       continue;
     }
     const uint64_t end = std::min(recv, first + span);
-    if (!read_span_fmt(in, A, L, bps, first, end - first, x)) {
+    if (!read_span(in, A, L, bps, first, end - first, x)) {
       fprintf(stderr, "short read\n");
       return 1;
     }

@@ -1,22 +1,21 @@
 // offline_decode.cpp -- the reference's offline mode (LTESniffer -i file.cf32: src/src/LTESniffer_Core.cc:365-444 feeding
 // SubframeWorker::work, results to LTESniffer_pcap_writer and DCIToFile) written against the C-ABI of libltephy_b200 from C++,
-// the way a maintainer would call it: read a cf32 capture in batches, ltephy_decode_subframes, write the MAC-LTE pcap and the
+// the way a maintainer would call it: read a capture in batches, ltephy_decode_subframes, write the MAC-LTE pcap and the
 // DCI trace.  Host code only; every computation happens in the library (there is no CPU fallback: without a GPU ltephy_create fails).
 //
 //   offline_decode <iq.cf32> <nof_prb> <nof_ports> <cell_id> <nof_rx> <out.pcap> <out_dci.tsv> [batch=500] [first_tti=0] [speculate_256qam=0]
 //                  [phich_resources=0] [phich_length=0]      (the MIB's PHICH configuration; the reference's file mode presets 1/6, normal)
+//                  [fmt=cf32|sc16|sc8]
 //
-// File layout: subframe after subframe, antenna after antenna, lte sf_len complex float32 samples each (what
-// srsran_filesource_read_multi hands SubframeWorker, src/src/SubframeWorker.cc:89).
-#include "ltephy_b200.h"
-#include "ltephy_search.h"
-#include "ltephy_sinks.h"
-#include <cstdio>
-#include <cstdlib>
-#include <vector>
+// File layout: subframe after subframe, antenna after antenna, lte sf_len complex samples each (what srsran_filesource_read_multi hands
+// SubframeWorker, src/src/SubframeWorker.cc:89): float32 (cf32, the default) or int16 / int8 I/Q pairs (sc16 / sc8), handed to the library as
+// read, so the host-to-device copy moves a half or a quarter of the bytes.
+#include "cell_chain.h"
 
 int main(int argc, char** argv)
 {
+  uint32_t fmt = LTEPHY_IQ_CF32;
+  if (int r = chain_take_fmt(argc, argv, &fmt)) return r;
   if (argc < 8) {
     fprintf(stderr, "usage: %s <iq.cf32> <nof_prb> <nof_ports> <cell_id> <nof_rx> <out.pcap> <out_dci.tsv> [batch] [first_tti] [speculate_256qam]\n", argv[0]);
     return 2;
@@ -27,7 +26,7 @@ int main(int argc, char** argv)
   const uint32_t B         = argc > 8 ? (uint32_t)atoi(argv[8]) : 500;
   uint32_t       tti       = argc > 9 ? (uint32_t)atoi(argv[9]) : 0;
   const int      speculate = argc > 10 ? atoi(argv[10]) : 0;
-  cfg.max_subframes = B, cfg.turbo_max_iter = 8, cfg.flags = LTEPHY_FLAG_SKIP_LOW_POWER;
+  cfg.max_subframes = B, cfg.turbo_max_iter = 8, cfg.flags = LTEPHY_FLAG_SKIP_LOW_POWER, cfg.iq_format = fmt;
   cfg.phich_resources = argc > 11 ? (uint32_t)atoi(argv[11]) : 0, cfg.phich_length = argc > 12 ? (uint32_t)atoi(argv[12]) : 0;
 
   ltephy_t* phy = nullptr;
@@ -44,9 +43,9 @@ int main(int argc, char** argv)
     fprintf(stderr, "cannot open inputs / outputs\n");
     return 1;
   }
-  const size_t sf_floats = (size_t)2 * cfg.nof_rx * ltephy_sf_len(phy);
+  const size_t sf_bytes = (size_t)chain_sample_bytes(fmt) * cfg.nof_rx * ltephy_sf_len(phy);
   const uint32_t max_dcis = 32 * B;
-  std::vector<float>               iq(sf_floats * B);
+  std::vector<uint8_t>             iq(sf_bytes * B);
   std::vector<uint32_t>            ttis(B);
   std::vector<ltephy_sf_info_t>    info(B);
   std::vector<ltephy_cand_t>       scratch((size_t)B * LTEPHY_MAX_LOC * LTEPHY_MAX_SIZES);
@@ -56,7 +55,7 @@ int main(int argc, char** argv)
   unsigned long long n_sf = 0, n_dci = 0, n_tb = 0, n_ok = 0;
   char               line[256];
   for (;;) {
-    const size_t got = fread(iq.data(), sizeof(float) * sf_floats, B, in);
+    const size_t got = fread(iq.data(), sf_bytes, B, in);
     if (!got) break;
     for (size_t i = 0; i < got; i++) ttis[i] = (tti + (uint32_t)i) % 10240;
     uint32_t nd = 0;

@@ -41,6 +41,13 @@ extern "C" {
 
 typedef struct ltephy ltephy_t;
 
+/* Sample formats of a narrowband or wideband input: interleaved I/Q, converted to float exactly where the kernels load them, so a run on integer
+ * samples equals the cf32 run on value * 2^-15 (sc16) or value * 2^-7 (sc8) bit for bit (DESIGN.md §2 "integer samples").  Outputs -- the
+ * tracker's cut, the channeliser's carrier streams -- are always cf32: a decode or search handle fed from them keeps iq_format = 0. */
+#define LTEPHY_IQ_CF32 0u /* float32 */
+#define LTEPHY_IQ_SC16 1u /* int16, value * 2^-15 */
+#define LTEPHY_IQ_SC8 2u  /* int8, value * 2^-7 */
+
 typedef struct {
   uint32_t nof_prb;        /* 15..100 (control region needs > 10) */
   uint32_t nof_ports;      /* CRS ports 1|2 */
@@ -64,7 +71,9 @@ typedef struct {
   uint32_t ul_nof_rx;       /* receive antennas of the uplink carrier: 0 or 1 one antenna, 2 two (PUSCH combined over both, DESIGN.md §2 "uplink
                                receive diversity"); any other value is INVALID_INPUTS.  Sets the shape of ltephy_submit_ul / _device and
                                LTEPHY_TAP_UL_SYM. */
-  uint32_t reserved[3];
+  uint32_t iq_format;       /* LTEPHY_IQ_CF32 (0), LTEPHY_IQ_SC16 or LTEPHY_IQ_SC8: the sample type of ltephy_submit_iq / _device and ltephy_submit_ul /
+                               _device (and so of ltephy_decode_subframes*); any other value is INVALID_INPUTS */
+  uint32_t reserved[2];
 } ltephy_cfg_t;
 
 #define LTEPHY_FLAG_SKIP_LOW_POWER 1u /* do not decode locations covering a CCE with mean|LLR| < 0.7 (they are never consulted) */
@@ -174,7 +183,7 @@ void ltephy_destroy(ltephy_t* h);
 const char* ltephy_last_error(void);
 
 /* static geometry queries (host only) */
-uint32_t ltephy_sf_len(const ltephy_t* h);                          /* cf32 samples per antenna-subframe */
+uint32_t ltephy_sf_len(const ltephy_t* h);                          /* complex samples per antenna-subframe (of the handle's iq_format) */
 uint32_t ltephy_nof_cce(const ltephy_t* h, uint32_t cfi);
 uint32_t ltephy_nof_sizes(const ltephy_t* h);                       /* distinct DCI payload sizes */
 uint32_t ltephy_dci_size(const ltephy_t* h, uint32_t format);       /* srsran_dci_format_sizeof */
@@ -182,10 +191,11 @@ uint32_t ltephy_size_index(const ltephy_t* h, uint32_t format);     /* format ->
 uint32_t ltephy_locations(const ltephy_t* h, uint32_t cfi, uint16_t* ncce, uint8_t* L, uint32_t max); /* falcon_pdcch.c:321-356 */
 
 /* ---- phase A ------------------------------------------------------------------------------ */
-/* iq: n * nof_rx * sf_len cf32 (interleaved re,im), subframe-major then antenna; host memory
+/* iq: n * nof_rx * sf_len samples in the handle's iq_format (interleaved re,im), subframe-major then antenna; host memory
  * (pinned memory makes the copy asynchronous).  tti[i] = 10*sfn + sf_idx.  Asynchronous. */
-int ltephy_submit_iq(ltephy_t* h, const float* iq, const uint32_t* tti, uint32_t n);
-/* same, but iq already lives in device memory (used to time the kernels alone) */
+int ltephy_submit_iq(ltephy_t* h, const void* iq, const uint32_t* tti, uint32_t n);
+/* same, but iq already lives in device memory (used to time the kernels alone); INVALID_INPUTS for integer samples whose pointer is not aligned
+ * to the sample (4 bytes sc16, 2 bytes sc8) */
 int ltephy_submit_iq_device(ltephy_t* h, const void* iq_dev, const uint32_t* tti, uint32_t n);
 /* blocks until phase A of the current batch is done and copies its results to the host:
  * info[n], cands[n][LTEPHY_MAX_LOC][LTEPHY_MAX_SIZES] */
@@ -267,7 +277,8 @@ typedef struct {
   uint32_t nof_rx;      /* 1 or 2 antennas */
   uint64_t max_samples; /* longest recording per antenna this handle accepts (device memory is sized for it) */
   int32_t  device;      /* CUDA device ordinal */
-  uint32_t reserved[4];
+  uint32_t iq_format;   /* LTEPHY_IQ_*: the sample type of ltephy_cell_search / _device; any other value is INVALID_INPUTS */
+  uint32_t reserved[3];
 } ltephy_sync_cfg_t;
 typedef struct {
   uint8_t  detected;        /* psr >= 2.5 and sss_ratio >= 1.75 */
@@ -283,10 +294,10 @@ typedef struct {
 } ltephy_cell_t;
 int  ltephy_sync_create(const ltephy_sync_cfg_t* cfg, ltephy_sync_t** h);
 void ltephy_sync_destroy(ltephy_sync_t* h);
-/* iq: cf32 [nof_rx][nof_samples], antenna-major, host memory; HF + N <= nof_samples <= max_samples (HF = 75 N, 5 ms).  out[3]: one result per
- * N_ID_2, by pss_peak descending, ties to the lower N_ID_2.  Blocks until done. */
-int  ltephy_cell_search(ltephy_sync_t* h, const float* iq, uint64_t nof_samples, ltephy_cell_t out[3]);
-/* same, with the samples already in device memory */
+/* iq: [nof_rx][nof_samples] samples in the handle's iq_format, antenna-major, host memory; HF + N <= nof_samples <= max_samples (HF = 75 N, 5 ms).
+ * out[3]: one result per N_ID_2, by pss_peak descending, ties to the lower N_ID_2.  Blocks until done. */
+int  ltephy_cell_search(ltephy_sync_t* h, const void* iq, uint64_t nof_samples, ltephy_cell_t out[3]);
+/* same, with the samples already in device memory (integer samples aligned to the sample) */
 int  ltephy_cell_search_device(ltephy_sync_t* h, const void* iq_dev, uint64_t nof_samples, ltephy_cell_t out[3]);
 enum {
   LTEPHY_SYNC_TAP_COARSE  = 0, /* f32 [3][9600]       folded coarse metric per N_ID_2 */
@@ -320,7 +331,8 @@ typedef struct {
   uint32_t max_subframes; /* most subframes one push cuts (device memory is sized for it) */
   uint32_t flags;         /* LTEPHY_TRACK_* */
   int32_t  device;        /* CUDA device ordinal */
-  uint32_t reserved[5];
+  uint32_t iq_format;     /* LTEPHY_IQ_*: the sample type of every push, the DL and the UL input alike (the cut is cf32); else INVALID_INPUTS */
+  uint32_t reserved[4];
 } ltephy_track_cfg_t;
 #define LTEPHY_TRACK_LOCKED 1u /* subframe: the last half-frame measured before it was locked (or none was measured yet); half-frame: locked */
 #define LTEPHY_TRACK_LOST   2u /* 4 or more half-frames in a row were not locked */
@@ -353,11 +365,11 @@ typedef struct {
 } ltephy_track_out_t;
 int  ltephy_track_create(const ltephy_track_cfg_t* cfg, ltephy_track_t** h);
 void ltephy_track_destroy(ltephy_track_t* h);
-/* iq: cf32 [nof_rx][nof_samples], antenna-major, host memory, absolute samples first_sample .. first_sample + nof_samples - 1, with
+/* iq: [nof_rx][nof_samples] samples in the handle's iq_format, antenna-major, host memory, absolute samples first_sample .. first_sample + nof_samples - 1, with
  * first_sample <= the previous push's next_sample.  Cuts every subframe (up to max_subframes) that lies wholly inside what has been fed.  The
  * results do not depend on how the recording is split into pushes.  Blocks until the cut is complete. */
-int  ltephy_track_push(ltephy_track_t* h, const float* iq, uint64_t first_sample, uint64_t nof_samples, ltephy_track_out_t* out);
-/* same, with the samples already in device memory */
+int  ltephy_track_push(ltephy_track_t* h, const void* iq, uint64_t first_sample, uint64_t nof_samples, ltephy_track_out_t* out);
+/* same, with the samples already in device memory (integer samples aligned to the sample) */
 int  ltephy_track_push_device(ltephy_track_t* h, const void* iq_dev, uint64_t first_sample, uint64_t nof_samples, ltephy_track_out_t* out);
 /* The uplink carrier of the same radio (the reference's -m 1: channel 1 of srsran_ue_sync_zerocopy, src/src/LTESniffer_Core.cc:174-181,365), cut
  * at the downlink's tracked timing.  UL subframe k starts at start_k + ul_offset and is rotated, with the DL cut's rule, by
@@ -372,13 +384,13 @@ typedef struct {
   uint32_t reserved[4];
 } ltephy_track_ul_cfg_t;
 int  ltephy_track_set_ul(ltephy_track_t* h, const ltephy_track_ul_cfg_t* cfg);
-/* iq as ltephy_track_push; iq_ul: cf32 [ul nof_rx][nof_samples], antenna-major like iq, the same absolute samples.  A subframe is cut only when its
+/* iq as ltephy_track_push; iq_ul: [ul nof_rx][nof_samples] in the same iq_format, antenna-major like iq, the same absolute samples.  A subframe is cut only when its
  * DL window and its UL window both lie inside what has been fed; out->next_sample is the lowest sample either pending window still needs.  The DL
  * records and cut equal those of a tracker without the uplink.  *ul_iq_dev: cf32 [nof_subframes][ul nof_rx][15 N] in device memory, valid until the
  * next push: the input ltephy_submit_ul_device takes with ltephy_cfg_t.ul_nof_rx = the same antenna count. */
-int  ltephy_track_push_ul(ltephy_track_t* h, const float* iq, const float* iq_ul, uint64_t first_sample, uint64_t nof_samples, ltephy_track_out_t* out,
+int  ltephy_track_push_ul(ltephy_track_t* h, const void* iq, const void* iq_ul, uint64_t first_sample, uint64_t nof_samples, ltephy_track_out_t* out,
                           const void** ul_iq_dev);
-/* same, with both carriers already in device memory */
+/* same, with both carriers already in device memory (integer samples aligned to the sample) */
 int  ltephy_track_push_ul_device(ltephy_track_t* h, const void* iq_dev, const void* iq_ul_dev, uint64_t first_sample, uint64_t nof_samples,
                                  ltephy_track_out_t* out, const void** ul_iq_dev);
 
@@ -395,10 +407,7 @@ int  ltephy_track_push_ul_device(ltephy_track_t* h, const void* iq_dev, const vo
  * L <= 2 M (upsampling at most 2x) and its phase table L * Kp has at most 2^15 taps.  Output m belongs to capture time m M / L and needs capture
  * samples floor(m M / L) - Ka .. floor(m M / L) + Kb (ltephy_chan_design).  A carrier of integer ratio keeps the integer rule, flag or not. */
 #define LTEPHY_CHAN_RATIONAL 1u
-/* Sample formats of the input: interleaved I/Q, complex sample i of antenna a at index a * nof_samples + i */
-#define LTEPHY_IQ_CF32 0u /* float32 */
-#define LTEPHY_IQ_SC16 1u /* int16, value * 2^-15 */
-#define LTEPHY_IQ_SC8 2u  /* int8, value * 2^-7 */
+/* The input is in one of the LTEPHY_IQ_* formats (ltephy_chan_cfg_t.iq_format): complex sample i of antenna a at index a * nof_samples + i */
 typedef struct ltephy_chan ltephy_chan_t;
 typedef struct {
   int32_t  offset_hz; /* carrier centre minus capture centre, a multiple of 1000 */
@@ -487,12 +496,12 @@ typedef struct {
   float ta_us;            /* .ta_us    timing offset from the phase slope of the DMRS estimates (meas_ta_en, UL_Sniffer_PUSCH.cc:424,574) */
 } ltephy_ul_chest_t;
 int ltephy_set_ul_cfg(ltephy_t* h, const ltephy_ul_cfg_t* cfg);
-/* iq_ul: cf32 [n][A][sf_len] of the UL carrier, A = ltephy_cfg_t.ul_nof_rx antennas (one antenna, A = 1, is what the reference decodes: antenna
+/* iq_ul: [n][A][sf_len] samples of the UL carrier in the handle's iq_format, A = ltephy_cfg_t.ul_nof_rx antennas (one antenna, A = 1, is what the reference decodes: antenna
  * buffer 1); host memory.  With A = 2 the PUSCH is estimated per antenna and equalised over both (DESIGN.md §2 "uplink receive diversity").
  * iq_ul may be NULL when the previous call demodulated the same n subframes: their symbols are decoded again with the new grants
  * (srsran_enb_ul_fft once, decode_run per grant).  L_prb >= 3: the 1- and 2-PRB DMRS base sequences (36.211 Tables 5.5.1.2-1 / -2) are not carried. */
-int ltephy_submit_ul(ltephy_t* h, const float* iq_ul, const uint32_t* tti, uint32_t n, const ltephy_ul_grant_t* grants, uint32_t ngrants);
-/* same, with iq_ul_dev cf32 [n][A][sf_len] already in device memory on the handle's device (e.g. ltephy_track_push_ul's cut), read in place: the
+int ltephy_submit_ul(ltephy_t* h, const void* iq_ul, const uint32_t* tti, uint32_t n, const ltephy_ul_grant_t* grants, uint32_t ngrants);
+/* same, with iq_ul_dev [n][A][sf_len] already in device memory on the handle's device (integer samples aligned to the sample) (e.g. ltephy_track_push_ul's cut), read in place: the
  * caller keeps it alive until ltephy_get_ul returns.  NULL re-decodes the previous call's symbols, as above. */
 int ltephy_submit_ul_device(ltephy_t* h, const void* iq_ul_dev, const uint32_t* tti, uint32_t n, const ltephy_ul_grant_t* grants, uint32_t ngrants);
 /* the uplink twin of ltephy_set_cfo: a constant carrier-offset correction of every UL subframe (phase restarting at each subframe, the table of

@@ -201,14 +201,14 @@ typedef struct {
 int ltephy_ul_grants_from_dcis(const ltephy_search_t* s, const ltephy_sf_info_t* info, const ltephy_dci_t* dcis, uint32_t nd, const ltephy_ul_ue_cfg_t* ue,
                                uint32_t n_ue, ltephy_ul_grant_t* grants, uint32_t* grant_dci, uint8_t* reading, uint32_t max_grants, uint32_t* n_grants);
 
-/* Whole batch: IQ in host memory -> accepted DCIs + transport blocks.  seq orders concurrent calls on
+/* Whole batch: IQ in host memory, in the handle's iq_format -> accepted DCIs + transport blocks.  seq orders concurrent calls on
  * different PHY handles that share one search object (the search runs strictly in seq order, starting
  * at 0); pass LTEPHY_SEQ_NONE for a single pipeline.  A call that fails, argument checks included, still passes its turn on.  A seq
  * whose turn is over (reused, or a restart from 0 on a search that has walked), or that another call on this search object is decoding,
  * returns LTEPHY_ERROR_INVALID_INPUTS at once and consumes no turn.
  *   info[n], cand_scratch[n*LTEPHY_MAX_LOC*LTEPHY_MAX_SIZES] (caller-owned, pinned if possible),
  *   dcis[max_dcis], tbs[2*max_dcis] (tbs[2*i+t] belongs to dcis[i]), payload. */
-int ltephy_decode_subframes(ltephy_t* h, ltephy_search_t* s, const float* iq, const uint32_t* tti, uint32_t n, uint64_t seq, ltephy_sf_info_t* info,
+int ltephy_decode_subframes(ltephy_t* h, ltephy_search_t* s, const void* iq, const uint32_t* tti, uint32_t n, uint64_t seq, ltephy_sf_info_t* info,
                             ltephy_cand_t* cand_scratch, ltephy_dci_t* dcis, uint32_t max_dcis, uint32_t* n_dcis, ltephy_tb_result_t* tbs,
                             uint8_t* payload, size_t payload_cap);
 

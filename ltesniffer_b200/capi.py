@@ -12,13 +12,16 @@ LLR_STRIDE = 72 * MAX_CCE
 TX_PORT0, TX_DIVERSITY, TX_CDD, TX_SPATIALMUX = 0, 1, 2, 3
 TAP_SYM, TAP_CE, TAP_LLR, TAP_PDSCH_LLR, TAP_TURBO_IN = 0, 1, 2, 3, 4
 FLAG_SKIP_LOW_POWER = 1
+# sample formats of every input (LTEPHY_IQ_*): complex64, or int16 / int8 interleaved I/Q (value * 2^-15 / value * 2^-7)
+IQ_FORMATS = {"cf32": 0, "sc16": 1, "sc8": 2}
+_IQ_DTYPES = {"cf32": np.complex64, "sc16": np.int16, "sc8": np.int8}
 
 
 class Cfg(C.Structure):
     _fields_ = [("nof_prb", C.c_uint32), ("nof_ports", C.c_uint32), ("cell_id", C.c_uint32), ("nof_rx", C.c_uint32),
                 ("max_subframes", C.c_uint32), ("max_grants", C.c_uint32), ("turbo_max_iter", C.c_uint32), ("device", C.c_int32),
                 ("flags", C.c_uint32), ("symbol_sz", C.c_uint32), ("phich_resources", C.c_uint32), ("phich_length", C.c_uint32),
-                ("ul_nof_rx", C.c_uint32), ("reserved", C.c_uint32 * 3)]
+                ("ul_nof_rx", C.c_uint32), ("iq_format", C.c_uint32), ("reserved", C.c_uint32 * 2)]
 
 
 class SfInfo(C.Structure):
@@ -156,16 +159,39 @@ def _p(a):
     return a.ctypes.data_as(C.c_void_p)
 
 
+def _host_iq(iq, fmt):
+    """-> (iq as a contiguous host array of the format's type, its shape in complex samples).  cf32: complex64; sc16 / sc8: int16 / int8 with a
+    last axis of 2 (I, Q)"""
+    iq = np.ascontiguousarray(iq, _IQ_DTYPES[fmt])
+    if fmt == "cf32":
+        return iq, iq.shape
+    assert iq.ndim >= 1 and iq.shape[-1] == 2, iq.shape
+    return iq, iq.shape[:-1]
+
+
+def _dev_shape(t, fmt):
+    """shape in complex samples of a contiguous device tensor of the format: complex64, or int16 / int8 with a last axis of 2"""
+    assert t.is_cuda and t.is_contiguous(), "a contiguous CUDA tensor"
+    if fmt == "cf32":
+        return tuple(t.shape)
+    import torch
+    want = {"sc16": torch.int16, "sc8": torch.int8}[fmt]
+    assert t.dtype == want and t.shape[-1] == 2, (t.dtype, tuple(t.shape), fmt)
+    return tuple(t.shape[:-1])
+
+
 class LtePhy:
     """One PHY context (cell + batch capacity) on one GPU."""
 
     def __init__(self, nof_prb, nof_ports, cell_id, nof_rx, max_subframes=16, turbo_max_iter=8, device=0, flags=0, symbol_sz=0, phich_resources=0, phich_length=0,
-                 ul_nof_rx=1):
-        """ul_nof_rx: receive antennas of the uplink carrier (1 or 2): decode_ul / decode_ul_device then take [n][ul_nof_rx][sf_len]"""
+                 ul_nof_rx=1, iq_format="cf32"):
+        """ul_nof_rx: receive antennas of the uplink carrier (1 or 2): decode_ul / decode_ul_device then take [n][ul_nof_rx][sf_len].
+        iq_format "cf32" takes complex64 samples, "sc16" / "sc8" int16 / int8 ones with a last axis of 2 (I, Q), DL and UL alike."""
         self.L = load_library()
+        self.iq_format = iq_format
         cfg = Cfg(nof_prb=nof_prb, nof_ports=nof_ports, cell_id=cell_id, nof_rx=nof_rx, max_subframes=max_subframes,
                   turbo_max_iter=turbo_max_iter, device=device, flags=flags, symbol_sz=symbol_sz, phich_resources=phich_resources, phich_length=phich_length,
-                  ul_nof_rx=ul_nof_rx)
+                  ul_nof_rx=ul_nof_rx, iq_format=IQ_FORMATS[iq_format])
         self.cfg = cfg
         self.h = C.c_void_p()
         r = self.L.ltephy_create(C.byref(cfg), C.byref(self.h))
@@ -206,13 +232,23 @@ class LtePhy:
 
     # ---- phase A
     def submit_iq(self, iq, tti):
-        """iq: complex64 [n][nof_rx][sf_len]"""
-        iq = np.ascontiguousarray(iq, np.complex64)
+        """iq: complex64 [n][nof_rx][sf_len] (int16 / int8 [n][nof_rx][sf_len][2] for sc16 / sc8)"""
+        iq, shape = _host_iq(iq, self.iq_format)
         tti = np.ascontiguousarray(tti, np.uint32)
         n = len(tti)
-        assert iq.shape == (n, self.cfg.nof_rx, self.sf_len), iq.shape
+        assert shape == (n, self.cfg.nof_rx, self.sf_len), iq.shape
         self._keep = (iq, tti)
         self._chk(self.L.ltephy_submit_iq(self.h, _p(iq), _p(tti), n), "submit_iq")
+        self.n = n
+
+    def submit_iq_device(self, iq_dev, tti):
+        """ltephy_submit_iq_device: iq_dev a torch tensor [n][nof_rx][sf_len] (of the handle's format, as submit_iq), contiguous, on this handle's
+        device, read in place until phase A is fetched"""
+        tti = np.ascontiguousarray(tti, np.uint32)
+        n = len(tti)
+        assert _dev_shape(iq_dev, self.iq_format) == (n, self.cfg.nof_rx, self.sf_len), tuple(iq_dev.shape)
+        self._keep = (iq_dev, tti)
+        self._chk(self.L.ltephy_submit_iq_device(self.h, C.c_void_p(iq_dev.data_ptr()), _p(tti), n), "submit_iq_device")
         self.n = n
 
     def get_phase_a(self, want_cands=True):
@@ -279,11 +315,13 @@ class LtePhy:
         self._chk(self.L.ltephy_set_ul_cfg(self.h, C.byref(cfg)), "set_ul_cfg")
 
     def decode_ul(self, iq_ul, tti, grants):
-        """iq_ul complex64 [n][sf_len] with one UL antenna, [n][ul_nof_rx][sf_len] with two (None: decode the subframes of the previous call
-        again); grants: list of UlGrant -> (results, chest, payload)"""
-        iq_ul = None if iq_ul is None else np.ascontiguousarray(iq_ul, np.complex64)
+        """iq_ul complex64 [n][sf_len] with one UL antenna, [n][ul_nof_rx][sf_len] with two (int16 / int8 with a last axis of 2 for sc16 / sc8;
+        None: decode the subframes of the previous call again); grants: list of UlGrant -> (results, chest, payload)"""
+        shape = None
+        if iq_ul is not None:
+            iq_ul, shape = _host_iq(iq_ul, self.iq_format)
         tti = np.ascontiguousarray(tti, np.uint32)
-        assert iq_ul is None or iq_ul.size == len(tti) * self.ul_nof_rx * self.sf_len, (iq_ul.shape, self.ul_nof_rx)
+        assert iq_ul is None or int(np.prod(shape)) == len(tti) * self.ul_nof_rx * self.sf_len, (iq_ul.shape, self.ul_nof_rx)
         arr = (UlGrant * max(1, len(grants)))(*grants)
         self._chk(self.L.ltephy_submit_ul(self.h, None if iq_ul is None else _p(iq_ul), _p(tti), len(tti), arr, len(grants)), "submit_ul")
         res = (TbResult * max(1, len(grants)))()
@@ -294,13 +332,14 @@ class LtePhy:
         return res, ch, pl
 
     def decode_ul_device(self, iq_dev, tti, grants):
-        """ltephy_submit_ul_device: iq_dev a torch complex64 tensor [n][sf_len] ([n][ul_nof_rx][sf_len] with two UL antennas), contiguous, on this
-        handle's device (None: decode the subframes of the previous call again), read in place -> (results, chest, payload) as decode_ul"""
+        """ltephy_submit_ul_device: iq_dev a torch complex64 tensor [n][sf_len] ([n][ul_nof_rx][sf_len] with two UL antennas; int16 / int8 with a
+        last axis of 2 for sc16 / sc8), contiguous, on this handle's device (None: decode the subframes of the previous call again), read in place ->
+        (results, chest, payload) as decode_ul"""
         self.L.ltephy_submit_ul_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32]
         tti = np.ascontiguousarray(tti, np.uint32)
         if iq_dev is not None:
             want = (len(tti), self.sf_len) if self.ul_nof_rx == 1 else (len(tti), self.ul_nof_rx, self.sf_len)
-            assert iq_dev.is_cuda and iq_dev.is_contiguous() and tuple(iq_dev.shape) == want, tuple(iq_dev.shape)
+            assert _dev_shape(iq_dev, self.iq_format) == want, tuple(iq_dev.shape)
         arr = (UlGrant * max(1, len(grants)))(*grants)
         ptr = None if iq_dev is None else C.c_void_p(iq_dev.data_ptr())
         self._chk(self.L.ltephy_submit_ul_device(self.h, ptr, _p(tti), len(tti), arr, len(grants)), "submit_ul_device")
@@ -570,10 +609,10 @@ def ul_grants_from_dcis(search, info, dcis, ue_cfgs=()):
 
 
 def decode_subframes(phy, search, iq, tti, seq=SEQ_NONE, max_dcis=None, scratch=None):
-    """One call through the reference-facing pipeline: host IQ -> (info, dcis, tb results, payload)."""
+    """One call through the reference-facing pipeline: host IQ in phy's iq_format -> (info, dcis, tb results, payload)."""
     L = phy.L
     _bind_search(L)
-    iq = np.ascontiguousarray(iq, np.complex64)
+    iq, _ = _host_iq(iq, phy.iq_format)
     tti = np.ascontiguousarray(tti, np.uint32)
     n = len(tti)
     max_dcis = max_dcis or 32 * n
@@ -732,7 +771,8 @@ SYNC_BINS = 9600
 
 
 class SyncCfg(C.Structure):
-    _fields_ = [("symbol_sz", C.c_uint32), ("nof_rx", C.c_uint32), ("max_samples", C.c_uint64), ("device", C.c_int32), ("reserved", C.c_uint32 * 4)]
+    _fields_ = [("symbol_sz", C.c_uint32), ("nof_rx", C.c_uint32), ("max_samples", C.c_uint64), ("device", C.c_int32), ("iq_format", C.c_uint32),
+                ("reserved", C.c_uint32 * 3)]
 
 
 class CellInfo(C.Structure):
@@ -746,9 +786,10 @@ assert C.sizeof(CellInfo) == 48
 
 
 class CellSearch:
-    """PSS / SSS cell search of continuous recordings of symbol_sz samples per symbol and nof_rx antennas, up to max_samples per antenna."""
+    """PSS / SSS cell search of continuous recordings of symbol_sz samples per symbol and nof_rx antennas, up to max_samples per antenna.
+    iq_format "cf32" takes complex64 [nof_rx][n], "sc16" / "sc8" int16 / int8 [nof_rx][n][2]."""
 
-    def __init__(self, symbol_sz, nof_rx, max_samples, device=0):
+    def __init__(self, symbol_sz, nof_rx, max_samples, device=0, iq_format="cf32"):
         self.L = load_library()
         L = self.L
         L.ltephy_sync_create.argtypes = [C.POINTER(SyncCfg), C.POINTER(C.c_void_p)]
@@ -756,7 +797,8 @@ class CellSearch:
         L.ltephy_cell_search.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]
         L.ltephy_cell_search_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]
         L.ltephy_sync_tap.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t]
-        self.cfg = SyncCfg(symbol_sz=symbol_sz, nof_rx=nof_rx, max_samples=max_samples, device=device)
+        self.iq_format = iq_format
+        self.cfg = SyncCfg(symbol_sz=symbol_sz, nof_rx=nof_rx, max_samples=max_samples, device=device, iq_format=IQ_FORMATS[iq_format])
         self.h = C.c_void_p()
         r = L.ltephy_sync_create(C.byref(self.cfg), C.byref(self.h))
         if r != 0:
@@ -780,17 +822,19 @@ class CellSearch:
         return [CellInfo.from_buffer_copy(out[i]) for i in range(3)]
 
     def search(self, iq):
-        """iq: complex64 [nof_rx][nof_samples] (host) -> three CellInfo, by pss_peak descending"""
-        iq = np.ascontiguousarray(iq, np.complex64)
-        assert iq.ndim == 2 and iq.shape[0] == self.cfg.nof_rx, iq.shape
+        """iq: complex64 [nof_rx][nof_samples] (host; int16 / int8 [nof_rx][nof_samples][2] for sc16 / sc8) -> three CellInfo, by pss_peak
+        descending"""
+        iq, shape = _host_iq(iq, self.iq_format)
+        assert len(shape) == 2 and shape[0] == self.cfg.nof_rx, iq.shape
         out = (CellInfo * 3)()
-        return self._done(self.L.ltephy_cell_search(self.h, _p(iq), iq.shape[1], out), out)
+        return self._done(self.L.ltephy_cell_search(self.h, _p(iq), shape[1], out), out)
 
     def search_device(self, iq):
-        """iq: torch complex64 tensor [nof_rx][nof_samples], contiguous, on this handle's device"""
-        assert iq.is_cuda and iq.is_contiguous() and iq.dim() == 2 and iq.shape[0] == self.cfg.nof_rx
+        """iq: torch complex64 tensor [nof_rx][nof_samples] (int16 / int8 [nof_rx][nof_samples][2]), contiguous, on this handle's device"""
+        shape = _dev_shape(iq, self.iq_format)
+        assert len(shape) == 2 and shape[0] == self.cfg.nof_rx
         out = (CellInfo * 3)()
-        return self._done(self.L.ltephy_cell_search_device(self.h, C.c_void_p(iq.data_ptr()), iq.shape[1], out), out)
+        return self._done(self.L.ltephy_cell_search_device(self.h, C.c_void_p(iq.data_ptr()), shape[1], out), out)
 
     def tap(self, what):
         """intermediate of the last search as float32: coarse [3][9600], refined [3][2D-1], cfo [3][2], sss [3][168][2]"""
@@ -812,7 +856,7 @@ TRACK_LOCKED, TRACK_LOST, TRACK_REACQUIRED = 1, 2, 4
 class TrackCfg(C.Structure):
     _fields_ = [("symbol_sz", C.c_uint32), ("nof_rx", C.c_uint32), ("pci", C.c_uint32), ("first_tti", C.c_uint32), ("frame_offset", C.c_uint64),
                 ("cfo_hz", C.c_float), ("max_ppm", C.c_float), ("max_subframes", C.c_uint32), ("flags", C.c_uint32), ("device", C.c_int32),
-                ("reserved", C.c_uint32 * 5)]
+                ("iq_format", C.c_uint32), ("reserved", C.c_uint32 * 4)]
 
 
 TRACK_SF_DTYPE = np.dtype([("start", "<i8"), ("tti", "<u4"), ("cfo_hz", "<f4"), ("flags", "<u4"), ("index", "<u4")])
@@ -838,9 +882,11 @@ class Tracker:
     [nof_rx][n] with its absolute first sample); each push returns the subframes that now lie wholly inside what was fed.  With ul=dict(cfo_ratio=..., ul_offset=...) the tracker also cuts the
     uplink carrier of the same radio (ltephy_track_set_ul); push both carriers with push_ul / push_ul_device.  ul=dict(..., nof_rx=2) cuts two UL
     antennas: push_ul then takes iq_ul [2][n] and ul_iq is [k][2][15 N] (one antenna: [n] and [k][15 N]).  With flags=TRACK_REACQUIRE a
-    lost cell is searched again frame by frame; the first subframe cut after it is found carries TRACK_REACQUIRED."""
+    lost cell is searched again frame by frame; the first subframe cut after it is found carries TRACK_REACQUIRED.  iq_format "sc16" / "sc8" takes
+    int16 / int8 pushes with a last axis of 2 (I, Q), DL and UL alike; the cuts stay complex64."""
 
-    def __init__(self, symbol_sz, nof_rx, pci, frame_offset, cfo_hz=0.0, first_tti=0, max_subframes=1000, max_ppm=50.0, flags=0, device=0, ul=None):
+    def __init__(self, symbol_sz, nof_rx, pci, frame_offset, cfo_hz=0.0, first_tti=0, max_subframes=1000, max_ppm=50.0, flags=0, device=0, ul=None,
+                 iq_format="cf32"):
         self.L = load_library()
         L = self.L
         L.ltephy_track_create.argtypes = [C.POINTER(TrackCfg), C.POINTER(C.c_void_p)]
@@ -851,7 +897,8 @@ class Tracker:
         L.ltephy_track_push_ul.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.POINTER(TrackOut), C.POINTER(C.c_void_p)]
         L.ltephy_track_push_ul_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.POINTER(TrackOut), C.POINTER(C.c_void_p)]
         self.cfg = TrackCfg(symbol_sz=symbol_sz, nof_rx=nof_rx, pci=pci, first_tti=first_tti, frame_offset=frame_offset, cfo_hz=cfo_hz,
-                            max_ppm=max_ppm, max_subframes=max_subframes, flags=flags, device=device)
+                            max_ppm=max_ppm, max_subframes=max_subframes, flags=flags, device=device, iq_format=IQ_FORMATS[iq_format])
+        self.iq_format = iq_format
         self.h = C.c_void_p()
         r = L.ltephy_track_create(C.byref(self.cfg), C.byref(self.h))
         if r != 0:
@@ -906,32 +953,34 @@ class Tracker:
     def push(self, iq, first_sample):
         """iq: complex64 [nof_rx][n] (host) of absolute samples first_sample ... -> dict(sf, hf: record arrays, iq: torch complex64
         [k][nof_rx][15 N] on the device (a copy of the tracker's cut), next_sample, remeasured, finds)"""
-        iq = np.ascontiguousarray(iq, np.complex64)
-        assert iq.ndim == 2 and iq.shape[0] == self.cfg.nof_rx, iq.shape
+        iq, shape = _host_iq(iq, self.iq_format)
+        assert len(shape) == 2 and shape[0] == self.cfg.nof_rx, iq.shape
         o = TrackOut()
-        return self._done(self.L.ltephy_track_push(self.h, _p(iq), first_sample, iq.shape[1], C.byref(o)), o)
+        return self._done(self.L.ltephy_track_push(self.h, _p(iq), first_sample, shape[1], C.byref(o)), o)
 
     def push_device(self, iq, first_sample):
-        """iq: torch complex64 tensor [nof_rx][n], contiguous, on this handle's device"""
-        assert iq.is_cuda and iq.is_contiguous() and iq.dim() == 2 and iq.shape[0] == self.cfg.nof_rx
+        """iq: torch complex64 tensor [nof_rx][n] (int16 / int8 [nof_rx][n][2]), contiguous, on this handle's device"""
+        shape = _dev_shape(iq, self.iq_format)
+        assert len(shape) == 2 and shape[0] == self.cfg.nof_rx
         o = TrackOut()
-        return self._done(self.L.ltephy_track_push_device(self.h, C.c_void_p(iq.data_ptr()), first_sample, iq.shape[1], C.byref(o)), o)
+        return self._done(self.L.ltephy_track_push_device(self.h, C.c_void_p(iq.data_ptr()), first_sample, shape[1], C.byref(o)), o)
 
     def push_ul(self, iq, iq_ul, first_sample):
         """iq as push, iq_ul: complex64 [n] of the uplink antenna ([A][n] with A = 2 UL antennas), the same absolute samples -> push's dict plus
         ul_iq: torch complex64 [k][15 N] ([k][A][15 N]) on the device (a copy of the tracker's UL cut)"""
-        iq = np.ascontiguousarray(iq, np.complex64)
-        iq_ul = np.ascontiguousarray(iq_ul, np.complex64).reshape(-1)
-        assert iq.ndim == 2 and iq.shape[0] == self.cfg.nof_rx and iq_ul.shape[0] == max(1, self.ul.nof_rx) * iq.shape[1], (iq.shape, iq_ul.shape)
+        iq, shape = _host_iq(iq, self.iq_format)
+        iq_ul, ushape = _host_iq(iq_ul, self.iq_format)
+        assert len(shape) == 2 and shape[0] == self.cfg.nof_rx and int(np.prod(ushape)) == max(1, self.ul.nof_rx) * shape[1], (iq.shape, iq_ul.shape)
         o, u = TrackOut(), C.c_void_p()
-        return self._done(self.L.ltephy_track_push_ul(self.h, _p(iq), _p(iq_ul), first_sample, iq.shape[1], C.byref(o), C.byref(u)), o, u)
+        return self._done(self.L.ltephy_track_push_ul(self.h, _p(iq), _p(iq_ul), first_sample, shape[1], C.byref(o), C.byref(u)), o, u)
 
     def push_ul_device(self, iq, iq_ul, first_sample):
         """iq: torch complex64 [nof_rx][n], iq_ul: torch complex64 [n] ([A][n] with A = 2 UL antennas), both contiguous on this handle's device"""
-        assert iq.is_cuda and iq.is_contiguous() and iq.dim() == 2 and iq.shape[0] == self.cfg.nof_rx
-        assert iq_ul.is_cuda and iq_ul.is_contiguous() and iq_ul.numel() == max(1, self.ul.nof_rx) * iq.shape[1]
+        shape, ushape = _dev_shape(iq, self.iq_format), _dev_shape(iq_ul, self.iq_format)
+        assert len(shape) == 2 and shape[0] == self.cfg.nof_rx
+        assert int(np.prod(ushape)) == max(1, self.ul.nof_rx) * shape[1]
         o, u = TrackOut(), C.c_void_p()
-        return self._done(self.L.ltephy_track_push_ul_device(self.h, C.c_void_p(iq.data_ptr()), C.c_void_p(iq_ul.data_ptr()), first_sample, iq.shape[1],
+        return self._done(self.L.ltephy_track_push_ul_device(self.h, C.c_void_p(iq.data_ptr()), C.c_void_p(iq_ul.data_ptr()), first_sample, shape[1],
                                                              C.byref(o), C.byref(u)), o, u)
 
 
@@ -939,8 +988,6 @@ class Tracker:
 # channeliser (ltephy_chan_*, include/ltephy_b200.h)
 CHAN_MAX_CARRIERS = 8
 CHAN_RATIONAL = 1
-IQ_FORMATS = {"cf32": 0, "sc16": 1, "sc8": 2}
-_IQ_DTYPES = {"cf32": np.complex64, "sc16": np.int16, "sc8": np.int8}
 
 
 class ChanCarrier(C.Structure):

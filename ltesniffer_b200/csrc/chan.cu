@@ -28,8 +28,6 @@ struct ltephy_chan {
   size_t         smem = 0;
 };
 
-static size_t chan_sample_bytes(uint32_t fmt) { return fmt == LTEPHY_IQ_SC16 ? 4 : fmt == LTEPHY_IQ_SC8 ? 2 : 8; }
-
 static uint32_t chan_max_prb(uint32_t N)
 {
   switch (N) {
@@ -198,7 +196,7 @@ extern "C" int ltephy_chan_create(const ltephy_chan_cfg_t* cfg, ltephy_chan_t** 
   ltephy_chan* const                                           h = owner.get();
   h->cfg                                                         = *cfg;
   CU(cudaStreamCreateWithFlags(&h->stream.raw, cudaStreamNonBlocking));
-  const size_t xbytes = (size_t)cfg->nof_rx * cfg->max_samples * chan_sample_bytes(cfg->iq_format);
+  const size_t xbytes = (size_t)cfg->nof_rx * cfg->max_samples * iq_sample_bytes(cfg->iq_format);
   if (h->d_x.reserve((xbytes + sizeof(float2) - 1) / sizeof(float2))) return fail(LTEPHY_ERROR, "chan_create: device allocation failed");
   for (uint32_t c = 0; c < cfg->nof_carriers; c++) {
     ltephy_chan::Carrier& k = h->car[c];
@@ -282,7 +280,7 @@ extern "C" int ltephy_chan_run(ltephy_chan_t* h, const void* iq, uint64_t first_
 {
   if (int r = chan_check(h, iq, first_sample, nof_samples, out, next_sample)) return r;
   CU(cudaSetDevice(h->cfg.device));
-  CU(cudaMemcpyAsync(h->d_x.p, iq, (size_t)h->cfg.nof_rx * nof_samples * chan_sample_bytes(h->cfg.iq_format), cudaMemcpyHostToDevice, h->stream));
+  CU(cudaMemcpyAsync(h->d_x.p, iq, (size_t)h->cfg.nof_rx * nof_samples * iq_sample_bytes(h->cfg.iq_format), cudaMemcpyHostToDevice, h->stream));
   return chan_run(h, h->d_x.p, first_sample, nof_samples, out, next_sample);
 }
 
@@ -290,8 +288,8 @@ extern "C" int ltephy_chan_run_device(ltephy_chan_t* h, const void* iq_dev, uint
                                       uint64_t* next_sample)
 {
   if (int r = chan_check(h, iq_dev, first_sample, nof_samples, out, next_sample)) return r;
-  if (h->cfg.iq_format != LTEPHY_IQ_CF32 && (uintptr_t)iq_dev % chan_sample_bytes(h->cfg.iq_format))
-    return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan_run_device: iq_dev not aligned to its %zu-byte samples", chan_sample_bytes(h->cfg.iq_format));
+  if (iq_misaligned(iq_dev, h->cfg.iq_format))
+    return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan_run_device: iq_dev not aligned to its %zu-byte samples", iq_sample_bytes(h->cfg.iq_format));
   CU(cudaSetDevice(h->cfg.device));
   return chan_run(h, iq_dev, first_sample, nof_samples, out, next_sample);
 }

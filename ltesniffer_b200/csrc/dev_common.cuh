@@ -50,6 +50,19 @@ struct DevSfInfo {
 };
 static_assert(sizeof(DevSfInfo) == sizeof(ltephy_sf_info_t), "DevSfInfo must mirror ltephy_sf_info_t");
 
+// One complex input sample as cf32, converted where a kernel loads it: sc16 is value * 2^-15, sc8 value * 2^-7, both exact in fp32, so a run on
+// integer samples equals the cf32 run on the converted samples bit for bit (DESIGN.md §2 "integer samples").
+__device__ __forceinline__ float2 chan_cf32(float2 v) { return v; }
+__device__ __forceinline__ float2 chan_cf32(short2 v) { return make_float2((float)v.x * 0x1p-15f, (float)v.y * 0x1p-15f); }
+__device__ __forceinline__ float2 chan_cf32(char2 v) { return make_float2((float)v.x * 0x1p-7f, (float)v.y * 0x1p-7f); }
+
+// host: f(X{}) with X the sample type of iq_format fmt (LTEPHY_IQ_CF32 float2, _SC16 short2, _SC8 char2); callers validate fmt beforehand
+template <typename F>
+inline auto with_iq_type(uint32_t fmt, F&& f)
+{
+  return fmt == LTEPHY_IQ_SC16 ? f(short2{}) : fmt == LTEPHY_IQ_SC8 ? f(char2{}) : f(float2{});
+}
+
 // deterministic warp sum: lane-strided partials already in v, then the fixed halving tree.
 __device__ __forceinline__ float warp_tree_sum(float v)
 {

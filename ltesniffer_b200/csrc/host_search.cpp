@@ -1520,7 +1520,7 @@ static int decode_common(ltephy_t* h, ltephy_search_t* s, const void* iq, bool i
   // batch must not leave the other pipelines of this search object waiting for a sequence number that never comes.
   TurnGuard turn(s->turn, seq);
   if (!h || !iq || !tti || !info || !cand_scratch || !dcis || !n_dcis || !tbs) return LTEPHY_ERROR_INVALID_INPUTS;
-  int r = iq_on_device ? ltephy_submit_iq_device(h, iq, tti, n) : ltephy_submit_iq(h, (const float*)iq, tti, n);
+  int r = iq_on_device ? ltephy_submit_iq_device(h, iq, tti, n) : ltephy_submit_iq(h, iq, tti, n);
   if (r) return r;
   double t1 = now_ms();
   r = ltephy_get_phase_a_compact(h, info, nullptr); // survivor form (4.5 KB / subframe) stays in the handle's pinned buffer
@@ -1559,7 +1559,7 @@ static int decode_common(ltephy_t* h, ltephy_search_t* s, const void* iq, bool i
   for (uint32_t gi = 0; gi < ng; gi++) ltephy_place_grant_result(tbs, grant_dci[gi], res[2 * gi], res[2 * gi + 1]);
   return LTEPHY_SUCCESS;
 }
-int ltephy_decode_subframes(ltephy_t* h, ltephy_search_t* s, const float* iq, const uint32_t* tti, uint32_t n, uint64_t seq, ltephy_sf_info_t* info,
+int ltephy_decode_subframes(ltephy_t* h, ltephy_search_t* s, const void* iq, const uint32_t* tti, uint32_t n, uint64_t seq, ltephy_sf_info_t* info,
                             ltephy_cand_t* cand_scratch, ltephy_dci_t* dcis, uint32_t max_dcis, uint32_t* n_dcis, ltephy_tb_result_t* tbs,
                             uint8_t* payload, size_t payload_cap)
 {

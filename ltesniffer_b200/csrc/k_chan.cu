@@ -3,12 +3,9 @@
 // Each sum is a serial k-ascending chain of separate fp32 products and adds (-fmad=false), as lteo_chan_run / lteo_chan_run_poly (oracle/)
 // compute it, so the results equal the oracles' bit for bit.  The input is converted to cf32 where it is staged into shared memory; sc16 and sc8
 // scale by a power of two, which is exact.
+#include "dev_common.cuh"
 #include "k_chan.cuh"
 #include <cstdint>
-
-__device__ __forceinline__ float2 chan_cf32(float2 v) { return v; }
-__device__ __forceinline__ float2 chan_cf32(short2 v) { return make_float2((float)v.x * 0x1p-15f, (float)v.y * 0x1p-15f); }
-__device__ __forceinline__ float2 chan_cf32(char2 v) { return make_float2((float)v.x * 0x1p-7f, (float)v.y * 0x1p-7f); }
 
 // The serial k-ascending chain of one output: taps t[0 .. Kp) against span positions s, s - 1, .., s - Kp + 1, position s at row s / Q of phase
 // s mod Q of xs.  LDG: the taps are read through L1, else from shared memory.

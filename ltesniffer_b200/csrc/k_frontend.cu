@@ -58,15 +58,16 @@ __device__ __forceinline__ void fft_pass(float2* work, const float2* __restrict_
 
 // R3: the symbol has 3 * 2^k samples (srsRAN's default sampling rates, 1536 at 100 PRB): three power-of-two transforms F_r of x[3 m + r] run
 // side by side (thread = (r, t)), then X[k] = (F0[k mod M] + W_N^k F1[k mod M]) + W_N^(2k) F2[k mod M] -- the oracle's expression.
-template <bool UL, bool R3, bool CFO>
-__global__ void __launch_bounds__(256) ofdm_rx_kernel(const __grid_constant__ DevCell c, const float2* __restrict__ iq, float2* __restrict__ sym)
+// X: the input's sample type (float2, short2 or char2), converted to cf32 on load, before the rotations.
+template <bool UL, bool R3, bool CFO, typename X>
+__global__ void __launch_bounds__(256) ofdm_rx_kernel(const __grid_constant__ DevCell c, const X* __restrict__ iq, float2* __restrict__ sym)
 {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const uint32_t l = blockIdx.x, a = blockIdx.y, sf = blockIdx.z, n = c.fft, M = c.sub, L = c.log2n, q8 = M >> 3;
   const uint32_t nt = R3 ? blockDim.x / 3 : blockDim.x, r = R3 ? threadIdx.x / nt : 0u, tid = R3 ? threadIdx.x % nt : threadIdx.x;
   float2*        work = reinterpret_cast<float2*>(smem_raw) + r * M; // [3][M] or [fft], swizzled
   const uint32_t nant = gridDim.y; // c.nof_rx, or c.ul_nof_rx on the UL carrier
-  const float2*  src = iq + ((size_t)sf * nant + a) * c.sf_len + c.sym_off[l];
+  const X*       src = iq + ((size_t)sf * nant + a) * c.sf_len + c.sym_off[l];
   const float2*  tw_st = c.tw_st;
 
   // ---- pass 1: stages 1..3 of group g = bitrev(t): A[8 g + j] = x_r[bitrev3(j) M/8 + t], x_r[i] = x[3 i + r] (x[i] for a power-of-two symbol)
@@ -79,7 +80,7 @@ __global__ void __launch_bounds__(256) ofdm_rx_kernel(const __grid_constant__ De
 #pragma unroll
       for (uint32_t j = 0; j < 8; j++) {
         const uint32_t m = ((j & 1u) << 2) | (j & 2u) | (j >> 2), idx = R3 ? 3 * (t + m * q8) + r : t + m * q8;
-        float2         x = src[idx];
+        float2         x = chan_cf32(src[idx]);
         if (CFO) { // constant frequency-offset correction of the file samples (srsran_cfo_correct in srsran_ue_sync's file mode)
           const float2 rr = __ldg(&(UL ? c.ul_cfo_rot : c.cfo_rot)[c.sym_off[l] + idx]);
           x               = make_float2(x.x * rr.x - x.y * rr.y, x.x * rr.y + x.y * rr.x);
@@ -333,23 +334,36 @@ extern "C" void launch_chest_interp(const DevCell& c, const float2* pil, float2*
   chest_interp_kernel<<<dim3(c.nof_ports * c.nof_rx, n), 256, 0, st>>>(c, pil, ce);
   *launches += 1;
 }
-extern "C" void launch_frontend(const DevCell& c, const float2* iq, float2* sym, float2* ce, float* llr, DevSfInfo* info, uint32_t n,
+
+// one launch of the OFDM receive over n subframes of nant antennas (the DL or the UL carrier), in the handle's sample format
+template <bool UL>
+static void launch_ofdm(const DevCell& c, const void* iq, uint32_t fmt, float2* sym, uint32_t nant, uint32_t n, bool cfo, cudaStream_t st)
+{
+  const size_t   smem_fft = (size_t)c.fft * sizeof(float2);
+  const dim3     grid(14, nant, n);
+  const uint32_t nt2 = c.fft / 8 < 32 ? 32 : c.fft / 8, nt3 = 3 * (c.sub / 8);
+  with_iq_type(fmt, [&](auto z) {
+    using X    = decltype(z);
+    const X* x = static_cast<const X*>(iq);
+    if (c.sub == c.fft) {
+      if (cfo)
+        ofdm_rx_kernel<UL, false, true, X><<<grid, nt2, smem_fft, st>>>(c, x, sym);
+      else
+        ofdm_rx_kernel<UL, false, false, X><<<grid, nt2, smem_fft, st>>>(c, x, sym);
+    } else {
+      if (cfo)
+        ofdm_rx_kernel<UL, true, true, X><<<grid, nt3, smem_fft, st>>>(c, x, sym);
+      else
+        ofdm_rx_kernel<UL, true, false, X><<<grid, nt3, smem_fft, st>>>(c, x, sym);
+    }
+    return 0;
+  });
+}
+
+extern "C" void launch_frontend(const DevCell& c, const void* iq, uint32_t fmt, float2* sym, float2* ce, float* llr, DevSfInfo* info, uint32_t n,
                                 cudaStream_t st, uint64_t* launches)
 {
-  const size_t smem_fft = (size_t)c.fft * sizeof(float2);
-  const dim3   grid(14, c.nof_rx, n);
-  const uint32_t nt2 = c.fft / 8 < 32 ? 32 : c.fft / 8, nt3 = 3 * (c.sub / 8);
-  if (c.sub == c.fft) {
-    if (c.cfo_rot)
-      ofdm_rx_kernel<false, false, true><<<grid, nt2, smem_fft, st>>>(c, iq, sym);
-    else
-      ofdm_rx_kernel<false, false, false><<<grid, nt2, smem_fft, st>>>(c, iq, sym);
-  } else {
-    if (c.cfo_rot)
-      ofdm_rx_kernel<false, true, true><<<grid, nt3, smem_fft, st>>>(c, iq, sym);
-    else
-      ofdm_rx_kernel<false, true, false><<<grid, nt3, smem_fft, st>>>(c, iq, sym);
-  }
+  launch_ofdm<false>(c, iq, fmt, sym, c.nof_rx, n, c.cfo_rot != nullptr, st);
   const size_t smem_ch = (size_t)2 * NPILSYM * 2 * c.nof_prb * sizeof(float2);
   chest_kernel<<<dim3(c.nof_ports * c.nof_rx, n), 256, smem_ch, st>>>(c, sym, ce, info);
   rb_power_kernel<<<n, 128, 0, st>>>(c, sym, info);
@@ -357,21 +371,8 @@ extern "C" void launch_frontend(const DevCell& c, const float2* iq, float2* sym,
   *launches += 4;
 }
 
-extern "C" void launch_ul_ofdm(const DevCell& c, const float2* iq, float2* sym, uint32_t n, cudaStream_t st, uint64_t* launches)
+extern "C" void launch_ul_ofdm(const DevCell& c, const void* iq, uint32_t fmt, float2* sym, uint32_t n, cudaStream_t st, uint64_t* launches)
 {
-  const size_t smem_fft = (size_t)c.fft * sizeof(float2);
-  const dim3   grid(14, c.ul_nof_rx, n);
-  const uint32_t nt2 = c.fft / 8 < 32 ? 32 : c.fft / 8, nt3 = 3 * (c.sub / 8);
-  if (c.sub == c.fft) {
-    if (c.ul_cfo_rot)
-      ofdm_rx_kernel<true, false, true><<<grid, nt2, smem_fft, st>>>(c, iq, sym);
-    else
-      ofdm_rx_kernel<true, false, false><<<grid, nt2, smem_fft, st>>>(c, iq, sym);
-  } else {
-    if (c.ul_cfo_rot)
-      ofdm_rx_kernel<true, true, true><<<grid, nt3, smem_fft, st>>>(c, iq, sym);
-    else
-      ofdm_rx_kernel<true, true, false><<<grid, nt3, smem_fft, st>>>(c, iq, sym);
-  }
+  launch_ofdm<true>(c, iq, fmt, sym, c.ul_nof_rx, n, c.ul_cfo_rot != nullptr, st);
   *launches += 1;
 }

@@ -6,10 +6,10 @@
 #include "dev_ul.cuh"
 
 extern "C" {
-void launch_frontend(const DevCell& c, const float2* iq, float2* sym, float2* ce, float* llr, DevSfInfo* info, uint32_t n, cudaStream_t st,
+void launch_frontend(const DevCell& c, const void* iq, uint32_t fmt, float2* sym, float2* ce, float* llr, DevSfInfo* info, uint32_t n, cudaStream_t st,
                      uint64_t* launches);
 void launch_chest_interp(const DevCell& c, const float2* pil, float2* ce, uint32_t n, cudaStream_t st, uint64_t* launches);
-void launch_ul_ofdm(const DevCell& c, const float2* iq, float2* sym, uint32_t n, cudaStream_t st, uint64_t* launches);
+void launch_ul_ofdm(const DevCell& c, const void* iq, uint32_t fmt, float2* sym, uint32_t n, cudaStream_t st, uint64_t* launches);
 void launch_viterbi(const DevCell& c, const float* llr, const DevSfInfo* info, ltephy_cand_t* cands, uint32_t* work, uint32_t n, cudaStream_t st,
                     uint64_t* launches);
 void launch_compact(const DevCell& c, const DevSfInfo* info, const ltephy_cand_t* cands, ltephy_compact_t* out, uint32_t n, cudaStream_t st,

@@ -1,6 +1,7 @@
 // k_sync.cu -- cell search kernels (DESIGN.md §2 "cell search", §4): coarse PSS correlation at stride D = N / 128, half-frame fold and peak,
 // stride-1 refinement with the CFO sums, 62-bin DFTs of the PSS / SSS symbols and the SSS hypothesis table.  Every float sum runs in the
 // order lteo_cell_search (oracle/lte_sync_oracle.c) restates, built with -fmad=false, so the results equal the oracle's bit for bit.
+#include "dev_common.cuh"
 #include "k_sync.cuh"
 #include <cstdint>
 
@@ -11,7 +12,9 @@
 // samples D apart, so an even D would put every lane of a half-warp on one bank pair; with the odd stride Ds they all land on different ones.
 static __device__ __forceinline__ uint32_t sync_pad_stride(uint32_t D) { return D | 1u; }
 
-// m[u][j] = sum_a |c_ua(jD)|^2 / (E_p[u] sum_a E_a(jD)); each thread keeps 4 offsets x 3 replicas of correlations and the 4 window energies in registers
+// m[u][j] = sum_a |c_ua(jD)|^2 / (E_p[u] sum_a E_a(jD)); each thread keeps 4 offsets x 3 replicas of correlations and the 4 window energies in registers.
+// X, here and below: the sample type of g.x, converted to cf32 where it is loaded.
+template <typename X>
 __global__ void __launch_bounds__(COARSE_THREADS) sync_coarse_kernel(SyncArgs g, float* __restrict__ m)
 {
   extern __shared__ float4 sm4[];
@@ -36,10 +39,10 @@ __global__ void __launch_bounds__(COARSE_THREADS) sync_coarse_kernel(SyncArgs g,
   }
   for (uint32_t a = 0; a < g.A; a++) {
     __syncthreads();
-    const float2* xa = g.x + (uint64_t)a * g.lda;
+    const X* xa = static_cast<const X*>(g.x) + (uint64_t)a * g.lda;
     for (uint32_t i = threadIdx.x; i < span; i += blockDim.x) {
       const uint64_t s    = s0 + i;
-      xs[(i / D) * Ds + i % D] = s < g.L ? xa[s] : make_float2(0.0f, 0.0f);
+      xs[(i / D) * Ds + i % D] = s < g.L ? chan_cf32(xa[s]) : make_float2(0.0f, 0.0f);
     }
     __syncthreads();
     float cr[3][COARSE_R], ci[3][COARSE_R], e[COARSE_R];
@@ -137,14 +140,15 @@ __global__ void __launch_bounds__(1024) sync_peak_kernel(const float* __restrict
 }
 
 // the metric of one window at stride 1, in lteo_cell_search's sync_metric order
+template <typename X>
 static __device__ float sync_window_metric(const SyncArgs& g, uint64_t t, const float2* __restrict__ p, float ep)
 {
   float P = 0.0f, E = 0.0f;
   for (uint32_t a = 0; a < g.A; a++) {
-    const float2* xa = g.x + (uint64_t)a * g.lda + t;
-    float         cr = 0.0f, ci = 0.0f, e = 0.0f;
+    const X* xa = static_cast<const X*>(g.x) + (uint64_t)a * g.lda + t;
+    float    cr = 0.0f, ci = 0.0f, e = 0.0f;
     for (uint32_t k = 0; k < g.N; k++) {
-      const float2 v = xa[k], w = p[k];
+      const float2 v = chan_cf32(xa[k]), w = p[k];
       cr             = cr + (v.x * w.x + v.y * w.y);
       ci             = ci + (v.y * w.x - v.x * w.y);
       e              = e + (v.x * v.x + v.y * v.y);
@@ -157,6 +161,7 @@ static __device__ float sync_window_metric(const SyncArgs& g, uint64_t t, const 
 }
 
 // rm[u][h][i]: metric at ((bp D + HF + i - (D - 1)) mod HF) + h HF, for the 2D - 1 offsets i around the coarse peak and every half-frame h
+template <typename X>
 __global__ void sync_refine_kernel(SyncArgs g, const SyncPeak* __restrict__ pk, float* __restrict__ rm)
 {
   const uint32_t NR = 2 * g.D - 1, t = blockIdx.x * blockDim.x + threadIdx.x;
@@ -164,10 +169,11 @@ __global__ void sync_refine_kernel(SyncArgs g, const SyncPeak* __restrict__ pk, 
   const uint32_t u = t / (g.nh * NR), h = (t / NR) % g.nh, i = t % NR;
   const uint64_t HF = 75ull * g.N, tt = ((uint64_t)pk[u].bin * g.D + HF + i - (g.D - 1)) % HF + h * HF;
   const float    ep = u == 0 ? g.ep[0] : u == 1 ? g.ep[1] : g.ep[2]; // no run-time index into the parameters (it would copy them to local memory)
-  if (tt + g.N <= g.L) rm[t] = sync_window_metric(g, tt, g.rep + u * g.N, ep);
+  if (tt + g.N <= g.L) rm[t] = sync_window_metric<X>(g, tt, g.rep + u * g.N, ep);
 }
 
 // one block per N_ID_2: fold the refined metrics, pick the best offset (ties to the lowest), then S = sum_h sum_a c2 conj(c1) at that timing
+template <typename X>
 __global__ void sync_select_kernel(SyncArgs g, const float* __restrict__ rm, float4* __restrict__ c12, SyncPeak* __restrict__ pk,
                                                           float* __restrict__ refined)
 {
@@ -201,15 +207,15 @@ __global__ void sync_select_kernel(SyncArgs g, const float* __restrict__ rm, flo
     const uint32_t h = w / g.A, a = w % g.A;
     const uint64_t t = tau + h * HF;
     if (t + g.N > g.L) continue;
-    const float2* xa = g.x + (uint64_t)a * g.lda + t;
-    float         c1r = 0.0f, c1i = 0.0f, c2r = 0.0f, c2i = 0.0f;
+    const X* xa  = static_cast<const X*>(g.x) + (uint64_t)a * g.lda + t;
+    float    c1r = 0.0f, c1i = 0.0f, c2r = 0.0f, c2i = 0.0f;
     for (uint32_t k = 0; k < g.N / 2; k++) {
-      const float2 v = xa[k], q = p[k];
+      const float2 v = chan_cf32(xa[k]), q = p[k];
       c1r            = c1r + (v.x * q.x + v.y * q.y);
       c1i            = c1i + (v.y * q.x - v.x * q.y);
     }
     for (uint32_t k = g.N / 2; k < g.N; k++) {
-      const float2 v = xa[k], q = p[k];
+      const float2 v = chan_cf32(xa[k]), q = p[k];
       c2r            = c2r + (v.x * q.x + v.y * q.y);
       c2i            = c2i + (v.y * q.x - v.x * q.y);
     }
@@ -233,6 +239,7 @@ template <typename T>
 static __device__ __forceinline__ T sss_pick(const T (&v)[3], uint32_t u) { return u == 0 ? v[0] : u == 1 ? v[1] : v[2]; }
 
 // Y[u][hs][a][sym][n]: 62-bin DFT of the PSS (sym 0, at tau + h HF) and SSS (sym 1, N + 9D earlier) windows, h = h0[u] + hs, twiddles in shared memory
+template <typename X>
 __global__ void __launch_bounds__(256) sync_dft_kernel(SyncArgs g, SyncSss s, float2* __restrict__ Y)
 {
   extern __shared__ float2 W[];
@@ -243,12 +250,12 @@ __global__ void __launch_bounds__(256) sync_dft_kernel(SyncArgs g, SyncSss s, fl
   const uint32_t u = t / per_u, n = t % 62, sym = (t / 62) % 2, a = (t / 124) % g.A, hs = (t / (124 * g.A)) % s.nhmax;
   if (hs >= sss_pick(s.nH, u)) return;
   const uint64_t tp = sss_pick(s.tau, u) + (uint64_t)(sss_pick(s.h0, u) + hs) * 75ull * g.N, t0 = sym ? tp - g.N - 9 * g.D : tp;
-  const float2*  xa = g.x + (uint64_t)a * g.lda + t0;
+  const X*       xa = static_cast<const X*>(g.x) + (uint64_t)a * g.lda + t0;
   const uint32_t f  = n < 31 ? g.N + n - 31 : n - 30;
   float          yr = 0.0f, yi = 0.0f;
   uint32_t       idx = 0; // (f m) mod N
   for (uint32_t m = 0; m < g.N; m++) {
-    const float2 v = xa[m], w = W[idx];
+    const float2 v = chan_cf32(xa[m]), w = W[idx];
     yr             = yr + (v.x * w.x - v.y * w.y);
     yi             = yi + (v.x * w.y + v.y * w.x);
     idx += f;
@@ -294,26 +301,33 @@ __global__ void __launch_bounds__(256) sync_sss_kernel(SyncArgs g, SyncSss s, co
   if (lane == 0) out[(u * 168 + n1) * 2] = A0, out[(u * 168 + n1) * 2 + 1] = A1;
 }
 
-extern "C" int launch_sync_pss(const SyncArgs& g, float* m, float* fold, SyncPeak* pk, float* rm, float4* c12, float* refined, cudaStream_t st,
-                               uint64_t* launches)
+extern "C" int launch_sync_pss(const SyncArgs& g, uint32_t fmt, float* m, float* fold, SyncPeak* pk, float* rm, float4* c12, float* refined,
+                               cudaStream_t st, uint64_t* launches)
 {
   const uint32_t T = COARSE_THREADS * COARSE_R, Ds = g.D | 1u;
   const size_t   smem = (size_t)g.N * 24 + (size_t)(T + g.N / g.D) * Ds * 8;
-  if (cudaFuncSetAttribute(sync_coarse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return -1;
-  sync_coarse_kernel<<<(unsigned)((g.J + T - 1) / T), COARSE_THREADS, smem, st>>>(g, m);
-  sync_fold_kernel<<<(3 * SYNC_BINS + 255) / 256, 256, 0, st>>>(g, m, fold);
-  sync_peak_kernel<<<3, 1024, 0, st>>>(fold, pk);
-  const uint32_t nr = 3 * g.nh * (2 * g.D - 1);
-  sync_refine_kernel<<<(nr + 127) / 128, 128, 0, st>>>(g, pk, rm);
-  sync_select_kernel<<<3, 256, 0, st>>>(g, rm, c12, pk, refined);
-  *launches += 5;
-  return cudaGetLastError() == cudaSuccess ? 0 : -1;
+  return with_iq_type(fmt, [&](auto z) {
+    using X = decltype(z);
+    if (cudaFuncSetAttribute(sync_coarse_kernel<X>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return -1;
+    sync_coarse_kernel<X><<<(unsigned)((g.J + T - 1) / T), COARSE_THREADS, smem, st>>>(g, m);
+    sync_fold_kernel<<<(3 * SYNC_BINS + 255) / 256, 256, 0, st>>>(g, m, fold);
+    sync_peak_kernel<<<3, 1024, 0, st>>>(fold, pk);
+    const uint32_t nr = 3 * g.nh * (2 * g.D - 1);
+    sync_refine_kernel<X><<<(nr + 127) / 128, 128, 0, st>>>(g, pk, rm);
+    sync_select_kernel<X><<<3, 256, 0, st>>>(g, rm, c12, pk, refined);
+    *launches += 5;
+    return cudaGetLastError() == cudaSuccess ? 0 : -1;
+  });
 }
 
-extern "C" int launch_sync_sss(const SyncArgs& g, const SyncSss& s, float2* Y, float* sss, cudaStream_t st, uint64_t* launches)
+extern "C" int launch_sync_sss(const SyncArgs& g, uint32_t fmt, const SyncSss& s, float2* Y, float* sss, cudaStream_t st, uint64_t* launches)
 {
   const uint32_t nt = 3 * s.nhmax * g.A * 124;
-  if (nt) sync_dft_kernel<<<(nt + 255) / 256, 256, g.N * sizeof(float2), st>>>(g, s, Y);
+  if (nt)
+    with_iq_type(fmt, [&](auto z) {
+      sync_dft_kernel<decltype(z)><<<(nt + 255) / 256, 256, g.N * sizeof(float2), st>>>(g, s, Y);
+      return 0;
+    });
   sync_sss_kernel<<<(3 * 168 * 32 + 255) / 256, 256, 0, st>>>(g, s, Y, sss);
   *launches += nt ? 2 : 1;
   return cudaGetLastError() == cudaSuccess ? 0 : -1;

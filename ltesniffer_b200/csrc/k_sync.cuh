@@ -7,7 +7,7 @@
 #define SYNC_BINS 9600 // coarse bins per half-frame: 75 N / D
 
 struct SyncArgs {
-  const float2* x;   // [A][lda] samples
+  const void*   x;   // [A][lda] samples in the handle's iq_format (float2, short2 or char2)
   uint64_t      lda, L, J; // J: coarse offsets whose window fits, (L - N) / D + 1
   uint32_t      N, D, A, nh; // nh: half-frames with a window start below L - N + 1, (L - N) / HF + 1
   const float2* rep; // [3][N] PSS replicas
@@ -36,8 +36,10 @@ struct SyncSss {
 float sync_pss_replica(uint32_t N, uint32_t u, float2* d, float2* rep);
 // host (sync.cu): the cell search of the L samples x[a * lda + i] (device memory, i < L <= max_samples) on h's stream; blocks until out[3] is
 // written.  ltephy_cell_search_device is lda = L; the tracker's find state (track.cu) searches a window of its own buffer in place.
-int sync_run(ltephy_sync_t* h, const float2* x, uint64_t lda, uint64_t L, ltephy_cell_t* out);
+// x holds samples in the handle's iq_format.
+int sync_run(ltephy_sync_t* h, const void* x, uint64_t lda, uint64_t L, ltephy_cell_t* out);
 
-extern "C" int launch_sync_pss(const SyncArgs& g, float* m, float* fold, SyncPeak* pk, float* rm, float4* c12, float* refined, cudaStream_t st,
+// fmt: the iq_format of g.x
+extern "C" int launch_sync_pss(const SyncArgs& g, uint32_t fmt, float* m, float* fold, SyncPeak* pk, float* rm, float4* c12, float* refined, cudaStream_t st,
                                uint64_t* launches);
-extern "C" int launch_sync_sss(const SyncArgs& g, const SyncSss& s, float2* Y, float* sss, cudaStream_t st, uint64_t* launches);
+extern "C" int launch_sync_sss(const SyncArgs& g, uint32_t fmt, const SyncSss& s, float2* Y, float* sss, cudaStream_t st, uint64_t* launches);

@@ -69,6 +69,7 @@ extern "C" int ltephy_create(const ltephy_cfg_t* cfg, ltephy_t** out)
       cfg->max_subframes == 0)
     return fail(LTEPHY_ERROR_INVALID_INPUTS, "unsupported cell/batch configuration");
   if (cfg->ul_nof_rx > 2) return fail(LTEPHY_ERROR_INVALID_INPUTS, "ul_nof_rx %u: 0 or 1 (one uplink antenna) or 2", cfg->ul_nof_rx);
+  if (cfg->iq_format > LTEPHY_IQ_SC8) return fail(LTEPHY_ERROR_INVALID_INPUTS, "iq_format %u: LTEPHY_IQ_CF32 (0), LTEPHY_IQ_SC16 (1) or LTEPHY_IQ_SC8 (2)", cfg->iq_format);
   // the front end puts the subframe index on gridDim.y / gridDim.z (k_frontend.cu), which stop at 65 535
   if (cfg->max_subframes > LTEPHY_MAX_BATCH_SUBFRAMES)
     return fail(LTEPHY_ERROR_INVALID_INPUTS, "max_subframes %u: at most %u subframes per batch", cfg->max_subframes, (uint32_t)LTEPHY_MAX_BATCH_SUBFRAMES);
@@ -242,7 +243,7 @@ extern "C" int ltephy_create(const ltephy_cfg_t* cfg, ltephy_t** out)
   }
   if (h->table_err != cudaSuccess) return fail(LTEPHY_ERROR, "table upload failed: %s", cudaGetErrorString(h->table_err));
   const size_t S = cfg->max_subframes, g = (size_t)14 * c.nsc;
-  if (h->d_iq.reserve(S * c.nof_rx * c.sf_len) || h->d_sym.reserve(S * c.nof_rx * g) || h->d_pil.reserve(S * c.nof_ports * c.nof_rx * 4 * 2 * c.nof_prb) ||
+  if (h->d_iq.reserve(S * c.nof_rx * c.sf_len * iq_sample_bytes(cfg->iq_format)) || h->d_sym.reserve(S * c.nof_rx * g) || h->d_pil.reserve(S * c.nof_ports * c.nof_rx * 4 * 2 * c.nof_prb) ||
       h->d_llr.reserve(S * LLR_STRIDE) || h->d_info.reserve(S) || h->d_cands.reserve(S * LTEPHY_MAX_LOC * LTEPHY_MAX_SIZES) || h->d_vwork.reserve(S * (LTEPHY_MAX_LOC / 2) * LTEPHY_MAX_SIZES * 2 + 16) ||
       h->h_info.reserve(S) || h->d_compact.reserve(S) || h->h_compact.reserve(S) || h->d_rm.reserve((size_t)4 << 20) || h->d_pi.reserve((size_t)188 * 6144))
     return fail(LTEPHY_ERROR, "device allocation failed");
@@ -315,7 +316,7 @@ extern "C" int      ltephy_last_timing(ltephy_t* h, float ms[4])
 // Phase A over n subframes.  iq_host != nullptr: the samples are still in (pinned) host memory and are copied first, as ONE
 // transfer: splitting it into chunks with per-chunk kernels was measured and is slower with several pipelines (the chunks of
 // different batches interleave on the copy engine, so every batch's front end finishes later: e2e 87-91 k -> 82 k subframes/s).
-static int phase_a_common(ltephy* h, const float2* iq_dev, const float2* iq_host, const uint32_t* tti, uint32_t n)
+static int phase_a_common(ltephy* h, const void* iq_dev, const void* iq_host, const uint32_t* tti, uint32_t n)
 {
   for (uint32_t i = 0; i < n; i++) {
     memset(&h->h_info.p[i], 0, sizeof(DevSfInfo));
@@ -329,11 +330,11 @@ static int phase_a_common(ltephy* h, const float2* iq_dev, const float2* iq_host
     std::lock_guard<std::mutex> lk(g_h2d_mtx);
     cudaEvent_t& last = g_h2d_last[h->cfg.device & 63];
     if (last && last != h->ev_h2d) CU(cudaStreamWaitEvent(h->stream, last, 0));
-    CU(cudaMemcpyAsync(h->d_iq.p, iq_host, (size_t)n * c.nof_rx * c.sf_len * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
+    CU(cudaMemcpyAsync(h->d_iq.p, iq_host, (size_t)n * c.nof_rx * c.sf_len * iq_sample_bytes(h->cfg.iq_format), cudaMemcpyHostToDevice, h->stream));
     CU(cudaEventRecord(h->ev_h2d, h->stream));
     last = h->ev_h2d;
   }
-  launch_frontend(c, iq_dev, h->d_sym.p, h->d_pil.p, h->d_llr.p, h->d_info.p, n, h->stream, &h->launches);
+  launch_frontend(c, iq_dev, h->cfg.iq_format, h->d_sym.p, h->d_pil.p, h->d_llr.p, h->d_info.p, n, h->stream, &h->launches);
   launch_viterbi(c, h->d_llr.p, h->d_info.p, h->d_cands.p, h->d_vwork.p, n, h->stream, &h->launches);
   launch_compact(c, h->d_info.p, h->d_cands.p, h->d_compact.p, n, h->stream, &h->launches);
   CU(cudaEventRecord(h->ev[1], h->stream));
@@ -341,19 +342,21 @@ static int phase_a_common(ltephy* h, const float2* iq_dev, const float2* iq_host
   h->n_cur = n;
   return LTEPHY_SUCCESS;
 }
-extern "C" int ltephy_submit_iq(ltephy_t* h, const float* iq, const uint32_t* tti, uint32_t n)
+extern "C" int ltephy_submit_iq(ltephy_t* h, const void* iq, const uint32_t* tti, uint32_t n)
 {
   if (!h || !iq || !tti || n == 0 || n > h->cfg.max_subframes) return fail(LTEPHY_ERROR_INVALID_INPUTS, "submit_iq: bad arguments");
   CU(cudaSetDevice(h->cfg.device));
   CU(cudaEventRecord(h->ev[0], h->stream));
-  return phase_a_common(h, h->d_iq.p, reinterpret_cast<const float2*>(iq), tti, n);
+  return phase_a_common(h, h->d_iq.p, iq, tti, n);
 }
 extern "C" int ltephy_submit_iq_device(ltephy_t* h, const void* iq_dev, const uint32_t* tti, uint32_t n)
 {
   if (!h || !iq_dev || !tti || n == 0 || n > h->cfg.max_subframes) return fail(LTEPHY_ERROR_INVALID_INPUTS, "submit_iq_device: bad arguments");
+  if (iq_misaligned(iq_dev, h->cfg.iq_format))
+    return fail(LTEPHY_ERROR_INVALID_INPUTS, "submit_iq_device: iq_dev not aligned to its %zu-byte samples", iq_sample_bytes(h->cfg.iq_format));
   CU(cudaSetDevice(h->cfg.device));
   CU(cudaEventRecord(h->ev[0], h->stream));
-  return phase_a_common(h, reinterpret_cast<const float2*>(iq_dev), nullptr, tti, n); // read in place: the caller keeps the buffer alive until phase A is fetched
+  return phase_a_common(h, iq_dev, nullptr, tti, n); // read in place: the caller keeps the buffer alive until phase A is fetched
 }
 // log10f / atan2f of the bit-exact device sums are taken on the host (DESIGN.md section 2); idempotent
 extern "C" void ltephy_finalize_info(ltephy_sf_info_t* info, uint32_t n, uint32_t nof_ports, uint32_t nof_rx)
@@ -1078,26 +1081,29 @@ static int ul_table_for(ltephy* h, uint32_t kind, uint32_t M, uint32_t ncs, uint
 }
 
 // ltephy_submit_ul / _device: iq_host is copied into d_uliq first; iq_dev is demodulated in place; both NULL re-decodes the previous symbols
-static int submit_ul_common(ltephy_t* h, const float2* iq_host, const float2* iq_dev, const uint32_t* tti, uint32_t n, const ltephy_ul_grant_t* gin,
+static int submit_ul_common(ltephy_t* h, const void* iq_host, const void* iq_dev, const uint32_t* tti, uint32_t n, const ltephy_ul_grant_t* gin,
                             uint32_t ng)
 {
   if (!h || !tti || n == 0 || n > h->cfg.max_subframes || (!gin && ng)) return fail(LTEPHY_ERROR_INVALID_INPUTS, "submit_ul: bad arguments");
   if (!h->ulcfg_set) return fail(LTEPHY_ERROR_INVALID_INPUTS, "submit_ul: ltephy_set_ul_cfg has not been called");
   const bool have_iq = iq_host || iq_dev;
   if (!have_iq && h->n_ul != n) return fail(LTEPHY_ERROR_INVALID_INPUTS, "submit_ul: no IQ given and the previous call demodulated %u subframes, not %u", h->n_ul, n);
+  if (iq_misaligned(iq_dev, h->cfg.iq_format))
+    return fail(LTEPHY_ERROR_INVALID_INPUTS, "submit_ul_device: iq_ul_dev not aligned to its %zu-byte samples", iq_sample_bytes(h->cfg.iq_format));
   CU(cudaSetDevice(h->cfg.device));
   const DevCell& c = h->dc;
   const size_t   A = c.ul_nof_rx; // samples and symbols are [n][A][..]: their offsets stay 64-bit (65 535 x 2 x 14 x 1200 x 8 bytes > 2^32)
-  if ((iq_host && h->d_uliq.reserve((size_t)h->cfg.max_subframes * A * c.sf_len)) || h->d_ulsym.reserve((size_t)h->cfg.max_subframes * A * 14 * c.nsc) ||
+  const size_t   xb = iq_sample_bytes(h->cfg.iq_format);
+  if ((iq_host && h->d_uliq.reserve((size_t)h->cfg.max_subframes * A * c.sf_len * xb)) || h->d_ulsym.reserve((size_t)h->cfg.max_subframes * A * 14 * c.nsc) ||
       h->d_ulpool.reserve((size_t)1 << 20))
     return fail(LTEPHY_ERROR, "device allocation failed");
   CU(cudaEventRecord(h->ev[2], h->stream));
   if (have_iq) { // NULL: the demodulated symbols of the previous call stay (srsran_enb_ul_fft once, then one decode per grant)
     if (iq_host) {
-      CU(cudaMemcpyAsync(h->d_uliq.p, iq_host, (size_t)n * A * c.sf_len * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
+      CU(cudaMemcpyAsync(h->d_uliq.p, iq_host, (size_t)n * A * c.sf_len * xb, cudaMemcpyHostToDevice, h->stream));
       iq_dev = h->d_uliq.p;
     }
-    launch_ul_ofdm(c, iq_dev, h->d_ulsym.p, n, h->stream, &h->launches);
+    launch_ul_ofdm(c, iq_dev, h->cfg.iq_format, h->d_ulsym.p, n, h->stream, &h->launches);
   }
   h->n_ul = n;
   // jobs
@@ -1155,13 +1161,13 @@ static int submit_ul_common(ltephy_t* h, const float2* iq_host, const float2* iq
   CU(cudaGetLastError());
   return LTEPHY_SUCCESS;
 }
-extern "C" int ltephy_submit_ul(ltephy_t* h, const float* iq_ul, const uint32_t* tti, uint32_t n, const ltephy_ul_grant_t* gin, uint32_t ng)
+extern "C" int ltephy_submit_ul(ltephy_t* h, const void* iq_ul, const uint32_t* tti, uint32_t n, const ltephy_ul_grant_t* gin, uint32_t ng)
 {
-  return submit_ul_common(h, reinterpret_cast<const float2*>(iq_ul), nullptr, tti, n, gin, ng);
+  return submit_ul_common(h, iq_ul, nullptr, tti, n, gin, ng);
 }
 extern "C" int ltephy_submit_ul_device(ltephy_t* h, const void* iq_ul_dev, const uint32_t* tti, uint32_t n, const ltephy_ul_grant_t* gin, uint32_t ng)
 {
-  return submit_ul_common(h, nullptr, static_cast<const float2*>(iq_ul_dev), tti, n, gin, ng); // read in place until ltephy_get_ul
+  return submit_ul_common(h, nullptr, iq_ul_dev, tti, n, gin, ng); // read in place until ltephy_get_ul
 }
 
 extern "C" int ltephy_get_ul(ltephy_t* h, ltephy_tb_result_t* results, ltephy_ul_chest_t* chest, uint8_t* payload, size_t payload_cap)

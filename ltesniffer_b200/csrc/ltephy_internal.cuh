@@ -26,6 +26,10 @@ static inline int fail(int code, const char* fmt, ...)
   ltephy_g_err = buf;
   return code;
 }
+// bytes of one complex sample of iq_format fmt (LTEPHY_IQ_*): sizes every sample buffer and host-to-device copy of an input
+static inline size_t iq_sample_bytes(uint32_t fmt) { return fmt == LTEPHY_IQ_SC16 ? 4 : fmt == LTEPHY_IQ_SC8 ? 2 : 8; }
+// integer samples in device memory are loaded as short2 / char2, so their pointer must be aligned to the sample; cf32 pointers are taken as given
+static inline bool iq_misaligned(const void* p, uint32_t fmt) { return fmt != LTEPHY_IQ_CF32 && (uintptr_t)p % iq_sample_bytes(fmt); }
 #define CU(x)                                                                                      \
   do {                                                                                             \
     cudaError_t e_ = (x);                                                                          \
@@ -141,7 +145,8 @@ struct ltephy {
   uint64_t                     launches  = 0;
 
   // phase A
-  DevBuf<float2>        d_iq, d_sym, d_pil, d_ce; // d_pil: smoothed CRS estimates [n][port][rx][4][2 nof_prb]; d_ce: interpolated grid, filled on demand (tap)
+  DevBuf<uint8_t>       d_iq;                     // samples of the batch in cfg.iq_format
+  DevBuf<float2>        d_sym, d_pil, d_ce; // d_pil: smoothed CRS estimates [n][port][rx][4][2 nof_prb]; d_ce: interpolated grid, filled on demand (tap)
   DevBuf<float>         d_llr;
   DevBuf<DevSfInfo>     d_info;
   DevBuf<ltephy_cand_t> d_cands;
@@ -209,7 +214,8 @@ struct ltephy {
   ltephy_ul_cfg_t            ulcfg{};
   bool                       ulcfg_set = false;
   uint32_t                   n_prs[20]{}, ul_u[20]{}, ul_v[20]{}; // per slot: n_PRS, base-sequence group u and sequence v
-  DevBuf<float2>             d_uliq, d_ulsym, d_ulpool; // d_ulpool: pool of DMRS sequences and IDFT twiddles (pool_append)
+  DevBuf<uint8_t>            d_uliq;                    // UL samples in cfg.iq_format
+  DevBuf<float2>             d_ulsym, d_ulpool; // d_ulpool: pool of DMRS sequences and IDFT twiddles (pool_append)
   DevBuf<DevUlGrant>         d_ulgrants;
   DevBuf<DevUlChest>         d_ulchest;
   PinBuf<DevUlChest>         h_ulchest;

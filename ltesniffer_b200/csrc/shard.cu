@@ -284,7 +284,7 @@ extern "C" int ltephy_decode_subframes_sharded(ltephy_shard_t* sh, ltephy_t* h, 
   double t[10];
   t[0]  = now_ms();
   // ---- phase A + pack (asynchronous) ----------------------------------------------------------------
-  int r = iq_on_device ? ltephy_submit_iq_device(h, iq, tti, n) : ltephy_submit_iq(h, (const float*)iq, tti, n);
+  int r = iq_on_device ? ltephy_submit_iq_device(h, iq, tti, n) : ltephy_submit_iq(h, iq, tti, n);
   if (r) return r;
   if ((r = pack_current(h, sl))) return r;
   t[1] = now_ms();

@@ -18,7 +18,8 @@ struct ltephy_sync {
   Stream            stream;
   float             ep[3]{};
   std::vector<float2> dpss; // [3][62]
-  DevBuf<float2>    d_x, d_rep, d_W, d_dpss, d_Y;
+  DevBuf<uint8_t>   d_x; // samples in cfg.iq_format
+  DevBuf<float2>    d_rep, d_W, d_dpss, d_Y;
   DevBuf<float>     d_seq, d_m, d_fold, d_rm, d_ref, d_sss;
   DevBuf<float4>    d_c12;
   DevBuf<SyncPeak>  d_pk;
@@ -87,6 +88,8 @@ extern "C" int ltephy_sync_create(const ltephy_sync_cfg_t* cfg, ltephy_sync_t** 
   if (N < 128 || N > 2048 || N % 128 || (M & (M - 1)) || cfg->nof_rx < 1 || cfg->nof_rx > 2)
     return fail(LTEPHY_ERROR_INVALID_INPUTS, "sync_create: symbol size %u / %u antennas not supported", N, cfg->nof_rx);
   if (cfg->max_samples < 75ull * N + N) return fail(LTEPHY_ERROR_INVALID_INPUTS, "sync_create: max_samples below one half-frame plus a symbol");
+  if (cfg->iq_format > LTEPHY_IQ_SC8)
+    return fail(LTEPHY_ERROR_INVALID_INPUTS, "sync_create: iq_format %u: LTEPHY_IQ_CF32 (0), LTEPHY_IQ_SC16 (1) or LTEPHY_IQ_SC8 (2)", cfg->iq_format);
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail(LTEPHY_ERROR, "no CUDA device: this library has no CPU path");
   CU(cudaSetDevice(cfg->device));
@@ -109,7 +112,7 @@ extern "C" int ltephy_sync_create(const ltephy_sync_cfg_t* cfg, ltephy_sync_t** 
     for (uint32_t n1 = 0; n1 < 168; n1++)
       for (uint32_t q = 0; q < 2; q++) sss_seq(n1, u, q, &seq[((u * 168 + n1) * 2 + q) * 62]);
   if (h->d_rep.reserve(rep.size()) || h->d_W.reserve(N) || h->d_dpss.reserve(3 * 62) || h->d_seq.reserve(seq.size()) ||
-      h->d_x.reserve((size_t)h->A * cfg->max_samples) || h->d_m.reserve(3 * h->Jmax) || h->d_fold.reserve(3 * SYNC_BINS) ||
+      h->d_x.reserve((size_t)h->A * cfg->max_samples * iq_sample_bytes(cfg->iq_format)) || h->d_m.reserve(3 * h->Jmax) || h->d_fold.reserve(3 * SYNC_BINS) ||
       h->d_rm.reserve((size_t)3 * h->nhmax * h->NR) || h->d_ref.reserve(3 * h->NR) || h->d_sss.reserve(3 * 336) ||
       h->d_c12.reserve((size_t)3 * h->nhmax * h->A) || h->d_pk.reserve(3) || h->d_Y.reserve((size_t)3 * h->nhmax * h->A * 124))
     return fail(LTEPHY_ERROR, "sync_create: device allocation failed");
@@ -137,7 +140,7 @@ static int sync_check(ltephy_sync_t* h, const void* iq, uint64_t L, ltephy_cell_
   return LTEPHY_SUCCESS;
 }
 
-int sync_run(ltephy_sync_t* h, const float2* x, uint64_t lda, uint64_t L, ltephy_cell_t* out)
+int sync_run(ltephy_sync_t* h, const void* x, uint64_t lda, uint64_t L, ltephy_cell_t* out)
 {
   const uint32_t N = h->N, D = h->D, CP6 = 9 * D;
   const uint64_t HF = 75ull * N, FR = 150ull * N;
@@ -145,7 +148,7 @@ int sync_run(ltephy_sync_t* h, const float2* x, uint64_t lda, uint64_t L, ltephy
   g.x = x, g.lda = lda, g.L = L, g.J = (L - N) / D + 1, g.N = N, g.D = D, g.A = h->A, g.nh = (uint32_t)((L - N) / HF + 1);
   g.rep = h->d_rep.p, g.W = h->d_W.p;
   for (int u = 0; u < 3; u++) g.ep[u] = h->ep[u];
-  if (launch_sync_pss(g, h->d_m.p, h->d_fold.p, h->d_pk.p, h->d_rm.p, h->d_c12.p, h->d_ref.p, h->stream, &h->launches))
+  if (launch_sync_pss(g, h->cfg.iq_format, h->d_m.p, h->d_fold.p, h->d_pk.p, h->d_rm.p, h->d_c12.p, h->d_ref.p, h->stream, &h->launches))
     return fail(LTEPHY_ERROR, "cell_search: PSS kernels failed: %s", cudaGetErrorString(cudaGetLastError()));
   SyncPeak pk[3];
   CU(cudaMemcpyAsync(pk, h->d_pk.p, sizeof(pk), cudaMemcpyDeviceToHost, h->stream));
@@ -172,7 +175,7 @@ int sync_run(ltephy_sync_t* h, const float2* x, uint64_t lda, uint64_t L, ltephy
     o.nof_half_frames  = s.nH[u];
   }
   s.nhmax = std::max(s.nH[0], std::max(s.nH[1], s.nH[2]));
-  if (launch_sync_sss(g, s, h->d_Y.p, h->d_sss.p, h->stream, &h->launches))
+  if (launch_sync_sss(g, h->cfg.iq_format, s, h->d_Y.p, h->d_sss.p, h->stream, &h->launches))
     return fail(LTEPHY_ERROR, "cell_search: SSS kernels failed: %s", cudaGetErrorString(cudaGetLastError()));
   std::vector<float> tab(3 * 336);
   CU(cudaMemcpyAsync(tab.data(), h->d_sss.p, tab.size() * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
@@ -207,19 +210,21 @@ int sync_run(ltephy_sync_t* h, const float2* x, uint64_t lda, uint64_t L, ltephy
   return LTEPHY_SUCCESS;
 }
 
-extern "C" int ltephy_cell_search(ltephy_sync_t* h, const float* iq, uint64_t nof_samples, ltephy_cell_t out[3])
+extern "C" int ltephy_cell_search(ltephy_sync_t* h, const void* iq, uint64_t nof_samples, ltephy_cell_t out[3])
 {
   if (int r = sync_check(h, iq, nof_samples, out)) return r;
   CU(cudaSetDevice(h->cfg.device));
-  CU(cudaMemcpyAsync(h->d_x.p, iq, (size_t)h->A * nof_samples * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
+  CU(cudaMemcpyAsync(h->d_x.p, iq, (size_t)h->A * nof_samples * iq_sample_bytes(h->cfg.iq_format), cudaMemcpyHostToDevice, h->stream));
   return sync_run(h, h->d_x.p, nof_samples, nof_samples, out);
 }
 
 extern "C" int ltephy_cell_search_device(ltephy_sync_t* h, const void* iq_dev, uint64_t nof_samples, ltephy_cell_t out[3])
 {
   if (int r = sync_check(h, iq_dev, nof_samples, out)) return r;
+  if (iq_misaligned(iq_dev, h->cfg.iq_format))
+    return fail(LTEPHY_ERROR_INVALID_INPUTS, "cell_search_device: iq_dev not aligned to its %zu-byte samples", iq_sample_bytes(h->cfg.iq_format));
   CU(cudaSetDevice(h->cfg.device));
-  return sync_run(h, static_cast<const float2*>(iq_dev), nof_samples, nof_samples, out);
+  return sync_run(h, iq_dev, nof_samples, nof_samples, out);
 }
 
 extern "C" int ltephy_sync_tap(ltephy_sync_t* h, int what, void* dst, size_t bytes)

@@ -21,7 +21,8 @@ struct ltephy_track {
   uint32_t           N = 0, A = 0, W = 0, SF = 0;
   float              ep = 0.0f, thr = 0.0f, max_ppm = 50.0f;
   Stream             stream;
-  DevBuf<float2>     d_rep, d_x, d_cut, d_tabA, d_tabB, d_c;
+  DevBuf<uint8_t>    d_x; // samples of the push in cfg.iq_format
+  DevBuf<float2>     d_rep, d_cut, d_tabA, d_tabB, d_c;
   DevBuf<float>      d_m;
   DevBuf<TrackWin>   d_win;
   DevBuf<uint64_t>   d_pos, d_start;
@@ -45,7 +46,8 @@ struct ltephy_track {
   double           ul_ratio = 1.0;
   int32_t          ul_off   = 0;
   uint32_t         ul_A     = 1;
-  DevBuf<float2>   d_xu, d_cutu, d_tabAu, d_tabBu;
+  DevBuf<uint8_t>  d_xu; // UL samples of the push in cfg.iq_format
+  DevBuf<float2>   d_cutu, d_tabAu, d_tabBu;
   DevBuf<uint64_t> d_startu;
 };
 
@@ -82,6 +84,8 @@ extern "C" int ltephy_track_create(const ltephy_track_cfg_t* cfg, ltephy_track_t
   if (!(cfg->max_ppm >= 0.0f && cfg->max_ppm <= 1000.0f)) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_create: max_ppm outside 0..1000");
   if (cfg->max_subframes < 1 || cfg->max_subframes > 20000) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_create: max_subframes outside 1..20000");
   if (cfg->flags & ~(LTEPHY_TRACK_NO_CFO | LTEPHY_TRACK_REACQUIRE)) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_create: unknown flags 0x%x", cfg->flags);
+  if (cfg->iq_format > LTEPHY_IQ_SC8)
+    return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_create: iq_format %u: LTEPHY_IQ_CF32 (0), LTEPHY_IQ_SC16 (1) or LTEPHY_IQ_SC8 (2)", cfg->iq_format);
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail(LTEPHY_ERROR, "no CUDA device: this library has no CPU path");
   CU(cudaSetDevice(cfg->device));
@@ -96,7 +100,7 @@ extern "C" int ltephy_track_create(const ltephy_track_cfg_t* cfg, ltephy_track_t
   // with 2 antennas) stays unused: the find reads the push's samples in place through sync_run.
   if (cfg->flags & LTEPHY_TRACK_REACQUIRE) {
     ltephy_sync_cfg_t sc{};
-    sc.symbol_sz = N, sc.nof_rx = h->A, sc.max_samples = 151ull * N, sc.device = cfg->device;
+    sc.symbol_sz = N, sc.nof_rx = h->A, sc.max_samples = 151ull * N, sc.device = cfg->device, sc.iq_format = cfg->iq_format;
     ltephy_sync_t* sync = nullptr;
     if (int r = ltephy_sync_create(&sc, &sync)) return r;
     h->sync.reset(sync);
@@ -131,7 +135,7 @@ static int track_metrics(ltephy_track_t* h, const TrackArgs& g, const std::vecto
   if (win.empty()) return LTEPHY_SUCCESS;
   if (h->d_win.reserve(win.size()) || h->d_m.reserve(m.size())) return fail(LTEPHY_ERROR, "track_push: device allocation failed");
   CU(cudaMemcpyAsync(h->d_win.p, win.data(), win.size() * sizeof(TrackWin), cudaMemcpyHostToDevice, h->stream));
-  if (launch_track_metric(g, h->d_win.p, (uint32_t)win.size(), stride, stride, h->d_m.p, h->stream))
+  if (launch_track_metric(g, h->cfg.iq_format, h->d_win.p, (uint32_t)win.size(), stride, stride, h->d_m.p, h->stream))
     return fail(LTEPHY_ERROR, "track_push: metric kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
   CU(cudaMemcpyAsync(m.data(), h->d_m.p, m.size() * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
   CU(cudaStreamSynchronize(h->stream));
@@ -140,13 +144,14 @@ static int track_metrics(ltephy_track_t* h, const TrackArgs& g, const std::vecto
 
 // one find window (lteo_track's track_find): the cell search on the samples [f0, f0 + FR + N) of x, read in place; found: resume at the
 // window's first subframe boundary with the subframe number of its SSS, otherwise step one frame on
-static int track_find(ltephy_track_t* h, const float2* x, uint64_t first, uint64_t n, bool& found)
+static int track_find(ltephy_track_t* h, const void* x, uint64_t first, uint64_t n, bool& found)
 {
   const uint32_t N = h->N, SF = h->SF;
   const uint64_t FR = 150ull * N;
   CU(cudaStreamSynchronize(h->stream)); // the push's copy of x runs on the tracker's stream, the search on the sync handle's
   ltephy_cell_t res[3];
-  if (int r = sync_run(h->sync.get(), x + (h->f0 - (int64_t)first), n, FR + N, res)) return r;
+  const uint8_t* w = static_cast<const uint8_t*>(x) + (uint64_t)(h->f0 - (int64_t)first) * iq_sample_bytes(h->cfg.iq_format);
+  if (int r = sync_run(h->sync.get(), w, n, FR + N, res)) return r;
   const ltephy_cell_t* c = nullptr;
   for (uint32_t i = 0; i < 3; i++)
     if (res[i].n_id_2 == h->cfg.pci % 3) c = &res[i];
@@ -166,7 +171,7 @@ static int track_find(ltephy_track_t* h, const float2* x, uint64_t first, uint64
   return LTEPHY_SUCCESS;
 }
 
-static int track_run(ltephy_track_t* h, const float2* x, const float2* xu, uint64_t first, uint64_t n, ltephy_track_out_t* out, const void** ul_iq_dev)
+static int track_run(ltephy_track_t* h, const void* x, const void* xu, uint64_t first, uint64_t n, ltephy_track_out_t* out, const void** ul_iq_dev)
 {
   const uint32_t N = h->N, SF = h->SF, W = h->W, maxsf = h->cfg.max_subframes;
   const uint64_t end = first + n;
@@ -287,7 +292,7 @@ static int track_run(ltephy_track_t* h, const float2* x, const float2* xu, uint6
   std::vector<float2> c((size_t)nh * h->A * 2);
   if (nh) {
     CU(cudaMemcpyAsync(h->d_pos.p, hpos.data(), nh * sizeof(uint64_t), cudaMemcpyHostToDevice, h->stream));
-    if (launch_track_sums(g, h->d_pos.p, nh, h->d_c.p, h->stream))
+    if (launch_track_sums(g, h->cfg.iq_format, h->d_pos.p, nh, h->d_c.p, h->stream))
       return fail(LTEPHY_ERROR, "track_push: sum kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
     CU(cudaMemcpyAsync(c.data(), h->d_c.p, c.size() * sizeof(float2), cudaMemcpyDeviceToHost, h->stream));
     CU(cudaStreamSynchronize(h->stream));
@@ -329,7 +334,7 @@ static int track_run(ltephy_track_t* h, const float2* x, const float2* xu, uint6
     CU(cudaMemcpyAsync(h->d_start.p, spos.data(), nsf * sizeof(uint64_t), cudaMemcpyHostToDevice, h->stream));
     CU(cudaMemcpyAsync(h->d_tabA.p, tabA.data(), tabA.size() * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
     CU(cudaMemcpyAsync(h->d_tabB.p, tabB.data(), tabB.size() * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
-    if (launch_track_cut(g, h->d_start.p, h->d_tabA.p, h->d_tabB.p, nsf, h->d_cut.p, h->stream))
+    if (launch_track_cut(g, h->cfg.iq_format, h->d_start.p, h->d_tabA.p, h->d_tabB.p, nsf, h->d_cut.p, h->stream))
       return fail(LTEPHY_ERROR, "track_push: cut kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
     if (xu) { // the same kernel on the UL carrier: its antennas, start + ul_offset, the UL tables
       std::vector<uint64_t> upos(nsf);
@@ -339,7 +344,7 @@ static int track_run(ltephy_track_t* h, const float2* x, const float2* xu, uint6
       CU(cudaMemcpyAsync(h->d_startu.p, upos.data(), nsf * sizeof(uint64_t), cudaMemcpyHostToDevice, h->stream));
       CU(cudaMemcpyAsync(h->d_tabAu.p, tabAu.data(), tabAu.size() * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
       CU(cudaMemcpyAsync(h->d_tabBu.p, tabBu.data(), tabBu.size() * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
-      if (launch_track_cut(gu, h->d_startu.p, h->d_tabAu.p, h->d_tabBu.p, nsf, h->d_cutu.p, h->stream))
+      if (launch_track_cut(gu, h->cfg.iq_format, h->d_startu.p, h->d_tabAu.p, h->d_tabBu.p, nsf, h->d_cutu.p, h->stream))
         return fail(LTEPHY_ERROR, "track_push: UL cut kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
     }
     CU(cudaStreamSynchronize(h->stream));
@@ -363,13 +368,14 @@ static int track_check(ltephy_track_t* h, const void* iq, uint64_t first, uint64
   return LTEPHY_SUCCESS;
 }
 
-extern "C" int ltephy_track_push(ltephy_track_t* h, const float* iq, uint64_t first_sample, uint64_t nof_samples, ltephy_track_out_t* out)
+extern "C" int ltephy_track_push(ltephy_track_t* h, const void* iq, uint64_t first_sample, uint64_t nof_samples, ltephy_track_out_t* out)
 {
   if (int r = track_check(h, iq, first_sample, nof_samples, out, false)) return r;
   CU(cudaSetDevice(h->cfg.device));
   if (nof_samples) {
-    if (h->d_x.reserve((size_t)h->A * nof_samples)) return fail(LTEPHY_ERROR, "track_push: device allocation failed");
-    CU(cudaMemcpyAsync(h->d_x.p, iq, (size_t)h->A * nof_samples * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
+    const size_t bytes = (size_t)h->A * nof_samples * iq_sample_bytes(h->cfg.iq_format);
+    if (h->d_x.reserve(bytes)) return fail(LTEPHY_ERROR, "track_push: device allocation failed");
+    CU(cudaMemcpyAsync(h->d_x.p, iq, bytes, cudaMemcpyHostToDevice, h->stream));
   }
   return track_run(h, h->d_x.p, nullptr, first_sample, nof_samples, out, nullptr);
 }
@@ -377,8 +383,10 @@ extern "C" int ltephy_track_push(ltephy_track_t* h, const float* iq, uint64_t fi
 extern "C" int ltephy_track_push_device(ltephy_track_t* h, const void* iq_dev, uint64_t first_sample, uint64_t nof_samples, ltephy_track_out_t* out)
 {
   if (int r = track_check(h, iq_dev, first_sample, nof_samples, out, false)) return r;
+  if (iq_misaligned(iq_dev, h->cfg.iq_format))
+    return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_push_device: iq_dev not aligned to its %zu-byte samples", iq_sample_bytes(h->cfg.iq_format));
   CU(cudaSetDevice(h->cfg.device));
-  return track_run(h, static_cast<const float2*>(iq_dev), nullptr, first_sample, nof_samples, out, nullptr);
+  return track_run(h, iq_dev, nullptr, first_sample, nof_samples, out, nullptr);
 }
 
 extern "C" int ltephy_track_set_ul(ltephy_track_t* h, const ltephy_track_ul_cfg_t* cfg)
@@ -400,17 +408,18 @@ extern "C" int ltephy_track_set_ul(ltephy_track_t* h, const ltephy_track_ul_cfg_
   return LTEPHY_SUCCESS;
 }
 
-extern "C" int ltephy_track_push_ul(ltephy_track_t* h, const float* iq, const float* iq_ul, uint64_t first_sample, uint64_t nof_samples,
+extern "C" int ltephy_track_push_ul(ltephy_track_t* h, const void* iq, const void* iq_ul, uint64_t first_sample, uint64_t nof_samples,
                                     ltephy_track_out_t* out, const void** ul_iq_dev)
 {
   if (!iq_ul && nof_samples) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_push_ul: null argument");
   if (int r = track_check(h, iq, first_sample, nof_samples, out, true)) return r;
   CU(cudaSetDevice(h->cfg.device));
   if (nof_samples) {
-    if (h->d_x.reserve((size_t)h->A * nof_samples) || h->d_xu.reserve((size_t)h->ul_A * nof_samples))
+    const size_t xb = iq_sample_bytes(h->cfg.iq_format);
+    if (h->d_x.reserve((size_t)h->A * nof_samples * xb) || h->d_xu.reserve((size_t)h->ul_A * nof_samples * xb))
       return fail(LTEPHY_ERROR, "track_push_ul: device allocation failed");
-    CU(cudaMemcpyAsync(h->d_x.p, iq, (size_t)h->A * nof_samples * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
-    CU(cudaMemcpyAsync(h->d_xu.p, iq_ul, (size_t)h->ul_A * nof_samples * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
+    CU(cudaMemcpyAsync(h->d_x.p, iq, (size_t)h->A * nof_samples * xb, cudaMemcpyHostToDevice, h->stream));
+    CU(cudaMemcpyAsync(h->d_xu.p, iq_ul, (size_t)h->ul_A * nof_samples * xb, cudaMemcpyHostToDevice, h->stream));
   }
   return track_run(h, h->d_x.p, h->d_xu.p, first_sample, nof_samples, out, ul_iq_dev);
 }
@@ -420,6 +429,8 @@ extern "C" int ltephy_track_push_ul_device(ltephy_track_t* h, const void* iq_dev
 {
   if (!iq_ul_dev && nof_samples) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_push_ul: null argument");
   if (int r = track_check(h, iq_dev, first_sample, nof_samples, out, true)) return r;
+  if (iq_misaligned(iq_dev, h->cfg.iq_format) || iq_misaligned(iq_ul_dev, h->cfg.iq_format))
+    return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_push_ul_device: iq_dev / iq_ul_dev not aligned to their %zu-byte samples", iq_sample_bytes(h->cfg.iq_format));
   CU(cudaSetDevice(h->cfg.device));
-  return track_run(h, static_cast<const float2*>(iq_dev), static_cast<const float2*>(iq_ul_dev), first_sample, nof_samples, out, ul_iq_dev);
+  return track_run(h, iq_dev, iq_ul_dev, first_sample, nof_samples, out, ul_iq_dev);
 }
