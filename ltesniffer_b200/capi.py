@@ -950,38 +950,38 @@ class Tracker:
             out["ul_iq"] = self._view(ul_ptr.value, (o.nof_subframes, 15 * self.cfg.symbol_sz) if A == 1 else (o.nof_subframes, A, 15 * self.cfg.symbol_sz))
         return out
 
+    def _push(self, dev, first_sample, *iqs):
+        """every push: iqs = (iq,) or (iq, iq_ul), host arrays or, with dev, contiguous tensors on this handle's device"""
+        if dev:
+            shapes, ptrs = [_dev_shape(q, self.iq_format) for q in iqs], [C.c_void_p(q.data_ptr()) for q in iqs]
+        else:
+            iqs = [_host_iq(q, self.iq_format) for q in iqs]
+            shapes, ptrs = [s for _, s in iqs], [_p(q) for q, _ in iqs]
+        ul = len(iqs) == 2
+        assert len(shapes[0]) == 2 and shapes[0][0] == self.cfg.nof_rx, shapes
+        assert not ul or int(np.prod(shapes[1])) == max(1, self.ul.nof_rx) * shapes[0][1], shapes
+        o, u = TrackOut(), C.c_void_p()
+        push = getattr(self.L, "ltephy_track_push" + "_ul" * ul + "_device" * dev)
+        r = push(self.h, *ptrs, first_sample, shapes[0][1], C.byref(o), *([C.byref(u)] if ul else []))
+        return self._done(r, o, u if ul else None)
+
     def push(self, iq, first_sample):
         """iq: complex64 [nof_rx][n] (host) of absolute samples first_sample ... -> dict(sf, hf: record arrays, iq: torch complex64
         [k][nof_rx][15 N] on the device (a copy of the tracker's cut), next_sample, remeasured, finds)"""
-        iq, shape = _host_iq(iq, self.iq_format)
-        assert len(shape) == 2 and shape[0] == self.cfg.nof_rx, iq.shape
-        o = TrackOut()
-        return self._done(self.L.ltephy_track_push(self.h, _p(iq), first_sample, shape[1], C.byref(o)), o)
+        return self._push(False, first_sample, iq)
 
     def push_device(self, iq, first_sample):
         """iq: torch complex64 tensor [nof_rx][n] (int16 / int8 [nof_rx][n][2]), contiguous, on this handle's device"""
-        shape = _dev_shape(iq, self.iq_format)
-        assert len(shape) == 2 and shape[0] == self.cfg.nof_rx
-        o = TrackOut()
-        return self._done(self.L.ltephy_track_push_device(self.h, C.c_void_p(iq.data_ptr()), first_sample, shape[1], C.byref(o)), o)
+        return self._push(True, first_sample, iq)
 
     def push_ul(self, iq, iq_ul, first_sample):
         """iq as push, iq_ul: complex64 [n] of the uplink antenna ([A][n] with A = 2 UL antennas), the same absolute samples -> push's dict plus
         ul_iq: torch complex64 [k][15 N] ([k][A][15 N]) on the device (a copy of the tracker's UL cut)"""
-        iq, shape = _host_iq(iq, self.iq_format)
-        iq_ul, ushape = _host_iq(iq_ul, self.iq_format)
-        assert len(shape) == 2 and shape[0] == self.cfg.nof_rx and int(np.prod(ushape)) == max(1, self.ul.nof_rx) * shape[1], (iq.shape, iq_ul.shape)
-        o, u = TrackOut(), C.c_void_p()
-        return self._done(self.L.ltephy_track_push_ul(self.h, _p(iq), _p(iq_ul), first_sample, shape[1], C.byref(o), C.byref(u)), o, u)
+        return self._push(False, first_sample, iq, iq_ul)
 
     def push_ul_device(self, iq, iq_ul, first_sample):
         """iq: torch complex64 [nof_rx][n], iq_ul: torch complex64 [n] ([A][n] with A = 2 UL antennas), both contiguous on this handle's device"""
-        shape, ushape = _dev_shape(iq, self.iq_format), _dev_shape(iq_ul, self.iq_format)
-        assert len(shape) == 2 and shape[0] == self.cfg.nof_rx
-        assert int(np.prod(ushape)) == max(1, self.ul.nof_rx) * shape[1]
-        o, u = TrackOut(), C.c_void_p()
-        return self._done(self.L.ltephy_track_push_ul_device(self.h, C.c_void_p(iq.data_ptr()), C.c_void_p(iq_ul.data_ptr()), first_sample, shape[1],
-                                                             C.byref(o), C.byref(u)), o, u)
+        return self._push(True, first_sample, iq, iq_ul)
 
 
 # ------------------------------------------------------------------------------------------------

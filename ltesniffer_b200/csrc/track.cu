@@ -16,16 +16,33 @@
 #define TRACK_MISS   4u    // half-frames in a row without lock after which records are flagged lost
 #define TRACK_LOCK_K 20.0f // lock: peak metric >= 20 / N; on noise-only captures no half-frame's peak came above 10.2 / N (DESIGN.md §2)
 
+// a carrier the tracker cuts: the downlink, and with ltephy_track_set_ul the uplink, whose A antennas are cut at start + off and rotated by
+// f ratio with their own factor tables
+struct TrackCarrier {
+  uint32_t         A     = 1;
+  int32_t          off   = 0;
+  double           ratio = 1.0;
+  DevBuf<uint8_t>  d_x; // samples of a host push in cfg.iq_format
+  DevBuf<float2>   d_cut, d_tabA, d_tabB;
+  DevBuf<uint64_t> d_start;
+  int              reserve(size_t nsf, uint32_t SF)
+  {
+    return d_cut.reserve(nsf * A * SF) || d_tabA.reserve(nsf * (SF / 128)) || d_tabB.reserve(nsf * 128) || d_start.reserve(nsf);
+  }
+};
+
 struct ltephy_track {
   ltephy_track_cfg_t cfg{};
-  uint32_t           N = 0, A = 0, W = 0, SF = 0;
+  uint32_t           N = 0, W = 0, SF = 0;
   float              ep = 0.0f, thr = 0.0f, max_ppm = 50.0f;
   Stream             stream;
-  DevBuf<uint8_t>    d_x; // samples of the push in cfg.iq_format
-  DevBuf<float2>     d_rep, d_cut, d_tabA, d_tabB, d_c;
+  DevBuf<float2>     d_rep, d_c;
   DevBuf<float>      d_m;
   DevBuf<TrackWin>   d_win;
-  DevBuf<uint64_t>   d_pos, d_start;
+  DevBuf<uint64_t>   d_pos;
+  TrackCarrier       car[2]; // the downlink, then the uplink
+  uint32_t           nc = 1; // carriers cut: 2 once the uplink is set
+  bool               pushed = false;
   // state: as lteo_track
   int64_t  s = 0;
   uint32_t k = 0;
@@ -41,30 +58,25 @@ struct ltephy_track {
   std::unique_ptr<ltephy_sync_t, decltype(&ltephy_sync_destroy)> sync{nullptr, ltephy_sync_destroy};
   std::vector<ltephy_track_sf_t> sf;
   std::vector<ltephy_track_hf_t> hf;
-  // the uplink carrier (ltephy_track_set_ul): ul_A antennas cut at start + ul_off with their own rotation tables
-  bool             pushed = false, ul = false;
-  double           ul_ratio = 1.0;
-  int32_t          ul_off   = 0;
-  uint32_t         ul_A     = 1;
-  DevBuf<uint8_t>  d_xu; // UL samples of the push in cfg.iq_format
-  DevBuf<float2>   d_cutu, d_tabAu, d_tabBu;
-  DevBuf<uint64_t> d_startu;
 };
 
-// the lowest absolute sample the pending DL window, and with the uplink set its UL window, still needs
-// in the find state, the window's first sample
+// the lowest absolute sample the pending window of any carrier still needs; in the find state, from the window's first sample
 static int64_t track_needed(const ltephy_track* h)
 {
-  const int64_t s = h->find ? h->f0 : h->s;
-  return h->ul && h->ul_off < 0 ? s + h->ul_off : s;
+  const int64_t s  = h->find ? h->f0 : h->s;
+  int64_t       lo = s;
+  for (uint32_t c = 0; c < h->nc; c++) lo = std::min(lo, s + h->car[c].off);
+  return lo;
 }
 
-// a subframe starting at s is cut only when its DL window, and with the uplink set its UL window, lie inside [first, end)
+// a subframe starting at s is cut only when the window of every carrier lies inside [first, end)
 static bool track_fits(const ltephy_track* h, int64_t s, uint64_t first, uint64_t end)
 {
-  if (!(s >= (int64_t)first && (uint64_t)s + h->SF <= end)) return false;
-  const int64_t su = s + (h->ul ? h->ul_off : 0);
-  return su >= (int64_t)first && (uint64_t)su + h->SF <= end;
+  for (uint32_t c = 0; c < h->nc; c++) {
+    const int64_t sc = s + h->car[c].off;
+    if (!(sc >= (int64_t)first && (uint64_t)sc + h->SF <= end)) return false;
+  }
+  return true;
 }
 
 static bool track_symbol_ok(uint32_t N)
@@ -91,7 +103,7 @@ extern "C" int ltephy_track_create(const ltephy_track_cfg_t* cfg, ltephy_track_t
   CU(cudaSetDevice(cfg->device));
   std::unique_ptr<ltephy_track, decltype(&ltephy_track_destroy)> owner(new ltephy_track(), ltephy_track_destroy);
   ltephy_track* const                                            h = owner.get();
-  h->cfg = *cfg, h->N = N, h->A = cfg->nof_rx, h->W = 9 * N / 128, h->SF = 15 * N;
+  h->cfg = *cfg, h->N = N, h->car[0].A = cfg->nof_rx, h->W = 9 * N / 128, h->SF = 15 * N;
   h->max_ppm = cfg->max_ppm > 0.0f ? cfg->max_ppm : 50.0f;
   h->thr     = TRACK_LOCK_K / (float)N;
   h->s = h->base = (int64_t)cfg->frame_offset, h->f = cfg->cfo_hz;
@@ -100,7 +112,7 @@ extern "C" int ltephy_track_create(const ltephy_track_cfg_t* cfg, ltephy_track_t
   // with 2 antennas) stays unused: the find reads the push's samples in place through sync_run.
   if (cfg->flags & LTEPHY_TRACK_REACQUIRE) {
     ltephy_sync_cfg_t sc{};
-    sc.symbol_sz = N, sc.nof_rx = h->A, sc.max_samples = 151ull * N, sc.device = cfg->device, sc.iq_format = cfg->iq_format;
+    sc.symbol_sz = N, sc.nof_rx = cfg->nof_rx, sc.max_samples = 151ull * N, sc.device = cfg->device, sc.iq_format = cfg->iq_format;
     ltephy_sync_t* sync = nullptr;
     if (int r = ltephy_sync_create(&sc, &sync)) return r;
     h->sync.reset(sync);
@@ -109,8 +121,8 @@ extern "C" int ltephy_track_create(const ltephy_track_cfg_t* cfg, ltephy_track_t
   std::vector<float2> rep(N), d62(62);
   h->ep = sync_pss_replica(N, cfg->pci % 3, d62.data(), rep.data());
   const size_t nsf = cfg->max_subframes;
-  if (h->d_rep.reserve(N) || h->d_cut.reserve(nsf * h->A * h->SF) || h->d_tabA.reserve(nsf * (h->SF / 128)) || h->d_tabB.reserve(nsf * 128) ||
-      h->d_start.reserve(nsf) || h->d_pos.reserve(nsf / 5 + 1) || h->d_c.reserve((nsf / 5 + 1) * h->A * 2) || h->d_win.reserve(nsf / 5 + 1))
+  if (h->d_rep.reserve(N) || h->car[0].reserve(nsf, h->SF) || h->d_pos.reserve(nsf / 5 + 1) || h->d_c.reserve((nsf / 5 + 1) * cfg->nof_rx * 2) ||
+      h->d_win.reserve(nsf / 5 + 1))
     return fail(LTEPHY_ERROR, "track_create: device allocation failed");
   CU(cudaMemcpy(h->d_rep.p, rep.data(), N * sizeof(float2), cudaMemcpyHostToDevice));
   h->sf.reserve(nsf), h->hf.reserve(nsf / 5 + 1);
@@ -171,12 +183,13 @@ static int track_find(ltephy_track_t* h, const void* x, uint64_t first, uint64_t
   return LTEPHY_SUCCESS;
 }
 
-static int track_run(ltephy_track_t* h, const void* x, const void* xu, uint64_t first, uint64_t n, ltephy_track_out_t* out, const void** ul_iq_dev)
+// x[c]: the device samples of carrier c
+static int track_run(ltephy_track_t* h, const void* const* x, uint64_t first, uint64_t n, ltephy_track_out_t* out, const void** ul_iq_dev)
 {
-  const uint32_t N = h->N, SF = h->SF, W = h->W, maxsf = h->cfg.max_subframes;
+  const uint32_t N = h->N, SF = h->SF, W = h->W, A = h->car[0].A, maxsf = h->cfg.max_subframes;
   const uint64_t end = first + n;
   TrackArgs      g{};
-  g.x = x, g.lda = n, g.N = N, g.A = h->A, g.rep = h->d_rep.p, g.ep = h->ep;
+  g.x = x[0], g.lda = n, g.N = N, g.A = A, g.rep = h->d_rep.p, g.ep = h->ep;
   // 1. predict: the subframes of this push from the state at its start (and again after a find), without corrections; each half-frame's
   //    window is the tracker's +-W plus the distance a clock max_ppm off moves the start over the predicted span, clamped to the samples fed
   std::vector<TrackWin> win;
@@ -215,7 +228,7 @@ static int track_run(ltephy_track_t* h, const void* x, const void* xu, uint64_t 
     if (h->find) { // a window is searched once all of its samples have been fed
       if ((uint64_t)h->f0 + 151ull * N > end) break;
       bool found = false;
-      if (int r = track_find(h, x, first, n, found)) return r;
+      if (int r = track_find(h, x[0], first, n, found)) return r;
       finds++;
       if (found) {
         if (int r = predict()) return r;
@@ -289,7 +302,7 @@ static int track_run(ltephy_track_t* h, const void* x, const void* xu, uint64_t 
   }
   const uint32_t nsf = (uint32_t)h->sf.size(), nh = (uint32_t)h->hf.size();
   // 3. the CFO sums at the chosen positions, then the loop in subframe order: each subframe keeps the offset that held before its half-frame
-  std::vector<float2> c((size_t)nh * h->A * 2);
+  std::vector<float2> c((size_t)nh * A * 2);
   if (nh) {
     CU(cudaMemcpyAsync(h->d_pos.p, hpos.data(), nh * sizeof(uint64_t), cudaMemcpyHostToDevice, h->stream));
     if (launch_track_sums(g, h->cfg.iq_format, h->d_pos.p, nh, h->d_c.p, h->stream))
@@ -297,15 +310,6 @@ static int track_run(ltephy_track_t* h, const void* x, const void* xu, uint64_t 
     CU(cudaMemcpyAsync(c.data(), h->d_c.p, c.size() * sizeof(float2), cudaMemcpyDeviceToHost, h->stream));
     CU(cudaStreamSynchronize(h->stream));
   }
-  // the cut's factor tables of subframe i for the offset f: exp(-j th 128 q) and exp(-j th q), th = 2 pi f / (15000 N), in double, rounded to float
-  auto tables = [&](std::vector<float2>& tA, std::vector<float2>& tB, uint32_t i, float f) {
-    const double th = 2.0 * M_PI * (double)f / (15000.0 * (double)N);
-    for (uint32_t q = 0; q < SF / 128; q++)
-      tA[(size_t)i * (SF / 128) + q] = make_float2((float)std::cos(-th * 128.0 * (double)q), (float)std::sin(-th * 128.0 * (double)q));
-    for (uint32_t q = 0; q < 128; q++) tB[(size_t)i * 128 + q] = make_float2((float)std::cos(-th * (double)q), (float)std::sin(-th * (double)q));
-  };
-  std::vector<float2> tabA((size_t)nsf * (SF / 128)), tabB((size_t)nsf * 128), tabAu, tabBu;
-  if (xu) tabAu.resize(tabA.size()), tabBu.resize(tabB.size());
   for (uint32_t i = 0, j = 0, ri = 0; i < nsf; i++) {
     ltephy_track_sf_t& o = h->sf[i];
     if (o.flags & LTEPHY_TRACK_REACQUIRED) {
@@ -313,13 +317,11 @@ static int track_run(ltephy_track_t* h, const void* x, const void* xu, uint64_t 
       ri++;
     }
     o.cfo_hz = h->f;
-    tables(tabA, tabB, i, h->f);
-    if (xu) tables(tabAu, tabBu, i, (float)((double)h->f * h->ul_ratio)); // f_ul = (float)(cfo_hz cfo_ratio)
     if (j < nh && h->hf[j].index == o.index) {
       ltephy_track_hf_t& q  = h->hf[j];
       float              sr = 0.0f, si = 0.0f;
-      for (uint32_t a = 0; a < h->A; a++) {
-        const float2 c1 = c[((size_t)j * h->A + a) * 2], c2 = c[((size_t)j * h->A + a) * 2 + 1];
+      for (uint32_t a = 0; a < A; a++) {
+        const float2 c1 = c[((size_t)j * A + a) * 2], c2 = c[((size_t)j * A + a) * 2 + 1];
         sr              = sr + (c2.x * c1.x + c2.y * c1.y);
         si              = si + (c2.y * c1.x - c2.x * c1.y);
       }
@@ -329,108 +331,100 @@ static int track_run(ltephy_track_t* h, const void* x, const void* xu, uint64_t 
       j++;
     }
   }
-  // 4. the cut
-  if (nsf) {
-    CU(cudaMemcpyAsync(h->d_start.p, spos.data(), nsf * sizeof(uint64_t), cudaMemcpyHostToDevice, h->stream));
-    CU(cudaMemcpyAsync(h->d_tabA.p, tabA.data(), tabA.size() * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
-    CU(cudaMemcpyAsync(h->d_tabB.p, tabB.data(), tabB.size() * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
-    if (launch_track_cut(g, h->cfg.iq_format, h->d_start.p, h->d_tabA.p, h->d_tabB.p, nsf, h->d_cut.p, h->stream))
-      return fail(LTEPHY_ERROR, "track_push: cut kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
-    if (xu) { // the same kernel on the UL carrier: its antennas, start + ul_offset, the UL tables
-      std::vector<uint64_t> upos(nsf);
-      for (uint32_t i = 0; i < nsf; i++) upos[i] = (uint64_t)((int64_t)spos[i] + h->ul_off);
-      TrackArgs gu = g;
-      gu.x = xu, gu.A = h->ul_A;
-      CU(cudaMemcpyAsync(h->d_startu.p, upos.data(), nsf * sizeof(uint64_t), cudaMemcpyHostToDevice, h->stream));
-      CU(cudaMemcpyAsync(h->d_tabAu.p, tabAu.data(), tabAu.size() * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
-      CU(cudaMemcpyAsync(h->d_tabBu.p, tabBu.data(), tabBu.size() * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
-      if (launch_track_cut(gu, h->cfg.iq_format, h->d_startu.p, h->d_tabAu.p, h->d_tabBu.p, nsf, h->d_cutu.p, h->stream))
-        return fail(LTEPHY_ERROR, "track_push: UL cut kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
+  // 4. the cut of each carrier: its antennas from start + off, rotated by f = (float)(cfo_hz ratio) (cfo_hz itself at ratio 1) with the factor
+  //    tables exp(-j th 128 q) and exp(-j th q) of each subframe, th = 2 pi f / (15000 N), in double, rounded to float
+  std::vector<float2>   tabA[2], tabB[2]; // kept until the stream is synchronised
+  std::vector<uint64_t> pos[2];
+  for (uint32_t ci = 0; ci < h->nc && nsf; ci++) {
+    TrackCarrier& cr = h->car[ci];
+    tabA[ci].resize((size_t)nsf * (SF / 128)), tabB[ci].resize((size_t)nsf * 128), pos[ci].resize(nsf);
+    for (uint32_t i = 0; i < nsf; i++) {
+      const double th = 2.0 * M_PI * (double)(float)((double)h->sf[i].cfo_hz * cr.ratio) / (15000.0 * (double)N);
+      for (uint32_t q = 0; q < SF / 128; q++)
+        tabA[ci][(size_t)i * (SF / 128) + q] = make_float2((float)std::cos(-th * 128.0 * (double)q), (float)std::sin(-th * 128.0 * (double)q));
+      for (uint32_t q = 0; q < 128; q++) tabB[ci][(size_t)i * 128 + q] = make_float2((float)std::cos(-th * (double)q), (float)std::sin(-th * (double)q));
+      pos[ci][i] = (uint64_t)((int64_t)spos[i] + cr.off);
     }
-    CU(cudaStreamSynchronize(h->stream));
+    TrackArgs gc = g;
+    gc.x = x[ci], gc.A = cr.A;
+    CU(cudaMemcpyAsync(cr.d_start.p, pos[ci].data(), nsf * sizeof(uint64_t), cudaMemcpyHostToDevice, h->stream));
+    CU(cudaMemcpyAsync(cr.d_tabA.p, tabA[ci].data(), tabA[ci].size() * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
+    CU(cudaMemcpyAsync(cr.d_tabB.p, tabB[ci].data(), tabB[ci].size() * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
+    if (launch_track_cut(gc, h->cfg.iq_format, cr.d_start.p, cr.d_tabA.p, cr.d_tabB.p, nsf, cr.d_cut.p, h->stream))
+      return fail(LTEPHY_ERROR, "track_push: %scut kernel failed: %s", ci ? "UL " : "", cudaGetErrorString(cudaGetLastError()));
   }
-  if (ul_iq_dev) *ul_iq_dev = h->d_cutu.p;
+  if (nsf) CU(cudaStreamSynchronize(h->stream));
+  if (ul_iq_dev) *ul_iq_dev = h->car[1].d_cut.p;
   out->nof_subframes = nsf, out->nof_half_frames = nh;
-  out->sf = h->sf.data(), out->hf = h->hf.data(), out->iq_dev = h->d_cut.p;
+  out->sf = h->sf.data(), out->hf = h->hf.data(), out->iq_dev = h->car[0].d_cut.p;
   out->next_sample = (uint64_t)track_needed(h), out->remeasured = remeasured, out->finds = finds;
   return LTEPHY_SUCCESS;
 }
 
-static int track_check(ltephy_track_t* h, const void* iq, uint64_t first, uint64_t n, ltephy_track_out_t* out, bool ul)
+// every push: the samples of the downlink (x0) and, with ul, of the uplink (xu), on the host or, with dev, on the device
+static int track_push(ltephy_track_t* h, const void* x0, const void* xu, bool dev, bool ul, uint64_t first, uint64_t n, ltephy_track_out_t* out,
+                      const void** ul_iq_dev)
 {
-  if (!h || !out || (!iq && n)) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_push: null argument");
-  if (ul != h->ul)
-    return fail(LTEPHY_ERROR_INVALID_INPUTS, h->ul ? "track_push: the uplink is set: push with ltephy_track_push_ul" : "track_push_ul: ltephy_track_set_ul has not been called");
+  const void* x[2] = {x0, xu};
+  if (ul && !xu && n) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_push_ul: null argument");
+  if (!h || !out || (!x[0] && n)) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_push: null argument");
+  if (ul != (h->nc == 2))
+    return fail(LTEPHY_ERROR_INVALID_INPUTS, ul ? "track_push_ul: ltephy_track_set_ul has not been called" : "track_push: the uplink is set: push with ltephy_track_push_ul");
   if ((int64_t)first > track_needed(h))
     return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_push: first_sample %llu is after the next sample needed, %lld", (unsigned long long)first,
                 (long long)track_needed(h));
   h->pushed = true;
-  return LTEPHY_SUCCESS;
+  const size_t xb = iq_sample_bytes(h->cfg.iq_format);
+  if (dev && (iq_misaligned(x[0], h->cfg.iq_format) || (ul && iq_misaligned(x[1], h->cfg.iq_format))))
+    return fail(LTEPHY_ERROR_INVALID_INPUTS, ul ? "track_push_ul_device: iq_dev / iq_ul_dev not aligned to their %zu-byte samples"
+                                                : "track_push_device: iq_dev not aligned to its %zu-byte samples", xb);
+  CU(cudaSetDevice(h->cfg.device));
+  if (dev) return track_run(h, x, first, n, out, ul_iq_dev);
+  for (uint32_t c = 0; n && c < h->nc; c++)
+    if (h->car[c].d_x.reserve((size_t)h->car[c].A * n * xb))
+      return fail(LTEPHY_ERROR, ul ? "track_push_ul: device allocation failed" : "track_push: device allocation failed");
+  for (uint32_t c = 0; n && c < h->nc; c++)
+    CU(cudaMemcpyAsync(h->car[c].d_x.p, x[c], (size_t)h->car[c].A * n * xb, cudaMemcpyHostToDevice, h->stream));
+  const void* xd[2] = {h->car[0].d_x.p, h->car[1].d_x.p};
+  return track_run(h, xd, first, n, out, ul_iq_dev);
 }
 
 extern "C" int ltephy_track_push(ltephy_track_t* h, const void* iq, uint64_t first_sample, uint64_t nof_samples, ltephy_track_out_t* out)
 {
-  if (int r = track_check(h, iq, first_sample, nof_samples, out, false)) return r;
-  CU(cudaSetDevice(h->cfg.device));
-  if (nof_samples) {
-    const size_t bytes = (size_t)h->A * nof_samples * iq_sample_bytes(h->cfg.iq_format);
-    if (h->d_x.reserve(bytes)) return fail(LTEPHY_ERROR, "track_push: device allocation failed");
-    CU(cudaMemcpyAsync(h->d_x.p, iq, bytes, cudaMemcpyHostToDevice, h->stream));
-  }
-  return track_run(h, h->d_x.p, nullptr, first_sample, nof_samples, out, nullptr);
+  return track_push(h, iq, nullptr, false, false, first_sample, nof_samples, out, nullptr);
 }
 
 extern "C" int ltephy_track_push_device(ltephy_track_t* h, const void* iq_dev, uint64_t first_sample, uint64_t nof_samples, ltephy_track_out_t* out)
 {
-  if (int r = track_check(h, iq_dev, first_sample, nof_samples, out, false)) return r;
-  if (iq_misaligned(iq_dev, h->cfg.iq_format))
-    return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_push_device: iq_dev not aligned to its %zu-byte samples", iq_sample_bytes(h->cfg.iq_format));
-  CU(cudaSetDevice(h->cfg.device));
-  return track_run(h, iq_dev, nullptr, first_sample, nof_samples, out, nullptr);
+  return track_push(h, iq_dev, nullptr, true, false, first_sample, nof_samples, out, nullptr);
 }
 
 extern "C" int ltephy_track_set_ul(ltephy_track_t* h, const ltephy_track_ul_cfg_t* cfg)
 {
   if (!h || !cfg) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_set_ul: null argument");
-  if (h->pushed || h->ul) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_set_ul: only before the first push, once");
+  if (h->pushed || h->nc == 2) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_set_ul: only before the first push, once");
   if (!(cfg->cfo_ratio > 0.0 && cfg->cfo_ratio <= 2.0)) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_set_ul: cfo_ratio outside (0, 2]");
   const int64_t off = cfg->ul_offset;
   if ((off < 0 ? -off : off) >= (int64_t)h->SF) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_set_ul: |ul_offset| %lld >= 15 N", (long long)off);
   if ((int64_t)h->cfg.frame_offset + off < 0)
     return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_set_ul: the first UL subframe would start before sample 0 (frame_offset + ul_offset < 0)");
   if (cfg->nof_rx > 2) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_set_ul: nof_rx %u: 0 or 1 (one UL antenna) or 2", cfg->nof_rx);
-  const uint32_t A = cfg->nof_rx ? cfg->nof_rx : 1;
   CU(cudaSetDevice(h->cfg.device));
-  const size_t nsf = h->cfg.max_subframes;
-  if (h->d_cutu.reserve(nsf * A * h->SF) || h->d_tabAu.reserve(nsf * (h->SF / 128)) || h->d_tabBu.reserve(nsf * 128) || h->d_startu.reserve(nsf))
-    return fail(LTEPHY_ERROR, "track_set_ul: device allocation failed");
-  h->ul = true, h->ul_ratio = cfg->cfo_ratio, h->ul_off = cfg->ul_offset, h->ul_A = A;
+  TrackCarrier& u = h->car[1];
+  u.A = cfg->nof_rx ? cfg->nof_rx : 1;
+  if (u.reserve(h->cfg.max_subframes, h->SF)) return fail(LTEPHY_ERROR, "track_set_ul: device allocation failed");
+  h->nc = 2, u.ratio = cfg->cfo_ratio, u.off = cfg->ul_offset;
   return LTEPHY_SUCCESS;
 }
 
 extern "C" int ltephy_track_push_ul(ltephy_track_t* h, const void* iq, const void* iq_ul, uint64_t first_sample, uint64_t nof_samples,
                                     ltephy_track_out_t* out, const void** ul_iq_dev)
 {
-  if (!iq_ul && nof_samples) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_push_ul: null argument");
-  if (int r = track_check(h, iq, first_sample, nof_samples, out, true)) return r;
-  CU(cudaSetDevice(h->cfg.device));
-  if (nof_samples) {
-    const size_t xb = iq_sample_bytes(h->cfg.iq_format);
-    if (h->d_x.reserve((size_t)h->A * nof_samples * xb) || h->d_xu.reserve((size_t)h->ul_A * nof_samples * xb))
-      return fail(LTEPHY_ERROR, "track_push_ul: device allocation failed");
-    CU(cudaMemcpyAsync(h->d_x.p, iq, (size_t)h->A * nof_samples * xb, cudaMemcpyHostToDevice, h->stream));
-    CU(cudaMemcpyAsync(h->d_xu.p, iq_ul, (size_t)h->ul_A * nof_samples * xb, cudaMemcpyHostToDevice, h->stream));
-  }
-  return track_run(h, h->d_x.p, h->d_xu.p, first_sample, nof_samples, out, ul_iq_dev);
+  return track_push(h, iq, iq_ul, false, true, first_sample, nof_samples, out, ul_iq_dev);
 }
 
 extern "C" int ltephy_track_push_ul_device(ltephy_track_t* h, const void* iq_dev, const void* iq_ul_dev, uint64_t first_sample, uint64_t nof_samples,
                                            ltephy_track_out_t* out, const void** ul_iq_dev)
 {
-  if (!iq_ul_dev && nof_samples) return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_push_ul: null argument");
-  if (int r = track_check(h, iq_dev, first_sample, nof_samples, out, true)) return r;
-  if (iq_misaligned(iq_dev, h->cfg.iq_format) || iq_misaligned(iq_ul_dev, h->cfg.iq_format))
-    return fail(LTEPHY_ERROR_INVALID_INPUTS, "track_push_ul_device: iq_dev / iq_ul_dev not aligned to their %zu-byte samples", iq_sample_bytes(h->cfg.iq_format));
-  CU(cudaSetDevice(h->cfg.device));
-  return track_run(h, iq_dev, iq_ul_dev, first_sample, nof_samples, out, ul_iq_dev);
+  return track_push(h, iq_dev, iq_ul_dev, true, true, first_sample, nof_samples, out, ul_iq_dev);
 }

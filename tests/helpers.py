@@ -1,4 +1,7 @@
-"""Shared helpers for the parity tests: run the CPU oracle over a capture, convert grants."""
+"""Shared helpers for the parity tests: run the CPU oracle over a capture, convert grants, and the UL-mode batch step of the examples driven
+through the binding."""
+import ctypes as C
+
 import numpy as np
 import ltelib
 from ltelib import Sim
@@ -89,3 +92,84 @@ def describe_mismatch(a, b, name):
     d = np.abs(a.astype(np.complex128) - b.astype(np.complex128))
     return "%s: %d/%d differ, first at %d (%r vs %r), max abs diff %.3g, rel %.3g" % (
         name, len(bad), len(a), bad[0], a[bad[0]], b[bad[0]], d.max(), d.max() / (np.abs(b).max() + 1e-30))
+
+
+def ul_records(grants, res, pl, tti):
+    """the UL records (0, rnti, tti, payload) of one ltephy_submit_ul: the first attempt of a DCI-0 that passed (PUSCH_Decoder::decode stops
+    there), as the examples write them"""
+    out, passed = [], False
+    for k, g in enumerate(grants):
+        if k == 0 or grants[k - 1].rnti != g.rnti or grants[k - 1].sf != g.sf:
+            passed = False
+        ok = res[k].crc and not passed
+        passed = passed or res[k].crc != 0
+        if ok and res[k].payload_len:
+            out.append((0, int(g.rnti), int(tti[g.sf]), bytes(pl[res[k].payload_off:res[k].payload_off + res[k].payload_len])))
+    return out
+
+
+class UlModeStep:
+    """The UL-mode batch step of examples/cell_chain.h driven through the binding: decode a batch of DL subframes in UL mode and record their DL
+    blocks; split the carried grants into this batch's and later ones; take msg-3 grants from RAR payloads (sf + 6) and activate their C-RNTIs;
+    take DCI-0 grants from ul_grants_from_dcis; shift the carry; decode the uplink and keep the first attempt of a DCI-0 that passed.  It owns
+    the search handle in UL mode, the DL and UL handles (the UL one with ul_nof_rx antennas), the scratch buffers and the carry.  beyond: the
+    largest number of carried grants that fell beyond a batch; carry: the grants still carried; now: the grants of the last batch's UL decode."""
+
+    def __init__(self, prb, ports, pci, B, ul_nof_rx=1, symbol_sz=0, phich_resources=0, phich_length=0):
+        import track_lib as T
+        mk = lambda A: capi.LtePhy(prb, ports, pci, 1, max_subframes=B, turbo_max_iter=8, flags=capi.FLAG_SKIP_LOW_POWER, symbol_sz=symbol_sz,
+                                   phich_resources=phich_resources, phich_length=phich_length, ul_nof_rx=A)
+        self.phy, self.ul = mk(1), mk(ul_nof_rx)
+        self.ul.set_ul_cfg(**T.UCFG)
+        self.srch = capi.Search(prb, ports, pci, 1, phich_resources=phich_resources)
+        self.L = self.phy.L
+        self.L.ltephy_search_set_ul_mode(self.srch.h, 1, 0)
+        self.L.ltephy_search_set_ul_hopping(self.srch.h, 0)
+        self.L.ltephy_search_activate.argtypes = [C.c_void_p, C.c_uint16, C.c_uint32, C.c_int]
+        self.md = 32 * B
+        self.info, self.cands = (capi.SfInfo * B)(), np.zeros((B, capi.MAX_LOC, capi.MAX_SIZES), capi.CAND_DTYPE)
+        self.dcis, self.tbs, self.pay = np.zeros(self.md, capi.DCI_DTYPE), (capi.TbResult * (2 * self.md))(), np.zeros(B * 64 * 1024, np.uint8)
+        self.carry, self.beyond, self.now = [], 0, []
+
+    def close(self):
+        self.phy.close(), self.ul.close(), self.srch.close()
+
+    def __call__(self, dl, tti, ul_iq):
+        """one batch: dl torch complex64 [m][1][15 N] on the device, tti its m ttis, ul_iq torch complex64 [m][15 N] ([m][A][15 N]) on the device
+        -> the batch's records in the examples' order: its DL blocks (1, rnti, tti, payload), then its UL blocks (0, rnti, tti, payload)"""
+        tti, m, L, tbs, pay = np.ascontiguousarray(tti, np.uint32), len(tti), self.L, self.tbs, self.pay
+        block = lambda rr: bytes(pay[rr.payload_off:rr.payload_off + rr.payload_len])
+        nd = C.c_uint32(0)
+        assert L.ltephy_decode_subframes_device(self.phy.h, self.srch.h, C.c_void_p(dl.data_ptr()), capi._p(tti), m, capi.SEQ_NONE, self.info,
+                                                capi._p(self.cands), capi._p(self.dcis), self.md, C.byref(nd), tbs, capi._p(pay), pay.nbytes) == 0
+        dcis = self.dcis[:nd.value].copy()
+        now, self.carry = [g for g in self.carry if g.sf < m], [g for g in self.carry if g.sf >= m]
+        self.beyond = max(self.beyond, len(self.carry))
+        out = []
+        for i, d in enumerate(dcis):
+            for t in range(2):
+                rr = tbs[2 * i + t]
+                if rr.crc and rr.payload_len:
+                    out.append((1, int(d["rnti"]), int(tti[int(d["sf"])]), block(rr)))
+        for i, d in enumerate(dcis):
+            rr = tbs[2 * i]
+            if not (1 <= int(d["rnti"]) <= 10 and rr.crc and rr.payload_len):
+                continue
+            rc, rars, _ = capi.rar_unpack(self.srch, block(rr))
+            if rc != 0:
+                continue
+            for a in rars:
+                L.ltephy_search_activate(self.srch.h, a.t_crnti, 0, 2)
+                if a.valid:
+                    g = capi.UlGrant.from_buffer_copy(a.grant)
+                    g.sf = int(d["sf"]) + 6
+                    (now if g.sf < m else self.carry).append(g)
+        for _, _, g in capi.ul_grants_from_dcis(self.srch, self.info, dcis):
+            (now if g.sf < m else self.carry).append(g)
+        for g in self.carry:
+            g.sf -= m
+        self.now = now
+        if now:
+            res, _, pl = self.ul.decode_ul_device(ul_iq, tti, now)
+            out += ul_records(now, res, pl, tti)
+        return out

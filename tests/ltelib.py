@@ -101,6 +101,9 @@ def sim():
         L.lte_dci_unpack.argtypes = [C.POINTER(Cell), C.c_int, C.c_uint16, C.c_void_p, C.c_uint32, C.POINTER(Dci)]
         L.lte_dci_pack.argtypes = [C.POINTER(Cell), C.POINTER(Dci), C.c_void_p, C.POINTER(C.c_uint32)]
         L.lte_dl_dci_to_grant.argtypes = [C.POINTER(Cell), C.c_uint32, C.c_uint32, C.c_int, C.POINTER(Dci), C.POINTER(DlGrant)]
+        L.lte_ul_dci_to_grant.argtypes = [C.POINTER(Cell), C.POINTER(Dci), C.c_int, C.POINTER(UlGrant)]
+        L.lte_sim_ul_subframe_rx.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(UlCfg), C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p,
+                                             C.c_void_p, C.c_uint32]
         L.lte_pdcch_validate_location.argtypes = [C.c_uint32] * 4 + [C.c_uint16]
         L.lte_pdcch_validate_location.restype = C.c_uint32
         L.lte_sf_len.argtypes = [C.c_uint32]
@@ -542,7 +545,6 @@ class UlChest(C.Structure):
 def make_ul_grants(cell, rng, n, table=1, min_prb=3):
     """n random non-overlapping valid UL grants (DCI format 0 fields -> lte_ul_dci_to_grant)"""
     S = sim()
-    S.lte_ul_dci_to_grant.argtypes = [C.POINTER(Cell), C.POINTER(Dci), C.c_int, C.POINTER(UlGrant)]
     S.lte_ul_valid_prb.argtypes = [C.c_uint32]
     out, start = [], 0
     N = cell.nof_prb

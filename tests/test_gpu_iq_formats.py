@@ -11,10 +11,8 @@ import numpy as np
 import pytest
 
 import ltelib
-import pusch_rx_lib as X
 import sync_lib as S
 import track_lib as T
-import track_reacq_lib as Q
 from helpers import make_capture
 from ltesniffer_b200 import capi
 
@@ -179,13 +177,13 @@ def test_tracker_uplink_equals_cf32_of_the_converted_samples(infra, phylib, A, f
     q, ref = quantise(x, fmt)
     qu, refu = quantise(xu, fmt)
     mk = lambda f: capi.Tracker(N, 1, 33, 1234, cfo_hz=650.0, max_subframes=200, ul=dict(cfo_ratio=0.948, ul_offset=-200, nof_rx=A), iq_format=f)
-    want = X.run_chunks_ul_rx(mk("cf32"), ref, refu, [ref.shape[1]])
+    want = T.run_chunks(mk("cf32"), ref, [ref.shape[1]], xu=refu)
     assert len(want["sf"]) >= 35
     for sizes in ([x.shape[1]], [7919, 3 * 15 * N + 17]):
         for dev in (False, True):
             tr = mk(fmt)
             push = (lambda a, b, f: tr.push_ul_device(_dev(a), _dev(b), f)) if dev else tr.push_ul
-            got = X.run_chunks_ul_rx(tr, q, qu, sizes, push=push)
+            got = T.run_chunks(tr, q, sizes, xu=qu, push=push)
             _same(got, want, ("sf", "hf", "iq", "ul_iq"))
             tr.close()
 
@@ -198,13 +196,13 @@ def test_tracker_reacquire_equals_cf32_of_the_converted_samples(infra, phylib, f
     x, _, _, _, lead = drop_capture(N, nrx, 20.0, "37SF+1234")
     q, ref = quantise(x, fmt)
     mk = lambda f: capi.Tracker(N, nrx, PCI, lead, cfo_hz=900.0, first_tti=T0, flags=capi.TRACK_REACQUIRE, max_subframes=300, iq_format=f)
-    want = Q.run_chunks(mk("cf32"), ref, [ref.shape[1]])
+    want = T.run_chunks(mk("cf32"), ref, [ref.shape[1]])
     assert want["finds"] >= 1 and ((want["sf"]["flags"] & capi.TRACK_REACQUIRED) != 0).sum() == 1
     for sizes in [[x.shape[1]], [SF - 1, FR + N + 1], [7919, 3 * SF + 17, 104729]]:
         for dev in (False, True):
             tr = mk(fmt)
             push = (lambda a, f: tr.push_device(_dev(a), f)) if dev else tr.push
-            got = Q.run_chunks(tr, q, sizes, push=push)
+            got = T.run_chunks(tr, q, sizes, push=push)
             _same(got, want, ("sf", "hf", "iq"))
             assert got["finds"] == want["finds"] and got["next_sample"] == want["next_sample"]
             tr.close()
@@ -287,17 +285,16 @@ def test_decode_recording_ul_sc16_files(infra, phylib, tmp_path):
     """decode_recording_ul fmt=sc16 with two UL antennas writes the pcap of the same example on the cf32 files of the converted samples, byte for
     byte, and the transport blocks of the example on the unquantised captures"""
     from test_gpu_track_ul import EXE, LEAD_E2E, N_E2E, OFF_E2E, PCI_E2E, RHO_E2E, _read_pcap
-    import track_ul_lib as U
     subprocess.run(["make", "-s", "-C", ROOT, "examples/decode_recording_ul"], check=True)
-    cap = X.TwoCarrierRx(N_E2E, PCI_E2E, 200, ppm=20.0, cfo=800.0, rho=RHO_E2E, lead=LEAD_E2E, ul_offset=OFF_E2E, seed=73, pbch=1, nof_ports=2,
-                         mcs_max=20, ul_snr=12.0)
+    cap = T.TwoCarrier(N_E2E, PCI_E2E, 200, ppm=20.0, cfo=800.0, rho=RHO_E2E, lead=LEAD_E2E, ul_offset=OFF_E2E, seed=73, pbch=1, nof_ports=2,
+                       mcs_max=20, ul_snr=12.0, ul_nof_rx=2)
     qd, rd = quantise(cap.x[0], "sc16")
     qu, ru = quantise(cap.xu, "sc16")
     out = {}
     for name, d, u, fmt in (("sc16", qd, qu, ["fmt=sc16"]), ("ref", rd, ru, []), ("orig", cap.x[0], cap.xu, [])):
         fd, fu = _tofile(d, tmp_path / ("%s_dl.iq" % name)), _tofile(u, tmp_path / ("%s_ul.iq" % name))
         pc = str(tmp_path / ("%s.pcap" % name))
-        stdout = _run([EXE, fd, fu, str(N_E2E), pc, str(RHO_E2E), str(OFF_E2E), str(U.UCFG["n_dmrs1"]), str(U.UCFG["delta_ss"]), "0", "2"] + fmt)
+        stdout = _run([EXE, fd, fu, str(N_E2E), pc, str(RHO_E2E), str(OFF_E2E), str(T.UCFG["n_dmrs1"]), str(T.UCFG["delta_ss"]), "0", "2"] + fmt)
         out[name] = (stdout, open(pc, "rb").read())
     assert out["sc16"] == out["ref"]
     got = _read_pcap(str(tmp_path / "sc16.pcap"))

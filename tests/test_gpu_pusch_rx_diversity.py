@@ -8,7 +8,8 @@ import pytest
 
 import ltelib
 import pusch_rx_lib as X
-from helpers import describe_mismatch
+import track_lib as T
+from helpers import UlModeStep, describe_mismatch
 from ltelib import Cell, Oracle, Sim, UlCfg
 from ltesniffer_b200 import capi
 from test_pusch_rx_diversity import CASES, _grants
@@ -185,12 +186,11 @@ def test_largest_two_antenna_batch(infra, phylib):
 def test_tracker_two_antenna_ul_cut(infra, phylib, N, off):
     """the two-antenna UL cut equals lteo_track_push_ul with two UL antennas bit for bit, through host and device pushes and in several chunkings"""
     import torch
-    import track_lib as T
     from test_track import chunk_cases
     x = T.capture(N, 33, 40, nrx=2, ppm=20.0, cfo=700.0, ramp=500.0, snr=12.0, lead=1234, seed=4)[0]
     rng = np.random.default_rng(N)
     xu = (rng.standard_normal((2, x.shape[1])) + 1j * rng.standard_normal((2, x.shape[1]))).astype(np.complex64)
-    ref = X.OracleUlRx(N, 2, 33, 1234, cfo_hz=650.0, cfo_ratio=0.948, ul_offset=off).push_ul(x, xu, 0)
+    ref = T.Oracle(N, 2, 33, 1234, cfo_hz=650.0, ul=dict(cfo_ratio=0.948, ul_offset=off, nof_rx=2)).push_ul(x, xu, 0)
     assert len(ref["sf"]) >= 35
     mk = lambda: capi.Tracker(N, 2, 33, 1234, cfo_hz=650.0, max_subframes=200, ul=dict(cfo_ratio=0.948, ul_offset=off, nof_rx=2))
     for sizes in [[x.shape[1]]] + chunk_cases(N)[:3]:
@@ -200,7 +200,7 @@ def test_tracker_two_antenna_ul_cut(infra, phylib, N, off):
                 push = lambda a, b, f: tr.push_ul_device(torch.from_numpy(np.ascontiguousarray(a)).cuda(), torch.from_numpy(np.ascontiguousarray(b)).cuda(), f)
             else:
                 push = tr.push_ul
-            got = X.run_chunks_ul_rx(tr, x, xu, sizes, push=push)
+            got = T.run_chunks(tr, x, sizes, xu=xu, push=push)
             assert got["sf"].tobytes() == ref["sf"].tobytes() and got["hf"].tobytes() == ref["hf"].tobytes()
             assert got["iq"].tobytes() == ref["iq"].tobytes() and got["ul_iq"].tobytes() == ref["ul_iq"].tobytes(), (sizes, dev)
             tr.close()
@@ -213,28 +213,16 @@ def _recording_chain_rx(cap, kv, B):
     DL decode in UL mode, RAR and DCI-0 grants with carry-over, ltephy_submit_ul_device on the [k][2][15 N] UL cut of a handle with
     ul_nof_rx = 2 -> the pcap records the example must write, in its order"""
     from test_gpu_track_ul import OFF_E2E, PCI_E2E, RHO_E2E
-    import track_ul_lib as U
     N, pci, SF = cap.N, PCI_E2E, cap.SF
     fo, sfn = int(kv["frame_offset"]), int(kv["sfn"])
     phich = dict(phich_resources=int(kv["phich_resources"]), phich_length=int(kv["phich_length"]))
-    mk = lambda A: capi.LtePhy(25, int(kv["nof_ports"]), pci, 1, max_subframes=B, turbo_max_iter=8, flags=capi.FLAG_SKIP_LOW_POWER, symbol_sz=N,
-                               ul_nof_rx=A, **phich)
-    phy, ul = mk(1), mk(2)
-    ul.set_ul_cfg(**U.UCFG)
-    srch = capi.Search(25, int(kv["nof_ports"]), pci, 1, phich_resources=phich["phich_resources"])
-    L_ = phy.L
-    L_.ltephy_search_set_ul_mode(srch.h, 1, 0)
-    L_.ltephy_search_set_ul_hopping(srch.h, 0)
-    L_.ltephy_search_activate.argtypes = [C.c_void_p, C.c_uint16, C.c_uint32, C.c_int]
+    step = UlModeStep(25, int(kv["nof_ports"]), pci, B, ul_nof_rx=2, symbol_sz=N, **phich)
     cs = capi.CellSearch(N, 1, 40 * SF)
     c = cs.search(cap.x[:, :40 * SF])[0]
     cs.close()
     assert c.detected and c.pci == pci and c.frame_offset == fo
     tr = capi.Tracker(N, 1, pci, fo, cfo_hz=c.cfo_hz, first_tti=10 * sfn, max_subframes=B, ul=dict(cfo_ratio=RHO_E2E, ul_offset=OFF_E2E, nof_rx=2))
-    md = 32 * B
-    info, cands = (capi.SfInfo * B)(), np.zeros((B, capi.MAX_LOC, capi.MAX_SIZES), capi.CAND_DTYPE)
-    dbuf, tbs, pay = np.zeros(md, capi.DCI_DTYPE), (capi.TbResult * (2 * md))(), np.zeros(B * 64 * 1024, np.uint8)
-    expect, recv, carry, L = [], 0, [], cap.x.shape[1]
+    expect, recv, L = [], 0, cap.x.shape[1]
     while True:
         if recv < L:
             recv = min(recv + B * SF, L)
@@ -250,45 +238,8 @@ def _recording_chain_rx(cap, kv, B):
                 break
             continue
         assert tuple(o["ul_iq"].shape) == (m, 2, SF)
-        tti = np.ascontiguousarray(o["sf"]["tti"], np.uint32)
-        nd = C.c_uint32(0)
-        assert L_.ltephy_decode_subframes_device(phy.h, srch.h, C.c_void_p(o["iq"].data_ptr()), capi._p(tti), m, capi.SEQ_NONE, info, capi._p(cands),
-                                                 capi._p(dbuf), md, C.byref(nd), tbs, capi._p(pay), pay.nbytes) == 0
-        dcis = dbuf[:nd.value].copy()
-        now, carry = [g for g in carry if g.sf < m], [g for g in carry if g.sf >= m]
-        for i, d in enumerate(dcis):
-            for t in range(2):
-                rr = tbs[2 * i + t]
-                if rr.crc and rr.payload_len:
-                    expect.append((1, int(d["rnti"]), int(tti[int(d["sf"])]), bytes(pay[rr.payload_off:rr.payload_off + rr.payload_len])))
-        for i, d in enumerate(dcis):
-            rr = tbs[2 * i]
-            if not (1 <= int(d["rnti"]) <= 10 and rr.crc and rr.payload_len):
-                continue
-            rc, rars, _ = capi.rar_unpack(srch, bytes(pay[rr.payload_off:rr.payload_off + rr.payload_len]))
-            if rc != 0:
-                continue
-            for a in rars:
-                L_.ltephy_search_activate(srch.h, a.t_crnti, 0, 2)
-                if a.valid:
-                    g = capi.UlGrant.from_buffer_copy(a.grant)
-                    g.sf = int(d["sf"]) + 6
-                    (now if g.sf < m else carry).append(g)
-        for _, _, g in capi.ul_grants_from_dcis(srch, info, dcis):
-            (now if g.sf < m else carry).append(g)
-        for g in carry:
-            g.sf -= m
-        if now:
-            res, _, pl = ul.decode_ul_device(o["ul_iq"], tti, now)
-            passed = False
-            for k, g in enumerate(now):      # the first attempt of a DCI-0 that passed, as the example keeps it
-                if k == 0 or now[k - 1].rnti != g.rnti or now[k - 1].sf != g.sf:
-                    passed = False
-                ok = res[k].crc and not passed
-                passed = passed or res[k].crc != 0
-                if ok and res[k].payload_len:
-                    expect.append((0, int(g.rnti), int(tti[g.sf]), bytes(pl[res[k].payload_off:res[k].payload_off + res[k].payload_len])))
-    tr.close(), phy.close(), ul.close(), srch.close()
+        expect += step(o["iq"], o["sf"]["tti"], o["ul_iq"])
+    tr.close(), step.close()
     return expect
 
 
@@ -299,10 +250,9 @@ def test_two_antenna_recording_to_pcap(infra, phylib, tmp_path):
     419 grants from antenna 0 and 337 from both)"""
     import subprocess
     from test_gpu_track_ul import EXE, LEAD_E2E, N_E2E, OFF_E2E, PCI_E2E, RHO_E2E, ROOT, _read_pcap
-    import track_ul_lib as U
     subprocess.run(["make", "-s", "-C", ROOT, "examples/decode_recording_ul"], check=True)
-    cap = X.TwoCarrierRx(N_E2E, PCI_E2E, 300, ppm=20.0, cfo=800.0, rho=RHO_E2E, lead=LEAD_E2E, ul_offset=OFF_E2E, seed=73, pbch=1, nof_ports=2,
-                         mcs_max=20, ul_snr=6.0)
+    cap = T.TwoCarrier(N_E2E, PCI_E2E, 300, ppm=20.0, cfo=800.0, rho=RHO_E2E, lead=LEAD_E2E, ul_offset=OFF_E2E, seed=73, pbch=1, nof_ports=2,
+                       mcs_max=20, ul_snr=6.0, ul_nof_rx=2)
     fd, fu2, fu1 = tmp_path / "dl.cf32", tmp_path / "ul2.cf32", tmp_path / "ul1.cf32"
     cap.x[0].tofile(str(fd))
     cap.xu.tofile(str(fu2))                                          # antenna-major: all of antenna 0, then all of antenna 1
@@ -310,7 +260,7 @@ def test_two_antenna_recording_to_pcap(infra, phylib, tmp_path):
     runs = {}
     for A, fu in ((2, fu2), (1, fu1)):
         pc = str(tmp_path / ("o%d.pcap" % A))
-        r = subprocess.run([EXE, str(fd), str(fu), str(N_E2E), pc, str(RHO_E2E), str(OFF_E2E), str(U.UCFG["n_dmrs1"]), str(U.UCFG["delta_ss"]), "0",
+        r = subprocess.run([EXE, str(fd), str(fu), str(N_E2E), pc, str(RHO_E2E), str(OFF_E2E), str(T.UCFG["n_dmrs1"]), str(T.UCFG["delta_ss"]), "0",
                             str(A)], capture_output=True, text=True)
         assert r.returncode == 0, r.stderr
         runs[A] = (r, _read_pcap(pc))

@@ -8,7 +8,6 @@ import pytest
 
 import track_lib as T
 import track_reacq_lib as Q
-import track_ul_lib as U
 from test_track_reacquire import PCI, T0, drop_capture
 
 pytestmark = pytest.mark.gpu
@@ -87,16 +86,16 @@ def test_dl_ul_tracker_with_a_drop_past_2_32(phylib):
     mk = lambda fo: capi.Tracker(N, 1, PCI, fo, cfo_hz=900.0, first_tti=T0, flags=capi.TRACK_REACQUIRE, max_subframes=300,
                                  ul=dict(cfo_ratio=rho, ul_offset=off))
     tr = mk(lead)
-    a = U.run_chunks_ul(tr, x, xu, sizes)
+    a = T.run_chunks(tr, x, sizes, xu=xu)
     tr.close()
     assert ((a["sf"]["flags"] & capi.TRACK_REACQUIRED) != 0).sum() == 1
-    o = U.run_chunks_ul(U.OracleUl(N, 1, PCI, F + lead, cfo_hz=900.0, first_tti=T0, flags=Q.REACQUIRE, cfo_ratio=rho, ul_offset=off), x, xu, sizes,
-                        first=F)
+    o = T.run_chunks(T.Oracle(N, 1, PCI, F + lead, cfo_hz=900.0, first_tti=T0, flags=Q.REACQUIRE, ul=dict(cfo_ratio=rho, ul_offset=off)), x,
+                     sizes, first=F, xu=xu)
     for device in (False, True):
         tr = mk(F + lead)
         seen, wrap = _spans()
         push = wrap(lambda xx, xxu, s: tr.push_ul_device(_dev(xx), _dev(xxu), s)) if device else wrap(tr.push_ul)
-        b = U.run_chunks_ul(tr, x, xu, sizes, first=F, push=push)
+        b = T.run_chunks(tr, x, sizes, first=F, xu=xu, push=push)
         tr.close()
         assert any(s < TWO32 < e for s, e in seen), seen
         assert any(s < TWO32 < s + SF for s in b["sf"]["start"].tolist())

@@ -37,7 +37,7 @@ def test_drop_bit_exact_with_the_oracle(phylib, case):
     N, nrx, snr, drop = CASES[case]
     SF, FR = 15 * N, 150 * N
     x, _, _, _, lead = drop_capture(N, nrx, snr, drop)
-    mk_o = lambda: Q.Oracle(N, nrx, PCI, lead, cfo_hz=900.0, first_tti=T0, flags=Q.REACQUIRE)
+    mk_o = lambda: T.Oracle(N, nrx, PCI, lead, cfo_hz=900.0, first_tti=T0, flags=Q.REACQUIRE)
     mk_g = lambda: capi.Tracker(N, nrx, PCI, lead, cfo_hz=900.0, first_tti=T0, flags=capi.TRACK_REACQUIRE, max_subframes=300)
     ref = mk_o().push(x, 0, max_sf=300)
     assert ref["finds"] == 1 and ((ref["sf"]["flags"] & capi.TRACK_REACQUIRED) != 0).sum() == 1
@@ -47,9 +47,9 @@ def test_drop_bit_exact_with_the_oracle(phylib, case):
     _same(ref, got)
     tr.close()
     for sizes in [[FR + N], [SF - 1, FR + N + 1], [7919, 3 * SF + 17, 104729]]:
-        o = Q.run_chunks(mk_o(), x, sizes)
+        o = T.run_chunks(mk_o(), x, sizes)
         tr = mk_g()
-        g = Q.run_chunks(tr, x, sizes, push=lambda xx, s: tr.push_device(torch.from_numpy(np.ascontiguousarray(xx)).cuda(), s))
+        g = T.run_chunks(tr, x, sizes, push=lambda xx, s: tr.push_device(torch.from_numpy(np.ascontiguousarray(xx)).cuda(), s))
         _same(o, g)
         tr.close()
 
@@ -58,14 +58,14 @@ def test_fade_bit_exact_with_the_oracle(phylib):
     from ltesniffer_b200 import capi
     N = 256
     x, _, _ = T.capture(N, 100, 400, nrx=1, ppm=20.0, snr=20.0, lead=500, seed=4, gap=(150 * 15 * N, 100 * 15 * N))
-    ref = Q.Oracle(N, 1, 100, 500, flags=Q.REACQUIRE).push(x, 0, max_sf=500)
+    ref = T.Oracle(N, 1, 100, 500, flags=Q.REACQUIRE).push(x, 0, max_sf=500)
     tr = capi.Tracker(N, 1, 100, 500, flags=capi.TRACK_REACQUIRE, max_subframes=500)
     got = tr.push(x, 0)
     assert ref["finds"] >= 1
     _same(ref, got)
     tr.close()
     tr = capi.Tracker(N, 1, 100, 500, flags=capi.TRACK_REACQUIRE | capi.TRACK_NO_CFO, max_subframes=37)
-    _same(Q.run_chunks(Q.Oracle(N, 1, 100, 500, flags=Q.REACQUIRE | T.NO_CFO), x, [15 * N * 7 + 3]), Q.run_chunks(tr, x, [15 * N * 7 + 3]))
+    _same(T.run_chunks(T.Oracle(N, 1, 100, 500, flags=Q.REACQUIRE | T.NO_CFO), x, [15 * N * 7 + 3]), T.run_chunks(tr, x, [15 * N * 7 + 3]))
     tr.close()
 
 
@@ -76,25 +76,24 @@ def test_short_fade_bit_exact_with_the_oracle(phylib, N):
     from ltesniffer_b200 import capi
     SF = 15 * N
     x, _, _ = T.capture(N, 100, 160, nrx=2, ppm=20.0, snr=20.0, lead=500, seed=N, gap=(40 * SF, 60 * SF))
-    ref = Q.Oracle(N, 2, 100, 500, flags=Q.REACQUIRE).push(x, 0, max_sf=300)
+    ref = T.Oracle(N, 2, 100, 500, flags=Q.REACQUIRE).push(x, 0, max_sf=300)
     assert ref["finds"] >= 1 and ((ref["sf"]["flags"] & capi.TRACK_REACQUIRED) != 0).sum() == 1
     tr = capi.Tracker(N, 2, 100, 500, flags=capi.TRACK_REACQUIRE, max_subframes=300)
     _same(ref, tr.push(x, 0))
     tr.close()
     sizes = [150 * N + 7, 3 * SF + 17]
     tr = capi.Tracker(N, 2, 100, 500, flags=capi.TRACK_REACQUIRE, max_subframes=300)
-    g = Q.run_chunks(tr, x, sizes, push=lambda xx, s: tr.push_device(torch.from_numpy(np.ascontiguousarray(xx)).cuda(), s))
-    _same(Q.run_chunks(Q.Oracle(N, 2, 100, 500, flags=Q.REACQUIRE), x, sizes), g)
+    g = T.run_chunks(tr, x, sizes, push=lambda xx, s: tr.push_device(torch.from_numpy(np.ascontiguousarray(xx)).cuda(), s))
+    _same(T.run_chunks(T.Oracle(N, 2, 100, 500, flags=Q.REACQUIRE), x, sizes), g)
     tr.close()
 
 
 def test_uplink_equals_the_oracle(phylib):
-    import track_ul_lib as U
     from ltesniffer_b200 import capi
     N, off, rho = 384, -(3 * 384 + 5), 0.95
     x, _, _, _, lead = drop_capture(N, 1, 20.0, "37SF+1234")
     xu = Q.noise(np.random.default_rng(5), 1, x.shape[1], 1.0)[0]
-    o = Q.OracleUl(N, 1, PCI, lead, cfo_hz=900.0, first_tti=T0, flags=Q.REACQUIRE, cfo_ratio=rho, ul_offset=off)
+    o = T.Oracle(N, 1, PCI, lead, cfo_hz=900.0, first_tti=T0, flags=Q.REACQUIRE, ul=dict(cfo_ratio=rho, ul_offset=off))
     ref = o.push_ul(x, xu, 0, max_sf=300)
     tr = capi.Tracker(N, 1, PCI, lead, cfo_hz=900.0, first_tti=T0, flags=capi.TRACK_REACQUIRE, max_subframes=300, ul=dict(cfo_ratio=rho, ul_offset=off))
     got = tr.push_ul(x, xu, 0)
@@ -103,10 +102,10 @@ def test_uplink_equals_the_oracle(phylib):
     assert got["ul_iq"].cpu().numpy().tobytes() == ref["ul_iq"].tobytes()
     tr.close()
     sizes = [15 * N * 150 + N + 1, 7919]
-    o = Q.OracleUl(N, 1, PCI, lead, cfo_hz=900.0, first_tti=T0, flags=Q.REACQUIRE, cfo_ratio=rho, ul_offset=off)
+    o = T.Oracle(N, 1, PCI, lead, cfo_hz=900.0, first_tti=T0, flags=Q.REACQUIRE, ul=dict(cfo_ratio=rho, ul_offset=off))
     tr = capi.Tracker(N, 1, PCI, lead, cfo_hz=900.0, first_tti=T0, flags=capi.TRACK_REACQUIRE, max_subframes=300, ul=dict(cfo_ratio=rho, ul_offset=off))
-    a = U.run_chunks_ul(o, x, xu, sizes)
-    b = U.run_chunks_ul(tr, x, xu, sizes)
+    a = T.run_chunks(o, x, sizes, xu=xu)
+    b = T.run_chunks(tr, x, sizes, xu=xu)
     assert a["sf"].tobytes() == b["sf"].tobytes() and a["ul_iq"].tobytes() == b["ul_iq"].tobytes()
     tr.close()
 

@@ -11,7 +11,7 @@ import pytest
 
 import ltelib
 import track_lib as T
-import track_ul_lib as U
+from helpers import UlModeStep, ul_records
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -52,7 +52,7 @@ def test_ul_cut_bit_exact_with_the_oracle(phylib, case):
     rng = np.random.default_rng(case)
     xu = np.ascontiguousarray(np.roll(x[nrx - 1], off) + 0.1 * (rng.standard_normal(x.shape[1]) + 1j * rng.standard_normal(x.shape[1])), np.complex64)
     mk = lambda: dict(cfo_hz=kw["cfo"] * 0.9, first_tti=2)
-    ref = U.OracleUl(N, nrx, 301, lead, cfo_ratio=rho, ul_offset=off, **mk()).push_ul(x, xu, 0)
+    ref = T.Oracle(N, nrx, 301, lead, ul=dict(cfo_ratio=rho, ul_offset=off), **mk()).push_ul(x, xu, 0)
     assert len(ref["sf"]) >= nsf - 3
     dl = T.Oracle(N, nrx, 301, lead, **mk()).push(x, 0)
     n = len(ref["sf"])
@@ -62,11 +62,11 @@ def test_ul_cut_bit_exact_with_the_oracle(phylib, case):
     tr.close()
     for sizes in ([15 * N + 1], [7919, 3 * 15 * N + 17, 104729], [13 * N // 2 + 3, 15 * N - 5 + abs(off) // 2]):
         tr = capi.Tracker(N, nrx, 301, lead, max_subframes=200, ul=dict(cfo_ratio=rho, ul_offset=off), **mk())
-        _same(ref, U.run_chunks_ul(tr, x, xu, sizes))
+        _same(ref, T.run_chunks(tr, x, sizes, xu=xu))
         tr.close()
         tr = capi.Tracker(N, nrx, 301, lead, max_subframes=200, ul=dict(cfo_ratio=rho, ul_offset=off), **mk())
         dev = lambda a, b, s: tr.push_ul_device(torch.from_numpy(np.ascontiguousarray(a)).cuda(), torch.from_numpy(np.ascontiguousarray(b)).cuda(), s)
-        _same(ref, U.run_chunks_ul(tr, x, xu, sizes, push=dev))
+        _same(ref, T.run_chunks(tr, x, sizes, xu=xu, push=dev))
         tr.close()
     # the same tracker without the uplink, over the subframes both cut
     tr = capi.Tracker(N, nrx, 301, lead, **mk())
@@ -108,7 +108,7 @@ def test_submit_ul_device_equals_host(phylib):
     import torch
     from ltesniffer_b200 import capi
     N, n = 768, 24
-    cap = U.TwoCarrier(N, 40, n, lead=200, seed=5, mcs_max=24)
+    cap = T.TwoCarrier(N, 40, n, lead=200, seed=5, mcs_max=24)
     grants = [_phy_grant(k, g) for k in range(n) for g in cap.grants[k]]
     assert len(grants) >= 20
     iq = np.stack(cap.ul).astype(np.complex64)
@@ -116,7 +116,7 @@ def test_submit_ul_device_equals_host(phylib):
         outs = []
         for dev in (False, True):
             phy = capi.LtePhy(50, 1, 40, 1, max_subframes=n, symbol_sz=N)
-            phy.set_ul_cfg(**U.UCFG)
+            phy.set_ul_cfg(**T.UCFG)
             phy.set_ul_cfo(cfo)
             run = (lambda a, g: phy.decode_ul_device(None if a is None else torch.from_numpy(a).cuda(), cap.tti, g)) if dev else \
                 (lambda a, g: phy.decode_ul(a, cap.tti, g))
@@ -211,7 +211,7 @@ def _example_and_chain(cap, tmp_path):
     cap.x[0].tofile(str(fd))
     cap.xu.tofile(str(fu))
     pc = str(tmp_path / "o.pcap")
-    r = subprocess.run([EXE, str(fd), str(fu), str(N), pc, str(rho), str(off), str(U.UCFG["n_dmrs1"]), str(U.UCFG["delta_ss"])],
+    r = subprocess.run([EXE, str(fd), str(fu), str(N), pc, str(rho), str(off), str(T.UCFG["n_dmrs1"]), str(T.UCFG["delta_ss"])],
                        capture_output=True, text=True)
     assert r.returncode == 0, r.stderr
     head = r.stdout.splitlines()[0].split()
@@ -224,34 +224,12 @@ def _example_and_chain(cap, tmp_path):
     sfn, fo = int(kv["sfn"]), int(c.frame_offset)
     assert sfn == 0
     phich = dict(phich_resources=int(kv["phich_resources"]), phich_length=int(kv["phich_length"]))
-    mk = lambda: capi.LtePhy(25, int(kv["nof_ports"]), pci, 1, max_subframes=B, turbo_max_iter=8, flags=capi.FLAG_SKIP_LOW_POWER, symbol_sz=N, **phich)
-    phy, ul, ul_ref = mk(), mk(), mk()
-    ul.set_ul_cfg(**U.UCFG)
-    ul_ref.set_ul_cfg(**U.UCFG)
-    srch = capi.Search(25, int(kv["nof_ports"]), pci, 1, phich_resources=phich["phich_resources"])
-    L_ = phy.L
-    L_.ltephy_search_set_ul_mode(srch.h, 1, 0)
-    L_.ltephy_search_set_ul_hopping(srch.h, 0)
-    L_.ltephy_search_activate.argtypes = [C.c_void_p, C.c_uint16, C.c_uint32, C.c_int]
+    step = UlModeStep(25, int(kv["nof_ports"]), pci, B, symbol_sz=N, **phich)
+    ul_ref = capi.LtePhy(25, int(kv["nof_ports"]), pci, 1, max_subframes=B, turbo_max_iter=8, flags=capi.FLAG_SKIP_LOW_POWER, symbol_sz=N, **phich)
+    ul_ref.set_ul_cfg(**T.UCFG)
     tr = capi.Tracker(N, 1, pci, fo, cfo_hz=c.cfo_hz, first_tti=10 * sfn, max_subframes=B, ul=dict(cfo_ratio=rho, ul_offset=off))
-    md = 32 * B
-    sc = dict(info=(capi.SfInfo * B)(), cands=np.zeros((B, capi.MAX_LOC, capi.MAX_SIZES), capi.CAND_DTYPE), dcis=np.zeros(md, capi.DCI_DTYPE),
-              tbs=(capi.TbResult * (2 * md))(), payload=np.zeros(B * 64 * 1024, np.uint8))
-
-    def kept(now, res, pl, tti):
-        """the UL records of one submit: the first attempt of a DCI-0 that passed (PUSCH_Decoder::decode stops there), as the example writes them"""
-        out, passed = [], False
-        for k, g in enumerate(now):
-            if k == 0 or now[k - 1].rnti != g.rnti or now[k - 1].sf != g.sf:
-                passed = False
-            ok = res[k].crc and not passed
-            passed = passed or res[k].crc != 0
-            if ok and res[k].payload_len:
-                out.append((0, int(g.rnti), int(tti[g.sf]), bytes(pl[res[k].payload_off:res[k].payload_off + res[k].payload_len])))
-        return out
-
     L = cap.x.shape[1]
-    expect, aligned, recv, done, carry, lost, beyond = [], [], 0, 0, [], 0, 0
+    expect, aligned, recv, done, lost = [], [], 0, 0, 0
     while True:
         if recv < L:
             recv = min(recv + B * SF, L)
@@ -267,46 +245,16 @@ def _example_and_chain(cap, tmp_path):
                 break
             continue
         lost += int((o["sf"]["flags"] & capi.TRACK_LOST).sum())
-        tti = np.ascontiguousarray(o["sf"]["tti"], np.uint32)
-        nd = C.c_uint32(0)
-        assert L_.ltephy_decode_subframes_device(phy.h, srch.h, C.c_void_p(o["iq"].data_ptr()), capi._p(tti), m, capi.SEQ_NONE, sc["info"],
-                                                 capi._p(sc["cands"]), capi._p(sc["dcis"]), md, C.byref(nd), sc["tbs"], capi._p(sc["payload"]),
-                                                 sc["payload"].nbytes) == 0
-        dcis = sc["dcis"][:nd.value].copy()
-        now = [g for g in carry if g.sf < m]
-        carry = [g for g in carry if g.sf >= m]
-        beyond = max(beyond, len(carry))
-        for i, d in enumerate(dcis):
-            for t in range(2):
-                rr = sc["tbs"][2 * i + t]
-                if rr.crc and rr.payload_len:
-                    expect.append((1, int(d["rnti"]), int(tti[int(d["sf"])]), bytes(sc["payload"][rr.payload_off:rr.payload_off + rr.payload_len])))
-        for i, d in enumerate(dcis):
-            rr = sc["tbs"][2 * i]
-            if not (1 <= int(d["rnti"]) <= 10 and rr.crc and rr.payload_len):
-                continue
-            rc, rars, _ = capi.rar_unpack(srch, bytes(sc["payload"][rr.payload_off:rr.payload_off + rr.payload_len]))
-            if rc != 0:
-                continue
-            for a in rars:
-                L_.ltephy_search_activate(srch.h, a.t_crnti, 0, 2)
-                if a.valid:
-                    g = capi.UlGrant.from_buffer_copy(a.grant)
-                    g.sf = int(d["sf"]) + 6
-                    (now if g.sf < m else carry).append(g)
-        for _, _, g in capi.ul_grants_from_dcis(srch, sc["info"], dcis):
-            (now if g.sf < m else carry).append(g)
-        for g in carry:
-            g.sf -= m
-        if now:
-            res, _, pl = ul.decode_ul_device(o["ul_iq"], tti, now)
-            expect += kept(now, res, pl, tti)
+        tti = o["sf"]["tti"]
+        expect += step(o["iq"], tti, o["ul_iq"])
+        if step.now:
             # the same grants on the simulator's own UL subframes of these ttis (no clock or carrier offset, no uplink delay)
-            res, _, pl = ul_ref.decode_ul(np.stack([cap.ul[int(t)] for t in tti]).astype(np.complex64), tti, now)
-            aligned += kept(now, res, pl, tti)
+            res, _, pl = ul_ref.decode_ul(np.stack([cap.ul[int(t)] for t in tti]).astype(np.complex64), tti, step.now)
+            aligned += ul_records(step.now, res, pl, tti)
         done += m
-    tr.close(), phy.close(), ul.close(), ul_ref.close(), srch.close()
-    return dict(r=r, got=_read_pcap(pc), expect=expect, aligned=aligned, done=done, lost=lost, carried_beyond=beyond, carry_left=len(carry))
+    tr.close(), step.close(), ul_ref.close()
+    return dict(r=r, got=_read_pcap(pc), expect=expect, aligned=aligned, done=done, lost=lost, carried_beyond=step.beyond,
+                carry_left=len(step.carry))
 
 
 def test_recording_ul_to_pcap_at_20ppm(infra, phylib, tmp_path):
@@ -315,7 +263,7 @@ def test_recording_ul_to_pcap_at_20ppm(infra, phylib, tmp_path):
     and every DL block that the same decoder in UL mode reads from the aligned DL subframes"""
     from ltesniffer_b200 import capi
     nsf, B = 2000, B_E2E
-    cap = U.TwoCarrier(N_E2E, PCI_E2E, nsf, ppm=20.0, cfo=800.0, rho=RHO_E2E, lead=LEAD_E2E, ul_offset=OFF_E2E, seed=71, pbch=1, nof_ports=2,
+    cap = T.TwoCarrier(N_E2E, PCI_E2E, nsf, ppm=20.0, cfo=800.0, rho=RHO_E2E, lead=LEAD_E2E, ul_offset=OFF_E2E, seed=71, pbch=1, nof_ports=2,
                        mcs_max=20)
     e = _example_and_chain(cap, tmp_path)
     got, done = e["got"], e["done"]
@@ -364,7 +312,7 @@ def test_recording_ul_with_a_short_last_push(infra, phylib, tmp_path):
     """a recording that ends two subframes after a push boundary: the last push cuts fewer subframes than the grants carried into it reach, those
     grants stay carried (counted as beyond the recording), and the example still decodes the rest of that push and prints its summary"""
     nsf = 202   # push 1 cuts subframes 0..198 (its last UL window ends before 200 subframes' worth of samples), push 2 cuts 199 and 200
-    cap = U.TwoCarrier(N_E2E, PCI_E2E, nsf, ppm=20.0, cfo=800.0, rho=RHO_E2E, lead=LEAD_E2E, ul_offset=OFF_E2E, seed=72, pbch=1, nof_ports=2,
+    cap = T.TwoCarrier(N_E2E, PCI_E2E, nsf, ppm=20.0, cfo=800.0, rho=RHO_E2E, lead=LEAD_E2E, ul_offset=OFF_E2E, seed=72, pbch=1, nof_ports=2,
                        mcs_max=20)
     e = _example_and_chain(cap, tmp_path)
     assert e["carried_beyond"] >= 1 and e["carry_left"] >= 1, (e["carried_beyond"], e["carry_left"])

@@ -189,19 +189,18 @@ def test_oracle_tracker_cuts_each_ul_antenna_as_a_one_antenna_tracker():
     """lteo_track_set_ul_rx with two UL antennas: UL antenna a of the cut equals the UL cut of a one-antenna tracker fed antenna a, records and DL
     cut unchanged; nof_rx 3 is refused"""
     import track_lib as T
-    import track_ul_lib as U
     N = 256
     x = T.capture(N, 33, 40, nrx=2, ppm=20.0, cfo=700.0, ramp=500.0, snr=12.0, lead=1234, seed=4)[0]
     rng = np.random.default_rng(9)
     xu = (rng.standard_normal((2, x.shape[1])) + 1j * rng.standard_normal((2, x.shape[1]))).astype(np.complex64)
-    got = X.OracleUlRx(N, 2, 33, 1234, cfo_hz=650.0, cfo_ratio=0.948, ul_offset=-200).push_ul(x, xu, 0)
+    got = T.Oracle(N, 2, 33, 1234, cfo_hz=650.0, ul=dict(cfo_ratio=0.948, ul_offset=-200, nof_rx=2)).push_ul(x, xu, 0)
     assert len(got["sf"]) >= 35
     for a in range(2):
-        one = U.OracleUl(N, 2, 33, 1234, cfo_hz=650.0, cfo_ratio=0.948, ul_offset=-200).push_ul(x, xu[a], 0)
+        one = T.Oracle(N, 2, 33, 1234, cfo_hz=650.0, ul=dict(cfo_ratio=0.948, ul_offset=-200)).push_ul(x, xu[a], 0)
         assert got["sf"].tobytes() == one["sf"].tobytes() and got["hf"].tobytes() == one["hf"].tobytes() and got["iq"].tobytes() == one["iq"].tobytes()
         assert np.ascontiguousarray(got["ul_iq"][:, a]).tobytes() == one["ul_iq"].tobytes()
     t = T.Oracle(N, 2, 33, 1234)
-    assert X.track_set_ul_rx(T.lib(), t.t, 1.0, 0, 3) == -2
+    assert T.lib().lteo_track_set_ul_rx(t.t, 1.0, 0, 3) == -2
 
 
 def test_three_ul_antennas_are_refused_without_a_gpu(phylib):

@@ -65,7 +65,7 @@ def check_reacquired(r, truth, ft, num, drop_at, N, cfo_tol=200.0):
 def test_drop_is_reacquired(case):
     N, nrx, snr, drop = DROP_CASES[case]
     x, truth, ft, num, lead = drop_capture(N, nrx, snr, drop)
-    r = Q.Oracle(N, nrx, PCI, lead, cfo_hz=900.0, first_tti=T0, flags=Q.REACQUIRE).push(x, 0, cut=False)
+    r = T.Oracle(N, nrx, PCI, lead, cfo_hz=900.0, first_tti=T0, flags=Q.REACQUIRE).push(x, 0, cut=False)
     i = check_reacquired(r, truth, ft, num, lead + 40 * 15 * N + 333, N)
     # the first window starts at the subframe after the lost one, 20 ms after the drop: wholly after it, so one window finds the cell
     assert r["finds"] == 1
@@ -82,7 +82,7 @@ def test_drop_of_whole_frames_keeps_the_timing(N):
     +-9 N / 128: nothing is lost and no window is searched, and the subframe numbers stay right, but the SFN is 12 frames ahead of the count --
     only the MIB can tell"""
     x, truth, ft, num, lead = drop_capture(N, 2, 15.0, 12 * 150 * N)
-    r = Q.Oracle(N, 2, PCI, lead, cfo_hz=900.0, first_tti=T0, flags=Q.REACQUIRE).push(x, 0, cut=False)
+    r = T.Oracle(N, 2, PCI, lead, cfo_hz=900.0, first_tti=T0, flags=Q.REACQUIRE).push(x, 0, cut=False)
     sf = r["sf"]
     assert r["finds"] == 0 and not (sf["flags"] & (T.LOST | Q.REACQUIRED)).any()
     k = sf["index"]
@@ -97,7 +97,7 @@ def test_fade_reacquires_at_the_old_timing():
     was dropped"""
     N = 256
     x, truth, _ = T.capture(N, 100, 400, nrx=1, ppm=20.0, snr=20.0, lead=500, seed=4, gap=(150 * 15 * N, 100 * 15 * N))
-    r = Q.Oracle(N, 1, 100, 500, flags=Q.REACQUIRE).push(x, 0, cut=False)
+    r = T.Oracle(N, 1, 100, 500, flags=Q.REACQUIRE).push(x, 0, cut=False)
     sf = r["sf"]
     ire = np.flatnonzero(sf["flags"] & Q.REACQUIRED)
     assert len(ire) == 1 and r["finds"] >= 1
@@ -119,7 +119,7 @@ def test_noise_is_never_found(case):
     x, _, _ = T.capture(N, PCI, 30, nrx=nrx, snr=20.0, lead=N, seed=case)
     rms = np.sqrt(np.mean(np.abs(x[:, N:]) ** 2))
     x = np.concatenate([x, Q.noise(np.random.default_rng(case), nrx, (nwin + 3) * FR, rms)], axis=1)
-    tr = Q.Oracle(N, nrx, PCI, N, flags=Q.REACQUIRE)
+    tr = T.Oracle(N, nrx, PCI, N, flags=Q.REACQUIRE)
     r = tr.push(x[:, :N + 30 * SF], 0, cut=False)           # locked up to the end of the cell
     assert r["finds"] == 0 and not (r["sf"]["flags"] & T.LOST).any()
     total, nxt = 0, tr.next_sample
@@ -140,11 +140,11 @@ def test_chunking_inside_and_at_find_windows():
     N, nrx = 128, 2
     SF, FR = 15 * N, 150 * N
     x, truth, ft, num, lead = drop_capture(N, nrx, 15.0, "37SF+1234")
-    mk = lambda: Q.Oracle(N, nrx, PCI, lead, cfo_hz=900.0, first_tti=T0, flags=Q.REACQUIRE)
+    mk = lambda: T.Oracle(N, nrx, PCI, lead, cfo_hz=900.0, first_tti=T0, flags=Q.REACQUIRE)
     ref = mk().push(x, 0)
     assert ref["finds"] == 1
     for sizes in [[FR + N], [FR], [FR // 3], [SF - 1, FR + N + 1], [7919, 3 * SF + 17, 104729]]:
-        got = Q.run_chunks(mk(), x, sizes)
+        got = T.run_chunks(mk(), x, sizes)
         assert got["sf"].tobytes() == ref["sf"].tobytes() and got["hf"].tobytes() == ref["hf"].tobytes(), sizes
         assert got["iq"].tobytes() == ref["iq"].tobytes() and got["finds"] == ref["finds"], sizes
 
@@ -156,8 +156,8 @@ def test_uplink_cut_follows_the_new_timing(ul_offset):
     N, rho = 128, 0.95
     x, truth, ft, num, lead = drop_capture(N, 1, 20.0, "37SF+1234")
     xu = Q.noise(np.random.default_rng(5), 1, x.shape[1], 1.0)[0]
-    dl = Q.Oracle(N, 1, PCI, lead, cfo_hz=900.0, first_tti=T0, flags=Q.REACQUIRE).push(x, 0, cut=False)
-    tr = Q.OracleUl(N, 1, PCI, lead, cfo_hz=900.0, first_tti=T0, flags=Q.REACQUIRE, cfo_ratio=rho, ul_offset=ul_offset)
+    dl = T.Oracle(N, 1, PCI, lead, cfo_hz=900.0, first_tti=T0, flags=Q.REACQUIRE).push(x, 0, cut=False)
+    tr = T.Oracle(N, 1, PCI, lead, cfo_hz=900.0, first_tti=T0, flags=Q.REACQUIRE, ul=dict(cfo_ratio=rho, ul_offset=ul_offset))
     r = tr.push_ul(x, xu, 0)
     assert r["sf"].tobytes() == dl["sf"].tobytes() and r["finds"] == dl["finds"] == 1
     i = int(np.flatnonzero(r["sf"]["flags"] & Q.REACQUIRED)[0])
@@ -175,7 +175,7 @@ def test_oracle_equals_float64_reference(case):
     import ref64_track_find as F
     N, nrx, snr, drop = DROP_CASES[case]
     x, _, _, _, lead = drop_capture(N, nrx, snr, drop)
-    o = Q.Oracle(N, nrx, PCI, lead, cfo_hz=900.0, first_tti=T0, flags=Q.REACQUIRE).push(x, 0, cut=False)
+    o = T.Oracle(N, nrx, PCI, lead, cfo_hz=900.0, first_tti=T0, flags=Q.REACQUIRE).push(x, 0, cut=False)
     f = F.track(N, x, PCI, lead, 900.0, first_tti=T0)
     assert (o["sf"]["flags"] & Q.REACQUIRED).any() and o["finds"] == f["finds"] == 1
     np.testing.assert_array_equal(o["sf"]["start"], f["start"])

@@ -10,7 +10,6 @@ import pytest
 
 import ltelib
 import track_lib as T
-import track_ul_lib as U
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 EXE = os.path.join(ROOT, "examples", "decode_recording_ul")
@@ -25,7 +24,7 @@ def test_ul_cut_of_downlink_antenna_equals_downlink_cut():
     those of a tracker without the uplink"""
     x = _dl_capture()
     ref = T.Oracle(256, 2, 33, 1234, cfo_hz=650.0).push(x, 0)
-    got = U.OracleUl(256, 2, 33, 1234, cfo_hz=650.0, cfo_ratio=1.0, ul_offset=0).push_ul(x, x[0], 0)
+    got = T.Oracle(256, 2, 33, 1234, cfo_hz=650.0, ul=dict(cfo_ratio=1.0, ul_offset=0)).push_ul(x, x[0], 0)
     assert got["sf"].tobytes() == ref["sf"].tobytes() and got["hf"].tobytes() == ref["hf"].tobytes()
     assert got["iq"].tobytes() == ref["iq"].tobytes()
     assert got["ul_iq"].tobytes() == np.ascontiguousarray(ref["iq"][:, 0]).tobytes()
@@ -42,7 +41,7 @@ def test_ul_cut_equals_float64_restatement(rho, off_n):
     rng = np.random.default_rng(off_n + 5)
     xu = (rng.standard_normal(x.shape[1]) + 1j * rng.standard_normal(x.shape[1])).astype(np.complex64)
     off = off_n * N
-    r = U.OracleUl(N, 2, 33, 1234, cfo_hz=650.0, cfo_ratio=rho, ul_offset=off).push_ul(x, xu, 0)
+    r = T.Oracle(N, 2, 33, 1234, cfo_hz=650.0, ul=dict(cfo_ratio=rho, ul_offset=off)).push_ul(x, xu, 0)
     assert len(r["sf"]) >= 35
     n = np.arange(15 * N)
     for k, s in enumerate(r["sf"]):
@@ -59,9 +58,9 @@ def test_ul_chunking_invariance(off, sizes_i):
     N = 256
     x = _dl_capture(N, 60, -20.0)
     xu = np.ascontiguousarray(x[1][::-1])
-    ref = U.OracleUl(N, 2, 33, 1234, cfo_hz=650.0, cfo_ratio=0.948, ul_offset=off).push_ul(x, xu, 0)
+    ref = T.Oracle(N, 2, 33, 1234, cfo_hz=650.0, ul=dict(cfo_ratio=0.948, ul_offset=off)).push_ul(x, xu, 0)
     sizes = chunk_cases(N)[sizes_i] + ([15 * N + off // 2 + 1] if off else [])
-    got = U.run_chunks_ul(U.OracleUl(N, 2, 33, 1234, cfo_hz=650.0, cfo_ratio=0.948, ul_offset=off), x, xu, sizes)
+    got = T.run_chunks(T.Oracle(N, 2, 33, 1234, cfo_hz=650.0, ul=dict(cfo_ratio=0.948, ul_offset=off)), x, sizes, xu=xu)
     assert got["sf"].tobytes() == ref["sf"].tobytes() and got["hf"].tobytes() == ref["hf"].tobytes()
     assert got["iq"].tobytes() == ref["iq"].tobytes() and got["ul_iq"].tobytes() == ref["ul_iq"].tobytes()
 
@@ -72,21 +71,21 @@ def test_tracked_ul_cut_decodes_what_the_aligned_uplink_does():
     frame_offset + k 15 N (rotated by the constant offset) and the tracked cut without the UL rotation each lose blocks."""
     N, nsf, lead, off, rho, cfo = 384, 500, 1000, 300, 0.948, 800.0
     SF = 15 * N
-    cap = U.TwoCarrier(N, 77, nsf, ppm=20.0, cfo=cfo, rho=rho, lead=lead, ul_offset=off, seed=11, mcs_max=20)
-    r = U.OracleUl(N, 1, 77, lead, cfo_hz=cfo - 30.0, cfo_ratio=rho, ul_offset=off).push_ul(cap.x, cap.xu, 0)
+    cap = T.TwoCarrier(N, 77, nsf, ppm=20.0, cfo=cfo, rho=rho, lead=lead, ul_offset=off, seed=11, mcs_max=20)
+    r = T.Oracle(N, 1, 77, lead, cfo_hz=cfo - 30.0, ul=dict(cfo_ratio=rho, ul_offset=off)).push_ul(cap.x, cap.xu, 0)
     k = r["sf"]["index"]
     assert len(k) >= nsf - 3 and np.array_equal(k, np.arange(len(k)))
-    ideal = U.decode_ul(cap, lambda q: cap.ul[q], k)
+    ideal = T.decode_ul(cap, lambda q: cap.ul[q], k)
     assert len(ideal) >= 0.95 * len([q for q in cap.sent if q[0] in set(k.tolist())]) and len(ideal) > 300
     qm = {(q, int(g.rnti), int(g.n_prb)): int(g.qm) for q in k for g in cap.grants[q]}
     assert any(qm[t] >= 4 for t in ideal)
-    tracked = U.decode_ul(cap, lambda q: r["ul_iq"][q], k)
+    tracked = T.decode_ul(cap, lambda q: r["ul_iq"][q], k)
     assert ideal <= tracked, sorted(ideal - tracked)[:10]
     n = np.arange(SF)
-    fixed = U.decode_ul(cap, lambda q: cap.xu[lead + off + q * SF:lead + off + (q + 1) * SF] * np.exp(-2j * np.pi * rho * cfo * n / (15000.0 * N)), k)
+    fixed = T.decode_ul(cap, lambda q: cap.xu[lead + off + q * SF:lead + off + (q + 1) * SF] * np.exp(-2j * np.pi * rho * cfo * n / (15000.0 * N)), k)
     assert len(ideal - fixed) >= 1, len(fixed)
     st = r["sf"]["start"]
-    unrot = U.decode_ul(cap, lambda q: cap.xu[st[q] + off:st[q] + off + SF], k)
+    unrot = T.decode_ul(cap, lambda q: cap.xu[st[q] + off:st[q] + off + SF], k)
     assert len(ideal - unrot) >= 1, len(unrot)
 
 
@@ -95,21 +94,21 @@ def test_constant_ul_cfo_correction():
     (8 of 28 measured: the slot-to-slot interpolation of the PUSCH estimate follows part of a 108 degree turn between the DMRS symbols) and
     1000 Hz loses every one."""
     N = 384
-    cap = U.TwoCarrier(N, 9, 40, lead=500, seed=21, mcs_max=24)
+    cap = T.TwoCarrier(N, 9, 40, lead=500, seed=21, mcs_max=24)
     ks = [k for k in range(40) if any(g.qm >= 4 for g in cap.grants[k])]
     hi = {(k, int(g.rnti), int(g.n_prb)) for k in ks for g in cap.grants[k] if g.qm >= 4}
     assert len(hi) >= 20
     n = np.arange(15 * N)
     rot = lambda f: (lambda k: cap.ul[k] * np.exp(2j * np.pi * f * n / (15000.0 * N)))
-    assert hi <= U.decode_ul(cap, lambda k: cap.ul[k], ks)
+    assert hi <= T.decode_ul(cap, lambda k: cap.ul[k], ks)
     for f in (600.0, 1000.0):
-        assert hi <= U.decode_ul(cap, rot(f), ks, cfo_hz=f), f
-    assert len(hi - U.decode_ul(cap, rot(600.0), ks)) >= 5
-    assert not (hi & U.decode_ul(cap, rot(1000.0), ks))
+        assert hi <= T.decode_ul(cap, rot(f), ks, cfo_hz=f), f
+    assert len(hi - T.decode_ul(cap, rot(600.0), ks)) >= 5
+    assert not (hi & T.decode_ul(cap, rot(1000.0), ks))
 
 
 def test_oracle_argument_checks():
-    L = U.lib()
+    L = T.lib()
     t = T.Oracle(256, 1, 1, 1000)
     for ratio, off in [(0.0, 0), (-1.0, 0), (2.01, 0), (float("nan"), 0), (1.0, 15 * 256), (1.0, -15 * 256), (1.0, -1001)]:
         assert L.lteo_track_set_ul(t.t, ratio, off) == -2, (ratio, off)

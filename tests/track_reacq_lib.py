@@ -1,20 +1,10 @@
-"""Captures and oracle bindings for the tracker's find state (LTEPHY_TRACK_REACQUIRE, DESIGN.md §2 "tracking"): a receiver that drops samples,
-the oracle with its count of find windows, and chunked pushes that sum it.  Imported only by tests/."""
-import ctypes as C
-
+"""Captures for the tracker's find state (LTEPHY_TRACK_REACQUIRE, DESIGN.md §2 "tracking"): a receiver that drops samples, the drops of the tests
+and noise.  Imported only by tests/."""
 import numpy as np
 
 import track_lib as T
-import track_ul_lib as U
 
 REACQUIRE, REACQUIRED = 2, 4
-
-
-def _lib():
-    L = T.lib()
-    L.lteo_track_finds.restype = C.c_uint32
-    L.lteo_track_finds.argtypes = [C.c_void_p]
-    return L
 
 
 def capture(N, pci, nsf, drop=None, **kw):
@@ -30,42 +20,6 @@ def capture(N, pci, nsf, drop=None, **kw):
         truth = np.where(truth >= a + c, truth - c, truth)[keep]
         ft, num = ft[keep], num[keep]
     return x, truth, ft, num
-
-
-def _counted(cls):
-    class Counted(cls):
-        """the oracle binding with `finds`: the find windows its push searched, as ltephy_track_out_t.finds"""
-
-        def _count(self, fn, *a, **kw):
-            n0 = _lib().lteo_track_finds(self.t)
-            o = fn(*a, **kw)
-            o["finds"] = _lib().lteo_track_finds(self.t) - n0
-            return o
-
-        def push(self, *a, **kw):
-            return self._count(super().push, *a, **kw)
-
-        def push_ul(self, *a, **kw):
-            return self._count(super().push_ul, *a, **kw)
-    return Counted
-
-
-Oracle = _counted(T.Oracle)
-OracleUl = _counted(U.OracleUl)
-
-
-def run_chunks(tr, x, sizes, push=None):
-    """track_lib.run_chunks, with the finds of every push summed and the tracker's last next_sample"""
-    push = push or tr.push
-    finds = []
-
-    def counted(xx, s):
-        o = push(xx, s)
-        finds.append(o["finds"])
-        return o
-    r = T.run_chunks(tr, x, sizes, push=counted)
-    r["finds"], r["next_sample"] = sum(finds), tr.next_sample
-    return r
 
 
 def drop_cases(N):
