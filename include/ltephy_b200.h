@@ -462,6 +462,47 @@ typedef struct {
  * ltephy_chan_taps's h, g and rot. */
 int  ltephy_chan_design(const ltephy_chan_cfg_t* cfg, uint32_t c, ltephy_chan_poly_t* out, float* hp, float* g, float* rot);
 
+/* Raster scan: find the cells of a wideband capture without knowing where they are.  Every point of the 100 kHz E-UTRA channel raster (36.101
+ * §5.7.2) inside the capture gets the channeliser's N = 128 stream (the central 62 sub-carriers hold the PSS and SSS of every bandwidth) and the
+ * cell search of that stream.  Point p has offset o_p = 100 000 k - center_hz, for every integer k whose N = 128 carrier passes the channeliser's
+ * band check (|o| + 540 kHz <= fs_in / 2) and lies in [lo_hz, hi_hz] (both 0: every offset), in ascending offset.  A point's three results are
+ * exactly what ltephy_cell_search_device returns on what ltephy_chan_run (LTEPHY_CHAN_RATIONAL, the one carrier (o_p, 128)) makes of capture
+ * samples [0, n): DESIGN.md §2 ("raster scan"), with lteo_chan_run_poly and lteo_cell_search as its oracle. */
+typedef struct ltephy_scan ltephy_scan_t;
+typedef struct {
+  uint32_t fs_in;               /* capture rate in Hz, as for the channeliser; fs_in -> 1.92 MHz must pass its rational rule */
+  uint32_t nof_rx;              /* 1 or 2 antennas */
+  uint32_t iq_format;           /* LTEPHY_IQ_CF32 (0), LTEPHY_IQ_SC16 or LTEPHY_IQ_SC8: the sample type of the capture */
+  uint32_t max_points_per_pass; /* raster points one batched pass holds; 0 = as many as a fixed device budget (2 GiB) holds.  No result depends on it */
+  uint64_t center_hz;           /* absolute centre frequency of the capture, a multiple of 1 kHz */
+  int32_t  lo_hz, hi_hz;        /* offset range of the points, lo_hz <= hi_hz; both 0 = every offset */
+  uint64_t max_samples;         /* longest capture per antenna, up to 2^31; its N = 128 stream must hold a half-frame plus a symbol (9 728 samples) */
+  int32_t  device;              /* CUDA device ordinal */
+  uint32_t reserved[5];
+} ltephy_scan_cfg_t;
+typedef struct {
+  int32_t       offset_hz; /* the raster point's offset from center_hz */
+  uint32_t      pad;
+  ltephy_cell_t cell;      /* its result, with frame_offset in N = 128 stream samples: at N' it is frame_offset * N' / 128, within one N = 128 sample */
+} ltephy_scan_cell_t;
+/* INVALID_INPUTS, before any device is looked for, for: center_hz off the 1 kHz grid, fs_in outside 1..LTEPHY_CHAN_MAX_FS or a ratio fs_in ->
+ * 1.92 MHz the rational rule refuses, nof_rx other than 1 or 2, an unknown iq_format, lo_hz > hi_hz, a configuration without raster points,
+ * and max_samples above 2^31 or too short for a half-frame plus a symbol at N = 128. */
+int  ltephy_scan_create(const ltephy_scan_cfg_t* cfg, ltephy_scan_t** h);
+void ltephy_scan_destroy(ltephy_scan_t* h);
+/* iq: [nof_rx][nof_samples] samples in the handle's iq_format, antenna-major, host memory: capture samples 0 .. nof_samples - 1 (nof_samples <=
+ * max_samples, its N = 128 stream at least a half-frame plus a symbol).  out[cap]: every result with detected = 1, by offset ascending, then by
+ * pss_peak descending; *nof_cells: how many there are (only the first cap are written).  Blocks until done. */
+int  ltephy_scan_run(ltephy_scan_t* h, const void* iq, uint64_t nof_samples, ltephy_scan_cell_t* out, uint32_t cap, uint32_t* nof_cells);
+/* same, with the samples already in device memory on the handle's device (integer samples aligned to the sample) */
+int  ltephy_scan_run_device(ltephy_scan_t* h, const void* iq_dev, uint64_t nof_samples, ltephy_scan_cell_t* out, uint32_t cap, uint32_t* nof_cells);
+/* the three results of every point of the last run, point-major, each point's by pss_peak descending as ltephy_cell_search gives them:
+ * out[3 * cap]; writes min(cap, points) points */
+int  ltephy_scan_points(ltephy_scan_t* h, ltephy_cell_t* out, uint32_t cap);
+/* host only, needs no device: the raster offsets of a configuration, ascending; *n: how many (only the first cap are written).  Fails as
+ * ltephy_scan_create does, except that a configuration without points gives *n = 0. */
+int  ltephy_scan_plan(const ltephy_scan_cfg_t* cfg, int32_t* offsets, uint32_t cap, uint32_t* n);
+
 /* nslots HARQ slots of LTEPHY_HARQ_SLOT_BYTES each (150 RNTIs x 8 processes x 2 TBs = 2400 slots = 1.4 GB); contents survive across batches */
 int ltephy_harq_reserve(ltephy_t* h, uint32_t nslots);
 

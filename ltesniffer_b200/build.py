@@ -13,7 +13,7 @@ INC = os.path.join(HERE, "..", "include")
 OBJ = os.path.join(HERE, "_obj")
 OUT = os.path.join(HERE, "libltephy_b200.so")
 COMPAT_OUT = os.path.join(HERE, "libltephy_srsran_compat.so")
-SOURCES = ["k_frontend.cu", "k_viterbi.cu", "k_pdsch.cu", "k_turbo.cu", "k_pusch.cu", "k_pbch.cu", "k_sync.cu", "k_track.cu", "k_chan.cu", "ltephy_capi.cu", "sync.cu", "track.cu", "chan.cu", "shard.cu", "lte_host.cpp",
+SOURCES = ["k_frontend.cu", "k_viterbi.cu", "k_pdsch.cu", "k_turbo.cu", "k_pusch.cu", "k_pbch.cu", "k_sync.cu", "k_track.cu", "k_chan.cu", "ltephy_capi.cu", "sync.cu", "track.cu", "chan.cu", "scan.cu", "shard.cu", "lte_host.cpp",
            "host_search.cpp", "sinks.cpp", "harq.cpp"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-fmad=false",
               "-Xcompiler", "-fPIC,-ffp-contract=off,-fno-fast-math,-Wall,-Wno-unused-function", "-Xptxas", "-v"]

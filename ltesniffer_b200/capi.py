@@ -1140,3 +1140,114 @@ class Channelizer:
         n = self._samples(iq)
         out, nxt = (ChanOut * CHAN_MAX_CARRIERS)(), C.c_uint64()
         return self._done(self.L.ltephy_chan_run_device(self.h, C.c_void_p(iq.data_ptr()), first_sample, n, out, C.byref(nxt)), out, nxt, copy)
+
+
+# ------------------------------------------------------------------------------------------------
+# raster scan (ltephy_scan_*, include/ltephy_b200.h)
+class ScanCfg(C.Structure):
+    _fields_ = [("fs_in", C.c_uint32), ("nof_rx", C.c_uint32), ("iq_format", C.c_uint32), ("max_points_per_pass", C.c_uint32), ("center_hz", C.c_uint64),
+                ("lo_hz", C.c_int32), ("hi_hz", C.c_int32), ("max_samples", C.c_uint64), ("device", C.c_int32), ("reserved", C.c_uint32 * 5)]
+
+
+class ScanCell(C.Structure):
+    """ltephy_scan_cell_t: a raster point's offset and its detected cell (timing in N = 128 stream samples)"""
+    _fields_ = [("offset_hz", C.c_int32), ("pad", C.c_uint32), ("cell", CellInfo)]
+
+
+assert C.sizeof(ScanCfg) == 64 and C.sizeof(ScanCell) == 56
+
+
+def _bind_scan(L):
+    L.ltephy_scan_create.argtypes = [C.POINTER(ScanCfg), C.POINTER(C.c_void_p)]
+    L.ltephy_scan_destroy.argtypes = [C.c_void_p]
+    L.ltephy_scan_run.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32)]
+    L.ltephy_scan_run_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32)]
+    L.ltephy_scan_points.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
+    L.ltephy_scan_plan.argtypes = [C.POINTER(ScanCfg), C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32)]
+
+
+def scan_cfg(fs_in, nof_rx, center_hz, max_samples, lo_hz=0, hi_hz=0, iq_format="cf32", max_points_per_pass=0, device=0):
+    return ScanCfg(fs_in=fs_in, nof_rx=nof_rx, iq_format=IQ_FORMATS[iq_format], max_points_per_pass=max_points_per_pass, center_hz=center_hz, lo_hz=lo_hz,
+                   hi_hz=hi_hz, max_samples=max_samples, device=device)
+
+
+def scan_plan(cfg):
+    """host only: the raster offsets of a ScanCfg, ascending (np.int32); RuntimeError when refused"""
+    L = load_library()
+    _bind_scan(L)
+    n = C.c_uint32()
+    r = L.ltephy_scan_plan(C.byref(cfg), None, 0, C.byref(n))
+    if r != 0:
+        raise RuntimeError("ltephy_scan_plan failed (%d): %s" % (r, L.ltephy_last_error().decode()))
+    off = np.zeros(n.value, np.int32)
+    L.ltephy_scan_plan(C.byref(cfg), _p(off), n.value, C.byref(n))
+    return off
+
+
+class Scanner:
+    """Cell search at every 100 kHz raster point of a capture at fs_in centred on center_hz (a multiple of 1 kHz), in [lo_hz, hi_hz] (both 0: every
+    offset), of up to max_samples per antenna.  iq_format "cf32" takes complex64 [nof_rx][n], "sc16" / "sc8" interleaved int16 / int8 [nof_rx][2n],
+    as Channelizer does.  run / run_device -> [(offset_hz, CellInfo)] of every detected cell, by offset, then pss_peak descending."""
+
+    def __init__(self, fs_in, nof_rx, center_hz, max_samples, lo_hz=0, hi_hz=0, iq_format="cf32", max_points_per_pass=0, device=0):
+        self.L = load_library()
+        _bind_scan(self.L)
+        self.iq_format = iq_format
+        self.cfg = scan_cfg(fs_in, nof_rx, center_hz, max_samples, lo_hz, hi_hz, iq_format, max_points_per_pass, device)
+        self.offsets = scan_plan(self.cfg)
+        self.h = C.c_void_p()
+        r = self.L.ltephy_scan_create(C.byref(self.cfg), C.byref(self.h))
+        if r != 0:
+            self.h = None
+            raise RuntimeError("ltephy_scan_create failed (%d): %s" % (r, self.L.ltephy_last_error().decode()))
+
+    def close(self):
+        if self.h:
+            self.L.ltephy_scan_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def plan(self):
+        return self.offsets.copy()
+
+    def _samples(self, shape):
+        assert len(shape) == 2 and shape[0] == self.cfg.nof_rx, shape
+        if self.iq_format == "cf32":
+            return shape[1]
+        assert shape[1] % 2 == 0, shape
+        return shape[1] // 2
+
+    def _done(self, r, out, n):
+        if r != 0:
+            raise RuntimeError("ltephy_scan_run failed (%d): %s" % (r, self.L.ltephy_last_error().decode()))
+        return [(out[i].offset_hz, CellInfo.from_buffer_copy(out[i].cell)) for i in range(min(n.value, len(out)))]
+
+    def run(self, iq, cap=1024):
+        """iq: capture samples 0 .. n - 1 on the host"""
+        iq = np.ascontiguousarray(iq, _IQ_DTYPES[self.iq_format])
+        out, n = (ScanCell * cap)(), C.c_uint32()
+        r = self.L.ltephy_scan_run(self.h, _p(iq), self._samples(iq.shape), out, cap, C.byref(n))
+        return self._done(r, out, n)
+
+    def run_device(self, iq, cap=1024):
+        """iq: torch complex64 [nof_rx][n] (int16 / int8 [nof_rx][2n] for sc16 / sc8), contiguous, on this handle's device"""
+        import torch
+        want = {"cf32": torch.complex64, "sc16": torch.int16, "sc8": torch.int8}[self.iq_format]
+        assert iq.is_cuda and iq.is_contiguous() and iq.dtype == want, (iq.dtype, want)
+        out, n = (ScanCell * cap)(), C.c_uint32()
+        r = self.L.ltephy_scan_run_device(self.h, C.c_void_p(iq.data_ptr()), self._samples(tuple(iq.shape)), out, cap, C.byref(n))
+        return self._done(r, out, n)
+
+    def points(self):
+        """the three CellInfo of every point of the last run: [points][3], each point's by pss_peak descending"""
+        P = len(self.offsets)
+        out = (CellInfo * (3 * P))()
+        r = self.L.ltephy_scan_points(self.h, out, P)
+        if r != 0:
+            raise RuntimeError("ltephy_scan_points failed (%d): %s" % (r, self.L.ltephy_last_error().decode()))
+        return [[CellInfo.from_buffer_copy(out[3 * p + i]) for i in range(3)] for p in range(P)]

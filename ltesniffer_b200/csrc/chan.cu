@@ -65,7 +65,7 @@ static int64_t chan_gcd(int64_t a, int64_t b)
 // geometry of a carrier under the plan's flags (DESIGN.md §2): fs_out / fs_in = L / M in lowest terms; an integer decimation D = 2..128 is L = 1,
 // M = D, Tp = Kp = T, Ka = Kb = H, flag or not, and with LTEPHY_CHAN_RATIONAL any other ratio within the limits is accepted.  0, or
 // INVALID_INPUTS with the reason in the last error
-static int chan_geometry(uint32_t fs_in, int32_t offset_hz, uint32_t N, uint32_t flags, ltephy_chan_poly_t* q)
+int chan_geometry(uint32_t fs_in, int32_t offset_hz, uint32_t N, uint32_t flags, ltephy_chan_poly_t* q)
 {
   const uint32_t prb = chan_max_prb(N);
   if (!prb) return fail(LTEPHY_ERROR_INVALID_INPUTS, "chan: symbol size %u not supported", N);
@@ -98,7 +98,7 @@ static int chan_geometry(uint32_t fs_in, int32_t offset_hz, uint32_t N, uint32_t
 }
 
 // the tables of a carrier under the plan's flags, in the arithmetic of lteo_chan_design_poly, and at L = 1 of lteo_chan_design
-static int chan_design(uint32_t fs_in, int32_t offset_hz, uint32_t N, uint32_t flags, ltephy_chan_poly_t* out, float* hp, float* g, float* rot)
+int chan_design(uint32_t fs_in, int32_t offset_hz, uint32_t N, uint32_t flags, ltephy_chan_poly_t* out, float* hp, float* g, float* rot)
 {
   ltephy_chan_poly_t q;
   if (int r = chan_geometry(fs_in, offset_hz, N, flags, &q)) return r;
@@ -143,6 +143,32 @@ static int chan_design(uint32_t fs_in, int32_t offset_hz, uint32_t N, uint32_t f
     }
   }
   return LTEPHY_SUCCESS;
+}
+
+void chan_tiles(const ltephy_chan_poly_t& q, uint32_t* R, uint32_t* Q, uint32_t* rows, size_t* smem)
+{
+  uint32_t r = 0;
+  *Q         = q.L == 1 ? q.M : 1;
+  if (*Q > 1) { // an integer carrier: R = min(1024, max(64, (CHAN_SPAN - T) / D + 1)) outputs, the span split into its D phases
+    r = (uint32_t)std::min<int64_t>(1024, std::max<int64_t>(64, ((int64_t)CHAN_SPAN - (int64_t)q.Kp) / (int64_t)q.M + 1));
+  } else { // rows per phase class: the span R M + Kp within CHAN_PSPAN; from 32 rows up, whole warps per class and about 4096 outputs a tile
+    r = (uint32_t)std::max<int64_t>(1, ((int64_t)CHAN_PSPAN - (int64_t)q.Kp) / (int64_t)q.M);
+    if (r >= 32) r = std::max<uint32_t>(32, std::min<uint32_t>(r, 4096 / q.L) / 32 * 32);
+  }
+  const uint64_t span = ((uint64_t)(q.L - 1) + ((uint64_t)q.L * r - 1) * q.M) / q.L + q.Kp; // the longest span of a tile
+  *R = r, *rows = (uint32_t)((span + *Q - 1) / *Q);
+  *smem = ((q.L == 1 ? q.Kp : 0) + (size_t)*Q * *rows) * sizeof(float2); // taps at L = 1, and the span
+}
+
+void chan_range(const ltephy_chan_poly_t& q, uint64_t first, uint64_t n, uint64_t* lo_, uint64_t* cnt_, uint64_t* next)
+{
+  // outputs m >= 0 whose window [n - Ka, n + Kb], n = floor(m M / L), has every non-negative sample inside [first, first + n)
+  const unsigned __int128 L = q.L, M = q.M, last = first + n - 1;
+  const uint64_t          lo   = first == 0 ? 0 : (uint64_t)(((first + q.Ka) * L + M - 1) / M);
+  const uint64_t          hi_n = last >= q.Kb ? (uint64_t)(((last - q.Kb + 1) * L - 1) / M + 1) : 0;
+  const uint64_t          cnt  = hi_n > lo ? hi_n - lo : 0;
+  const uint64_t          mn = cnt ? hi_n : lo, nn = (uint64_t)(mn * M / L);
+  *lo_ = lo, *cnt_ = cnt, *next = nn >= q.Ka ? nn - q.Ka : 0;
 }
 
 static int chan_check_cfg(const ltephy_chan_cfg_t* cfg)
@@ -204,17 +230,10 @@ extern "C" int ltephy_chan_create(const ltephy_chan_cfg_t* cfg, ltephy_chan_t** 
     chan_geometry(cfg->fs_in, cfg->carrier[c].offset_hz, cfg->carrier[c].symbol_sz, cfg->flags, &q);
     std::vector<float> g(2 * (size_t)q.L * q.Kp), rot(2 * (size_t)q.P);
     chan_design(cfg->fs_in, cfg->carrier[c].offset_hz, cfg->carrier[c].symbol_sz, cfg->flags, nullptr, nullptr, g.data(), rot.data());
-    k.Q = q.L == 1 ? q.M : 1;
-    if (k.Q > 1) { // an integer carrier: R = min(1024, max(64, (CHAN_SPAN - T) / D + 1)) outputs, the span split into its D phases
-      k.R = (uint32_t)std::min<int64_t>(1024, std::max<int64_t>(64, ((int64_t)CHAN_SPAN - (int64_t)q.Kp) / (int64_t)q.M + 1));
-    } else { // rows per phase class: the span R M + Kp within CHAN_PSPAN; from 32 rows up, whole warps per class and about 4096 outputs a tile
-      k.R = (uint32_t)std::max<int64_t>(1, ((int64_t)CHAN_PSPAN - (int64_t)q.Kp) / (int64_t)q.M);
-      if (k.R >= 32) k.R = std::max<uint32_t>(32, std::min<uint32_t>(k.R, 4096 / q.L) / 32 * 32);
-    }
-    const uint64_t span = ((uint64_t)(q.L - 1) + ((uint64_t)q.L * k.R - 1) * q.M) / q.L + q.Kp; // the longest span of a tile
-    k.rows              = (uint32_t)((span + k.Q - 1) / k.Q);
-    k.cap               = (uint64_t)(((unsigned __int128)cfg->max_samples * q.L) / q.M) + 2;
-    h->smem             = std::max(h->smem, ((q.L == 1 ? q.Kp : 0) + (size_t)k.Q * k.rows) * sizeof(float2)); // taps at L = 1, and the span
+    size_t smem = 0;
+    chan_tiles(q, &k.R, &k.Q, &k.rows, &smem);
+    k.cap   = (uint64_t)(((unsigned __int128)cfg->max_samples * q.L) / q.M) + 2;
+    h->smem = std::max(h->smem, smem);
     if (k.g.reserve(g.size() / 2) || k.rot.reserve(q.P) || k.out.reserve((size_t)cfg->nof_rx * k.cap))
       return fail(LTEPHY_ERROR, "chan_create: device allocation failed");
     CU(cudaMemcpy(k.g.p, g.data(), g.size() * sizeof(float), cudaMemcpyHostToDevice));
@@ -250,13 +269,10 @@ static int chan_run(ltephy_chan_t* h, const void* x, uint64_t first, uint64_t n,
   for (uint32_t c = 0; c < h->cfg.nof_carriers; c++) {
     const ltephy_chan::Carrier& k = h->car[c];
     const ltephy_chan_poly_t&   q = k.q;
-    // outputs m >= 0 whose window [n - Ka, n + Kb], n = floor(m M / L), has every non-negative sample inside [first, first + n)
-    const unsigned __int128 L = q.L, M = q.M, last = first + n - 1;
-    const uint64_t          lo   = first == 0 ? 0 : (uint64_t)(((first + q.Ka) * L + M - 1) / M);
-    const uint64_t          hi_n = last >= q.Kb ? (uint64_t)(((last - q.Kb + 1) * L - 1) / M + 1) : 0;
-    const uint64_t          cnt  = hi_n > lo ? hi_n - lo : 0;
-    const uint64_t          mn = cnt ? hi_n : lo, nn = (uint64_t)(mn * M / L);
-    nx                         = std::min<uint64_t>(nx, nn >= q.Ka ? nn - q.Ka : 0);
+    uint64_t                    lo = 0, cnt = 0, nc = 0;
+    chan_range(q, first, n, &lo, &cnt, &nc);
+    const unsigned __int128     L = q.L, M = q.M;
+    nx = std::min<uint64_t>(nx, nc);
     out[c].first = lo, out[c].count = cnt, out[c].iq_dev = k.out.p;
     if (!cnt) continue;
     const uint64_t per   = (uint64_t)q.L * k.R;

@@ -36,15 +36,18 @@ __device__ __forceinline__ void chan_store(const ChanSeg& q, uint64_t i, uint32_
 // a fixed tap the threads of a warp (consecutive r) read consecutive 8-byte words; a rational one has Q = 1 and reads words M apart.  At L = 1
 // the tile has one phase class: its Kp taps sit in shared memory ahead of the span and the whole CTA reads one tap address per term (a broadcast,
 // two taps per 16-byte load).  At L > 1 a warp's tap reads are one address when R >= 32, through L1 (the [L][Kp] table, up to 256 KB, stays in
-// global memory and L2).
-template <typename X>
+// global memory and L2).  TAB: the segment of a tile is entry tile / tps of the device table g.tab (the raster scan's thousands of (point, antenna)
+// segments, every one of tps tiles), else the one of g.seg whose tiles hold it.
+template <typename X, bool TAB>
 __global__ void __launch_bounds__(CHAN_THREADS) chan_kernel(const __grid_constant__ ChanArgs g)
 {
   extern __shared__ float2 csm[];
   const uint32_t tile = blockIdx.x;
   uint32_t       si   = 0;
-  while (si + 1 < g.nseg && tile >= g.seg[si + 1].tile0) si++;
-  const ChanSeg& q = g.seg[si];
+  if (TAB) si = tile / g.tps;
+  else
+    while (si + 1 < g.nseg && tile >= g.seg[si + 1].tile0) si++;
+  const ChanSeg& q = TAB ? g.tab[si] : g.seg[si];
   const uint32_t L = q.L, M = q.M, Kp = q.Kp, R = q.R, Q = q.Q, rows = q.rows, t = tile - q.tile0;
   const uint64_t i0   = (uint64_t)t * L * R;
   const uint32_t Mt   = (uint32_t)min((uint64_t)L * R, q.count - i0);
@@ -80,7 +83,8 @@ __global__ void __launch_bounds__(CHAN_THREADS) chan_kernel(const __grid_constan
 extern "C" int launch_chan(const ChanArgs& g, uint32_t ntiles, size_t smem, uint32_t fmt, cudaStream_t st)
 {
   if (!ntiles) return 0;
-  const auto k = fmt == 0 ? chan_kernel<float2> : fmt == 1 ? chan_kernel<short2> : fmt == 2 ? chan_kernel<char2> : nullptr;
+  const auto k = g.tab ? (fmt == 0 ? chan_kernel<float2, true> : fmt == 1 ? chan_kernel<short2, true> : fmt == 2 ? chan_kernel<char2, true> : nullptr)
+                      : (fmt == 0 ? chan_kernel<float2, false> : fmt == 1 ? chan_kernel<short2, false> : fmt == 2 ? chan_kernel<char2, false> : nullptr);
   if (!k || cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return -1;
   k<<<ntiles, CHAN_THREADS, smem, st>>>(g);
   return cudaGetLastError() == cudaSuccess ? 0 : -1;

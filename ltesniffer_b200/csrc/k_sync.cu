@@ -23,6 +23,7 @@ __global__ void __launch_bounds__(COARSE_THREADS) sync_coarse_kernel(SyncArgs g,
   float2*        rB = reinterpret_cast<float2*>(rA + N);    // p2 per tap
   float2*        xs = rB + N;                               // (T + N / D) * Ds samples
   const uint64_t j0 = (uint64_t)blockIdx.x * T, s0 = j0 * D;
+  m += (uint64_t)blockIdx.y * 3 * g.J;
   const uint32_t span = T * D + N;
   for (uint32_t i = threadIdx.x; i < N; i += blockDim.x) {
     const float2 a = g.rep[i], b = g.rep[N + i];
@@ -39,7 +40,7 @@ __global__ void __launch_bounds__(COARSE_THREADS) sync_coarse_kernel(SyncArgs g,
   }
   for (uint32_t a = 0; a < g.A; a++) {
     __syncthreads();
-    const X* xa = static_cast<const X*>(g.x) + (uint64_t)a * g.lda;
+    const X* xa = static_cast<const X*>(g.x) + blockIdx.y * g.ps + (uint64_t)a * g.lda;
     for (uint32_t i = threadIdx.x; i < span; i += blockDim.x) {
       const uint64_t s    = s0 + i;
       xs[(i / D) * Ds + i % D] = s < g.L ? chan_cf32(xa[s]) : make_float2(0.0f, 0.0f);
@@ -96,6 +97,7 @@ __global__ void sync_fold_kernel(SyncArgs g, const float* __restrict__ m, float*
   const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= 3 * SYNC_BINS) return;
   const uint32_t u = t / SYNC_BINS, b = t % SYNC_BINS;
+  m += (uint64_t)blockIdx.y * 3 * g.J, fold += blockIdx.y * 3 * SYNC_BINS;
   float          sum = 0.0f;
   uint32_t       cnt = 0;
   for (uint64_t j = b; j < g.J; j += SYNC_BINS, cnt++) sum = sum + m[u * g.J + j];
@@ -107,7 +109,8 @@ __global__ void __launch_bounds__(1024) sync_peak_kernel(const float* __restrict
 {
   __shared__ float    sv[1024];
   __shared__ uint32_t si[1024];
-  const float*        f = fold + blockIdx.x * SYNC_BINS;
+  const uint32_t      up = blockIdx.y * 3 + blockIdx.x; // (capture, N_ID_2)
+  const float*        f  = fold + up * SYNC_BINS;
   float               bv = -1.0f;
   uint32_t            bi = 0xFFFFFFFFu;
   for (uint32_t b = threadIdx.x; b < SYNC_BINS; b += blockDim.x)
@@ -136,16 +139,16 @@ __global__ void __launch_bounds__(1024) sync_peak_kernel(const float* __restrict
     if (threadIdx.x < off) sv[threadIdx.x] = fmaxf(sv[threadIdx.x], sv[threadIdx.x + off]);
     __syncthreads();
   }
-  if (threadIdx.x == 0) pk[blockIdx.x] = SyncPeak{bp, peak, sv[0], 0, 0.0f, 0.0f, 0.0f};
+  if (threadIdx.x == 0) pk[up] = SyncPeak{bp, peak, sv[0], 0, 0.0f, 0.0f, 0.0f};
 }
 
 // the metric of one window at stride 1, in lteo_cell_search's sync_metric order
 template <typename X>
-static __device__ float sync_window_metric(const SyncArgs& g, uint64_t t, const float2* __restrict__ p, float ep)
+static __device__ float sync_window_metric(const SyncArgs& g, const X* x, uint64_t t, const float2* __restrict__ p, float ep)
 {
   float P = 0.0f, E = 0.0f;
   for (uint32_t a = 0; a < g.A; a++) {
-    const X* xa = static_cast<const X*>(g.x) + (uint64_t)a * g.lda + t;
+    const X* xa = x + (uint64_t)a * g.lda + t;
     float    cr = 0.0f, ci = 0.0f, e = 0.0f;
     for (uint32_t k = 0; k < g.N; k++) {
       const float2 v = chan_cf32(xa[k]), w = p[k];
@@ -167,9 +170,10 @@ __global__ void sync_refine_kernel(SyncArgs g, const SyncPeak* __restrict__ pk, 
   const uint32_t NR = 2 * g.D - 1, t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= 3 * g.nh * NR) return;
   const uint32_t u = t / (g.nh * NR), h = (t / NR) % g.nh, i = t % NR;
+  pk += blockIdx.y * 3, rm += (uint64_t)blockIdx.y * 3 * g.nh * NR;
   const uint64_t HF = 75ull * g.N, tt = ((uint64_t)pk[u].bin * g.D + HF + i - (g.D - 1)) % HF + h * HF;
   const float    ep = u == 0 ? g.ep[0] : u == 1 ? g.ep[1] : g.ep[2]; // no run-time index into the parameters (it would copy them to local memory)
-  if (tt + g.N <= g.L) rm[t] = sync_window_metric<X>(g, tt, g.rep + u * g.N, ep);
+  if (tt + g.N <= g.L) rm[t] = sync_window_metric<X>(g, static_cast<const X*>(g.x) + blockIdx.y * g.ps, tt, g.rep + u * g.N, ep);
 }
 
 // one block per N_ID_2: fold the refined metrics, pick the best offset (ties to the lowest), then S = sum_h sum_a c2 conj(c1) at that timing
@@ -181,6 +185,7 @@ __global__ void sync_select_kernel(SyncArgs g, const float* __restrict__ rm, flo
   __shared__ uint32_t s_tau;
   const uint32_t u = blockIdx.x, NR = 2 * g.D - 1;
   const uint64_t HF = 75ull * g.N;
+  rm += (uint64_t)blockIdx.y * 3 * g.nh * NR, c12 += (uint64_t)blockIdx.y * 3 * g.nh * g.A, pk += blockIdx.y * 3, refined += blockIdx.y * 3 * NR;
   const uint32_t bp = pk[u].bin;
   if (threadIdx.x < NR) {
     const uint32_t i  = threadIdx.x;
@@ -207,7 +212,7 @@ __global__ void sync_select_kernel(SyncArgs g, const float* __restrict__ rm, flo
     const uint32_t h = w / g.A, a = w % g.A;
     const uint64_t t = tau + h * HF;
     if (t + g.N > g.L) continue;
-    const X* xa  = static_cast<const X*>(g.x) + (uint64_t)a * g.lda + t;
+    const X* xa  = static_cast<const X*>(g.x) + blockIdx.y * g.ps + (uint64_t)a * g.lda + t;
     float    c1r = 0.0f, c1i = 0.0f, c2r = 0.0f, c2i = 0.0f;
     for (uint32_t k = 0; k < g.N / 2; k++) {
       const float2 v = chan_cf32(xa[k]), q = p[k];
@@ -234,10 +239,6 @@ __global__ void sync_select_kernel(SyncArgs g, const float* __restrict__ rm, flo
   }
 }
 
-// element u of a kernel-parameter array without a run-time index
-template <typename T>
-static __device__ __forceinline__ T sss_pick(const T (&v)[3], uint32_t u) { return u == 0 ? v[0] : u == 1 ? v[1] : v[2]; }
-
 // Y[u][hs][a][sym][n]: 62-bin DFT of the PSS (sym 0, at tau + h HF) and SSS (sym 1, N + 9D earlier) windows, h = h0[u] + hs, twiddles in shared memory
 template <typename X>
 __global__ void __launch_bounds__(256) sync_dft_kernel(SyncArgs g, SyncSss s, float2* __restrict__ Y)
@@ -248,9 +249,10 @@ __global__ void __launch_bounds__(256) sync_dft_kernel(SyncArgs g, SyncSss s, fl
   const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x, per_u = s.nhmax * g.A * 2 * 62;
   if (t >= 3 * per_u) return;
   const uint32_t u = t / per_u, n = t % 62, sym = (t / 62) % 2, a = (t / 124) % g.A, hs = (t / (124 * g.A)) % s.nhmax;
-  if (hs >= sss_pick(s.nH, u)) return;
-  const uint64_t tp = sss_pick(s.tau, u) + (uint64_t)(sss_pick(s.h0, u) + hs) * 75ull * g.N, t0 = sym ? tp - g.N - 9 * g.D : tp;
-  const X*       xa = static_cast<const X*>(g.x) + (uint64_t)a * g.lda + t0;
+  const SyncPt&  q = s.pt[blockIdx.y];
+  if (hs >= q.nH[u]) return;
+  const uint64_t tp = q.tau[u] + (uint64_t)(q.h0[u] + hs) * 75ull * g.N, t0 = sym ? tp - g.N - 9 * g.D : tp;
+  const X*       xa = static_cast<const X*>(g.x) + blockIdx.y * g.ps + (uint64_t)a * g.lda + t0;
   const uint32_t f  = n < 31 ? g.N + n - 31 : n - 30;
   float          yr = 0.0f, yi = 0.0f;
   uint32_t       idx = 0; // (f m) mod N
@@ -261,7 +263,7 @@ __global__ void __launch_bounds__(256) sync_dft_kernel(SyncArgs g, SyncSss s, fl
     idx += f;
     if (idx >= g.N) idx -= g.N;
   }
-  Y[t] = make_float2(yr, yi);
+  Y[(uint64_t)blockIdx.y * 3 * per_u + t] = make_float2(yr, yi);
 }
 
 // one warp per (N_ID_2, N_ID_1): z[n] = sum_a Y_sss conj(Y_pss conj(d_u) exp(-j phi)) (real part), then for every half-frame the two SSS
@@ -272,8 +274,9 @@ __global__ void __launch_bounds__(256) sync_sss_kernel(SyncArgs g, SyncSss s, co
   if (wid >= 3 * 168) return;
   const uint32_t u = wid / 168, n1 = wid % 168, per_u = s.nhmax * g.A * 124;
   const float*   q0 = s.seq + ((u * 168 + n1) * 2 + 0) * 62, *q1 = q0 + 62;
-  const float    rc = u == 0 ? s.rot[0][0] : u == 1 ? s.rot[1][0] : s.rot[2][0], rs = u == 0 ? s.rot[0][1] : u == 1 ? s.rot[1][1] : s.rot[2][1];
-  const uint32_t nH = sss_pick(s.nH, u), h0 = sss_pick(s.h0, u);
+  const SyncPt&  q  = s.pt[blockIdx.y];
+  const uint32_t nH = q.nH[u], h0 = q.h0[u];
+  const float2*  Yu = Y + (blockIdx.y * 3 + u) * per_u;
   float          A0 = 0.0f, A1 = 0.0f;
   for (uint32_t hs = 0; hs < nH; hs++) {
     float p0 = 0.0f, p1 = 0.0f;
@@ -281,9 +284,10 @@ __global__ void __launch_bounds__(256) sync_sss_kernel(SyncArgs g, SyncSss s, co
       const float2 d  = s.dpss[u * 62 + n];
       float        zr = 0.0f;
       for (uint32_t a = 0; a < g.A; a++) {
-        const float2* Ya = Y + u * per_u + (hs * g.A + a) * 124;
+        const float2* Ya = Yu + (hs * g.A + a) * 124;
         const float2  yp = Ya[n], ys = Ya[62 + n];
         const float   hr = yp.x * d.x + yp.y * d.y, hi = yp.y * d.x - yp.x * d.y;
+        const float   rc = __ldg(&q.rot[u][0]), rs = __ldg(&q.rot[u][1]); // loaded where used: hoisted, they spilled
         const float   gr = hr * rc - hi * rs, gi = hr * rs + hi * rc;
         zr               = zr + (ys.x * gr + ys.y * gi);
       }
@@ -298,10 +302,10 @@ __global__ void __launch_bounds__(256) sync_sss_kernel(SyncArgs g, SyncSss s, co
     A0               = A0 + ((h & 1) ? p1 : p0);
     A1               = A1 + ((h & 1) ? p0 : p1);
   }
-  if (lane == 0) out[(u * 168 + n1) * 2] = A0, out[(u * 168 + n1) * 2 + 1] = A1;
+  if (lane == 0) out[((blockIdx.y * 3 + u) * 168 + n1) * 2] = A0, out[((blockIdx.y * 3 + u) * 168 + n1) * 2 + 1] = A1;
 }
 
-extern "C" int launch_sync_pss(const SyncArgs& g, uint32_t fmt, float* m, float* fold, SyncPeak* pk, float* rm, float4* c12, float* refined,
+extern "C" int launch_sync_pss(const SyncArgs& g, uint32_t np, uint32_t fmt, float* m, float* fold, SyncPeak* pk, float* rm, float4* c12, float* refined,
                                cudaStream_t st, uint64_t* launches)
 {
   const uint32_t T = COARSE_THREADS * COARSE_R, Ds = g.D | 1u;
@@ -309,26 +313,26 @@ extern "C" int launch_sync_pss(const SyncArgs& g, uint32_t fmt, float* m, float*
   return with_iq_type(fmt, [&](auto z) {
     using X = decltype(z);
     if (cudaFuncSetAttribute(sync_coarse_kernel<X>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return -1;
-    sync_coarse_kernel<X><<<(unsigned)((g.J + T - 1) / T), COARSE_THREADS, smem, st>>>(g, m);
-    sync_fold_kernel<<<(3 * SYNC_BINS + 255) / 256, 256, 0, st>>>(g, m, fold);
-    sync_peak_kernel<<<3, 1024, 0, st>>>(fold, pk);
+    sync_coarse_kernel<X><<<dim3((unsigned)((g.J + T - 1) / T), np), COARSE_THREADS, smem, st>>>(g, m);
+    sync_fold_kernel<<<dim3((3 * SYNC_BINS + 255) / 256, np), 256, 0, st>>>(g, m, fold);
+    sync_peak_kernel<<<dim3(3, np), 1024, 0, st>>>(fold, pk);
     const uint32_t nr = 3 * g.nh * (2 * g.D - 1);
-    sync_refine_kernel<X><<<(nr + 127) / 128, 128, 0, st>>>(g, pk, rm);
-    sync_select_kernel<X><<<3, 256, 0, st>>>(g, rm, c12, pk, refined);
+    sync_refine_kernel<X><<<dim3((nr + 127) / 128, np), 128, 0, st>>>(g, pk, rm);
+    sync_select_kernel<X><<<dim3(3, np), 256, 0, st>>>(g, rm, c12, pk, refined);
     *launches += 5;
     return cudaGetLastError() == cudaSuccess ? 0 : -1;
   });
 }
 
-extern "C" int launch_sync_sss(const SyncArgs& g, uint32_t fmt, const SyncSss& s, float2* Y, float* sss, cudaStream_t st, uint64_t* launches)
+extern "C" int launch_sync_sss(const SyncArgs& g, uint32_t np, uint32_t fmt, const SyncSss& s, float2* Y, float* sss, cudaStream_t st, uint64_t* launches)
 {
   const uint32_t nt = 3 * s.nhmax * g.A * 124;
   if (nt)
     with_iq_type(fmt, [&](auto z) {
-      sync_dft_kernel<decltype(z)><<<(nt + 255) / 256, 256, g.N * sizeof(float2), st>>>(g, s, Y);
+      sync_dft_kernel<decltype(z)><<<dim3((nt + 255) / 256, np), 256, g.N * sizeof(float2), st>>>(g, s, Y);
       return 0;
     });
-  sync_sss_kernel<<<(3 * 168 * 32 + 255) / 256, 256, 0, st>>>(g, s, Y, sss);
+  sync_sss_kernel<<<dim3((3 * 168 * 32 + 255) / 256, np), 256, 0, st>>>(g, s, Y, sss);
   *launches += nt ? 2 : 1;
   return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }

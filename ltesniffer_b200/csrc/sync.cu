@@ -13,7 +13,7 @@
 
 struct ltephy_sync {
   ltephy_sync_cfg_t cfg{};
-  uint32_t          N = 0, D = 0, A = 0, NR = 0, nhmax = 0;
+  uint32_t          N = 0, D = 0, A = 0, NR = 0, nhmax = 0, points = 1; // points: captures a batch may hold
   uint64_t          Jmax = 0;
   Stream            stream;
   float             ep[3]{};
@@ -23,6 +23,7 @@ struct ltephy_sync {
   DevBuf<float>     d_seq, d_m, d_fold, d_rm, d_ref, d_sss;
   DevBuf<float4>    d_c12;
   DevBuf<SyncPeak>  d_pk;
+  DevBuf<SyncPt>    d_pt;
   uint64_t          launches = 0;
   bool              searched = false;
 };
@@ -81,7 +82,8 @@ static void sss_seq(uint32_t n_id_1, uint32_t n_id_2, uint32_t sf5, float* d)
   }
 }
 
-extern "C" int ltephy_sync_create(const ltephy_sync_cfg_t* cfg, ltephy_sync_t** out)
+// points: captures a batch holds; stage: keep a buffer for the host input of ltephy_cell_search
+static int sync_create(const ltephy_sync_cfg_t* cfg, uint32_t points, bool stage, ltephy_sync_t** out)
 {
   if (!cfg || !out) return fail(LTEPHY_ERROR_INVALID_INPUTS, "sync_create: null argument");
   const uint32_t N = cfg->symbol_sz, M = N % 3 ? N : N / 3;
@@ -95,7 +97,7 @@ extern "C" int ltephy_sync_create(const ltephy_sync_cfg_t* cfg, ltephy_sync_t** 
   CU(cudaSetDevice(cfg->device));
   std::unique_ptr<ltephy_sync, decltype(&ltephy_sync_destroy)> owner(new ltephy_sync(), ltephy_sync_destroy);
   ltephy_sync* const                                           h = owner.get();
-  h->cfg = *cfg, h->N = N, h->D = N / 128, h->A = cfg->nof_rx, h->NR = 2 * h->D - 1;
+  h->cfg = *cfg, h->N = N, h->D = N / 128, h->A = cfg->nof_rx, h->NR = 2 * h->D - 1, h->points = points;
   h->Jmax  = (cfg->max_samples - N) / h->D + 1;
   h->nhmax = (uint32_t)((cfg->max_samples - N) / (75ull * N) + 1);
   CU(cudaStreamCreateWithFlags(&h->stream.raw, cudaStreamNonBlocking));
@@ -111,10 +113,11 @@ extern "C" int ltephy_sync_create(const ltephy_sync_cfg_t* cfg, ltephy_sync_t** 
   for (uint32_t u = 0; u < 3; u++)
     for (uint32_t n1 = 0; n1 < 168; n1++)
       for (uint32_t q = 0; q < 2; q++) sss_seq(n1, u, q, &seq[((u * 168 + n1) * 2 + q) * 62]);
+  const size_t P = points;
   if (h->d_rep.reserve(rep.size()) || h->d_W.reserve(N) || h->d_dpss.reserve(3 * 62) || h->d_seq.reserve(seq.size()) ||
-      h->d_x.reserve((size_t)h->A * cfg->max_samples * iq_sample_bytes(cfg->iq_format)) || h->d_m.reserve(3 * h->Jmax) || h->d_fold.reserve(3 * SYNC_BINS) ||
-      h->d_rm.reserve((size_t)3 * h->nhmax * h->NR) || h->d_ref.reserve(3 * h->NR) || h->d_sss.reserve(3 * 336) ||
-      h->d_c12.reserve((size_t)3 * h->nhmax * h->A) || h->d_pk.reserve(3) || h->d_Y.reserve((size_t)3 * h->nhmax * h->A * 124))
+      (stage && h->d_x.reserve((size_t)h->A * cfg->max_samples * iq_sample_bytes(cfg->iq_format))) || h->d_m.reserve(P * 3 * h->Jmax) ||
+      h->d_fold.reserve(P * 3 * SYNC_BINS) || h->d_rm.reserve(P * 3 * h->nhmax * h->NR) || h->d_ref.reserve(P * 3 * h->NR) || h->d_sss.reserve(P * 3 * 336) ||
+      h->d_c12.reserve(P * 3 * h->nhmax * h->A) || h->d_pk.reserve(P * 3) || h->d_Y.reserve(P * 3 * h->nhmax * h->A * 124) || h->d_pt.reserve(P))
     return fail(LTEPHY_ERROR, "sync_create: device allocation failed");
   CU(cudaMemcpy(h->d_rep.p, rep.data(), rep.size() * sizeof(float2), cudaMemcpyHostToDevice));
   CU(cudaMemcpy(h->d_W.p, W.data(), W.size() * sizeof(float2), cudaMemcpyHostToDevice));
@@ -123,6 +126,13 @@ extern "C" int ltephy_sync_create(const ltephy_sync_cfg_t* cfg, ltephy_sync_t** 
   *out = owner.release();
   return LTEPHY_SUCCESS;
 }
+
+extern "C" int ltephy_sync_create(const ltephy_sync_cfg_t* cfg, ltephy_sync_t** out) { return sync_create(cfg, 1, true, out); }
+
+// the raster scan's handle searches its captures in place and stages no input of its own
+int sync_create_batch(const ltephy_sync_cfg_t* cfg, uint32_t points, ltephy_sync_t** out) { return sync_create(cfg, points, false, out); }
+
+cudaStream_t sync_stream(ltephy_sync_t* h) { return h->stream; }
 
 extern "C" void ltephy_sync_destroy(ltephy_sync_t* h)
 {
@@ -140,72 +150,84 @@ static int sync_check(ltephy_sync_t* h, const void* iq, uint64_t L, ltephy_cell_
   return LTEPHY_SUCCESS;
 }
 
-int sync_run(ltephy_sync_t* h, const void* x, uint64_t lda, uint64_t L, ltephy_cell_t* out)
+int sync_run(ltephy_sync_t* h, const void* x, uint64_t lda, uint64_t L, ltephy_cell_t* out) { return sync_run_batch(h, x, lda, 0, L, 1, out); }
+
+int sync_run_batch(ltephy_sync_t* h, const void* x, uint64_t lda, uint64_t ps, uint64_t L, uint32_t np, ltephy_cell_t* out)
 {
+  if (np < 1 || np > h->points) return fail(LTEPHY_ERROR_INVALID_INPUTS, "cell_search: %u captures, not 1..%u", np, h->points);
   const uint32_t N = h->N, D = h->D, CP6 = 9 * D;
   const uint64_t HF = 75ull * N, FR = 150ull * N;
   SyncArgs       g{};
-  g.x = x, g.lda = lda, g.L = L, g.J = (L - N) / D + 1, g.N = N, g.D = D, g.A = h->A, g.nh = (uint32_t)((L - N) / HF + 1);
+  g.x = x, g.lda = lda, g.ps = ps, g.L = L, g.J = (L - N) / D + 1, g.N = N, g.D = D, g.A = h->A, g.nh = (uint32_t)((L - N) / HF + 1);
   g.rep = h->d_rep.p, g.W = h->d_W.p;
   for (int u = 0; u < 3; u++) g.ep[u] = h->ep[u];
-  if (launch_sync_pss(g, h->cfg.iq_format, h->d_m.p, h->d_fold.p, h->d_pk.p, h->d_rm.p, h->d_c12.p, h->d_ref.p, h->stream, &h->launches))
+  if (launch_sync_pss(g, np, h->cfg.iq_format, h->d_m.p, h->d_fold.p, h->d_pk.p, h->d_rm.p, h->d_c12.p, h->d_ref.p, h->stream, &h->launches))
     return fail(LTEPHY_ERROR, "cell_search: PSS kernels failed: %s", cudaGetErrorString(cudaGetLastError()));
-  SyncPeak pk[3];
-  CU(cudaMemcpyAsync(pk, h->d_pk.p, sizeof(pk), cudaMemcpyDeviceToHost, h->stream));
+  std::vector<SyncPeak> pks((size_t)3 * np);
+  CU(cudaMemcpyAsync(pks.data(), h->d_pk.p, pks.size() * sizeof(SyncPeak), cudaMemcpyDeviceToHost, h->stream));
   CU(cudaStreamSynchronize(h->stream));
-  ltephy_cell_t res[3];
-  SyncSss       s{};
-  s.dpss = h->d_dpss.p, s.seq = h->d_seq.p;
-  for (uint32_t u = 0; u < 3; u++) {
-    ltephy_cell_t& o = res[u];
-    memset(&o, 0, sizeof(o));
-    o.n_id_2   = (uint8_t)u;
-    o.psr      = pk[u].side > 0.0f ? pk[u].peak / pk[u].side : (pk[u].peak > 0.0f ? INFINITY : 0.0f);
-    o.pss_peak = pk[u].rpeak;
-    o.cfo_re = pk[u].s_re, o.cfo_im = pk[u].s_im;
-    o.cfo_hz   = atan2f(pk[u].s_im, pk[u].s_re) * (float)(15000.0 / M_PI);
-    const double phi = 2.0 * M_PI * (double)o.cfo_hz * (double)(N + CP6) / (15000.0 * (double)N);
-    s.rot[u][0] = (float)std::cos(phi), s.rot[u][1] = (float)-std::sin(phi);
-    // half-frames h with the PSS window at tau + h HF inside the capture and the SSS window N + CP6 before it at or after sample 0
-    const uint64_t tau = pk[u].tau;
-    s.tau[u]           = tau;
-    s.h0[u]            = tau < N + CP6 ? 1 : 0;
-    const uint64_t last = (L - N - tau) / HF; // tau + HF > L - N cannot leave h = 0 without a PSS window
-    s.nH[u]            = tau + N <= L && last >= s.h0[u] ? (uint32_t)(last - s.h0[u] + 1) : 0;
-    o.nof_half_frames  = s.nH[u];
-  }
-  s.nhmax = std::max(s.nH[0], std::max(s.nH[1], s.nH[2]));
-  if (launch_sync_sss(g, h->cfg.iq_format, s, h->d_Y.p, h->d_sss.p, h->stream, &h->launches))
-    return fail(LTEPHY_ERROR, "cell_search: SSS kernels failed: %s", cudaGetErrorString(cudaGetLastError()));
-  std::vector<float> tab(3 * 336);
-  CU(cudaMemcpyAsync(tab.data(), h->d_sss.p, tab.size() * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-  CU(cudaStreamSynchronize(h->stream));
-  for (uint32_t u = 0; u < 3; u++) {
-    ltephy_cell_t& o = res[u];
-    const int64_t  st = (int64_t)pk[u].tau - (int64_t)(13 * N / 2); // first sample of the subframe whose symbol 6 starts at tau
-    if (!s.nH[u]) {
-      o.n_id_1 = o.pci = 0xFFFF;
-      o.frame_offset   = (uint64_t)(((st % (int64_t)FR) + (int64_t)FR) % (int64_t)FR);
-      continue;
+  std::vector<ltephy_cell_t> all((size_t)3 * np);
+  std::vector<SyncPt>        pts(np);
+  SyncSss                    s{};
+  s.pt = h->d_pt.p, s.dpss = h->d_dpss.p, s.seq = h->d_seq.p;
+  for (uint32_t p = 0; p < np; p++)
+    for (uint32_t u = 0; u < 3; u++) {
+      const SyncPeak* pk = &pks[3 * p];
+      SyncPt&         q  = pts[p];
+      ltephy_cell_t&  o  = all[3 * p + u];
+      memset(&o, 0, sizeof(o));
+      o.n_id_2   = (uint8_t)u;
+      o.psr      = pk[u].side > 0.0f ? pk[u].peak / pk[u].side : (pk[u].peak > 0.0f ? INFINITY : 0.0f);
+      o.pss_peak = pk[u].rpeak;
+      o.cfo_re = pk[u].s_re, o.cfo_im = pk[u].s_im;
+      o.cfo_hz   = atan2f(pk[u].s_im, pk[u].s_re) * (float)(15000.0 / M_PI);
+      const double phi = 2.0 * M_PI * (double)o.cfo_hz * (double)(N + CP6) / (15000.0 * (double)N);
+      q.rot[u][0] = (float)std::cos(phi), q.rot[u][1] = (float)-std::sin(phi);
+      // half-frames h with the PSS window at tau + h HF inside the capture and the SSS window N + CP6 before it at or after sample 0
+      const uint64_t tau = pk[u].tau;
+      q.tau[u]           = tau;
+      q.h0[u]            = tau < N + CP6 ? 1 : 0;
+      const uint64_t last = (L - N - tau) / HF; // tau + HF > L - N cannot leave h = 0 without a PSS window
+      q.nH[u]            = tau + N <= L && last >= q.h0[u] ? (uint32_t)(last - q.h0[u] + 1) : 0;
+      o.nof_half_frames  = q.nH[u];
+      s.nhmax            = std::max(s.nhmax, q.nH[u]);
     }
-    const float* Au   = &tab[u * 336];
-    uint32_t     best = 0;
-    for (uint32_t i = 1; i < 336; i++)
-      if (Au[i] > Au[best]) best = i; // ties: lowest N_ID_1, then q = 0
-    float second = -INFINITY;
-    for (uint32_t i = 0; i < 336; i++)
-      if (i != best && Au[i] > second) second = Au[i];
-    o.n_id_1       = (uint16_t)(best / 2);
-    o.pci          = (uint16_t)(3 * (best / 2) + u);
-    o.sss_peak     = Au[best];
-    o.sss_ratio    = second > 0.0f ? Au[best] / second : (Au[best] > 0.0f ? INFINITY : 0.0f);
-    const int64_t fs = (best & 1) ? st - (int64_t)HF : st; // q = 1: the half-frame at tau is subframe 5
-    o.frame_offset = (uint64_t)(((fs % (int64_t)FR) + (int64_t)FR) % (int64_t)FR);
-    o.detected     = o.psr >= SYNC_PSR_MIN && o.sss_ratio >= SYNC_SSS_MIN;
+  CU(cudaMemcpyAsync(h->d_pt.p, pts.data(), pts.size() * sizeof(SyncPt), cudaMemcpyHostToDevice, h->stream));
+  if (launch_sync_sss(g, np, h->cfg.iq_format, s, h->d_Y.p, h->d_sss.p, h->stream, &h->launches))
+    return fail(LTEPHY_ERROR, "cell_search: SSS kernels failed: %s", cudaGetErrorString(cudaGetLastError()));
+  std::vector<float> tabs((size_t)np * 3 * 336);
+  CU(cudaMemcpyAsync(tabs.data(), h->d_sss.p, tabs.size() * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  CU(cudaStreamSynchronize(h->stream));
+  for (uint32_t p = 0; p < np; p++) {
+    const float*   tab = &tabs[(size_t)p * 3 * 336];
+    ltephy_cell_t* res = &all[3 * p];
+    for (uint32_t u = 0; u < 3; u++) {
+      ltephy_cell_t& o  = res[u];
+      const int64_t  st = (int64_t)pks[3 * p + u].tau - (int64_t)(13 * N / 2); // first sample of the subframe whose symbol 6 starts at tau
+      if (!pts[p].nH[u]) {
+        o.n_id_1 = o.pci = 0xFFFF;
+        o.frame_offset   = (uint64_t)(((st % (int64_t)FR) + (int64_t)FR) % (int64_t)FR);
+        continue;
+      }
+      const float* Au   = &tab[u * 336];
+      uint32_t     best = 0;
+      for (uint32_t i = 1; i < 336; i++)
+        if (Au[i] > Au[best]) best = i; // ties: lowest N_ID_1, then q = 0
+      float second = -INFINITY;
+      for (uint32_t i = 0; i < 336; i++)
+        if (i != best && Au[i] > second) second = Au[i];
+      o.n_id_1       = (uint16_t)(best / 2);
+      o.pci          = (uint16_t)(3 * (best / 2) + u);
+      o.sss_peak     = Au[best];
+      o.sss_ratio    = second > 0.0f ? Au[best] / second : (Au[best] > 0.0f ? INFINITY : 0.0f);
+      const int64_t fs = (best & 1) ? st - (int64_t)HF : st; // q = 1: the half-frame at tau is subframe 5
+      o.frame_offset = (uint64_t)(((fs % (int64_t)FR) + (int64_t)FR) % (int64_t)FR);
+      o.detected     = o.psr >= SYNC_PSR_MIN && o.sss_ratio >= SYNC_SSS_MIN;
+    }
+    uint32_t ord[3] = {0, 1, 2};
+    std::stable_sort(ord, ord + 3, [&](uint32_t a, uint32_t b) { return res[a].pss_peak > res[b].pss_peak; });
+    for (uint32_t i = 0; i < 3; i++) out[3 * p + i] = res[ord[i]];
   }
-  uint32_t ord[3] = {0, 1, 2};
-  std::stable_sort(ord, ord + 3, [&](uint32_t a, uint32_t b) { return res[a].pss_peak > res[b].pss_peak; });
-  for (uint32_t i = 0; i < 3; i++) out[i] = res[ord[i]];
   h->searched = true;
   return LTEPHY_SUCCESS;
 }
