@@ -89,6 +89,12 @@ struct DevGrant {          // one PDSCH grant
   uint32_t scr_off[2];     // offset (words) of the scrambling sequence in the sequence pool
 };
 
+struct DevScr {            // one PDSCH or PUSCH codeword's scrambling sequence (scr_seq_kernel)
+  uint32_t c_init;         // Gold-sequence initialisation, 36.211 6.3.1 (PDSCH) / 5.3.1 (PUSCH)
+  uint32_t words;          // sequence words
+  uint32_t scr_off;        // offset (words) of the sequence in the sequence pool
+};
+
 // The soft-bit, turbo-stream and HARQ pools of one batch pass 2^32 elements (8.6 GB of soft bits after ~24 000 subframes of a loaded
 // 20 MHz cell), so offsets into them are 64-bit.  Scrambling-word and payload-byte offsets (scr_off, DevPair.out_byte, DevTb.byte_off) stay
 // 32-bit: they would need ~2^37 soft bits or ~200 GB of turbo pool before they wrap, which no 80 GB card holds.

@@ -1,5 +1,6 @@
 // dev_eq.cuh -- per-RE equalisers shared by the PDCCH and PDSCH kernels (zero forcing: the reference
-// leaves decoder_type = 0, SURVEY.md App. B.7).  Operation order mirrors the CPU oracle exactly.
+// leaves decoder_type = 0, SURVEY.md App. B.7), the zero-denominator rule they share with the PUSCH kernel, and the int16 soft
+// demapper with descrambling of the PDSCH and PUSCH kernels.  Operation order mirrors the CPU oracles exactly.
 #pragma once
 #include "dev_common.cuh"
 
@@ -40,6 +41,56 @@ __device__ __forceinline__ float2 h_at(const DevCell& c, const SfView& v, uint32
 // numerator / denominator of an equaliser, with an exactly zero denominator (no channel at all: a zero-filled capture, a dead antenna, a singular
 // 2x2) giving 0 instead of 0/0 = NaN, so that the RE becomes an erasure (LLR 0) -- DESIGN.md section 2.  Every other quotient is unchanged.
 __device__ __forceinline__ float eq_div(float n, float d) { return d == 0.0f ? 0.0f : n / d; }
+
+// ---- int16 soft demodulation (srsran_demod_soft_demodulate_s: scales 100*sqrt2 / 400 / 700 / 1000) and descrambling
+__device__ __forceinline__ short f2s(float v)
+{
+  if (isnan(v)) return 0; // fmaxf would turn NaN into -32767, a full-confidence bit
+  v = fminf(fmaxf(v, -32767.0f), 32767.0f);
+  return (short)(int)v; // truncation toward zero
+}
+__device__ __forceinline__ int iabs(int v) { return v < 0 ? -v : v; }
+__device__ __forceinline__ void demod_s(float2 x, uint32_t qm, short* z)
+{
+  if (qm == 2) {
+    const float s = 141.421356f;
+    z[0] = (short)-f2s(x.x * s), z[1] = (short)-f2s(x.y * s);
+  } else if (qm == 4) {
+    const int yr = f2s(x.x * 400.0f), yi = f2s(x.y * 400.0f);
+    z[0] = (short)-yr, z[1] = (short)-yi;
+    z[2] = (short)(iabs(yr) - 252), z[3] = (short)(iabs(yi) - 252);
+  } else if (qm == 6) {
+    const int yr = f2s(x.x * 700.0f), yi = f2s(x.y * 700.0f);
+    z[0] = (short)-yr, z[1] = (short)-yi;
+    z[2] = (short)(iabs(yr) - 432), z[3] = (short)(iabs(yi) - 432);
+    z[4] = (short)(iabs(z[2]) - 216), z[5] = (short)(iabs(z[3]) - 216);
+  } else { // 256QAM (on the PUSCH: third attempt of PUSCH_Decoder::decode, reference src/src/UL_Sniffer_PUSCH.cc:508-520)
+    const int yr = f2s(x.x * 1000.0f), yi = f2s(x.y * 1000.0f);
+    z[0] = (short)-yr, z[1] = (short)-yi;
+    z[2] = (short)(iabs(yr) - 613), z[3] = (short)(iabs(yi) - 613);
+    z[4] = (short)(iabs(z[2]) - 306), z[5] = (short)(iabs(z[3]) - 306);
+    z[6] = (short)(iabs(z[4]) - 153), z[7] = (short)(iabs(z[5]) - 153);
+  }
+}
+// The Qm soft bits of symbol x * scl: demodulate, flip the sign of bit b where bit b0 + b of the sequence seq is set (Qm bits taken from a
+// 64-bit window), store Qm / 2 packed int16 pairs at out.  An exactly zero x is an erasure (DESIGN.md section 2): LLR 0.  The zero test is on
+// x, before the scale, as in the oracles: a subnormal x that scl rounds to zero still demodulates.  Two conditions make the accesses safe:
+// out is 4-byte aligned because Qm is even and alloc_codeword (ltephy_capi.cu) rounds every codeword's soft-bit offset to 8, and the
+// window's second word lies inside the pool because alloc_codeword reserves one word past every codeword's sequence.
+__device__ __forceinline__ void soft_bits(float2 x, float scl, uint32_t qm, const uint32_t* __restrict__ seq, uint32_t b0, short* __restrict__ out)
+{
+  short z[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  if (x.x != 0.0f || x.y != 0.0f) demod_s(make_float2(x.x * scl, x.y * scl), qm, z);
+  const uint32_t           w0  = b0 >> 5;
+  const unsigned long long win = ((unsigned long long)seq[w0] | ((unsigned long long)seq[w0 + 1] << 32)) >> (b0 & 31u);
+  uint32_t*                o   = reinterpret_cast<uint32_t*>(out);
+#pragma unroll
+  for (uint32_t i = 0; i < 8; i += 2) {
+    if (i >= qm) break;
+    const int a = ((win >> i) & 1ull) ? -(int)z[i] : (int)z[i], b = ((win >> (i + 1)) & 1ull) ? -(int)z[i + 1] : (int)z[i + 1];
+    o[i >> 1]   = ((uint32_t)a & 0xFFFFu) | ((uint32_t)b << 16);
+  }
+}
 
 __device__ __forceinline__ float2 eq_port0(const DevCell& c, const SfView& v, uint32_t idx)
 {

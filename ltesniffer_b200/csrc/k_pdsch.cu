@@ -7,73 +7,28 @@
 #include "k_launch.cuh"
 #include "dev_eq.cuh"
 
-// ---- scrambling sequences: c = x1 ^ XOR_{b in c_init} basis[b]  (36.211 7.2 without the 1600-step warm-up)
-// Grid: x = (grant, codeword), y = block of 256 words.  The grant count goes on x because gridDim.y stops at 65 535 and a batch
-// may carry more than 32 767 grants; a codeword needs a few dozen word blocks at most.
-__global__ void __launch_bounds__(256) scr_seq_kernel(const DevGrant* __restrict__ grants, const uint32_t* __restrict__ x1,
-                                                      const uint32_t* __restrict__ basis, uint32_t basis_words, uint32_t cell_id,
-                                                      uint32_t* __restrict__ seq_pool)
+// ---- scrambling sequences of every codeword of a PDSCH or PUSCH batch: c = x1 ^ XOR_{b in c_init} basis[b]  (36.211 7.2 without the
+// 1600-step warm-up).  Grid: x = codeword, y = block of 256 words.  The codeword count goes on x because gridDim.y stops at 65 535 and a
+// batch may carry more codewords than that; a codeword needs a few dozen word blocks at most.
+__global__ void __launch_bounds__(256) scr_seq_kernel(const DevScr* __restrict__ cws, const uint32_t* __restrict__ x1,
+                                                      const uint32_t* __restrict__ basis, uint32_t basis_words, uint32_t* __restrict__ seq_pool)
 {
-  const DevGrant& g  = grants[blockIdx.x >> 1];
-  const uint32_t  cw = blockIdx.x & 1u;
-  if (cw >= g.ncw) return;
-  const uint32_t nwords = (g.nof_re * g.qm[cw] + 31) / 32;
-  const uint32_t wi     = blockIdx.y * blockDim.x + threadIdx.x;
-  if (wi >= nwords || wi >= basis_words) return;
-  const uint32_t c_init = (g.rnti << 14) + (cw << 13) + (g.sf_idx << 9) + cell_id;
-  uint32_t       v      = x1[wi];
+  const DevScr&  cw = cws[blockIdx.x];
+  const uint32_t wi = blockIdx.y * blockDim.x + threadIdx.x;
+  if (wi >= cw.words || wi >= basis_words) return;
+  uint32_t v = x1[wi];
 #pragma unroll
   for (uint32_t b = 0; b < 31; b++)
-    if ((c_init >> b) & 1u) v ^= basis[(size_t)b * basis_words + wi];
-  seq_pool[g.scr_off[cw] + wi] = v;
+    if ((cw.c_init >> b) & 1u) v ^= basis[(size_t)b * basis_words + wi];
+  seq_pool[cw.scr_off + wi] = v;
 }
 
-__device__ __forceinline__ short f2s(float v)
-{
-  if (isnan(v)) return 0; // fmaxf would turn NaN into -32767, a full-confidence bit
-  v = fminf(fmaxf(v, -32767.0f), 32767.0f);
-  return (short)(int)v; // truncation toward zero
-}
-__device__ __forceinline__ int iabs(int v) { return v < 0 ? -v : v; }
-__device__ __forceinline__ void demod_s(float2 x, uint32_t qm, short* z)
-{
-  if (qm == 2) {
-    z[0] = (short)-f2s(x.x * 141.421356f);
-    z[1] = (short)-f2s(x.y * 141.421356f);
-  } else if (qm == 4) {
-    const int yr = f2s(x.x * 400.0f), yi = f2s(x.y * 400.0f);
-    z[0] = (short)-yr, z[1] = (short)-yi;
-    z[2] = (short)(iabs(yr) - 252), z[3] = (short)(iabs(yi) - 252);
-  } else if (qm == 6) {
-    const int yr = f2s(x.x * 700.0f), yi = f2s(x.y * 700.0f);
-    z[0] = (short)-yr, z[1] = (short)-yi;
-    z[2] = (short)(iabs(yr) - 432), z[3] = (short)(iabs(yi) - 432);
-    z[4] = (short)(iabs(z[2]) - 216), z[5] = (short)(iabs(z[3]) - 216);
-  } else {
-    const int yr = f2s(x.x * 1000.0f), yi = f2s(x.y * 1000.0f);
-    z[0] = (short)-yr, z[1] = (short)-yi;
-    z[2] = (short)(iabs(yr) - 613), z[3] = (short)(iabs(yi) - 613);
-    z[4] = (short)(iabs(z[2]) - 306), z[5] = (short)(iabs(z[3]) - 306);
-    z[6] = (short)(iabs(z[4]) - 153), z[7] = (short)(iabs(z[5]) - 153);
-  }
-}
-// soft-demodulate one equalised symbol, descramble with Qm bits taken from a 64-bit window of the sequence, store
+// soft bits of one equalised symbol of codeword cw at its data-RE index gi
 __device__ __forceinline__ void emit(const DevGrant& g, uint32_t cw, uint32_t gi, float2 x, const uint32_t* __restrict__ seq_pool,
                                      short* __restrict__ llr_pool)
 {
   const uint32_t qm = g.qm[cw];
-  short          z[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-  if (x.x != 0.0f || x.y != 0.0f) demod_s(x, qm, z); // an exactly zero symbol is an erasure (DESIGN.md section 2): LLR 0
-  const uint32_t*    seq = seq_pool + g.scr_off[cw];
-  const uint32_t     b0  = gi * qm, w0 = b0 >> 5;
-  const unsigned long long win = ((unsigned long long)seq[w0] | ((unsigned long long)seq[w0 + 1] << 32)) >> (b0 & 31u);
-  uint32_t*          out = reinterpret_cast<uint32_t*>(llr_pool + g.llr_off[cw] + (size_t)gi * qm); // Qm even, offsets 8-aligned
-#pragma unroll
-  for (uint32_t i = 0; i < 8; i += 2) {
-    if (i >= qm) break;
-    const int a = ((win >> i) & 1ull) ? -(int)z[i] : (int)z[i], b = ((win >> (i + 1)) & 1ull) ? -(int)z[i + 1] : (int)z[i + 1];
-    out[i >> 1] = ((uint32_t)a & 0xFFFFu) | ((uint32_t)b << 16);
-  }
+  soft_bits(x, 1.0f, qm, seq_pool + g.scr_off[cw], gi * qm, llr_pool + g.llr_off[cw] + (size_t)gi * qm);
 }
 
 // One CTA per grant.  Work items are (OFDM symbol, allocated PRB, subcarrier) slots; the 12-bit data-RE
@@ -231,14 +186,19 @@ __global__ void __launch_bounds__(256) rm_turbo_rx_kernel(const DevCb* __restric
   }
 }
 
-extern "C" void launch_pdsch_front(const DevCell& c, const DevGrant* grants, uint32_t ngrants, uint32_t max_words, const float2* sym,
-                                   const float2* ce, const uint32_t* gold_x1, const uint32_t* gold_basis, uint32_t basis_words,
-                                   uint32_t* seq_pool, short* llr_pool, cudaStream_t st, uint64_t* launches)
+extern "C" void launch_scr_seq(const DevScr* cws, uint32_t ncw, uint32_t max_words, const uint32_t* gold_x1, const uint32_t* gold_basis,
+                               uint32_t basis_words, uint32_t* seq_pool, cudaStream_t st, uint64_t* launches)
+{
+  if (!ncw) return;
+  scr_seq_kernel<<<dim3(ncw, (max_words + 255) / 256), 256, 0, st>>>(cws, gold_x1, gold_basis, basis_words, seq_pool);
+  *launches += 1;
+}
+extern "C" void launch_pdsch_front(const DevCell& c, const DevGrant* grants, uint32_t ngrants, const float2* sym, const float2* ce,
+                                   const uint32_t* seq_pool, short* llr_pool, cudaStream_t st, uint64_t* launches)
 {
   if (!ngrants) return;
-  scr_seq_kernel<<<dim3(2 * ngrants, (max_words + 255) / 256), 256, 0, st>>>(grants, gold_x1, gold_basis, basis_words, c.cell_id, seq_pool);
   pdsch_demod_kernel<<<ngrants, 256, 0, st>>>(c, grants, sym, ce, seq_pool, llr_pool);
-  *launches += 2;
+  *launches += 1;
 }
 extern "C" void launch_rm_turbo_rx(const DevCb* cbs, const DevPair* pairs, uint32_t npairs, const short* llr_pool, const uint16_t* rm_pool,
                                    uint32_t* turbo_pool, short* harq_pool, uint32_t gen, cudaStream_t st, uint64_t* launches)

@@ -14,51 +14,6 @@
 #include "dev_ul.cuh"
 #include "dev_eq.cuh"
 
-__device__ __forceinline__ short ul_f2s(float v)
-{
-  if (isnan(v)) return 0; // as f2s (k_pdsch.cu) and the oracle's demodulator
-  v = fminf(fmaxf(v, -32767.0f), 32767.0f);
-  return (short)(int)v;
-}
-__device__ __forceinline__ int ul_iabs(int v) { return v < 0 ? -v : v; }
-__device__ __forceinline__ void ul_demod_s(float2 x, uint32_t qm, short* z)
-{
-  if (qm == 2) {
-    z[0] = (short)-ul_f2s(x.x * 141.421356f);
-    z[1] = (short)-ul_f2s(x.y * 141.421356f);
-  } else if (qm == 4) {
-    const int yr = ul_f2s(x.x * 400.0f), yi = ul_f2s(x.y * 400.0f);
-    z[0] = (short)-yr, z[1] = (short)-yi;
-    z[2] = (short)(ul_iabs(yr) - 252), z[3] = (short)(ul_iabs(yi) - 252);
-  } else if (qm == 6) {
-    const int yr = ul_f2s(x.x * 700.0f), yi = ul_f2s(x.y * 700.0f);
-    z[0] = (short)-yr, z[1] = (short)-yi;
-    z[2] = (short)(ul_iabs(yr) - 432), z[3] = (short)(ul_iabs(yi) - 432);
-    z[4] = (short)(ul_iabs(z[2]) - 216), z[5] = (short)(ul_iabs(z[3]) - 216);
-  } else { // 256QAM (third attempt of PUSCH_Decoder::decode, src/src/UL_Sniffer_PUSCH.cc:508-520)
-    const int yr = ul_f2s(x.x * 1000.0f), yi = ul_f2s(x.y * 1000.0f);
-    z[0] = (short)-yr, z[1] = (short)-yi;
-    z[2] = (short)(ul_iabs(yr) - 613), z[3] = (short)(ul_iabs(yi) - 613);
-    z[4] = (short)(ul_iabs(z[2]) - 306), z[5] = (short)(ul_iabs(z[3]) - 306);
-    z[6] = (short)(ul_iabs(z[4]) - 153), z[7] = (short)(ul_iabs(z[5]) - 153);
-  }
-}
-
-__global__ void __launch_bounds__(256) scr_seq_ul_kernel(const DevUlGrant* __restrict__ grants, const uint32_t* __restrict__ x1,
-                                                         const uint32_t* __restrict__ basis, uint32_t basis_words, uint32_t cell_id,
-                                                         uint32_t* __restrict__ seq_pool)
-{
-  const DevUlGrant& g = grants[blockIdx.x]; // grant on x, word block on y: gridDim.y stops at 65 535 (scr_seq_kernel, k_pdsch.cu)
-  const uint32_t nwords = (12 * g.M * g.qm + 31) / 32, wi = blockIdx.y * blockDim.x + threadIdx.x;
-  if (wi >= nwords || wi >= basis_words) return;
-  const uint32_t c_init = (g.rnti << 14) + (g.sf_idx << 9) + cell_id;
-  uint32_t       v      = x1[wi];
-#pragma unroll
-  for (uint32_t b = 0; b < 31; b++)
-    if ((c_init >> b) & 1u) v ^= basis[(size_t)b * basis_words + wi];
-  seq_pool[g.scr_off + wi] = v;
-}
-
 // RI / ACK / CQI position of the symbol in row k, column c of the R' = M x 12 channel-interleaver matrix (36.212 5.2.2.7 / 5.2.2.8, normal CP:
 // RI in columns {1,4,7,10}, ACK in {2,3,8,9}, both filled from the bottom row upwards in column-set order 0,3,2,1; CQI first in the row-major stream).
 // kind 0 data, 1 CQI, 2 RI, 3 ACK over data (erasure), 4 ACK over CQI; dpos = index of the symbol in the UL-SCH stream
@@ -238,25 +193,17 @@ __global__ void __launch_bounds__(256) pusch_kernel(const __grid_constant__ DevC
       uint32_t       dpos;
       const uint32_t kind = uci_pos(M, k, cc, g.qp_ack, g.qp_ri, g.qp_cqi, dpos);
       if (kind != 0 && kind != 3) continue;
-      const float2 zz = src[s * M + k];
-      short        z[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-      if (zz.x != 0.0f || zz.y != 0.0f) ul_demod_s(make_float2(zz.x * scl, zz.y * scl), qm, z); // an exactly zero sample is an erasure: LLR 0
-      const uint32_t hb0 = (cc * M + k) * qm;
-      for (uint32_t b = 0; b < qm; b++) {
-        const uint32_t hb = hb0 + b, sbit = (seq[hb >> 5] >> (hb & 31)) & 1u;
-        out[dpos * qm + b] = kind == 3 ? (short)0 : (sbit ? (short)-z[b] : z[b]);
-      }
+      const float2 zz = kind == 3 ? make_float2(0.0f, 0.0f) : src[s * M + k]; // ACK over data: erased, zero soft bits
+      soft_bits(zz, scl, qm, seq, (cc * M + k) * qm, out + dpos * qm);
     }
     __syncthreads();
   }
 }
 
-extern "C" void launch_pusch(const DevCell& c, const DevUlGrant* grants, uint32_t ngrants, uint32_t max_M, uint32_t max_words, const float2* ulsym,
-                             const float2* dmrs_pool, const float2* idft_pool, const uint32_t* x1, const uint32_t* basis, uint32_t basis_words,
-                             uint32_t* seq_pool, short* llr_pool, DevUlChest* chest, cudaStream_t st, uint64_t* launches)
+extern "C" void launch_pusch(const DevCell& c, const DevUlGrant* grants, uint32_t ngrants, uint32_t max_M, const float2* ulsym, const float2* dmrs_pool,
+                             const float2* idft_pool, const uint32_t* seq_pool, short* llr_pool, DevUlChest* chest, cudaStream_t st, uint64_t* launches)
 {
   if (!ngrants) return;
-  scr_seq_ul_kernel<<<dim3(ngrants, (max_words + 255) / 256), 256, 0, st>>>(grants, x1, basis, basis_words, c.cell_id, seq_pool);
   // ls [2][M], sm [A][2][M], W [M] and the two IDFT buffers: 86 KB at M = 1200 with one antenna, 106 KB with two (two CTAs per SM either way)
   const size_t smem = ((size_t)(3 + 2 * c.ul_nof_rx) * max_M + 2 * PUSCH_PASS_CAP) * sizeof(float2);
   const int    cap  = (int)(((3 + 2 * c.ul_nof_rx) * 1200 + 2 * PUSCH_PASS_CAP) * sizeof(float2));
@@ -267,5 +214,5 @@ extern "C" void launch_pusch(const DevCell& c, const DevUlGrant* grants, uint32_
     cudaFuncSetAttribute(pusch_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap);
     pusch_kernel<1><<<ngrants, 256, smem, st>>>(c, grants, ulsym, dmrs_pool, idft_pool, seq_pool, llr_pool, chest, max_M);
   }
-  *launches += 2;
+  *launches += 1;
 }

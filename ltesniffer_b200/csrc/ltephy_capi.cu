@@ -50,14 +50,18 @@ void ltephy_pull(ltephy* h, void* dst_dev, const void* src_pinned, size_t bytes,
   h->launches++;
 }
 static void pull(ltephy* h, void* dst_dev, const void* src_pinned, size_t bytes) { ltephy_pull(h, dst_dev, src_pinned, bytes, h->stream); }
-// stage `bytes` from pageable memory into the handle's pinned arena (16-byte slots) and pull them to dst_dev
+// copy `bytes` from pageable memory into the handle's pinned arena (16-byte slots, consecutive calls take consecutive slots)
+static uint8_t* stage(ltephy* h, const void* src, size_t bytes)
+{
+  uint8_t* slot = h->h_stage.p + h->stage_used;
+  if (bytes) memcpy(slot, src, bytes);
+  h->stage_used += (bytes + 15) & ~(size_t)15;
+  return slot;
+}
+// stage `bytes` and pull them to dst_dev
 static void stage_and_pull(ltephy* h, void* dst_dev, const void* src, size_t bytes)
 {
-  if (!bytes) return;
-  uint8_t* slot = h->h_stage.p + h->stage_used;
-  memcpy(slot, src, bytes);
-  h->stage_used += (bytes + 15) & ~(size_t)15;
-  pull(h, dst_dev, slot, bytes);
+  if (bytes) pull(h, dst_dev, stage(h, src, bytes), bytes);
 }
 
 extern "C" const char* ltephy_last_error(void) { return ltephy_g_err.c_str(); }
@@ -514,14 +518,15 @@ static int add_transport_block(ltephy* h, uint32_t tbs, uint32_t G, uint32_t qm,
   b.tbs.push_back(tb);
   return LTEPHY_SUCCESS;
 }
-// LLR and scrambling space of one codeword: G soft bits, scrambled with the first `bits` bits of the Gold sequence (PDSCH: G, PUSCH: 12 M Qm);
-// false if the scrambling basis is shorter
-static bool alloc_codeword(ltephy* h, uint32_t bits, uint32_t G, uint64_t& llr_off, uint32_t& scr_off)
+// LLR and scrambling space of one codeword: G soft bits, scrambled with the first `bits` bits of the Gold sequence of c_init (PDSCH: G,
+// PUSCH: 12 M Qm), whose words go on scr_seq_kernel's list; false if the scrambling basis is shorter
+static bool alloc_codeword(ltephy* h, uint32_t bits, uint32_t G, uint32_t c_init, uint64_t& llr_off, uint32_t& scr_off)
 {
   ltephy::PhaseB& b = h->pb;
   const uint32_t  w = (bits + 31) / 32;
   if (w > h->gold_words) return false;
   llr_off = b.pllr_elems, scr_off = (uint32_t)b.seq_words;
+  b.scr.push_back(DevScr{c_init, w, scr_off});
   b.max_scr_words = std::max(b.max_scr_words, w);
   b.seq_words += w + 1; // +1: the demapper reads a 64-bit window
   b.pllr_elems += (G + 7) & ~7u;
@@ -662,7 +667,8 @@ static int build_jobs(ltephy* h, const ltephy_grant_t* gin, uint32_t n)
       const uint32_t qm = g.tb[t].qm, G = acc * qm;
       if (qm != 2 && qm != 4 && qm != 6 && qm != 8) return fail(LTEPHY_ERROR_INVALID_INPUTS, "grant %u: bad modulation order", gi);
       d.qm[cw] = qm;
-      if (!alloc_codeword(h, G, G, d.llr_off[cw], d.scr_off[cw])) return fail(LTEPHY_ERROR, "grant %u: codeword longer than the scrambling basis", gi);
+      const uint32_t c_init = (d.rnti << 14) + (cw << 13) + (d.sf_idx << 9) + c.cell_id; // 36.211 6.3.1
+      if (!alloc_codeword(h, G, G, c_init, d.llr_off[cw], d.scr_off[cw])) return fail(LTEPHY_ERROR, "grant %u: codeword longer than the scrambling basis", gi);
       if (g.tb[t].tbs > 0) {
         uint32_t tbi;
         int r = add_transport_block(h, (uint32_t)g.tb[t].tbs, G, qm, g.tb[t].rv, g.tx_scheme == LTEPHY_TX_DIVERSITY ? 2 : 1, d.llr_off[cw], tbi,
@@ -741,13 +747,28 @@ static int reserve_phase_b(ltephy* h, size_t grant_bytes)
   const ltephy::PhaseB& b = h->pb;
   if (h->stage_busy) CU(cudaStreamSynchronize(h->stream)); // a phase B that was never fetched may still be pulling from the arena
   h->stage_used = 0, h->stage_busy = true;
-  if (h->h_stage.reserve(grant_bytes + b.tbs.size() * sizeof(DevTb) + b.pairs.size() * (sizeof(DevPair) + 4) + b.cbs.size() * sizeof(DevCb) + 256))
+  const size_t scr_bytes = b.scr.size() * sizeof(DevScr);
+  if (h->h_stage.reserve(grant_bytes + b.tbs.size() * sizeof(DevTb) + scr_bytes + b.pairs.size() * (sizeof(DevPair) + 4) + b.cbs.size() * sizeof(DevCb) + 256))
     return fail(LTEPHY_ERROR, "pinned allocation failed");
-  if (h->d_tbs.reserve(b.tbs.size() + 1) || h->d_seq.reserve(b.seq_words + 1) || h->d_pllr.reserve(b.pllr_elems + 8) || h->d_turbo.reserve(b.turbo_words + 1) ||
-      h->d_payload.reserve(b.payload_bytes + 4) || h->d_cb_iters.reserve(b.cbs.size() + 1) || h->d_cb_crc.reserve(b.cbs.size() + 1) ||
+  if (h->d_tbs.reserve(b.tbs.size() + (scr_bytes + sizeof(DevTb) - 1) / sizeof(DevTb) + 1) || h->d_seq.reserve(b.seq_words + 1) ||
+      h->d_pllr.reserve(b.pllr_elems + 8) || h->d_turbo.reserve(b.turbo_words + 1) || h->d_payload.reserve(b.payload_bytes + 4) || h->d_cb_iters.reserve(b.cbs.size() + 1) || h->d_cb_crc.reserve(b.cbs.size() + 1) ||
       h->d_res.reserve(b.tbs.size() + 1) || h->h_res.reserve(b.tbs.size() + 1) || h->h_payload.reserve(b.payload_bytes + 4))
     return fail(LTEPHY_ERROR, "device allocation failed");
   return LTEPHY_SUCCESS;
+}
+
+// The start of every PDSCH / PUSCH phase B, after the caller has staged its grants: stage the transport blocks (tb_crc) and the codeword
+// list (scr_seq_kernel) behind them, both into d_tbs with one pull, then write every codeword's scrambling sequence
+static void stage_tbs_and_scramble(ltephy* h)
+{
+  static_assert(sizeof(DevTb) % 16 == 0, "the codeword list must start in the arena slot right behind the transport blocks");
+  const ltephy::PhaseB& b = h->pb;
+  const size_t          tb_bytes = b.tbs.size() * sizeof(DevTb), scr_bytes = b.scr.size() * sizeof(DevScr);
+  uint8_t*              slot = stage(h, b.tbs.data(), tb_bytes);
+  stage(h, b.scr.data(), scr_bytes);
+  pull(h, h->d_tbs.p, slot, tb_bytes + scr_bytes);
+  launch_scr_seq(reinterpret_cast<const DevScr*>(h->d_tbs.p + b.tbs.size()), (uint32_t)b.scr.size(), b.max_scr_words, h->d_gold_x1, h->d_gold_basis,
+                 h->gold_words, h->d_seq.p, h->stream, &h->launches);
 }
 
 extern "C" int ltephy_submit_grants(ltephy_t* h, const ltephy_grant_t* gin, uint32_t n)
@@ -761,9 +782,8 @@ extern "C" int ltephy_submit_grants(ltephy_t* h, const ltephy_grant_t* gin, uint
   CU(cudaEventRecord(h->ev[2], h->stream));
   if (n) {
     stage_and_pull(h, h->d_grants.p, b.grants.data(), n * sizeof(DevGrant));
-    stage_and_pull(h, h->d_tbs.p, b.tbs.data(), b.tbs.size() * sizeof(DevTb));
-    launch_pdsch_front(h->dc, h->d_grants.p, n, b.max_scr_words, h->d_sym.p, h->d_pil.p, h->d_gold_x1, h->d_gold_basis, h->gold_words, h->d_seq.p,
-                       h->d_pllr.p, h->stream, &h->launches);
+    stage_tbs_and_scramble(h);
+    launch_pdsch_front(h->dc, h->d_grants.p, n, h->d_sym.p, h->d_pil.p, h->d_seq.p, h->d_pllr.p, h->stream, &h->launches);
     CU(cudaGetLastError()); // a front kernel that could not launch would leave the previous batch's sequences and soft bits behind
     if (int r = decode_code_blocks(h)) return r;
   }
@@ -1137,7 +1157,8 @@ static int submit_ul_common(ltephy_t* h, const void* iq_host, const void* iq_dev
     }
     if (ul_table_for(h, 1, M, 0, 0, 0, d.idft_off)) return fail(LTEPHY_ERROR, "UL table upload failed");
     const uint32_t G = L.G;
-    if (!alloc_codeword(h, 12 * M * g.qm, G, d.llr_off, d.scr_off)) return fail(LTEPHY_ERROR, "UL grant %u: codeword longer than the scrambling basis", gi);
+    const uint32_t c_init = (d.rnti << 14) + (d.sf_idx << 9) + c.cell_id; // 36.211 5.3.1
+    if (!alloc_codeword(h, 12 * M * g.qm, G, c_init, d.llr_off, d.scr_off)) return fail(LTEPHY_ERROR, "UL grant %u: codeword longer than the scrambling basis", gi);
     if (G < g.qm * 12) return fail(LTEPHY_ERROR_INVALID_INPUTS, "UL grant %u: the control information leaves no room for the transport block", gi);
     max_M = std::max(max_M, M);
     uint32_t tbi;
@@ -1151,9 +1172,8 @@ static int submit_ul_common(ltephy_t* h, const void* iq_host, const void* iq_dev
   if (h->d_ulgrants.reserve(ng + 1) || h->d_ulchest.reserve(ng + 1) || h->h_ulchest.reserve(ng + 1)) return fail(LTEPHY_ERROR, "device allocation failed");
   if (ng) {
     stage_and_pull(h, h->d_ulgrants.p, b.ulgrants.data(), ng * sizeof(DevUlGrant));
-    stage_and_pull(h, h->d_tbs.p, b.tbs.data(), b.tbs.size() * sizeof(DevTb));
-    launch_pusch(c, h->d_ulgrants.p, ng, max_M, b.max_scr_words, h->d_ulsym.p, h->d_ulpool.p, h->d_ulpool.p, h->d_gold_x1, h->d_gold_basis, h->gold_words,
-                 h->d_seq.p, h->d_pllr.p, h->d_ulchest.p, h->stream, &h->launches);
+    stage_tbs_and_scramble(h);
+    launch_pusch(c, h->d_ulgrants.p, ng, max_M, h->d_ulsym.p, h->d_ulpool.p, h->d_ulpool.p, h->d_seq.p, h->d_pllr.p, h->d_ulchest.p, h->stream, &h->launches);
     CU(cudaGetLastError()); // as in ltephy_submit_grants
     if (int r = decode_code_blocks(h)) return r;
   }

@@ -167,6 +167,7 @@ struct ltephy {
     std::vector<CbHalf>     cb_half; // [code block]
     std::vector<DevPair>    pairs;
     std::vector<DevTb>      tbs;
+    std::vector<DevScr>     scr;     // [codeword] scrambling sequence to write (alloc_codeword)
     std::vector<uint32_t>   pair_pi_off;
     std::vector<uint32_t>   tb_slot; // result slot (DL: grant*2 + tb, UL: grant) -> tb index or ~0
     std::map<uint32_t, uint32_t> harq_uses; // slot -> uses in this batch
@@ -176,7 +177,7 @@ struct ltephy {
     uint32_t                max_scr_words = 0;              // longest codeword's scrambling words
     void reset(size_t nslots)
     {
-      grants.clear(), ulgrants.clear(), cbs.clear(), cb_half.clear(), pairs.clear(), tbs.clear(), pair_pi_off.clear(), harq_uses.clear();
+      grants.clear(), ulgrants.clear(), cbs.clear(), cb_half.clear(), pairs.clear(), tbs.clear(), scr.clear(), pair_pi_off.clear(), harq_uses.clear();
       tb_slot.assign(nslots, 0xFFFFFFFFu);
       harq_max_gen = 0, payload_bytes = 0, pllr_elems = 0, seq_words = 0, turbo_words = 0, max_scr_words = 0;
     }
@@ -184,7 +185,7 @@ struct ltephy {
   DevBuf<DevGrant>      d_grants;
   DevBuf<DevCb>         d_cbs;
   DevBuf<DevPair>       d_pairs;
-  DevBuf<DevTb>         d_tbs;
+  DevBuf<DevTb>         d_tbs;       // pb.tbs, then pb.scr (stage_tbs_and_scramble)
   DevBuf<uint32_t>      d_pair_pi_off;
   DevBuf<uint32_t>      d_seq, d_turbo;
   DevBuf<uint16_t>      d_rm;        // pool of rate-matching inverse tables (pool_append), rm_used entries filled
